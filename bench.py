@@ -2,7 +2,7 @@
 """Benchmark of the ChronoEdit denoising hot path (BASELINE.json metric: DiT denoising steps/sec at 14B, 720x1280,
 5 pixel frames = 2 latent frames).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" = one iteration of the sampling loop of ChronoEditPipeline.__call__ (pipeline_chronoedit.py:695-753) for ONE
 edit with classifier-free guidance: two DiT forwards (prompt / negative prompt — evaluated as one batch-2 call, which the
@@ -16,10 +16,14 @@ Printed JSON (one line, rank 0):
   value     steps/s summed over ranks, inputs resident in HBM, timed with CUDA events, max over ranks
   e2e       the same step through the host-buffer C-ABI call (ce_dit_forward_host): pinned-host inputs H2D every step,
             sample D2H every step, CFG combine + latent update on the host
-  roofline  the dominant kernel class (tcgen05 GEMM): algorithmic FLOPs / device time of those launches measured live
-            with CUDA events inside the timed region, against MEASURED_PEAKS.json bf16_tflops_sustained
+  roofline  the dominant kernel class (wgmma GEMM): algorithmic FLOPs / device time of those launches measured live
+            with CUDA events inside the timed region, against the H100 SXM data-sheet rate (989 TFLOP/s dense bf16 at
+            700 W; a power-limited card runs below it)
   cpu_baseline  the oracle (CPU restatement of the reference) timed on the host cores on a bounded sample
---impl reference times that CPU path alone with the same metric/config (the reference has no faster path on this box).
+--impl reference times that CPU path alone with the same metric/config.
+--dump-outputs DIR writes, after the timed steps, what the timed path returned in its last step as DIR/<name>.npy (float32):
+the DiT sample of the CFG pair and the updated latents (--impl reference: a seeded sample of the block output).  Inputs and
+weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -45,16 +49,32 @@ def model_config(layers: int):
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured"
-    return 1400.0, 6650.0, "fallback"
+    """Denominators of the roofline fractions: NVIDIA's data sheet for the H100 SXM at 700 W (dense bf16 TFLOP/s, HBM3 GB/s).  A
+    power-limited card runs below them; the card's name, clocks and power draw are printed beside the numbers."""
+    return 989.0, 3350.0, "H100 SXM data sheet (700 W)"
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(directory: str, arrays: dict):
+    """DIR/<name>.npy in float32, at most 64 MB in all: an array over its share is replaced by a fixed, seeded sample of its elements."""
+    import numpy as np
+
+    os.makedirs(directory, exist_ok=True)
+    if not arrays:   # no timed step ran
+        return
+    share = DUMP_LIMIT_BYTES // (4 * len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.size > share:
+            idx = np.random.default_rng(0).choice(a.size, size=share, replace=False)
+            a = a.reshape(-1)[np.sort(idx)]
+        np.save(os.path.join(directory, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / power / throttle reasons DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -107,7 +127,7 @@ def cpu_reference_step_rate(reps: int, warmup: int = 0):
     the 720p / 2-latent-frame sequence, 769 context tokens -- in fp32 on the host cores with the oracle, `reps` times (each ~3-10 s).
     A denoising step with CFG is 2 forwards x 40 such blocks (identical work; the embedders / head are < 0.1 %), so the step rate is
     1 / (80 x the measured block time): the only scaling is the count of identical blocks, no token-count or FLOP extrapolation.
-    Returns (steps_per_sec, seconds per block list, threads, description)."""
+    Returns (steps_per_sec, seconds per block list, threads, description, output of the last timed block)."""
     import torch
 
     from oracle import dit_oracle as O
@@ -140,7 +160,7 @@ def cpu_reference_step_rate(reps: int, warmup: int = 0):
         torch.set_num_threads(cores)
         for i in range(warmup + reps):
             t0 = time.perf_counter()
-            O.block(sd, 0, one, x, ctx, temb6, freqs)
+            y = O.block(sd, 0, one, x, ctx, temb6, freqs)
             dt = time.perf_counter() - t0
             if i >= warmup:
                 times.append(dt)
@@ -148,7 +168,7 @@ def cpu_reference_step_rate(reps: int, warmup: int = 0):
     step_s = 2 * 40 * t_block
     desc = (f"one full 14B-width DiT block (oracle, fp32) on all 7200 tokens, measured {reps}x ({t_block:.2f} s each), {cores} threads; "
             f"step = 2 CFG forwards x 40 identical blocks = 80 x the measured block")
-    return 1.0 / step_s, times, cores, desc
+    return 1.0 / step_s, times, cores, desc, y
 
 
 def cpu_extras(threads: int):
@@ -183,7 +203,9 @@ def run_reference_arm(args):
     if rank != 0:
         return
     t0 = time.perf_counter()
-    rate, times, cores, desc = cpu_reference_step_rate(args.steps, args.warmup)
+    rate, times, cores, desc, y = cpu_reference_step_rate(args.steps, args.warmup)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"block_output": y})
     ms_per_step = 1000.0 / rate
     line = {
         "impl": "reference", "metric": METRIC, "value": rate, "unit": "steps/s", "n_gpus": args.gpus, "steps": args.steps,
@@ -218,17 +240,6 @@ def dit_flops_per_forward(layers: int, frames: int, lat_h: int, lat_w: int, text
 
 VAE_ENCODE_FLOP = 24577494220800.0   # conv FLOPs of one 5 x 720 x 1280 encode / decode (SURVEY 8d: 24.58 / 41.04 TFLOP)
 VAE_DECODE_FLOP = 41036724633600.0
-
-
-def traffic(kernel: str, field: str = "dram_bytes"):
-    """Per-launch DRAM traffic of a kernel class from profiles/traffic.json (written by scripts/summarize_profiles.py from the
-    committed `ncu --set full` captures); None when there is no capture for it."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if not os.path.exists(p):
-        return None
-    with open(p) as f:
-        d = json.load(f)
-    return (d.get(kernel) or {}).get(field)
 
 
 def library_bar_step_rate(model, d_in, d_text, d_img, dev, layers: int, steps: int = 2):
@@ -272,7 +283,7 @@ def library_bar_step_rate(model, d_in, d_text, d_img, dev, layers: int, steps: i
 
 
 def init_weights_(model, seed: int):
-    """Random-init weights of the 14B architecture directly on the device (there is no checkpoint on the box):
+    """Random-init weights of the 14B architecture directly on the device (the benchmark needs no checkpoint):
     Linear ~ N(0, 0.02), norms ~ 1 + 0.1 N, scale_shift_table ~ N(0,1)/sqrt(D) (as transformer_chronoedit.py:265, 393)."""
     import math
 
@@ -350,6 +361,8 @@ def run_ours(args):
     d_lat = d_lat.to(torch.bfloat16)   # the diffusers pipeline keeps bf16 latents (pipeline_chronoedit.py:676-687)
     d_in = torch.cat([d_lat, d_cond], dim=1).contiguous()
 
+    last = {}   # what the last device_step returned to its caller (--dump-outputs)
+
     def device_step(i):
         nonlocal d_lat
         if sched.step_index is None or sched.step_index >= 50:
@@ -357,6 +370,7 @@ def run_ours(args):
         t = sched.timesteps[sched.step_index or 0]
         out = model(d_in.expand(2, -1, -1, -1, -1), t.expand(2), d_text, d_img, return_dict=False)[0]
         d_lat = sched.step_cfg(out[0:1], out[1:2], GUIDANCE, t, d_lat, model_input_out=d_in)
+        last["sample"], last["latents"] = out, d_lat
 
     # host-buffer (e2e) step = the SAME loop body through the host-facing call: every step the model input (built on the host from
     # the host copy of the latents), the timestep and the prompt / image embeddings go pinned-host -> device inside
@@ -441,6 +455,8 @@ def run_ours(args):
         model.clear_context_cache()
     dev_ms, wall_ms, _, clocks = timed(counted_step, args.steps, 0, sampler, profile=False)
     model.use_cuda_graph = False
+    if args.dump_outputs and rank == 0:   # before the later passes step the latents further
+        dump_outputs(args.dump_outputs, last)
     launches = launch_count["n"]
     value = world * args.steps / (dev_ms / 1000.0)
     # pass 2 -- the per-class split (CUDA events around every launch; slightly slower, not the reported value)
@@ -507,7 +523,7 @@ def run_ours(args):
 
     # library bar (SURVEY 8d "reference GPU path"): the oracle's functional restatement of the reference evaluated by torch eager on
     # this GPU in the reference's bf16 configuration = cuBLAS GEMMs + SDPA (cuDNN fused attention as the reference's own dispatch
-    # picks on cc 10.0, chronoedit/_src/modules/attention.py:129-138) + ATen elementwise, same weights, same step (2 forwards + CFG
+    # prefers where it is available, chronoedit/_src/modules/attention.py:129-138) + ATen elementwise, same weights, same step (2 forwards + CFG
     # + scheduler glue in torch).  A reported bar next to `value`, timed with CUDA events; not part of any timed region above.
     library_bar = None
     if rank == 0 and world == 1 and not args.no_library_bar:
@@ -549,19 +565,11 @@ def run_ours(args):
                     "steps": e2e_steps, "ms_per_step": e2e_wall_ms / e2e_steps},
             "gpu_launches": launches,
             "roofline": {
-                "bound": "tensor", "kernel": "gemm_bf16_2cta_kernel / gemm_bf16_kernel (tcgen05, all Linear layers)",
-                "achieved": gemm_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": gemm_tf / peak_tf, "peak_source": peak_src + " bf16_tflops_sustained",
-                # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full captures, as summarised
-                # into profiles/traffic.json by scripts/summarize_profiles.py (null when that file has no entry for the kernel)
-                "traffic": traffic("gemm"), "traffic_launch": traffic("gemm", "launch"),
-                "algorithmic_bytes_of_that_launch": traffic("gemm", "algorithmic_bytes"),
+                "bound": "tensor", "kernel": "gemm_bf16_kernel (wgmma, all Linear layers)",
+                "achieved": gemm_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": gemm_tf / peak_tf, "peak_source": peak_src,
                 "launches": prof["count"][0], "ms_total": prof["ms"][0], "split_pass_steps": split_steps, "split_pass_ms_per_step": split_ms / split_steps,
                 "share_of_kernel_time": prof["ms"][0] / kernel_ms if kernel_ms else None,
-                "attention": {"achieved": attn_tf, "frac": attn_tf / peak_tf, "ms_total": prof["ms"][1], "launches": prof["count"][1],
-                              "traffic": traffic("attention"), "traffic_launch": traffic("attention", "launch"),
-                              "algorithmic_bytes_of_that_launch": traffic("attention", "algorithmic_bytes")},
-                "conv": {"traffic": traffic("conv"), "traffic_launch": traffic("conv", "launch"),
-                         "algorithmic_bytes_of_that_launch": traffic("conv", "algorithmic_bytes")},
+                "attention": {"achieved": attn_tf, "frac": attn_tf / peak_tf, "ms_total": prof["ms"][1], "launches": prof["count"][1]},
                 "rows_ms_total": prof["ms"][2], "other_ms_total": prof["ms"][3],
                 "whole_step": {"algorithmic_tflop_per_step": flops_fwd / 1e12, "achieved": flops_fwd / 1e12 / (dev_ms / args.steps / 1000.0),
                                "frac": flops_fwd / 1e12 / (dev_ms / args.steps / 1000.0) / peak_tf},
@@ -572,7 +580,7 @@ def run_ours(args):
         }
         line["library_bar"] = library_bar
         if world == 1 and not args.no_cpu_baseline:
-            rate, times, cores, desc = cpu_reference_step_rate(reps=2, warmup=1)
+            rate, times, cores, desc, _ = cpu_reference_step_rate(reps=2, warmup=1)
             line["cpu_baseline"] = {"value": rate, "unit": "steps/s", "cores": cores, "kind": "port", "sample": desc,
                                     "extrapolated": "x80 identical blocks only (full token count measured)"}
             try:
@@ -595,6 +603,8 @@ def main():
     ap.add_argument("--no-library-bar", action="store_true")
     ap.add_argument("--cuda-graph", action="store_true", help="replay the DiT forward as a CUDA graph in the value pass (A/B)")
     ap.add_argument("--no-context-cache", action="store_true", help="recompute the step-invariant context every step (round-1 behaviour)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<name>.npy (float32, at most 64 MB in all)")
     ap.add_argument("--no-vae", action="store_true", help="skip the (untimed-region) VAE encode/decode measurement")
     ap.add_argument("--latent-frames", type=int, default=2, choices=[2, 8],
                     help="DEV ONLY: 8 = the temporal-reasoning geometry of configs[2] (28 800 tokens); not the headline workload")

@@ -1,4 +1,4 @@
-"""chronoedit_b200 — B200-native (sm_100a) implementation of the ChronoEdit denoising hot path.
+"""chronoedit_b200 — H100-native (sm_90a) implementation of the ChronoEdit denoising hot path.
 
 Public surface (drop-in for the objects `ChronoEditPipeline` registers, pipeline_chronoedit.py:175-183):
   ChronoEditTransformer3DModel   <- chronoedit_diffusers/transformer_chronoedit.py:298-476

@@ -1,7 +1,7 @@
 """ctypes binding of libchronoedit_b200.so (the C ABI declared in include/chronoedit_b200.h).
 
 There is no CPU or PyTorch fallback: if the shared library is missing this module raises, and every compute
-entry point fails on a machine without an sm_100 GPU.
+entry point fails on a machine without an sm_90 GPU.
 """
 from __future__ import annotations
 

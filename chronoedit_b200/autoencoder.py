@@ -1,4 +1,4 @@
-"""B200-native drop-in for diffusers `AutoencoderKLWan` as `ChronoEditPipeline` uses it.
+"""H100-native drop-in for diffusers `AutoencoderKLWan` as `ChronoEditPipeline` uses it.
 
 What the unchanged pipeline touches (pipeline_chronoedit.py:119-129, 185-186, 427-445, 672, 765-781):
     vae.encode(x).latent_dist.mode() / .sample(generator)      x  [B,3,T,H,W] in [-1,1]
@@ -8,7 +8,7 @@ diffusers' class is un-vendored; the arithmetic follows the in-tree twin
 /root/reference/chronoedit/_src/tokenizers/wan2pt1.py (WanVAE_, :467-581) with the diffusers deltas of SURVEY.md
 section 8c: no latent mean/std inside encode/decode, decode clamps to [-1,1].  Parameter names are the twin's
 (`encoder.downsamples.0.residual.2.weight`, ...); `diffusers_key_map()` gives the best-effort rename from a diffusers
-checkpoint.  All arithmetic runs in libchronoedit_b200.so (tcgen05 implicit-GEMM convolutions etc.); no PyTorch fallback.
+checkpoint.  All arithmetic runs in libchronoedit_b200.so (wgmma implicit-GEMM convolutions etc.); no PyTorch fallback.
 """
 from __future__ import annotations
 
@@ -223,7 +223,7 @@ class AutoencoderKLWan(nn.Module):
     def pack_weights(self) -> None:
         L = _lib.lib()
         if self.device.type != "cuda":
-            raise CEError("AutoencoderKLWan must live on a CUDA (sm_100) device; there is no CPU path")
+            raise CEError("AutoencoderKLWan must live on a CUDA (sm_90) device; there is no CPU path")
         if self._handle is None:
             c = self.config
             cfg = VAEConfigC(c.base_dim, c.z_dim, (_lib.c_int32 * 4)(*c.dim_mult), c.num_res_blocks,

@@ -1,4 +1,4 @@
-"""Build libchronoedit_b200.so in-tree with nvcc for sm_100a (cross-compiles on a GPU-less box).
+"""Build libchronoedit_b200.so in-tree with nvcc for sm_90a (cross-compiles on a GPU-less box).
 
     python -m chronoedit_b200.build [--force]
 
@@ -19,7 +19,7 @@ LIB = os.path.join(HERE, "lib", "libchronoedit_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
     "-I", INCLUDE, "-I", CSRC,
 ]
@@ -29,7 +29,7 @@ def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found: chronoedit_b200 needs the CUDA 12.9 toolkit to build its sm_100a kernels")
+    raise RuntimeError("nvcc not found: chronoedit_b200 needs the CUDA 12.9 toolkit to build its sm_90a kernels")
 
 
 def sources():
@@ -63,7 +63,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         for l in logs:
             sys.stderr.write(l)
     if jobs or not os.path.exists(LIB):
-        run([nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"])
+        run([nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

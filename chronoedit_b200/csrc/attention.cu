@@ -1,27 +1,22 @@
-// Non-causal multi-head attention forward for sm_100a (head_dim 128), flash-style, on tcgen05.
+// Non-causal multi-head attention forward for sm_90a (head_dim 128), flash-style, on wgmma.
 //
 //   out[b, i, h*128:(h+1)*128] = softmax_j( q[b,i,h,:] . k[b,j,h,:] * scale ) @ v[b,j,h,:]
 //
 // One CTA per (128-query tile, head, batch); 384 threads = 3 warpgroups (registers re-partitioned with setmaxnreg):
-//   warp 0      TMA producer: Q tile once, then K_j / V_j tiles (128 keys) through 2-deep rings
-//   warp 1      MMA issuer:   S_j = Q K_j^T  (M128 N128 K128, accumulator S_{j&1} in TMEM)
-//                             O_{j&1} += P_j V_j (P_j from shared memory, V_j as MN-major B operand)
-//   warps 4-7   softmax group 0 (even key tiles), warps 8-11 softmax group 1 (odd key tiles): the thread's whole
-//               128-wide score row TMEM -> registers in one go, max / exp2 / sum as independent chains (fp32),
-//               bf16 P -> shared memory (128B-swizzled A tile)
-// The two groups keep INDEPENDENT online-softmax streams (own max, sum and O accumulator) that are merged once
-// at the end, so S_{j+1} and softmax_j / PV_j overlap without any cross-group exchange in the loop.
-// O is rescaled lazily: only when the row max grows by more than 2^8 (values stay bounded, result identical
-// after the final normalisation).
+//   warpgroup 0     TMA producer (one lane of warp 0): Q tile once, then K_j / V_j tiles (128 keys) through 2-deep rings
+//   warpgroups 1,2  one 64-query half of the tile each, everything in registers:
+//                   S_j = Q K_j^T (wgmma, both operands from shared memory), online softmax (fp32: running max, exp2, running sum),
+//                   O += P_j V_j (wgmma, bf16 P_j straight from the S accumulator registers as the A operand, V_j as MN-major B)
+// The two warpgroups run independently, so the softmax of one overlaps the MMAs of the other on the tensor cores.
+// With a second key/value source (text + image cross-attention) the same CTA walks the second source after the first and adds
+// its separately normalised, bf16-rounded result to the first one's.
 //
-// TMEM (512 columns): S0 [0,128) S1 [128,256) O0 [256,384) O1 [384,512).
-// Shared memory: Q 32K | K 2x32K | V 2x32K | P 2x32K | barriers.
+// Shared memory: Q 32K | K 2x32K | V 2x32K | barriers.
 //
-// Replaces F.scaled_dot_product_attention at /root/reference/chronoedit_diffusers/transformer_chronoedit.py:91-99
+// Replaces F.scaled_dot_product_attention at chronoedit_diffusers/transformer_chronoedit.py:91-99 of the reference
 // (self-attention, text cross-attention and image cross-attention; the latter two are summed, :103-104).
-#include <stdlib.h>
-
 #include "attention.cuh"
+#include "wgmma.cuh"
 
 namespace ce {
 
@@ -33,19 +28,17 @@ constexpr int BKV = 128;
 constexpr int ATTN_THREADS = 384;
 constexpr uint32_t TILE_BYTES = 128 * 128 * 2;  // 32 KB: two 16 KB [128 x 64] swizzled blocks
 constexpr uint32_t HALF_BYTES = TILE_BYTES / 2;
-constexpr float RESCALE_THRESHOLD = 8.0f;       // log2 units
 
 struct SmemLayout {
   static constexpr uint32_t q = 0;
   static constexpr uint32_t k = q + TILE_BYTES;
   static constexpr uint32_t v = k + 2 * TILE_BYTES;
-  static constexpr uint32_t p = v + 2 * TILE_BYTES;
-  static constexpr uint32_t bars = p + 2 * TILE_BYTES;
+  static constexpr uint32_t bars = v + 2 * TILE_BYTES;
   static constexpr uint32_t total = bars + 256;
 };
 
 // barrier indices
-enum { Q_FULL = 0, K_FULL = 1, K_EMPTY = 3, V_FULL = 5, V_EMPTY = 7, S_FULL = 9, P_FULL = 11, PV_DONE = 13, S_FREE = 15, NUM_BARS = 17 };
+enum { Q_FULL = 0, K_FULL = 1, K_EMPTY = 3, V_FULL = 5, V_EMPTY = 7, NUM_BARS = 9 };
 
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
@@ -53,28 +46,19 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_con
                      const __grid_constant__ CUtensorMap tma_v2, AttnArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SmemLayout::bars);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NUM_BARS);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * BQ;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
-  // Key tiles are dealt to the two softmax groups g = 0, 1 as (g, t), t = 0..T[g]-1:
-  //   single source: tile index 2t + g of k/v (even / odd tiles), streams merged as ONE softmax at the end;
-  //   dual source  : group 0 walks k/v (Lk keys), group 1 walks k2/v2 (Lk2 keys); the two attention results are summed.
-  const bool dual = a.Lk2 > 0;
-  const int n_tiles = (a.Lk + BKV - 1) / BKV;
-  const int T0 = dual ? n_tiles : (n_tiles + 1) / 2;
-  const int T1 = dual ? (a.Lk2 + BKV - 1) / BKV : n_tiles / 2;
-  const int Tmax = T0 > T1 ? T0 : T1;
+  // key tiles of source 0 (k / v, Lk keys), then of source 1 (k2 / v2, Lk2 keys; none for a single source), through one ring
+  const int T0 = (a.Lk + BKV - 1) / BKV;
+  const int T1 = (a.Lk2 + BKV - 1) / BKV;
 
   if (threadIdx.x == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) {
-      printf("[chronoedit_b200] attention: dynamic shared memory not 1024-byte aligned\n");
-      __trap();
-    }
-    for (int i = 0; i < NUM_BARS; ++i) mbar_init(&bars[i], (i == P_FULL || i == P_FULL + 1 || i == S_FREE || i == S_FREE + 1) ? 128 : 1);
+    if ((smem_u32(smem) & 1023u) != 0) __trap();  // the swizzled tiles need 1024-byte alignment
+    for (int i = 0; i < NUM_BARS; ++i) mbar_init(&bars[i], (i >= K_EMPTY && i < K_EMPTY + 2) || (i >= V_EMPTY && i < V_EMPTY + 2) ? 2 : 1);
     fence_mbar_init();
     tma_prefetch_desc(&tma_q);
     tma_prefetch_desc(&tma_k);
@@ -82,344 +66,166 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_con
     tma_prefetch_desc(&tma_k2);
     tma_prefetch_desc(&tma_v2);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // register re-partition (warpgroup-aligned): the producer / MMA warpgroup gives its registers to the softmax warpgroups
   if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
-  if (warp == 0) {
     // ---------------------------------------------------------------- TMA producer
-    if (elect_one_sync()) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one_sync()) {
       mbar_arrive_expect_tx(&bars[Q_FULL], TILE_BYTES);
       tma_load_3d(smem + SmemLayout::q, &tma_q, &bars[Q_FULL], h * HD, q0, b);
       tma_load_3d(smem + SmemLayout::q + HALF_BYTES, &tma_q, &bars[Q_FULL], h * HD + 64, q0, b);
-      // Event-driven: each (group, K|V) stream advances as soon as ITS slot is free, so a K load never queues behind a V wait.
-      int k_next[2] = {0, 0}, v_next[2] = {0, 0};
-      const int T[2] = {T0, T1};
-      uint64_t t_start = 0;
-      uint32_t idle = 0;
-      while (k_next[0] < T0 || k_next[1] < T1 || v_next[0] < T0 || v_next[1] < T1) {
-        bool progress = false;
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          const CUtensorMap* mk = (dual && g) ? &tma_k2 : &tma_k;
-          const CUtensorMap* mv = (dual && g) ? &tma_v2 : &tma_v;
-          int t = k_next[g];
-          if (t < T[g] && mbar_test_wait(&bars[K_EMPTY + g], (t & 1) ^ 1)) {
-            const int row0 = (dual ? t : 2 * t + g) * BKV;
-            uint8_t* ks = smem + SmemLayout::k + g * TILE_BYTES;
-            mbar_arrive_expect_tx(&bars[K_FULL + g], TILE_BYTES);
-            tma_load_3d(ks, mk, &bars[K_FULL + g], h * HD, row0, b);
-            tma_load_3d(ks + HALF_BYTES, mk, &bars[K_FULL + g], h * HD + 64, row0, b);
-            ++k_next[g];
-            progress = true;
-          }
-          t = v_next[g];
-          if (t < T[g] && mbar_test_wait(&bars[V_EMPTY + g], (t & 1) ^ 1)) {
-            const int row0 = (dual ? t : 2 * t + g) * BKV;
-            uint8_t* vs = smem + SmemLayout::v + g * TILE_BYTES;
-            mbar_arrive_expect_tx(&bars[V_FULL + g], TILE_BYTES);
-            tma_load_3d(vs, mv, &bars[V_FULL + g], h * HD, row0, b);
-            tma_load_3d(vs + HALF_BYTES, mv, &bars[V_FULL + g], h * HD + 64, row0, b);
-            ++v_next[g];
-            progress = true;
-          }
-        }
-        if (progress) {
-          idle = 0;
-        } else if ((++idle & 0xFFF) == 0) {
-          if (t_start == 0) t_start = global_timer_ns();
-          else if (global_timer_ns() - t_start > CE_MBAR_TIMEOUT_NS) {
-            printf("[chronoedit_b200] attention producer stalled: block=(%d,%d,%d) k=%d,%d v=%d,%d\n", blockIdx.x, blockIdx.y, blockIdx.z,
-                   k_next[0], k_next[1], v_next[0], v_next[1]);
-            __trap();
-          }
-        }
+      for (int t = 0; t < T0 + T1; ++t) {
+        const int s = t & 1;
+        const uint32_t free_parity = ((t >> 1) & 1) ^ 1;
+        const CUtensorMap* mk = t < T0 ? &tma_k : &tma_k2;
+        const CUtensorMap* mv = t < T0 ? &tma_v : &tma_v2;
+        const int row0 = (t < T0 ? t : t - T0) * BKV;
+        uint8_t* ks = smem + SmemLayout::k + s * TILE_BYTES;
+        uint8_t* vs = smem + SmemLayout::v + s * TILE_BYTES;
+        mbar_wait(&bars[K_EMPTY + s], free_parity);
+        mbar_arrive_expect_tx(&bars[K_FULL + s], TILE_BYTES);
+        tma_load_3d(ks, mk, &bars[K_FULL + s], h * HD, row0, b);
+        tma_load_3d(ks + HALF_BYTES, mk, &bars[K_FULL + s], h * HD + 64, row0, b);
+        mbar_wait(&bars[V_EMPTY + s], free_parity);
+        mbar_arrive_expect_tx(&bars[V_FULL + s], TILE_BYTES);
+        tma_load_3d(vs, mv, &bars[V_FULL + s], h * HD, row0, b);
+        tma_load_3d(vs + HALF_BYTES, mv, &bars[V_FULL + s], h * HD + 64, row0, b);
       }
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer (one elected lane; every descriptor is fixed
-    // per group -- one K, V and P buffer each -- so all of them are built once and the MMAs go out eight per asm statement)
-    if (elect_one_sync()) {
-      constexpr uint32_t IDESC_S = umma_idesc_bf16(128, 128, 0);   // Q (K-major) x K^T (K-major)
-      constexpr uint32_t IDESC_PV = umma_idesc_bf16(128, 128, 1);  // P (K-major) x V (MN-major)
-      // Descriptors are rebuilt from one base word per operand right before each batch of MMAs (a few integer adds ahead of the asm
-      // statement, nothing between the MMAs).  Keeping all 56 of them live spilled them to local memory in this 80-register warp, and a
-      // reload is an L2 round trip on the critical chain (local memory does not stay in what is left of L1 next to 200+ KB of shared
-      // memory): measured on attention6.cu, 400-500 cycles per key tile (profiles/r2s_attention6_event_log.log).
-      const uint32_t hi_k = uint32_t(umma_desc_kmajor_sw128(0) >> 32), hi_v = uint32_t(umma_desc_mnmajor_sw128(0, HALF_BYTES) >> 32);
-      auto desc = [](uint32_t lo, uint32_t hi) { return (uint64_t(hi) << 32) | lo; };
-      const uint32_t q_lo = uint32_t(umma_desc_kmajor_sw128(smem_u32(smem + SmemLayout::q)));
-      const uint32_t k_lo = uint32_t(umma_desc_kmajor_sw128(smem_u32(smem + SmemLayout::k)));
-      const uint32_t p_lo = uint32_t(umma_desc_kmajor_sw128(smem_u32(smem + SmemLayout::p)));
-      const uint32_t v_lo = uint32_t(umma_desc_mnmajor_sw128(smem_u32(smem + SmemLayout::v), HALF_BYTES));
-      auto issue_s = [&](int g, int t) {
-        mbar_wait(&bars[K_FULL + g], t & 1, 30 + g);
-        tc_fence_after();
-        uint32_t qb = q_lo, kb = k_lo + g * (TILE_BYTES >> 4);
-        asm volatile("" : "+r"(qb), "+r"(kb));   // opaque: nothing is carried (= spilled) from one batch to the next
-        uint64_t da[8], db[8];
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint32_t off = (kk >> 2) * (HALF_BYTES >> 4) + 2 * (kk & 3);
-          da[kk] = desc(qb + off, hi_k);
-          db[kk] = desc(kb + off, hi_k);
-        }
-        umma_bf16_ss_x8(tmem_base + g * 128, da, db, IDESC_S, 0);
-        umma_commit(&bars[K_EMPTY + g]);
-        umma_commit(&bars[S_FULL + g]);
-      };
-      auto issue_pv = [&](int g, int t) {
-        tc_fence_after();
-        uint32_t pb = p_lo + g * (TILE_BYTES >> 4), vb = v_lo + g * (TILE_BYTES >> 4);
-        asm volatile("" : "+r"(pb), "+r"(vb));
-        uint64_t da[8], db[8];
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          da[kk] = desc(pb + (kk >> 2) * (HALF_BYTES >> 4) + 2 * (kk & 3), hi_k);
-          db[kk] = desc(vb + kk * (2048 >> 4), hi_v);
-        }
-        umma_bf16_ss_x8(tmem_base + 256 + g * 128, da, db, IDESC_PV, t != 0);
-        umma_commit(&bars[V_EMPTY + g]);
-        umma_commit(&bars[PV_DONE + g]);
-      };
-      mbar_wait(&bars[Q_FULL], 0, 1);
-      // Event-driven issue: whichever of {S(g, next), P.V(g, next)} has its inputs ready goes to the tensor pipe next.
-      //   S(g,t)   needs K(g,t) in shared memory and the S buffer of group g drained (the group copied S(g,t-1) to registers)
-      //   P.V(g,t) needs P(g,t) written by the group and V(g,t) in shared memory
-      int s_next[2] = {0, 0}, pv_next[2] = {0, 0};
-      const int T[2] = {T0, T1};
-      uint64_t t_start = 0;
-      uint32_t idle = 0;
-      while (pv_next[0] < T0 || pv_next[1] < T1) {
-        bool progress = false;
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          int t = s_next[g];
-          if (t < T[g] && (t == 0 || mbar_test_wait(&bars[S_FREE + g], (t - 1) & 1)) && mbar_test_wait(&bars[K_FULL + g], t & 1)) {
-            issue_s(g, t);
-            ++s_next[g];
-            progress = true;
-          }
-          t = pv_next[g];
-          if (t < s_next[g] && mbar_test_wait(&bars[P_FULL + g], t & 1) && mbar_test_wait(&bars[V_FULL + g], t & 1)) {
-            issue_pv(g, t);
-            ++pv_next[g];
-            progress = true;
-          }
-        }
-        if (progress) {
-          idle = 0;
-        } else if ((++idle & 0xFFF) == 0) {
-          if (t_start == 0) t_start = global_timer_ns();
-          else if (global_timer_ns() - t_start > CE_MBAR_TIMEOUT_NS) {
-            printf("[chronoedit_b200] attention MMA stalled: block=(%d,%d,%d) s=%d,%d pv=%d,%d\n", blockIdx.x, blockIdx.y, blockIdx.z, s_next[0],
-                   s_next[1], pv_next[0], pv_next[1]);
-            __trap();
-          }
-        }
-      }
-    }
+    return;
   }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-    // ---------------------------------------------------------------- softmax groups
-    const int g = (warp - 4) >> 2;       // 0: even key tiles, 1: odd key tiles
-    const int quad = warp & 3;           // TMEM lane quadrant of this warp
-    const int r = quad * 32 + lane;      // query row inside the tile
-    const uint32_t lane_base = uint32_t(quad * 32) << 16;
-    const uint32_t s_tmem = tmem_base + lane_base + g * 128;
-    const uint32_t o_tmem = tmem_base + lane_base + 256 + g * 128;
-    uint8_t* p_smem = smem + SmemLayout::p + g * TILE_BYTES;
-    const float sl2 = a.scale * 1.4426950408889634f;
-    const int my_tiles = g ? T1 : T0;
-    const int my_len = (dual && g) ? a.Lk2 : a.Lk;
-    float m = -INFINITY, l = 0.f;
-    const bool timed = a.timing != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 128;
-    long long tacc[6] = {0, 0, 0, 0, 0, 0};
-    long long tc0 = 0;
-#define CE_TICK(slot)                      \
-  if (timed) {                             \
-    const long long _t = clock64();        \
-    tacc[slot] += _t - tc0;                \
-    tc0 = _t;                              \
-  }
-    if (timed) tc0 = clock64();
 
-    for (int t = 0; t < my_tiles; ++t) {
-      const int valid = my_len - (dual ? t : 2 * t + g) * BKV;  // >= 1; >= 128 means no masking
-      mbar_wait(&bars[S_FULL + g], t & 1, 60 + g);
-      tc_fence_after();
-      CE_TICK(0)
-      // the whole 128-wide score row of this thread goes to registers with one wait (4 x tcgen05.ld in flight)
-      uint32_t s[128];
+  // ------------------------------------------------------------------ consumers: 64 query rows per warpgroup
+  setmaxnreg_inc<232>();
+  const int wg = (warp >> 2) - 1;
+  const bool signaller = (threadIdx.x & 127) == 0;
+  const int quad = lane & 3;
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // the thread's rows of the query tile: r0 and r0 + 8
+  const float sl2 = a.scale * 1.4426950408889634f;
+  const uint32_t q_smem = smem_u32(smem + SmemLayout::q) + wg * 64 * 128;
+  const bool timed = a.timing != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 128;
+  long long tacc[3] = {0, 0, 0};   // cycles in S = Q K^T (incl. the wait for K), softmax, P V (incl. the wait for V)
+  long long tc0 = timed ? clock64() : 0;
+#define CE_TICK(slot)               \
+  if (timed) {                      \
+    const long long _t = clock64(); \
+    tacc[slot] += _t - tc0;         \
+    tc0 = _t;                       \
+  }
+
+  mbar_wait(&bars[Q_FULL], 0);
+  int t = 0;   // position in the ring, over both sources
+  for (int src = 0; src < (T1 > 0 ? 2 : 1); ++src) {
+    const int my_tiles = src ? T1 : T0;
+    const int my_len = src ? a.Lk2 : a.Lk;
+    float o[64];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) tmem_ld_32x32(s_tmem + c * 32, *reinterpret_cast<uint32_t(*)[32]>(&s[32 * c]));
-      tmem_ld_wait();
-      CE_TICK(1)
-      tc_fence_before();
-      mbar_arrive(&bars[S_FREE + g]);  // S buffer drained
+    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // per row; l is this lane's share of the row sum
+
+    for (int j = 0; j < my_tiles; ++j, ++t) {
+      const int s = t & 1;
+      const uint32_t parity = (t >> 1) & 1;
+      const int valid = my_len - j * BKV;  // >= 1; >= 128 means no masking
+      // ---- S = Q K^T: 8 K16 steps over head_dim (two 64-wide swizzled blocks)
+      float sc[64];
+      mbar_wait(&bars[K_FULL + s], parity);
+      {
+        const uint32_t k_smem = smem_u32(smem + SmemLayout::k) + s * TILE_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+          const uint32_t off = (kk >> 2) * HALF_BYTES + (kk & 3) * 32;
+          wgmma_ss<128, 0>(sc, wgmma_desc_kmajor_sw128(q_smem + off), wgmma_desc_kmajor_sw128(k_smem + off), kk != 0);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (signaller) mbar_arrive(&bars[K_EMPTY + s]);
+      }
+      CE_TICK(0)
+      // ---- online softmax on the accumulator registers: sc[4 * c + e + 2 * hh] is row r0 + 8 * hh, key 8 * c + 2 * quad + e
       if (valid < BKV) {  // last key tile only (warp-uniform): masked scores -> -inf -> p = 0
 #pragma unroll
-        for (int i = 0; i < 128; ++i) s[i] = (i < valid) ? s[i] : 0xff800000u;
+        for (int i = 0; i < 64; ++i)
+          if (8 * (i >> 2) + 2 * quad + (i & 1) >= valid) sc[i] = -INFINITY;
       }
-      // row max with 8 independent chains (a single fmax chain would cost 128 x 4 dependent cycles)
-      float mx8[8];
+      uint32_t p[32];   // bf16 pairs: p[2 * c + hh] = keys 8 * c + 2 * quad + {0, 1} of row r0 + 8 * hh
 #pragma unroll
-      for (int i = 0; i < 8; ++i) mx8[i] = __uint_as_float(s[i]);
+      for (int hh = 0; hh < 2; ++hh) {
+        float mx = -INFINITY;
 #pragma unroll
-      for (int i = 8; i < 128; ++i) mx8[i & 7] = fmaxf(mx8[i & 7], __uint_as_float(s[i]));
-      float mx = fmaxf(fmaxf(fmaxf(mx8[0], mx8[1]), fmaxf(mx8[2], mx8[3])), fmaxf(fmaxf(mx8[4], mx8[5]), fmaxf(mx8[6], mx8[7])));
-      mx *= sl2;
-      // lazy rescale decision (registers only): take the new max only if it grew by more than 2^8
-      float alpha = 1.0f;
-      bool need = false;
-      if (t == 0) {
-        m = mx;
-      } else {
-        need = mx > m + RESCALE_THRESHOLD;
-        if (need) {
-          alpha = fast_exp2(m - mx);
-          m = mx;
+        for (int c = 0; c < 16; ++c) mx = fmaxf(mx, fmaxf(sc[4 * c + 2 * hh], sc[4 * c + 2 * hh + 1]));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float m_new = fmaxf(m[hh], mx * sl2);   // finite: every tile has at least one valid key
+        const float alpha = fast_exp2(m[hh] - m_new); // 0 on the first tile (m = -inf)
+        m[hh] = m_new;
+        float sum = 0.f;
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+          const float p0 = fast_exp2(fmaf(sc[4 * c + 2 * hh], sl2, -m_new));
+          const float p1 = fast_exp2(fmaf(sc[4 * c + 2 * hh + 1], sl2, -m_new));
+          sum += p0 + p1;
+          p[2 * c + hh] = pack_bf16x2(p0, p1);
         }
+        l[hh] = l[hh] * alpha + sum;
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+          o[4 * c + 2 * hh] *= alpha;
+          o[4 * c + 2 * hh + 1] *= alpha;
+        }
+      }
+      CE_TICK(1)
+      // ---- O += P V: 8 K16 steps over the keys; the A fragment of step kk is {rows r0, r0+8} x {keys 16kk + 2quad, + 8}
+      mbar_wait(&bars[V_FULL + s], parity);
+      {
+        const uint32_t v_smem = smem_u32(smem + SmemLayout::v) + s * TILE_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+          const uint32_t frag[4] = {p[4 * kk], p[4 * kk + 1], p[4 * kk + 2], p[4 * kk + 3]};
+          wgmma_rs<128, 1>(o, frag, wgmma_desc_mnmajor_sw128(v_smem + kk * 2048, HALF_BYTES), 1);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (signaller) mbar_arrive(&bars[V_EMPTY + s]);
       }
       CE_TICK(2)
-      // p = exp2(s*scale*log2e - m) -> packed bf16 in registers; this MUFU-bound phase overlaps the previous P.V of this group
-      const float neg_m = -m;
-      // packed fp32 pairs: FFMA2 for the scale-and-shift, FADD2 for the row sums (2 MUFU + 3 other instructions per pair)
-      const uint64_t sl2_2 = f2_pack(sl2, sl2), negm_2 = f2_pack(neg_m, neg_m);
-      uint64_t sum2[4] = {0ull, 0ull, 0ull, 0ull};
-      uint32_t pk[64];
-#pragma unroll
-      for (int i = 0; i < 64; ++i) {
-        float x0, x1;
-        f2_unpack(f2_fma(f2_pack_bits(s[2 * i], s[2 * i + 1]), sl2_2, negm_2), x0, x1);
-        const float p0 = fast_exp2(x0), p1 = fast_exp2(x1);
-        sum2[i & 3] = f2_add(sum2[i & 3], f2_pack(p0, p1));
-        pk[i] = pack_bf16x2(p0, p1);
-      }
-      float sum4[4];
-      {
-        float a0, a1, b0, b1;
-        f2_unpack(f2_add(sum2[0], sum2[1]), a0, a1);
-        f2_unpack(f2_add(sum2[2], sum2[3]), b0, b1);
-        sum4[0] = a0; sum4[1] = a1; sum4[2] = b0; sum4[3] = b1;
-      }
-      CE_TICK(3)
-      if (t > 0) {
-        mbar_wait(&bars[PV_DONE + g], (t - 1) & 1, 70 + g);  // previous P.V of this group done: O stable, P buffer free
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, need)) {
-          l *= alpha;
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            uint32_t o[32];
-            tmem_ld_32x32(o_tmem + c * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_32x32(o_tmem + c * 32, o);
-          }
-          tmem_st_wait();
-        }
-      }
-      CE_TICK(4)
-      // P -> shared memory (K-major, 128B swizzle: 16-byte chunk index ^= row & 7)
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint8_t* row_base = p_smem + (c >> 1) * HALF_BYTES + r * 128;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int chunk = ((c & 1) * 4 + i) ^ (r & 7);
-          *reinterpret_cast<uint4*>(row_base + chunk * 16) =
-              make_uint4(pk[16 * c + 4 * i], pk[16 * c + 4 * i + 1], pk[16 * c + 4 * i + 2], pk[16 * c + 4 * i + 3]);
-        }
-      }
-      l += (sum4[0] + sum4[1]) + (sum4[2] + sum4[3]);
-      tc_fence_before();
-      fence_proxy_async_smem();
-      mbar_arrive(&bars[P_FULL + g]);
-      CE_TICK(5)
-    }
-    if (timed) {
-      for (int i = 0; i < 6; ++i) a.timing[i] = tacc[i];
-      a.timing[6] = my_tiles;
     }
 
-    // ---- merge the two streams and write the output tile
-    if (my_tiles > 0) {
-      mbar_wait(&bars[PV_DONE + g], (my_tiles - 1) & 1, 80 + g);
-      tc_fence_after();
-    }
-    float2* xch = reinterpret_cast<float2*>(p_smem);  // own P buffer is free now
-    xch[r] = make_float2(m, l);
-    tc_fence_before();
-    named_bar_sync(1, 256);
-    tc_fence_after();
-    const float2 other = reinterpret_cast<const float2*>(smem + SmemLayout::p + (g ^ 1) * TILE_BYTES)[r];
-    const float m_e = g == 0 ? m : other.x, l_e = g == 0 ? l : other.y;
-    const float m_o = g == 0 ? other.x : m, l_o = g == 0 ? other.y : l;
-    const bool has_o = T1 > 0;
-    float w_e, w_o;
-    if (dual) {  // two separate softmaxes (text keys, image keys): each normalised on its own, results added (:103-104)
-      w_e = 1.0f / l_e;
-      w_o = has_o ? 1.0f / l_o : 0.f;
-    } else {
-      const float mm = has_o ? fmaxf(m_e, m_o) : m_e;
-      const float a_e = fast_exp2(m_e - mm);
-      const float a_o = has_o ? fast_exp2(m_o - mm) : 0.f;
-      const float inv = 1.0f / (l_e * a_e + l_o * a_o);
-      w_e = a_e * inv;
-      w_o = a_o * inv;
-    }
-    const int row = q0 + r;
-    bf16* orow = a.out + ((size_t)b * a.Lq + row) * a.ldo + h * HD + g * 64;
-    const uint32_t oe_tmem = tmem_base + lane_base + 256 + g * 64;
-    const uint32_t oo_tmem = tmem_base + lane_base + 384 + g * 64;
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      uint32_t oe[32], oo[32];
-      tmem_ld_32x32(oe_tmem + c * 32, oe);
-      if (has_o) tmem_ld_32x32(oo_tmem + c * 32, oo);
-      tmem_ld_wait();
-      if (row < a.Lq) {
+    // ---- normalise and store this source's result
 #pragma unroll
-        for (int v4 = 0; v4 < 4; ++v4) {
-          float y[8];
+    for (int hh = 0; hh < 2; ++hh) {
+      float lr = l[hh];
+      lr += __shfl_xor_sync(0xffffffffu, lr, 1);
+      lr += __shfl_xor_sync(0xffffffffu, lr, 2);
+      const float inv = 1.0f / lr;
+      const int row = q0 + r0 + 8 * hh;
+      if (row >= a.Lq) continue;
+      bf16* orow = a.out + ((size_t)b * a.Lq + row) * a.ldo + h * HD;
+      if (a.peer_rows > 0)   // sequence parallel: the token's owner gets the row (peer store over NVLink)
+        orow = a.out_peer[row / a.peer_rows] + ((size_t)b * a.peer_rows + row % a.peer_rows) * a.ldo + a.out_col0 + h * HD;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            y[i] = __uint_as_float(oe[v4 * 8 + i]) * w_e;
-            if (dual) {  // each SDPA result is a bf16 tensor in the reference before the add
-              y[i] = bf16_round(y[i]);
-              if (has_o) y[i] += bf16_round(__uint_as_float(oo[v4 * 8 + i]) * w_o);
-            } else if (has_o) {
-              y[i] += __uint_as_float(oo[v4 * 8 + i]) * w_o;
-            }
-          }
-          uint4* dst = reinterpret_cast<uint4*>(orow + c * 32 + v4 * 8);
-          if (a.accumulate) {
-            const uint4 pv = *dst;
-            const float2 p0 = unpack_bf16x2(pv.x), p1 = unpack_bf16x2(pv.y), p2 = unpack_bf16x2(pv.z),
-                         p3 = unpack_bf16x2(pv.w);
-            const float prev[8] = {p0.x, p0.y, p1.x, p1.y, p2.x, p2.y, p3.x, p3.y};
-#pragma unroll
-            for (int i = 0; i < 8; ++i) y[i] = bf16_round(y[i]) + prev[i];
-          }
-          *dst = make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]), pack_bf16x2(y[4], y[5]),
-                            pack_bf16x2(y[6], y[7]));
+      for (int c = 0; c < 16; ++c) {
+        float y0 = o[4 * c + 2 * hh] * inv, y1 = o[4 * c + 2 * hh + 1] * inv;
+        uint32_t* dst = reinterpret_cast<uint32_t*>(orow + 8 * c + 2 * quad);
+        if (a.accumulate || src == 1) {   // each SDPA result is a bf16 tensor in the reference before the add
+          const float2 prev = unpack_bf16x2(*dst);
+          y0 = bf16_round(y0) + prev.x;
+          y1 = bf16_round(y1) + prev.y;
         }
+        *dst = pack_bf16x2(y0, y1);
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
+  if (timed) {
+    for (int i = 0; i < 3; ++i) a.timing[i] = tacc[i];
+    a.timing[3] = T0 + T1;
+  }
+#undef CE_TICK
 }
+
 
 int make_qkv_tmap(CUtensorMap* m, const bf16* base, int B, int L, int H, int ld) {
   uint64_t dims[3] = {(uint64_t)H * HD, (uint64_t)L, (uint64_t)B};
@@ -430,37 +236,10 @@ int make_qkv_tmap(CUtensorMap* m, const bf16* base, int B, int L, int H, int ld)
 
 }  // namespace
 
-int launch_attention2(const AttnArgs& a, cudaStream_t stream);  // attention2.cu
-int launch_attention5(const AttnArgs& a, cudaStream_t stream);  // attention5.cu
-int launch_attention6(const AttnArgs& a, cudaStream_t stream);  // attention6.cu
-
-// Which kernel serves long single-source problems (the self-attention): 6 = attention6.cu (two softmax threads per row; default:
-// +6 % isolated, +5.8 % inside the step over attention2.cu, profiles/r2u_*, r2v_*), 2 = attention2.cu (one thread per row),
-// 5 = attention5.cu (cta_group::2, experimental), 0 = this file's kernel for everything.  CE_ATTN_V2 in the environment, or
-// ce_debug_attention_kernel() at run time (tests exercise the non-default kernels through it).
-static int g_attn_override = -1;
-void set_attention_kernel(int v) { g_attn_override = v; }
-static int attn_version() {
-  if (g_attn_override >= 0) return g_attn_override;
-  static const int v = [] {
-    const char* e = getenv("CE_ATTN_V2");
-    return !e ? 6 : (e[0] == '0' ? 0 : (e[0] == '5' ? 5 : (e[0] == '2' ? 2 : 6)));
-  }();
-  return v;
-}
-
 int launch_attention(const AttnArgs& a, cudaStream_t stream) {
   CE_REQUIRE(a.B > 0 && a.H > 0 && a.Lq > 0 && a.Lk > 0, "attention: empty problem");
-  // long single-source problems (the self-attention): two query tiles per CTA sharing every K/V tile, P in TMEM
-  if (a.Lk2 == 0 && !a.accumulate && a.Lq >= 256 && a.Lk >= 256 && a.head_dim == HD && attn_version() != 0)
-    return (attn_version() == 5 && a.peer_rows == 0) ? launch_attention5(a, stream)
-           : attn_version() == 2                     ? launch_attention2(a, stream)
-                                                     : launch_attention6(a, stream);
-  // The two-source cross-attention stays with this file's two-group kernel.  Two re-builds on attention6.cu's machinery were
-  // measured and dropped (patches + logs under profiles/): the sources one after the other in a 256-query CTA (0.439 ms, r2x) and
-  // one stream per source over a 128-query tile, started together or staggered (0.495 / 0.513 ms, r2I / r2J) against 0.405 ms here:
-  // with 4 + 3 key tiles per CTA the fixed cost of a 640-thread CTA outweighs the faster softmax.
-  CE_REQUIRE(a.peer_rows == 0, "attention: the sequence-parallel output scatter is built into the self-attention kernel (attention2.cu) only");
+  CE_REQUIRE(a.peer_rows == 0 || (a.Lk2 == 0 && !a.accumulate && (a.Lq + a.peer_rows - 1) / a.peer_rows <= 8),
+             "attention: the sequence-parallel output scatter serves the self-attention, with at most 8 peers");
   CE_REQUIRE(a.head_dim == HD, "attention: only head_dim 128 is built");
   CE_REQUIRE(a.ldq % 8 == 0 && a.ldk % 8 == 0 && a.ldv % 8 == 0 && a.ldo % 8 == 0, "attention: leading dims % 8");
   CE_REQUIRE(a.q && a.k && a.v && a.out, "attention: null pointer");

@@ -1,4 +1,4 @@
-// Interface of the tcgen05 attention forward (attention.cu).
+// Interface of the wgmma attention forward (attention.cu).
 #pragma once
 #include "host_common.h"
 #include "ptx.cuh"
@@ -23,7 +23,7 @@ struct AttnArgs {
   bf16* out = nullptr;      // out[b, i, h*hd + d]
   int ldo = 0;
   float scale = 0.f;        // 1/sqrt(head_dim)
-  long long* timing = nullptr;  // optional [16] device counters: phase cycles of softmax warp 4 lane 0 of block (0,0,0) (profiling aid)
+  long long* timing = nullptr;  // optional [16] device counters: phase cycles of thread 128 of block (0,0,0) (profiling aid)
   // sequence-parallel output scatter (csrc/seqpar.cu): when peer_rows > 0, query row i of sample b is stored at
   //   out_peer[i / peer_rows] + ((b * peer_rows + i % peer_rows) * ldo + h * head_dim + out_col0)
   // i.e. straight into the attention-output buffer of the rank that owns that token (its own pointer or a peer's, NVLink).
@@ -34,6 +34,5 @@ struct AttnArgs {
 };
 
 int launch_attention(const AttnArgs& a, cudaStream_t stream);
-void set_attention_kernel(int version);  // -1 default / environment, 0, 2, 5, 6, 7 (see attention.cu)
 
 }  // namespace ce

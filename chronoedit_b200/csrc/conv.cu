@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution for the Wan 3D causal VAE on sm_100a (tcgen05 + TMA), channels-last activations.
+// Implicit-GEMM convolution for the Wan 3D causal VAE on sm_90a (wgmma + TMA), channels-last activations.
 //
 // GEMM view: M = output voxels (tiles of 8 x 16 pixels of one frame = 128 rows), N = output channels, K = taps x Cin.
 // For every tap (dt,dh,dw) and 64-channel block the producer issues ONE 4-D TMA box load {64 ch, 16 w, 8 h, 1 t} at the
@@ -6,20 +6,21 @@
 // out-of-bounds zero fill IS the convolution's spatial zero padding (negative / overflowing coordinates) and the channel
 // padding of Cin up to 64.  Stride-2 convolutions use the tensor map's element strides.  The temporal halo is real data:
 // the caller keeps the causal history frames in front of the chunk (wan2pt1.py:49-60, CACHE_T = 2).
-// Weights are pre-packed [Cout, taps, Cin_pad] so the B tile is a plain 2-D box.  Pipeline / warp roles / TMEM double
-// buffering are those of gemm.cu; the epilogue adds bias, optional residual, the upsample3d frame interleave and an
-// optional planar (NCTHW) clamped store for the decoder head.
+// Weights are pre-packed [Cout, taps, Cin_pad] so the B tile is a plain 2-D box.  Pipeline and warpgroup roles are those of
+// gemm.cu (one TMA producer warpgroup, two wgmma consumer warpgroups of 64 rows each); the epilogue adds bias, optional
+// residual, the upsample3d frame interleave and an optional planar (NCTHW) clamped store for the decoder head.
 //
-// Replaces cuDNN's conv3d/conv2d behind CausalConv3d / nn.Conv2d of /root/reference/chronoedit/_src/tokenizers/wan2pt1.py
+// Replaces cuDNN's conv3d/conv2d behind CausalConv3d / nn.Conv2d of the reference's chronoedit/_src/tokenizers/wan2pt1.py
 // (:42-60, :98-110, :186-220) plus F.pad / torch.cat cache handling and the residual add (:220).
 #include "conv.cuh"
+#include "wgmma.cuh"
 
 namespace ce {
 
 namespace {
 
 constexpr int TILE_H = 8, TILE_W = 16, BM = 128, BK = 64;
-constexpr int CONV_THREADS = 192;
+constexpr int CONV_THREADS = 384;
 
 struct ConvGeom {
   int tiles_w, tiles_h, tiles_n, num_tiles;
@@ -40,19 +41,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv3d_cl_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_constant__ CUtensorMap tma_w, ConvArgs a, ConvGeom g) {
   constexpr uint32_t A_BYTES = BM * BK * 2;
   constexpr uint32_t B_BYTES = BN * BK * 2;
-  constexpr uint32_t TMEM_COLS = BN <= 32 ? 64 : (BN <= 64 ? 128 : (BN <= 128 ? 256 : 512));
-  constexpr uint32_t IDESC = umma_idesc_bf16(BM, BN, 0);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));
-  uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES;
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));
+  uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -60,24 +55,17 @@ conv3d_cl_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_constan
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 4);
+      mbar_init(&empty[i], 2);  // one arrive per consumer warpgroup
     }
     fence_mbar_init();
     tma_prefetch_desc(&tma_x);
     tma_prefetch_desc(&tma_w);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (elect_one_sync()) {  // one lane, known to the compiler as such: no per-instruction serialisation loops around UTMALDG / UTCHMMA
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one_sync()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < g.num_tiles; t += gridDim.x) {
@@ -91,7 +79,7 @@ conv3d_cl_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_constan
           for (int dh = 0; dh < a.kh; ++dh)
             for (int dw = 0; dw < a.kw; ++dw, ++tap)
               for (int cb = 0; cb < g.cblocks; ++cb) {
-                mbar_wait(&empty[stage], phase ^ 1, 100 + stage);
+                mbar_wait(&empty[stage], phase ^ 1);
                 mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
                 tma_load_4d(sA + stage * A_BYTES, &tma_x, &full[stage], cb * BK, w_in0 + dw, h_in0 + dh, t_in0 + dt);
                 tma_load_2d(sB + stage * B_BYTES, &tma_w, &full[stage], tap * a.Cin_pad + cb * BK, nb * BN);
@@ -102,120 +90,75 @@ conv3d_cl_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_constan
               }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one_sync()) {  // one lane, known to the compiler as such: no per-instruction serialisation loops around UTMALDG / UTCHMMA
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int t = blockIdx.x; t < g.num_tiles; t += gridDim.x) {
-        mbar_wait(&tempty[acc], acc_phase ^ 1, 200 + acc);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < g.kblocks; ++kb) {
-          mbar_wait(&full[stage], phase, 300 + stage);
-          tc_fence_after();
-          const uint64_t da = umma_desc_kmajor_sw128(smem_u32(sA + stage * A_BYTES));
-          const uint64_t db = umma_desc_kmajor_sw128(smem_u32(sB + stage * B_BYTES));
-umma_bf16_ss_x4(d_tmem, da, db, IDESC, kb != 0);   // the four K16 steps of the k-block, one asm statement
-          umma_commit(&empty[stage]);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tfull[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const int c_half = a.split_time ? a.Cout / 2 : a.Cout;  // channels per stored voxel
-    for (int t = blockIdx.x; t < g.num_tiles; t += gridDim.x) {
-      int to, th, tw, nb;
-      conv_tile_coords(t, g, to, th, tw, nb);
-      mbar_wait(&tfull[acc], acc_phase, 400 + acc);
-      tc_fence_after();
+    return;
+  }
+
+  setmaxnreg_inc<232>();
+  const int wg = (warp >> 2) - 1;
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // the thread's rows of the tile: r0 and r0 + 8
+  const int c_in_group = 2 * (lane & 3);
+  const int c_half = a.split_time ? a.Cout / 2 : a.Cout;  // channels per stored voxel
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BN / 2];
+  for (int t = blockIdx.x; t < g.num_tiles; t += gridDim.x) {
+    int to, th, tw, nb;
+    conv_tile_coords(t, g, to, th, tw, nb);
+    wgmma_ring_tile<BN, STAGES>(acc, smem_u32(sA) + wg * 64 * 128, smem_u32(sB), A_BYTES, B_BYTES, full, empty, g.kblocks, stage, phase);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = r0 + 8 * h;
       const int oh = th * TILE_H + (r >> 4), ow = tw * TILE_W + (r & 15);
-      const bool pix_ok = oh < a.Hout && ow < a.Wout;
-      const uint32_t t_row = tmem_base + (uint32_t(q * 32) << 16) + acc * BN;
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int n0 = nb * BN + c * 32;
-        if (n0 >= a.Cout) break;
-        uint32_t v[32];
-        tmem_ld_32x32(t_row + c * 32, v);
-        tmem_ld_wait();
-        if (!pix_ok) continue;
+      if (oh >= a.Hout || ow >= a.Wout) continue;
 #pragma unroll
-        for (int v8 = 0; v8 < 4; ++v8) {
-          const int n = n0 + v8 * 8;
-          if (n >= a.Cout) break;
-          float y[8];
+      for (int j = 0; j < BN / 8; ++j) {   // 8-channel groups, two channels per lane
+        const int n = nb * BN + j * 8 + c_in_group;
+        if (n >= a.Cout) continue;
+        float y[2];
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            y[j] = __uint_as_float(v[v8 * 8 + j]);
-            if (a.bias && n + j < a.Cout) y[j] += __bfloat162float(a.bias[n + j]);
-            y[j] = bf16_round(y[j]);  // the convolution returns a bf16 tensor
-          }
-          if (a.planar_out) {
-            // decoder head: [Cout, Tout, Hout, Wout], optional clamp (diffusers AutoencoderKLWan.decode)
+        for (int e = 0; e < 2; ++e) {
+          y[e] = acc[4 * j + 2 * h + e];
+          if (a.bias && n + e < a.Cout) y[e] += __bfloat162float(a.bias[n + e]);
+          y[e] = bf16_round(y[e]);  // the convolution returns a bf16 tensor
+        }
+        if (a.planar_out) {
+          // decoder head: [Cout, Tout, Hout, Wout], optional clamp (diffusers AutoencoderKLWan.decode)
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              if (n + j < a.Cout) {
-                float o = y[j];
-                if (a.clamp) o = fminf(fmaxf(o, -1.0f), 1.0f);
-                a.y[(((size_t)(n + j) * a.planar_T + a.planar_t0 + to) * a.Hout + oh) * a.Wout + ow] = __float2bfloat16_rn(o);
-              }
+          for (int e = 0; e < 2; ++e) {
+            if (n + e < a.Cout) {
+              float o = y[e];
+              if (a.clamp) o = fminf(fmaxf(o, -1.0f), 1.0f);
+              a.y[(((size_t)(n + e) * a.planar_T + a.planar_t0 + to) * a.Hout + oh) * a.Wout + ow] = __float2bfloat16_rn(o);
             }
-            continue;
           }
-          int frame = to, ch = n;
-          if (a.split_time) {
-            frame = 2 * to + (n >= c_half ? 1 : 0);
-            ch = n >= c_half ? n - c_half : n;
+          continue;
+        }
+        int frame = to, ch = n;
+        if (a.split_time) {
+          frame = 2 * to + (n >= c_half ? 1 : 0);
+          ch = n >= c_half ? n - c_half : n;
+        }
+        const size_t off = (((size_t)frame * a.Hout + oh) * a.Wout + ow) * c_half + ch;
+        if ((c_half & 1) == 0 && n + 2 <= a.Cout) {
+          if (a.resid) {
+            const float2 x = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(a.resid + off));
+            y[0] += x.x;
+            y[1] += x.y;
           }
-          const size_t off = (((size_t)frame * a.Hout + oh) * a.Wout + ow) * c_half + ch;
-          if ((c_half & 7) == 0 && n + 8 <= a.Cout) {
-            if (a.resid) {
-              const uint4 xv = *reinterpret_cast<const uint4*>(a.resid + off);
-              const float2 x0 = unpack_bf16x2(xv.x), x1 = unpack_bf16x2(xv.y), x2 = unpack_bf16x2(xv.z), x3 = unpack_bf16x2(xv.w);
-              y[0] += x0.x; y[1] += x0.y; y[2] += x1.x; y[3] += x1.y;
-              y[4] += x2.x; y[5] += x2.y; y[6] += x3.x; y[7] += x3.y;
-            }
-            *reinterpret_cast<uint4*>(a.y + off) =
-                make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]), pack_bf16x2(y[4], y[5]), pack_bf16x2(y[6], y[7]));
-          } else {
+          *reinterpret_cast<uint32_t*>(a.y + off) = pack_bf16x2(y[0], y[1]);
+        } else {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              if (n + j < a.Cout) {
-                float o = y[j];
-                if (a.resid) o += __bfloat162float(a.resid[off + j]);
-                a.y[off + j] = __float2bfloat16_rn(o);
-              }
+          for (int e = 0; e < 2; ++e) {
+            if (n + e < a.Cout) {
+              float o = y[e];
+              if (a.resid) o += __bfloat162float(a.resid[off + e]);
+              a.y[off + e] = __float2bfloat16_rn(o);
             }
           }
         }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 template <int BN, int STAGES>

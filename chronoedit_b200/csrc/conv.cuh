@@ -1,4 +1,4 @@
-// Interface of the tcgen05 implicit-GEMM convolution used by the Wan VAE path (conv.cu).
+// Interface of the wgmma implicit-GEMM convolution used by the Wan VAE path (conv.cu).
 #pragma once
 #include "host_common.h"
 #include "ptx.cuh"

@@ -1,4 +1,4 @@
-// ce_dit: the ChronoEdit DiT per-step forward as a chain of hand-written sm_100a kernels behind the C ABI.
+// ce_dit: the ChronoEdit DiT per-step forward as a chain of hand-written sm_90a kernels behind the C ABI.
 //
 // Mirrors ChronoEditTransformer3DModel.forward (/root/reference/chronoedit_diffusers/transformer_chronoedit.py:397-476)
 // with every rounding point of the reference's bf16 path kept (SURVEY.md section 8a).  Per block
@@ -792,19 +792,16 @@ int ce_linear_bf16(const void* A, int lda, const void* W, int ldw, const void* b
 }
 
 static long long* g_attn_timing = nullptr;
-// Profiling aid: subsequent ce_attention_bf16 calls record the phase cycles of one softmax warp (block 0) into `buf`
+// Profiling aid: subsequent ce_attention_bf16 calls record the phase cycles of the first consumer thread of block 0 into `buf`
 // ([16] int64 on the device); pass NULL to stop.
 int ce_debug_attention_timing(long long* buf) {
   g_attn_timing = buf;
   return CE_OK;
 }
 
-// Test / A-B aid: which kernel serves the self-attention from now on (6 default = attention6.cu, 2 = attention2.cu, 5 cta_group::2
-// cluster kernel, 0 the single-tile kernel of attention.cu; -1 back to the CE_ATTN_V2 / built-in default).
+// Test aid: attention.cu is the only attention kernel of the sm_90a build (version 0, also the default -1).
 int ce_debug_attention_kernel(int version) {
-  if (version != -1 && version != 0 && version != 2 && version != 5 && version != 6)
-    return ce::fail(ce::CE_ERR_INVALID, "attention kernel version must be -1, 0, 2, 5 or 6");
-  ce::set_attention_kernel(version);
+  if (version != -1 && version != 0) return ce::fail(ce::CE_ERR_INVALID, "attention kernel version must be -1 or 0");
   return CE_OK;
 }
 

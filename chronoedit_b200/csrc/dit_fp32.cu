@@ -4,10 +4,10 @@
 // SURVEY.md section 7 hard part 3).  Same operator order as ChronoEditTransformer3DModel.forward
 // (/root/reference/chronoedit_diffusers/transformer_chronoedit.py:397-476) evaluated in fp32 like the reference's own fp32 run.
 //
-// Every matrix product still runs on the tcgen05 GEMM of gemm.cu / gemm2.cu: an fp32 operand x is split into two bf16 terms
+// Every matrix product still runs on the wgmma GEMM of gemm.cu: an fp32 operand x is split into two bf16 terms
 // hi = bf16(x), lo = bf16(x - hi) (|x - hi - lo| <= 2^-17 |x|), and A.W^T is evaluated as ONE bf16 GEMM over a K axis three times
 // as long -- A' = [A_hi | A_lo | A_hi], W' = [W_hi | W_hi | W_lo], i.e. A_hi.W_hi + A_lo.W_hi + A_hi.W_lo, fp32 accumulation in
-// TMEM, fp32 store (the dropped A_lo.W_lo term is 2^-18 relative).  Attention is S = Q.K^T (same split GEMM, fp32 S in HBM),
+// registers, fp32 store (the dropped A_lo.W_lo term is 2^-18 relative).  Attention is S = Q.K^T (same split GEMM, fp32 S in HBM),
 // an fp32 row softmax, and O = P.V with P and V^T split the same way.  Everything elementwise is a plain fp32 SIMT kernel.
 // This path trades speed for precision (3x the MMA work, S materialised) and exists for parity checks only.
 #include <math.h>
@@ -25,7 +25,7 @@ namespace {
 constexpr int TPB = 256;
 inline int grid_for(size_t n) {
   size_t g = (n + TPB - 1) / TPB;
-  return (int)(g < 148 * 16 ? (g ? g : 1) : 148 * 16);
+  return (int)(g < device_sm_count() * 16 ? (g ? g : 1) : device_sm_count() * 16);
 }
 
 // out[r, :] (bf16, 3*Kp wide) from x[r, 0:K] fp32 (leading dim ldx); A layout [hi | lo | hi], W layout [hi | hi | lo]; columns

@@ -510,7 +510,7 @@ int launch_rmsnorm_rope_stats(bf16* x, int ldx, int rows, int D, float eps, cons
 int launch_patchify(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, cudaStream_t stream) {
   CE_REQUIRE(H % 2 == 0 && W % 2 == 0, "patchify: H, W must be even");
   const size_t total = (size_t)B * T * (H / 2) * (W / 2) * C * 4;
-  const int grid = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const int grid = (int)((total + 255) / 256 < device_sm_count() * 16 ? (total + 255) / 256 : device_sm_count() * 16);
   patchify_kernel<<<grid, 256, 0, stream>>>(x, patches, B, C, T, H, W);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
@@ -518,7 +518,7 @@ int launch_patchify(const bf16* x, bf16* patches, int B, int C, int T, int H, in
 
 int launch_unpatchify(const bf16* y, int ldy, bf16* out, int B, int C, int T, int H, int W, cudaStream_t stream) {
   const size_t total = (size_t)B * C * T * H * W;
-  const int grid = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const int grid = (int)((total + 255) / 256 < device_sm_count() * 16 ? (total + 255) / 256 : device_sm_count() * 16);
   unpatchify_kernel<<<grid, 256, 0, stream>>>(y, ldy, out, B, C, T, H, W);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
@@ -547,7 +547,7 @@ int launch_timestep_sinusoid(const float* t, float* emb, int B, int dim, cudaStr
 int launch_add_table(const float* table, int table_rows, const bf16* src, int src_ld, float* dst, int B, int n,
                      int chunks, cudaStream_t stream, unsigned plus_one_mask) {
   const size_t total = (size_t)table_rows * B * chunks * n;
-  const int grid = (int)((total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8);
+  const int grid = (int)((total + 255) / 256 < device_sm_count() * 8 ? (total + 255) / 256 : device_sm_count() * 8);
   const int src_per_chunk = src_ld >= chunks * n ? 1 : 0;
   add_table_kernel<<<grid, 256, 0, stream>>>(table, table_rows, src, src_ld, src_per_chunk, dst, B, n, chunks, plus_one_mask);
   CE_CHECK_CUDA(cudaGetLastError());

@@ -1,10 +1,10 @@
-// ce_encoder: the two once-per-edit encoders in front of the sampling loop (SURVEY.md section 8(f) row 3), on the same tcgen05
+// ce_encoder: the two once-per-edit encoders in front of the sampling loop (SURVEY.md section 8(f) row 3), on the same wgmma
 // GEMM as the DiT:
 //   UMT5 text encoder   -- `self.text_encoder(input_ids, mask).last_hidden_state`  (chronoedit_diffusers/pipeline_chronoedit.py:205-244;
 //                          transformers UMT5EncoderModel: T5LayerNorm, per-layer relative-position bias, un-scaled QK^T, gated GELU)
 //   CLIP vision encoder -- `self.image_encoder(**image, output_hidden_states=True).hidden_states[-2]`  (:246-254; transformers
 //                          CLIPVisionModel: patch conv + class token + position embedding, pre-LN blocks, penultimate hidden state)
-// Every Linear is one launch of the tcgen05 GEMM (fused bias / GELU / residual epilogues); LayerNorm / T5 RMSNorm are the row
+// Every Linear is one launch of the wgmma GEMM (fused bias / GELU / residual epilogues); LayerNorm / T5 RMSNorm are the row
 // kernels of elementwise.cu.  Head dims are 64 (UMT5) and 80 (CLIP ViT-H), sequence lengths 512 and 257: attention is S = Q K^T
 // per head (fp32 accumulator out of the GEMM), one row-softmax launch per layer over ALL heads (which applies the reference's
 // bf16 rounding of the scores, the T5 position bias / key mask or the CLIP scale), and O = P V per head with V^T produced for all
@@ -33,7 +33,7 @@ namespace {
 constexpr int TPB = 256;
 inline int grid_for(size_t n) {
   size_t g = (n + TPB - 1) / TPB;
-  return (int)(g < 148 * 16 ? (g ? g : 1) : 148 * 16);
+  return (int)(g < device_sm_count() * 16 ? (g ? g : 1) : device_sm_count() * 16);
 }
 inline int up8(int v) { return (v + 7) & ~7; }
 

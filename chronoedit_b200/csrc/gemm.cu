@@ -1,23 +1,23 @@
-// bf16 GEMM for sm_100a: TMA -> shared-memory ring -> tcgen05.mma (accumulators in TMEM) -> fused epilogue.
+// bf16 GEMM for sm_90a: TMA -> shared-memory ring -> wgmma (accumulators in registers) -> fused epilogue.
 //
 //   out[M,N] = epilogue( A[M,K] * W[N,K]^T )        A: activations (row-major), W: nn.Linear weight (row-major)
 //
-// Persistent, warp-specialised, one CTA per SM:
-//   warp 0      TMA producer (one lane): A tile 128x64, W tile BNx64 per k-block, 128B swizzle, STAGES-deep ring
-//   warp 1      MMA issuer (one lane): 4 x tcgen05.mma (M128, N=BN, K16) per k-block; tcgen05.commit frees the
-//               ring slot and, after the last k-block, publishes the accumulator; also owns the TMEM allocation
-//   warps 2..5  epilogue: tcgen05.ld 32 lanes x 32 columns -> bias / activation / gate / residual -> global
-// Two accumulator stages in TMEM (2 x BN columns) let the epilogue of tile i overlap the MMAs of tile i+1.
+// Persistent, warp-specialised, one CTA per SM, 384 threads = 3 warpgroups (registers re-partitioned with setmaxnreg):
+//   warpgroup 0     TMA producer (one lane of warp 0): A tile 128x64, W tile BNx64 per k-block, 128B swizzle, STAGES-deep ring
+//   warpgroups 1,2  consumers: 64 rows x BN columns of the tile each, 4 x wgmma (M64, N=BN, K16) per k-block with both operands
+//                   read from the ring, then bias / activation / gate / residual from the accumulator registers -> global
+// While the consumers run the epilogue of tile i the producer already fills the ring for tile i+1.
 // Tile order is grouped along M so that concurrently resident tiles share W column panels through L2.
 //
 // Replaces the cuBLASLt calls behind every nn.Linear of the reference DiT block
-// (/root/reference/chronoedit_diffusers/transformer_chronoedit.py:58-60, 84-87, 106, 292) plus the elementwise
+// (chronoedit_diffusers/transformer_chronoedit.py:58-60, 84-87, 106, 292) plus the elementwise
 // launches that follow them (:281, :286, :293).
 #include <stdlib.h>
 
 #include <cstdlib>
 
 #include "gemm.cuh"
+#include "wgmma.cuh"
 
 namespace ce {
 
@@ -25,7 +25,7 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int GEMM_THREADS = 192;
+constexpr int GEMM_THREADS = 384;
 
 __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int group_m, int& mb, int& nb) {
   const int per_group = group_m * tiles_n;
@@ -50,19 +50,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g) {
   constexpr uint32_t A_BYTES = BM * BK * 2;
   constexpr uint32_t B_BYTES = BN * BK * 2;
-  constexpr uint32_t TMEM_COLS = 2 * BN;  // power of two >= 32 for BN in {64,128,256}
-  constexpr uint32_t IDESC = umma_idesc_bf16(BM, BN, 0);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));
-  uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES;
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));
+  uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -74,32 +68,25 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 4);  // one arrive per epilogue warp
+      mbar_init(&empty[i], 2);  // one arrive per consumer warpgroup
     }
     fence_mbar_init();
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ------------------------------------------------------------------ TMA producer
-    if (elect_one_sync()) {  // one lane, known to the compiler as such: no per-instruction serialisation loops around UTMALDG / UTCHMMA
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one_sync()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         int mb, nb;
         tile_coords(t, tiles_m, tiles_n, g.group_m, mb, nb);
         for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1, 100 + stage);
+          mbar_wait(&empty[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
           tma_load_2d(sA + stage * A_BYTES, &tma_a, &full[stage], kb * BK, mb * BM);
           tma_load_2d(sB + stage * B_BYTES, &tma_b, &full[stage], kb * BK, nb * BN);
@@ -110,155 +97,101 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (elect_one_sync()) {  // one lane, known to the compiler as such: no per-instruction serialisation loops around UTMALDG / UTCHMMA
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        mbar_wait(&tempty[acc], acc_phase ^ 1, 200 + acc);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&full[stage], phase, 300 + stage);
-          tc_fence_after();
-          const uint64_t da = umma_desc_kmajor_sw128(smem_u32(sA + stage * A_BYTES));
-          const uint64_t db = umma_desc_kmajor_sw128(smem_u32(sB + stage * B_BYTES));
-          // four K16 steps (+32 bytes each inside the 128-byte swizzle row: start-address field += 2), one asm statement
-          umma_bf16_ss_x4(d_tmem, da, db, IDESC, kb != 0);
-          umma_commit(&empty[stage]);  // slot reusable once these MMAs have read it
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tfull[acc]);  // accumulator complete
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..5)
-    const int q = warp & 3;  // TMEM lane quadrant this warp may access
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      int mb, nb;
-      tile_coords(t, tiles_m, tiles_n, g.group_m, mb, nb);
-      mbar_wait(&tfull[acc], acc_phase, 400 + acc);
-      tc_fence_after();
-      const int row = mb * BM + q * 32 + lane;
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers: main loop + epilogue
+  setmaxnreg_inc<232>();
+  const int wg = (warp >> 2) - 1;                           // rows [64 wg, 64 wg + 64) of the tile
+  const int r_in_tile = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int c_in_group = 2 * (lane & 3);
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BN / 2];
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    int mb, nb;
+    tile_coords(t, tiles_m, tiles_n, g.group_m, mb, nb);
+    wgmma_ring_tile<BN, STAGES>(acc, smem_u32(sA) + wg * 64 * 128, smem_u32(sB), A_BYTES, B_BYTES, full, empty, kblocks, stage, phase);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {   // the thread's two rows
+      const int row = mb * BM + r_in_tile + 8 * h;
       const bool row_ok = row < g.M;
       const int batch = row_ok ? row / g.rows_per_batch : 0;
-      const uint32_t t_row = tmem_base + (uint32_t(q * 32) << 16) + acc * BN;
-      float st_pivot = 0.f, st_s = 0.f, st_ss = 0.f;   // row statistics of this tile (GemmArgs::stats_out)
+      // row statistics of this tile (GemmArgs::stats_out): the four lanes that share a row keep partial sums about one pivot
+      float st_pivot = 0.f, st_s = 0.f, st_ss = 0.f;
       int st_n = 0;
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int n0 = nb * BN + c * 32;
-        if (n0 >= g.N) break;  // warp-uniform
-        uint32_t r[32];
-        tmem_ld_32x32(t_row + c * 32, r);
-        tmem_ld_wait();
-        if (row_ok) {
 #pragma unroll
-          for (int v = 0; v < 4; ++v) {  // 8 columns per step
-            const int n = n0 + v * 8;
-            if (n >= g.N) break;
-            float y[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) y[j] = __uint_as_float(r[v * 8 + j]);
-            if (g.bias) {
-              const uint4 bv = *reinterpret_cast<const uint4*>(g.bias + n);
-              const float2 b0 = unpack_bf16x2(bv.x), b1 = unpack_bf16x2(bv.y), b2 = unpack_bf16x2(bv.z),
-                           b3 = unpack_bf16x2(bv.w);
-              y[0] += b0.x; y[1] += b0.y; y[2] += b1.x; y[3] += b1.y;
-              y[4] += b2.x; y[5] += b2.y; y[6] += b3.x; y[7] += b3.y;
-            }
-            if (g.bias_row) {
-              const float br = __bfloat162float(g.bias_row[row]);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) y[j] += br;
-            }
-            if (g.out_f32) {
-              float4* o = reinterpret_cast<float4*>(g.out_f32 + (size_t)row * (g.ld_f32 ? g.ld_f32 : g.N) + n);
-              o[0] = make_float4(y[0], y[1], y[2], y[3]);
-              o[1] = make_float4(y[4], y[5], y[6], y[7]);
-              if (!g.out) continue;
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j) y[j] = bf16_round(y[j]);  // nn.Linear returns bf16
+      for (int j = 0; j < BN / 8; ++j) {   // 8-column groups, two columns per lane
+        const int n = nb * BN + j * 8 + c_in_group;
+        const bool ok = row_ok && nb * BN + j * 8 < g.N;
+        float y0 = acc[4 * j + 2 * h], y1 = acc[4 * j + 2 * h + 1];
+        bool stored = false;
+        if (ok) {
+          if (g.bias) {
+            const float2 bv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(g.bias + n));
+            y0 += bv.x;
+            y1 += bv.y;
+          }
+          if (g.bias_row) {
+            const float br = __bfloat162float(g.bias_row[row]);
+            y0 += br;
+            y1 += br;
+          }
+          if (g.out_f32) *reinterpret_cast<float2*>(g.out_f32 + (size_t)row * (g.ld_f32 ? g.ld_f32 : g.N) + n) = make_float2(y0, y1);
+          if (g.out) {
+            y0 = bf16_round(y0);  // nn.Linear returns bf16
+            y1 = bf16_round(y1);
             if (g.epi == EPI_BIAS_GELU_TANH) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) y[j] = gelu_tanh_f(y[j]);
+              y0 = gelu_tanh_f(y0);
+              y1 = gelu_tanh_f(y1);
             } else if (g.epi == EPI_BIAS_GELU_ERF) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) y[j] = gelu_erf_f(y[j]);
+              y0 = gelu_erf_f(y0);
+              y1 = gelu_erf_f(y1);
             } else if (g.epi == EPI_BIAS_GATE_RESID || g.epi == EPI_BIAS_RESID) {
-              const uint4 xv = *reinterpret_cast<const uint4*>(g.resid + (size_t)row * g.ldr + n);
-              const float2 x0 = unpack_bf16x2(xv.x), x1 = unpack_bf16x2(xv.y), x2 = unpack_bf16x2(xv.z),
-                           x3 = unpack_bf16x2(xv.w);
-              const float x[8] = {x0.x, x0.y, x1.x, x1.y, x2.x, x2.y, x3.x, x3.y};
+              const float2 x = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(g.resid + (size_t)row * g.ldr + n));
               if (g.epi == EPI_BIAS_GATE_RESID) {
-                const float4* gp = reinterpret_cast<const float4*>(g.gate + (size_t)batch * g.gate_stride + n);
-                const float4 g0 = gp[0], g1 = gp[1];
-                const float gt[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-#pragma unroll
-                for (int j = 0; j < 8; ++j) y[j] = x[j] + y[j] * gt[j];
+                const float2 gt = *reinterpret_cast<const float2*>(g.gate + (size_t)batch * g.gate_stride + n);
+                y0 = x.x + y0 * gt.x;
+                y1 = x.y + y1 * gt.y;
               } else {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) y[j] = x[j] + y[j];
+                y0 = x.x + y0;
+                y1 = x.y + y1;
               }
             }
-            if (g.stats_mode) {   // statistics of the values as stored (bf16), pivot-shifted inside the tile
-              float z[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) z[j] = bf16_round(y[j]);
-              if (st_n == 0) st_pivot = g.stats_mode == 1 ? z[0] : 0.f;
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float d = z[j] - st_pivot;
-                st_s += d;
-                st_ss = fmaf(d, d, st_ss);
-              }
-              st_n += 8;
-            }
-            uint4 o;
-            o.x = pack_bf16x2(y[0], y[1]);
-            o.y = pack_bf16x2(y[2], y[3]);
-            o.z = pack_bf16x2(y[4], y[5]);
-            o.w = pack_bf16x2(y[6], y[7]);
-            *reinterpret_cast<uint4*>(g.out + (size_t)row * g.ldo + n) = o;
+            *reinterpret_cast<uint32_t*>(g.out + (size_t)row * g.ldo + n) = pack_bf16x2(y0, y1);
+            stored = true;
+          }
+        }
+        if (g.stats_mode) {   // statistics of the values as stored (bf16), pivot-shifted inside the tile
+          const float z0 = bf16_round(y0), z1 = bf16_round(y1);
+          if (j == 0) st_pivot = g.stats_mode == 1 ? __shfl_sync(0xffffffffu, z0, lane & ~3) : 0.f;  // the row's first column
+          if (stored) {
+            const float d0 = z0 - st_pivot, d1 = z1 - st_pivot;
+            st_s += d0 + d1;
+            st_ss = fmaf(d0, d0, st_ss);
+            st_ss = fmaf(d1, d1, st_ss);
+            st_n += 8;
           }
         }
       }
-      if (g.stats_mode && row_ok && st_n > 0) {
-        float2 pr;
-        if (g.stats_mode == 1) {   // (mean, M2) of this tile's st_n columns
-          const float md = st_s / (float)st_n;
-          pr = make_float2(st_pivot + md, fmaxf(st_ss - st_s * md, 0.f));
-        } else {
-          pr = make_float2(st_ss, 0.f);
+      if (g.stats_mode) {   // warp-uniform; the quad's partial sums are added in a fixed order
+        st_s += __shfl_xor_sync(0xffffffffu, st_s, 1);
+        st_ss += __shfl_xor_sync(0xffffffffu, st_ss, 1);
+        st_s += __shfl_xor_sync(0xffffffffu, st_s, 2);
+        st_ss += __shfl_xor_sync(0xffffffffu, st_ss, 2);
+        if (row_ok && st_n > 0 && (lane & 3) == 0) {
+          float2 pr;
+          if (g.stats_mode == 1) {   // (mean, M2) of this tile's st_n columns
+            const float md = __fdividef(st_s, (float)st_n);  // no call: a subroutine would serialise the wgmma pipeline
+            pr = make_float2(st_pivot + md, fmaxf(st_ss - st_s * md, 0.f));
+          } else {
+            pr = make_float2(st_ss, 0.f);
+          }
+          g.stats_out[(size_t)row * g.stats_ld + nb] = pr;
         }
-        g.stats_out[(size_t)row * g.stats_ld + nb] = pr;
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 template <int BN, int STAGES>
@@ -273,16 +206,6 @@ int launch_variant(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs&
 }
 
 }  // namespace
-
-int launch_gemm_bf16_2cta(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, cudaStream_t stream);  // gemm2.cu
-
-static bool use_2cta() {
-  static const bool on = [] {
-    const char* e = getenv("CE_GEMM_2CTA");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
 
 int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmArgs& g, cudaStream_t stream) {
   CE_REQUIRE(g.M > 0 && g.N > 0 && g.K > 0, "gemm: empty problem");
@@ -300,8 +223,7 @@ int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmA
                                (g.stats_mode == 1 || g.stats_mode == 2), "gemm: stats_out / stats_ld / stats_mode");
   GemmArgs a = g;
   // Tiles are rasterised in groups of group_m M-tiles x all N-tiles so that the A panel of a group stays in L2 while the W
-  // panels stream past it.  Measured at the 14B shapes (CE_GEMM_GROUP_M sweep, repeated A/B): 16 beats 8 by 2 % at K = 5120,
-  // no significant difference at K = 13824 or for 29 M-tiles, 4 is -3..6 %, a single group (57) -16 %.
+  // panels stream past it (16 M-tiles x 128 rows x K = 5120 is 20 MB of A, inside the H100's 50 MB L2).
   if (a.group_m <= 0) a.group_m = 16;
   {
     static const int env_gm = [] {   // developer knob (A/B)
@@ -314,10 +236,8 @@ int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmA
   CUtensorMap ta, tb;
   int rc = make_tmap_2d(&ta, A, (uint64_t)a.M, (uint64_t)a.K, (uint64_t)lda, BM);
   if (rc) return rc;
-  const bool pair = bn == 256 && a.M >= 512 && use_2cta();  // 256 x 256 tiles on CTA pairs (gemm2.cu)
-  rc = make_tmap_2d(&tb, W, (uint64_t)a.N, (uint64_t)a.K, (uint64_t)ldw, (uint32_t)(pair ? 128 : bn));
+  rc = make_tmap_2d(&tb, W, (uint64_t)a.N, (uint64_t)a.K, (uint64_t)ldw, (uint32_t)bn);
   if (rc) return rc;
-  if (pair) return launch_gemm_bf16_2cta(ta, tb, a, stream);
   if (bn == 256) return launch_variant<256, 4>(ta, tb, a, stream);
   if (bn == 128) return launch_variant<128, 6>(ta, tb, a, stream);
   return launch_variant<64, 8>(ta, tb, a, stream);

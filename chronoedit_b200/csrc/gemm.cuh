@@ -1,4 +1,4 @@
-// Interface of the tcgen05 GEMM used by the DiT path (gemm.cu).
+// Interface of the wgmma GEMM used by the DiT path (gemm.cu).
 #pragma once
 #include "host_common.h"
 #include "ptx.cuh"

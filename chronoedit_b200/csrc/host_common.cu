@@ -99,9 +99,9 @@ int check_device() {
                                       "); chronoedit_b200 has no CPU fallback");
   int major = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10)
+  if (major != 9)
     return fail(CE_ERR_NO_DEVICE, "device compute capability " + std::to_string(major) +
-                                      ".x is not sm_100; this library is built for sm_100a only");
+                                      ".x is not sm_90; this library is built for sm_90a only");
   return CE_OK;
 }
 

@@ -17,7 +17,7 @@ enum Status : int {
   CE_OK = 0,
   CE_ERR_INVALID = -1,      // bad argument / unsupported shape
   CE_ERR_CUDA = -2,         // CUDA runtime / driver error
-  CE_ERR_NO_DEVICE = -3,    // no sm_100 device: there is NO CPU fallback
+  CE_ERR_NO_DEVICE = -3,    // no sm_90 device: there is NO CPU fallback
   CE_ERR_MISSING_WEIGHT = -4,
   CE_ERR_WORKSPACE = -5,
 };
@@ -56,6 +56,6 @@ int ensure_dynamic_smem(const void* kernel, int bytes);
   do {                                                                                             \
     int _rc = ::ce::ensure_dynamic_smem(reinterpret_cast<const void*>(kernel), (int)(bytes));      \
     if (_rc) return _rc;                                                                           \
-  } while (0)  // CE_OK iff the current device is compute capability 10.x
+  } while (0)  // CE_OK iff the current device is compute capability 9.x
 
 }  // namespace ce

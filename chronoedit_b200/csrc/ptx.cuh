@@ -1,12 +1,10 @@
-// sm_100a primitives used by every kernel in this library: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / st / fences) and UMMA descriptor builders.
-// Hand-written inline PTX; no CUTLASS/CuTe dependency.
+// sm_90a primitives shared by the kernels of this library: mbarrier, TMA (cp.async.bulk.tensor), named barriers and small
+// numeric helpers.  The warpgroup MMA wrappers are in wgmma.cuh.  Hand-written inline PTX; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>  // CUtensorMap (types only; libcuda is reached through cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 namespace ce {
 
@@ -18,7 +16,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 
 // One lane of a converged warp (elect.sync): code under `if (elect_one_sync())` is known to the compiler to run in exactly one
-// thread, so warp-uniform operands (tcgen05 descriptors, TMEM addresses) go to uniform registers without a serialisation loop.
+// thread, so the TMA instructions it issues need no serialisation loop.
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile(
@@ -53,67 +51,38 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity
       : "memory");
   return ok;
 }
-// Non-blocking probe (try_wait may suspend the thread for a system-dependent time when the phase is not complete, which is
-// what a blocking wait wants but is poison for a loop that polls several barriers).
-__device__ __forceinline__ uint32_t mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok;
-}
 __device__ __forceinline__ uint64_t global_timer_ns() {
   uint64_t t;
   asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
   return t;
 }
-// Bounded wait: a protocol bug becomes a trapped launch (reported through cudaGetLastError /
-// the next sync) instead of a hung GPU.  The bound is wall time, far above any legitimate wait.
+// Bounded wait: a protocol bug becomes a trapped launch (reported through cudaGetLastError / the next sync) instead of a hung
+// GPU.  The bound is wall time, far above any legitimate wait.  It traps without a message: with a printf in this function ptxas
+// reported, for every kernel that waits on a barrier between wgmma.mma_async and its wait_group, "(C7510) Potential Performance
+// Loss: wgmma.mma_async instructions are serialized due to wgmma pipeline crossing function boundary at a function call".
 #ifndef CE_MBAR_TIMEOUT_NS
 #define CE_MBAR_TIMEOUT_NS 4000000000ull
 #endif
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   uint64_t t0 = global_timer_ns();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3FF) == 0 && global_timer_ns() - t0 > CE_MBAR_TIMEOUT_NS) {
-      printf("[chronoedit_b200] mbarrier timeout: tag=%d block=(%d,%d,%d) thread=%d parity=%u\n", tag, blockIdx.x,
-             blockIdx.y, blockIdx.z, threadIdx.x, parity);
-      __trap();
-    }
-  }
-}
-
-// Spinning wait (test_wait never suspends the thread): lowest wake-up latency, for the one or two threads whose reaction time is
-// on a critical chain.  Same wall-clock bound as mbar_wait.
-__device__ __forceinline__ void mbar_spin(uint64_t* bar, uint32_t parity, int tag = 0) {
-  if (mbar_test_wait(bar, parity)) return;
-  uint64_t t0 = 0;
-  uint32_t spins = 0;
-  while (!mbar_test_wait(bar, parity)) {
-    if ((++spins & 0xFFFF) == 0) {
-      if (t0 == 0) t0 = global_timer_ns();
-      else if (global_timer_ns() - t0 > CE_MBAR_TIMEOUT_NS) {
-        printf("[chronoedit_b200] mbarrier (spin) timeout: tag=%d block=(%d,%d,%d) thread=%d parity=%u\n", tag, blockIdx.x, blockIdx.y,
-               blockIdx.z, threadIdx.x, parity);
-        __trap();
-      }
-    }
+    if ((++spins & 0x3FF) == 0 && global_timer_ns() - t0 > CE_MBAR_TIMEOUT_NS) __trap();
   }
 }
 
 // ------------------------------------------------------------------ proxies / fences
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Register re-partition between the warpgroups of a CTA (executed by every thread of a warpgroup): the TMA producer warpgroup
+// gives registers up, the MMA warpgroups that hold the accumulators take them.
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
 
 // ------------------------------------------------------------------ TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -134,16 +103,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// multicast: the box lands at the same CTA-relative offset in every CTA of `cta_mask`, and each of those CTAs' barrier at the
-// CTA-relative offset of `bar` receives the complete_tx
-__device__ __forceinline__ void tma_load_3d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                               uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], "
-      "[%2], %6;" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
                                             int c2, int c3) {
   asm volatile(
@@ -151,271 +110,6 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       "[%2];" ::"r"(smem_u32(smem_dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
-}
-__device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                            int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, "
-      "%7}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-
-// ------------------------------------------------------------------ TMEM
-// All .sync.aligned: must be executed by every lane of one warp.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; bf16 inputs, fp32 accumulate.  Issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]: A = 128 lanes x K bf16 packed two per 32-bit column (K-major only).  Issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Eight / four MMAs in ONE asm statement: nothing but the UTCHMMA instructions themselves between consecutive issues.  The
-// issuing thread's own work between two tcgen05.mma (descriptor arithmetic, predicate set-up) is NOT hidden behind the previous
-// MMA when that work is longer than the MMA itself (64 cycles at M128 x N128 x K16): measured in the attention kernel, 95-115
-// cycles per MMA with the descriptors computed inline vs the 64-cycle floor (profiles/r2d_attention_per_mma_issue_stamps.log).
-// The first MMA overwrites D when acc_first == 0, the others accumulate.
-__device__ __forceinline__ void umma_bf16_ss_x8(uint32_t tmem_d, const uint64_t (&da)[8], const uint64_t (&db)[8], uint32_t idesc,
-                                                uint32_t acc_first) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %18, 0;\n\t"
-      "setp.eq.b32 q, 0, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %9, %17, p;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %2, %10, %17, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %3, %11, %17, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %4, %12, %17, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %5, %13, %17, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %6, %14, %17, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %7, %15, %17, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %8, %16, %17, q;\n\t}" ::"r"(tmem_d),
-      "l"(da[0]), "l"(da[1]), "l"(da[2]), "l"(da[3]), "l"(da[4]), "l"(da[5]), "l"(da[6]), "l"(da[7]), "l"(db[0]), "l"(db[1]), "l"(db[2]),
-      "l"(db[3]), "l"(db[4]), "l"(db[5]), "l"(db[6]), "l"(db[7]), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-// Four K16 steps of one 64-wide k-block: descriptors base + 2*k (32 bytes along K inside the 128-byte swizzle row)
-__device__ __forceinline__ void umma_bf16_ss_x4(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc_first) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 a1, a2, a3, b1, b2, b3;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "setp.eq.b32 q, 0, 0;\n\t"
-      "add.u64 a1, %1, 2;\n\tadd.u64 a2, %1, 4;\n\tadd.u64 a3, %1, 6;\n\t"
-      "add.u64 b1, %2, 2;\n\tadd.u64 b2, %2, 4;\n\tadd.u64 b3, %2, 6;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], a1, b1, %3, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], a2, b2, %3, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], a3, b3, %3, q;\n\t}" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_2sm_x4(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc_first) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 a1, a2, a3, b1, b2, b3;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "setp.eq.b32 q, 0, 0;\n\t"
-      "add.u64 a1, %1, 2;\n\tadd.u64 a2, %1, 4;\n\tadd.u64 a3, %1, 6;\n\t"
-      "add.u64 b1, %2, 2;\n\tadd.u64 b2, %2, 4;\n\tadd.u64 b3, %2, 6;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], a1, b1, %3, q;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], a2, b2, %3, q;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], a3, b3, %3, q;\n\t}" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-// A from TMEM at tmem_a, tmem_a + a_step, ... (packed bf16 columns), B descriptors db[0..3]
-__device__ __forceinline__ void umma_bf16_ts_x4(uint32_t tmem_d, uint32_t tmem_a, uint32_t a_step, uint64_t db0, uint64_t db1, uint64_t db2,
-                                                uint64_t db3, uint32_t idesc, uint32_t acc_first) {
-  const uint32_t a1 = tmem_a + a_step, a2 = tmem_a + 2 * a_step, a3 = tmem_a + 3 * a_step;
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %10, 0;\n\t"
-      "setp.eq.b32 q, 0, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %5, %9, p;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%2], %6, %9, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%3], %7, %9, q;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%4], %8, %9, q;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "r"(a1), "r"(a2), "r"(a3), "l"(db0), "l"(db1), "l"(db2), "l"(db3), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ts_x2(uint32_t tmem_d, uint32_t tmem_a, uint32_t a_step, uint64_t db0, uint64_t db1, uint32_t idesc,
-                                                uint32_t acc_first) {
-  const uint32_t a1 = tmem_a + a_step;
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "setp.eq.b32 q, 0, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %3, %5, p;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%2], %4, %5, q;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "r"(a1), "l"(db0), "l"(db1), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-// Arrive on an mbarrier once every tcgen05.mma issued so far by this thread has completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i of the warp = lane base + i).
-// 1-CTA MMAs, completion signalled on the barrier at the same CTA-relative offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]),
-      "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
-               "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------ 2-CTA (cta_group::2) variants
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-// TMA load whose completion bytes are credited to the LEADER CTA's mbarrier (peer bit of the barrier address cleared)
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  const uint64_t hint = 0x1000000000000000ull;  // EVICT_NORMAL
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint "
-      "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "l"(hint)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::
-          "r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A (256 rows, 128 per CTA) * B (N rows, N/2 per CTA); issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_bf16_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once all prior MMAs of this thread completed) on the mbarrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_bf16_ts_2sm(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// ------------------------------------------------------------------ UMMA descriptors
-// Shared-memory matrix descriptor (64-bit):
-//   [0,14)  start address >> 4        [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
-//   [46,48) version (1 on sm_100)     [49,52) base offset                [61,64) layout (2 = SWIZZLE_128B)
-// K-major, 128B swizzle: rows of 128 B (64 bf16 along K), 8-row groups 1024 B apart (SBO); LBO unused (1).
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-// MN-major, 128B swizzle: 128-B rows hold 64 consecutive MN elements for one k; 8 k-rows = 1024 B (SBO, between
-// 8-k groups); the next 64-element MN chunk lies `lbo_bytes` further on.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t saddr, uint32_t lbo_bytes) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-// Instruction descriptor (32-bit) for kind::f16, bf16 x bf16 -> fp32:
-//   [4,6) D format (1 = f32)  [7,10) A format (1 = bf16)  [10,13) B format (1 = bf16)
-//   [15] A major (0 = K)  [16] B major (0 = K, 1 = MN)  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int m, int n, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(n >> 3) << 17) |
-         ((uint32_t)(m >> 4) << 24);
 }
 
 // ------------------------------------------------------------------ small helpers
@@ -432,58 +126,6 @@ __device__ __forceinline__ float fast_exp2(float x) {  // MUFU.EX2; exp2(-inf) =
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-// same instruction, but ordered against the other volatile asm statements (tcgen05.ld / wait::ld): used where exponentials must be
-// issued BEFORE a later TMEM wait so that they overlap the loads still in flight
-__device__ __forceinline__ float fast_exp2_ordered(float x) {
-  float y;
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-// packed fp32 pairs (sm_100 FFMA2 / FADD2): one instruction for two lanes of work
-__device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ uint64_t f2_pack_bits(uint32_t lo, uint32_t hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// 2^x for a packed pair on the FMA pipe instead of the MUFU (16 ex2/clk/SM is what bounds the attention softmax):
-// round-to-nearest split x = n + f with the 1.5*2^23 trick, degree-3 minimax polynomial for 2^f on [-0.5, 0.5]
-// (max relative error 7.6e-5, far below the bf16 rounding of P), exponent added as an integer.  Valid for x <= 127.
-__device__ __forceinline__ void f2_exp2_poly(uint64_t x2, float& p0, float& p1) {
-  float x0, x1;
-  f2_unpack(x2, x0, x1);
-  x0 = fmaxf(x0, -126.0f);
-  x1 = fmaxf(x1, -126.0f);
-  const uint64_t xc = f2_pack(x0, x1);
-  const uint64_t t = f2_add(xc, f2_pack(12582912.0f, 12582912.0f));
-  const uint64_t n = f2_add(t, f2_pack(-12582912.0f, -12582912.0f));
-  const uint64_t f = f2_fma(n, f2_pack(-1.0f, -1.0f), xc);
-  uint64_t p = f2_fma(f2_pack(0.05520550534129143f, 0.05520550534129143f), f, f2_pack(0.24261397123336792f, 0.24261397123336792f));
-  p = f2_fma(p, f, f2_pack(0.6932547688484192f, 0.6932547688484192f));
-  p = f2_fma(p, f, f2_pack(0.9999276995658875f, 0.9999276995658875f));
-  uint32_t tl, th, pl, ph;
-  asm("mov.b64 {%0, %1}, %2;" : "=r"(tl), "=r"(th) : "l"(t));
-  asm("mov.b64 {%0, %1}, %2;" : "=r"(pl), "=r"(ph) : "l"(p));
-  p0 = __uint_as_float(pl + (tl << 23));
-  p1 = __uint_as_float(ph + (th << 23));
 }
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -78,7 +78,7 @@ __global__ void patchify_range_kernel(const bf16* __restrict__ x, bf16* __restri
 
 inline int grid_for(size_t n) {
   size_t g = (n + 255) / 256;
-  return (int)(g < 148 * 16 ? (g ? g : 1) : 148 * 16);
+  return (int)(g < device_sm_count() * 16 ? (g ? g : 1) : device_sm_count() * 16);
 }
 
 }  // namespace

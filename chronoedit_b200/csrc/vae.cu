@@ -1,11 +1,11 @@
-// ce_vae: Wan2.1 3D causal VAE encode / decode as a chain of sm_100a kernels behind the C ABI.
+// ce_vae: Wan2.1 3D causal VAE encode / decode as a chain of sm_90a kernels behind the C ABI.
 //
 // Follows WanVAE_.encode / .decode of /root/reference/chronoedit/_src/tokenizers/wan2pt1.py:502-560 (the arithmetic twin
 // of diffusers AutoencoderKLWan, which the pipeline calls at pipeline_chronoedit.py:436-443, 776-781): chunked causal
 // streaming (frame 0 alone, then 4-frame chunks when encoding; one latent frame per iteration when decoding) with a
 // 2-frame history per causal convolution.  Activations are channels-last bf16; every convolution with Cin >= 64 is the
-// tcgen05 implicit GEMM of conv.cu reading its input (history frames + chunk) in place; the three small-Cin convolutions
-// (3->dim, z->top, 2z->2z) go through im2row + the tcgen05 GEMM; RMS_norm+SiLU / upsample / softmax are the row kernels
+// wgmma implicit GEMM of conv.cu reading its input (history frames + chunk) in place; the three small-Cin convolutions
+// (3->dim, z->top, 2z->2z) go through im2row + the wgmma GEMM; RMS_norm+SiLU / upsample / softmax are the row kernels
 // of vae_kernels.cu; the single-head mid attention is GEMM (QK^T, fp32) -> row softmax -> GEMM (P V).
 #include <math.h>
 #include <stdlib.h>

@@ -152,7 +152,7 @@ __global__ void cl_to_planar_kernel(const bf16* __restrict__ cl, int C, bf16* __
 
 int grid_for(size_t total, int block) {
   size_t g = (total + block - 1) / block;
-  const size_t cap = (size_t)148 * 16;
+  const size_t cap = (size_t)device_sm_count() * 16;
   return (int)(g < cap ? (g == 0 ? 1 : g) : cap);
 }
 

@@ -1,11 +1,11 @@
-"""B200-native drop-ins for the two encoders the pipeline runs once per edit (SURVEY.md section 8(f) row 3):
+"""H100-native drop-ins for the two encoders the pipeline runs once per edit (SURVEY.md section 8(f) row 3):
 
     transformers.UMT5EncoderModel   `self.text_encoder(input_ids, attention_mask).last_hidden_state`   pipeline_chronoedit.py:205-244
     transformers.CLIPVisionModel    `self.image_encoder(**image, output_hidden_states=True).hidden_states[-2]`     :246-254
 
 Same constructor configuration fields, same parameter names as the transformers modules (their `state_dict()` loads unchanged),
 same call surface as far as the pipeline touches it.  All arithmetic runs in libchronoedit_b200.so (`ce_umt5_encode`,
-`ce_clip_vision_encode`: tcgen05 GEMMs + row kernels, csrc/encoders.cu); PyTorch owns memory and streams.  No CPU path.
+`ce_clip_vision_encode`: wgmma GEMMs + row kernels, csrc/encoders.cu); PyTorch owns memory and streams.  No CPU path.
 """
 from __future__ import annotations
 
@@ -137,7 +137,7 @@ class UMT5EncoderModel(_Base):
     @torch.no_grad()
     def _pack(self) -> None:
         if self.device.type != "cuda":
-            raise CEError("UMT5EncoderModel must live on a CUDA (sm_100) device; there is no CPU path")
+            raise CEError("UMT5EncoderModel must live on a CUDA (sm_90) device; there is no CPU path")
         c = self.config
         self._create(EncoderConfigC(0, c.vocab_size, c.d_model, c.d_kv, c.d_ff, c.num_layers, c.num_heads, c.layer_norm_epsilon, 0, 0, 0))
         self._keep = {}
@@ -257,7 +257,7 @@ class CLIPVisionModel(_Base):
     @torch.no_grad()
     def _pack(self) -> None:
         if self.device.type != "cuda":
-            raise CEError("CLIPVisionModel must live on a CUDA (sm_100) device; there is no CPU path")
+            raise CEError("CLIPVisionModel must live on a CUDA (sm_90) device; there is no CPU path")
         c = self.config
         self._create(EncoderConfigC(1, 0, c.hidden_size, c.hidden_size // c.num_attention_heads, c.intermediate_size, c.num_hidden_layers,
                                     c.num_attention_heads, c.layer_norm_eps, c.image_size, c.patch_size, 1 if c.hidden_act == "gelu" else 0))

@@ -1,10 +1,10 @@
-"""B200-native drop-in for `ChronoEditTransformer3DModel`.
+"""H100-native drop-in for `ChronoEditTransformer3DModel`.
 
 Host-side mirror of /root/reference/chronoedit_diffusers/transformer_chronoedit.py:298-476: same constructor
 arguments, same parameter names (so a diffusers checkpoint / `state_dict` loads unchanged), same
 `forward(hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image=None, return_dict=True,
 attention_kwargs=None)` signature and return types, `.config`, `.dtype`, `from_pretrained`.  All arithmetic happens in
-libchronoedit_b200.so (hand-written sm_100a kernels) through the C ABI of include/chronoedit_b200.h; PyTorch only
+libchronoedit_b200.so (hand-written sm_90a kernels) through the C ABI of include/chronoedit_b200.h; PyTorch only
 owns the memory and the stream.  There is no PyTorch fallback path.
 """
 from __future__ import annotations
@@ -246,7 +246,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         `forward_fp32`.  The bf16 parameters of this module are untouched."""
         dev = self.device
         if dev.type != "cuda":
-            raise CEError("fp32 validation mode needs the module on a CUDA (sm_100) device; there is no CPU path")
+            raise CEError("fp32 validation mode needs the module on a CUDA (sm_90) device; there is no CPU path")
         L = _lib.lib()
         self._ensure_handle()
         own = {n for n, _ in self.named_parameters()}
@@ -264,7 +264,7 @@ class ChronoEditTransformer3DModel(nn.Module):
     def forward_fp32(self, hidden_states: torch.Tensor, timestep: torch.Tensor, encoder_hidden_states: torch.Tensor,
                      encoder_hidden_states_image: Optional[torch.Tensor] = None, return_block0: bool = False):
         """VALIDATION mode (include/chronoedit_b200.h, ce_dit_forward_fp32): fp32 in, fp32 weights, fp32 out, every matrix product
-        on the tcgen05 GEMM with split-bf16 operands.  Meets rtol 1e-3 / atol 1e-4 against the reference's fp32 run end to end
+        on the wgmma GEMM with split-bf16 operands.  Meets rtol 1e-3 / atol 1e-4 against the reference's fp32 run end to end
         (tests/test_gpu_fp32_mode.py); far slower than forward() and not part of any benchmark."""
         if not getattr(self, "_fp32_keepalive", None):
             raise CEError("call enable_fp32_validation(fp32_state_dict) first")
@@ -300,7 +300,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         L = _lib.lib()
         dev = self.device
         if dev.type != "cuda":
-            raise CEError("ChronoEditTransformer3DModel must live on a CUDA (sm_100) device; there is no CPU path")
+            raise CEError("ChronoEditTransformer3DModel must live on a CUDA (sm_90) device; there is no CPU path")
         for n, p in self.named_parameters():
             want = torch.float32 if any(k in n for k in KEEP_FP32) else torch.bfloat16
             if p.dtype != want:

@@ -1,5 +1,5 @@
 /*
- * chronoedit_b200 — C ABI of the B200-native ChronoEdit denoising hot path.
+ * chronoedit_b200 — C ABI of the H100-native ChronoEdit denoising hot path.
  *
  * The reference (nv-tlabs/ChronoEdit) has no FFI for this path: the boundary is two Python objects registered
  * into a diffusers pipeline (pipeline_chronoedit.py:175-183).  This header is the C-ABI underneath the Python
@@ -12,7 +12,7 @@
  *   - `stream` is a cudaStream_t passed as void*; calls are asynchronous on it and never synchronise the device
  *     (the *_host variants synchronise `stream` before returning because they hand results back in host memory);
  *   - return value 0 = success, negative = failure (ce_last_error() holds the message of the calling thread's last
- *     failure); there is NO CPU fallback: on a machine without an sm_100 GPU every compute entry point fails;
+ *     failure); there is NO CPU fallback: on a machine without an sm_90 GPU every compute entry point fails;
  *   - one handle may be used from one thread at a time; distinct handles are independent.
  */
 #ifndef CHRONOEDIT_B200_H_
@@ -29,7 +29,7 @@ extern "C" {
 
 int ce_abi_version(void);
 const char* ce_last_error(void);
-/* 0 iff the current CUDA device is sm_100 (B200). */
+/* 0 iff the current CUDA device is sm_90 (H100). */
 int ce_device_check(void);
 
 /* ------------------------------------------------------------------------------------------------------------
@@ -141,7 +141,7 @@ int64_t ce_dit_host_staging_sample_offset(const ce_dit* h, int batch, int frames
 
 /* VALIDATION mode: the same forward in fp32 -- fp32 inputs, fp32 parameters (registered under their REFERENCE names, unfused:
  * blocks.N.attn1.to_q.weight ..., blocks.N.scale_shift_table [6*D], scale_shift_table [2*D], patch_embedding.weight [D, Cin*4]),
- * fp32 residual stream, fp32 outputs.  Matrix products run on the same tcgen05 GEMM with every fp32 operand split into two bf16
+ * fp32 residual stream, fp32 outputs.  Matrix products run on the same wgmma GEMM with every fp32 operand split into two bf16
  * terms (A_hi.W_hi + A_lo.W_hi + A_hi.W_lo, fp32 accumulate; csrc/dit_fp32.cu).  It exists so that north_star's
  * rtol 1e-3 / atol 1e-4 can be asserted end to end against the reference's fp32 run (tests/test_gpu_fp32_mode.py); it is about
  * 5-10x slower than the bf16 path and is not what bench.py measures.  block_out: optional, block 0's output [B*L, D] fp32. */
@@ -156,7 +156,7 @@ int64_t ce_dit_last_launch_count(const ce_dit* h);
 
 /* Device-side timing of the kernels of subsequent forwards: a CUDA event pair on the launch stream around every
  * launch (up to max_launches; later launches are not recorded).  ce_dit_profile_end waits for the last recorded event
- * and returns, per category c in {0: tcgen05 GEMM, 1: tcgen05 attention, 2: LayerNorm / RMSNorm row kernels,
+ * and returns, per category c in {0: wgmma GEMM, 1: wgmma attention, 2: LayerNorm / RMSNorm row kernels,
  * 3: everything else}: total milliseconds, total algorithmic work (FLOPs for 0/1, bytes for 2) and launch count
  * (each array has 4 entries).  This is what bench.py's "roofline" object is computed from. */
 int ce_dit_profile_begin(ce_dit* h, int max_launches);
@@ -237,7 +237,7 @@ int ce_clip_vision_encode(ce_encoder* h, const void* pixel_values, void* out, in
  * Individual hot-path operators (used by the handles above; exported for operator-level parity tests / profiling)
  * ------------------------------------------------------------------------------------------------------------ */
 
-/* One channels-last convolution on the tcgen05 implicit-GEMM kernel (CausalConv3d / Conv2d of wan2pt1.py:42-60, 98-110):
+/* One channels-last convolution on the wgmma implicit-GEMM kernel (CausalConv3d / Conv2d of wan2pt1.py:42-60, 98-110):
  *   y[to,oh,ow,n] = bias[n] + sum W[n,(dt,dh,dw),c] * x[t_base + to*st + dt, oh*sh + dh - ph, ow*sw + dw - pw, c]
  * x [Tin,Hin,Win,Cin], w packed [Cout, taps, Cin_pad64], y [Tout,Hout,Wout,Cout] (split_time: [2*Tout,...,Cout/2]),
  * resid optional (same geometry as y). */
@@ -257,13 +257,12 @@ int ce_linear_bf16(const void* A, int lda, const void* W, int ldw, const void* b
 int ce_attention_bf16(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo, int B,
                       int H, int Lq, int Lk, float scale, int accumulate, void* stream);
 
-/* Profiling aid: subsequent ce_attention_bf16 calls record per-phase cycle counts of one softmax warp of block 0 into `buf`
- * (device, 16 x int64); NULL stops. */
+/* Profiling aid: subsequent ce_attention_bf16 calls record, for the first consumer thread of block 0, into `buf` (device,
+ * 16 x int64): [0] cycles in S = Q K^T, [1] in the softmax, [2] in P V, [3] key tiles walked; NULL stops. */
 int ce_debug_attention_timing(long long* buf);
 
-/* Test / A-B aid: select the kernel that serves long single-source (self-)attention from now on: 6 = two query tiles per CTA, two
- * softmax threads per score row (default), 2 = two query tiles per CTA, one thread per row, 5 = cta_group::2 cluster kernel
- * (experimental), 0 = single-tile kernel, -1 = back to the default / CE_ATTN_V2. */
+/* Kept for ABI stability only: earlier builds selected between several attention kernels here.  The sm_90a build has one, so
+ * this call selects nothing: it accepts 0 and -1 (both mean that kernel) and rejects every other version. */
 int ce_debug_attention_kernel(int version);
 
 /* Cross-attention with TWO key/value sources in one launch: out = bf16(SDPA(q,k,v)) + bf16(SDPA(q,k2,v2)) — the text and

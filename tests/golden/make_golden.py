@@ -133,8 +133,6 @@ def main():
         if inter["block0"].shape[1] <= 512:  # per-layer checkpoints only for the small cases (fixture size)
             tensors.update({
                 "block0_fp32": inter["block0"].contiguous(), "block0_bf16": inter16["block0"].contiguous(),
-                "patch_embed_fp32": inter["patch_embed"].contiguous(),
-                "context_fp32": inter["context"][:, :, :64].contiguous(),
             })
         save_file(tensors, os.path.join(OUT, f"dit_{name}.safetensors"))
         manifest["cases"][f"dit_{name}"] = {

@@ -41,10 +41,10 @@ def main():
         assert torch.equal(ref16, ora16), (name, float((ref16.float() - ora16.float()).abs().max()))
         d32 = float((ref32.float() - ora32.float()).abs().max())
         assert d32 <= 2e-2, (name, d32)   # fp32 modules, bf16 latents between steps: bf16-ulp flips can appear
-        save_file({"video_ref_bf16": ref16.contiguous(), "video_ref_fp32modules": ref32.float().contiguous()},
-                  os.path.join(OUT, f"pipeline_{name}.safetensors"))
+        stride = 2 if ref16.numel() * 2 > 900_000 else 1   # long videos: every second frame, so that no fixture exceeds 1 MB
+        save_file({"video_ref_bf16": ref16[:, ::stride].contiguous()}, os.path.join(OUT, f"pipeline_{name}.safetensors"))
         manifest["cases"][name] = {
-            "shape": list(ref16.shape), "oracle_vs_reference_bf16_equal": True, "oracle_vs_reference_fp32modules_maxabs": d32,
+            "shape": list(ref16.shape), "frame_stride": stride, "oracle_vs_reference_bf16_equal": True, "oracle_vs_reference_fp32modules_maxabs": d32,
             "bf16_vs_fp32modules_meanabs": float((ref16.float() - ref32.float()).abs().mean()),
             "video_meanabs": float(ref32.float().abs().mean()), "inputs_checksum": pipeline_cases.inputs_checksum(case),
         }

@@ -4,7 +4,7 @@ The CPU oracle cannot follow these sizes in seconds (one 14B forward = 222 TFLOP
 oracle's functional restatement (oracle/dit_oracle.py, oracle/vae_oracle.py -- plain torch ops on a state dict) is
 evaluated on CUDA tensors on the test box: in fp32 with TF32 disabled (the "exact" answer) and in the reference's bf16
 configuration (torch eager = cuBLAS / cuDNN / SDPA, i.e. the library path the unmodified reference itself executes on a
-GPU).  The oracle stays the checker; the thing under test goes through the Python mirror -> C ABI -> sm_100a kernels.
+GPU).  The oracle stays the checker; the thing under test goes through the Python mirror -> C ABI -> sm_90a kernels.
 
 Acceptance rule = tests/test_gpu_dit.py: the reference does not meet rtol=1e-3/atol=1e-4 against itself across precisions,
 so OUR bf16 output must be as close to the fp32 answer as the REFERENCE's bf16 output is (mean-abs <= 1.25x, max-abs <= 2x);
@@ -45,6 +45,14 @@ def _init_dit_weights_(model, seed):
             p.data.normal_(0, 0.02, generator=g)
 
 
+class _AsFloat32(dict):
+    """The same bf16-representable weights, computed exactly: each tensor is widened to fp32 when the oracle reads it, so the 14B
+    model is never held in fp32 as a whole (65.6 GB beside the 32.8 GB bf16 copy would not fit the H100's 80 GB)."""
+
+    def __getitem__(self, key):
+        return super().__getitem__(key).float()
+
+
 def _dit_inputs(frames, seed, dev):
     g = torch.Generator(device="cpu").manual_seed(seed)
     x = torch.randn(1, 36, frames, 90, 160, generator=g)
@@ -78,8 +86,7 @@ def _run_dit_case(layers, frames, seed, curve_file=None):
         ref16 = ref16.float()
         r16_layers = [inter16[f"block{i}"][0].float() for i in range(layers)]
         del inter16
-        sd32 = {k: v.float() for k, v in sd16.items()}   # the same bf16-representable weights, computed exactly
-        ref32, inter32 = O.dit_forward(sd32, cfg, x, t, text, img, return_intermediates=True)
+        ref32, inter32 = O.dit_forward(_AsFloat32(sd16), cfg, x, t, text, img, return_intermediates=True)
     curve = []
     for i in range(layers):
         r32 = inter32[f"block{i}"][0]

@@ -3,7 +3,7 @@
 In bf16 that band cannot be met by any implementation -- the reference misses it against itself across precisions (SURVEY.md
 section 7, hard part 3) -- so the bf16 path is held to "as close to the fp32 answer as the reference's own bf16 run"
 (tests/test_gpu_dit.py, tests/test_gpu_baseline_sizes.py).  Here the VALIDATION mode of the CUDA path (ce_dit_forward_fp32: fp32
-I/O and residual stream, every matrix product on the tcgen05 GEMM with split-bf16 operands, csrc/dit_fp32.cu) is compared with
+I/O and residual stream, every matrix product on the wgmma GEMM with split-bf16 operands, csrc/dit_fp32.cu) is compared with
 the golden outputs of the UNMODIFIED reference run in fp32 (tests/golden/dit_*.safetensors: `out_fp32`, `block0_fp32`), and every
 element must satisfy |ours - ref| <= 1e-4 + 1e-3 |ref| -- torch.allclose(rtol=1e-3, atol=1e-4), no forgiven fraction -- on all
 BASELINE configs[0] cases incl. the 64x64 latent (2048 tokens), the 8-frame RoPE branch, batch 2 and the ragged 3-head case."""

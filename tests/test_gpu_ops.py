@@ -1,4 +1,4 @@
-"""Operator-level parity of the sm_100a kernels, called through the C ABI (ctypes), against a plain PyTorch fp32
+"""Operator-level parity of the sm_90a kernels, called through the C ABI (ctypes), against a plain PyTorch fp32
 restatement of the same op on the same seeded inputs.  Tolerance: north_star's rtol=1e-3 / atol=1e-4 wherever the
 op can expose an fp32 result (GEMM accumulators); for bf16 outputs the check is "equal to the fp32 reference rounded
 to bf16, up to 1 bf16 ulp at rounding ties" expressed as rtol=2^-7 on |y|, plus a mean-error bound that a systematic
@@ -185,11 +185,10 @@ def _rows_sum_property():
 
 
 @gpu
-@pytest.mark.parametrize("version", [2, 5, 0])
+@pytest.mark.parametrize("version", [0])
 def test_attention_alternative_kernels(version):
-    """The non-default self-attention kernels (2: one softmax thread per score row, 5: cta_group::2 cluster kernel with two softmax groups feeding one accumulator,
-    0: single-tile kernel) against the same oracle comparisons and the full-size row-sum property -- the latter has thousands of
-    lazy-rescale events (scores scaled x2), which is what exercises the shared-running-max protocol of kernel 5."""
+    """The attention kernel selected by its explicit version number (the sm_90a build has one, version 0) against the same oracle
+    comparisons and the full-size row-sum property -- the latter has thousands of running-maximum updates (scores scaled x2)."""
     L = _lib()
     L.check(L.lib().ce_debug_attention_kernel(version))
     try:
@@ -270,11 +269,9 @@ def test_rmsnorm_rope(rows, H, rope):
 
 
 @gpu
-@pytest.mark.parametrize("Lq,Lk,Lk2,version", [(300, 512, 257, -1), (7200, 512, 257, -1), (130, 7, 300, -1), (300, 7, 300, -1), (513, 640, 129, -1),
-                                               (300, 512, 257, 2)])
+@pytest.mark.parametrize("Lq,Lk,Lk2,version", [(300, 512, 257, -1), (7200, 512, 257, -1), (130, 7, 300, -1), (300, 7, 300, -1), (513, 640, 129, -1)])
 def test_attention_dual_source(Lq, Lk, Lk2, version):
-    """text + image cross-attention in one launch == sum of two separate bf16 SDPAs (transformer_chronoedit.py:84-104): attention.cu's
-    two-group kernel whatever serves the self-attention."""
+    """text + image cross-attention in one launch == sum of two separate bf16 SDPAs (transformer_chronoedit.py:84-104)."""
     L = _lib()
     lib = L.lib()
     L.check(lib.ce_debug_attention_kernel(version))

@@ -1,6 +1,6 @@
 """Sequence-parallel DiT forward (tokens of one edit split over the GPUs of a node, q/k/v and attention output exchanged by peer
-stores inside the kernels, csrc/seqpar.cuh) against the single-GPU forward: bit-identical on every rank.  Needs >= 2 GPUs in the
-box (gpurun --gpus 2); skipped on a single-GPU box."""
+stores inside the kernels, csrc/seqpar.cuh) against the single-GPU forward: bit-identical on every rank.  Needs >= 2 GPUs;
+skipped on a single-GPU machine."""
 import os
 import subprocess
 import sys

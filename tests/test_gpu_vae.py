@@ -1,4 +1,4 @@
-"""Parity of the VAE path on the GPU: the tcgen05 implicit-GEMM convolution against torch's fp32 conv3d on the same
+"""Parity of the VAE path on the GPU: the wgmma implicit-GEMM convolution against torch's fp32 conv3d on the same
 bf16 inputs, and full encode / decode against the golden fixtures recorded from the UNMODIFIED reference VAE
 (chronoedit/_src/tokenizers/wan2pt1.py) — same acceptance rule as the DiT (tests/test_gpu_dit.py): our bf16 result must
 be as close to the reference's fp32 result as the reference's own bf16 run is."""

@@ -150,6 +150,23 @@ def test_wan_to_diffusers_module_map_matches_reference_converter():
         assert f'"{dif}.weight": "{wan}.weight"' in src, (wan, dif)
 
 
+def test_wan_to_diffusers_module_map_matches_stored_reference_map(golden_dir):
+    """The same check against the converter's weight-name pairs as recorded from the reference (tests/golden/LORA_KEY_MAP.json)."""
+    import json
+    import os
+
+    import chronoedit_b200 as ce
+    ref = json.load(open(os.path.join(golden_dir, "LORA_KEY_MAP.json")))["weight_names"]
+    for wan, dif in ce.ChronoEditTransformer3DModel._WAN_TO_DIFFUSERS:
+        if "k_img" in wan or "v_img" in wan:
+            continue
+        assert ref[f"blocks.0.{dif}.weight"] == f"blocks.0.{wan}.weight", (wan, dif)
+    assert ref["blocks.0.attn2.add_k_proj.weight"] == "blocks.0.cross_attn.k_img.weight"
+    assert ref["blocks.0.attn2.add_v_proj.weight"] == "blocks.0.cross_attn.v_img.weight"
+    for wan, dif in ce.ChronoEditTransformer3DModel._WAN_TO_DIFFUSERS_GLOBAL.items():
+        assert ref[f"{dif}.weight"] == f"{wan}.weight", (wan, dif)
+
+
 def test_new_weights_drop_the_context_cache():
     """The step-invariant context cache is keyed on the conditioning tensors only, so anything that changes the weights has to empty
     it: load_state_dict (also mid-session), fuse_lora (tested above through its effect on the weights), .to()."""

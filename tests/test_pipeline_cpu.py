@@ -13,6 +13,7 @@
     place, LoRA loading through `pipe.load_lora_weights / fuse_lora`) is the product code, and the video must equal the
     reference's.  The GPU twin of this test (tests/test_gpu_pipeline.py) runs the real kernels under the same loop.
 """
+import json
 import os
 
 import pytest
@@ -40,6 +41,9 @@ def test_pipeline_restatement_matches_stored_reference_output(name):
     case = PC.PIPELINE_CASES[name]
     gold = load_file(os.path.join(GOLDEN, f"pipeline_{name}.safetensors"))
     ora = PC.run_oracle_pipeline(case, torch.bfloat16).float()
+    man = json.load(open(os.path.join(GOLDEN, "PIPELINE_MANIFEST.json")))["cases"][name]
+    assert list(ora.shape) == man["shape"]
+    ora = ora[:, ::man["frame_stride"]]   # the fixture of a long video stores every second frame
     ref = gold["video_ref_bf16"].float()
     assert ora.shape == ref.shape
     # same torch build / CPU kernels -> identical; a different CPU (other bf16 GEMM paths) may flip isolated bf16 ulps
