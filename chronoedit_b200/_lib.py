@@ -50,6 +50,15 @@ class UniPCStepArgsC(ctypes.Structure):   # ce_unipc_step_args (field order = in
     ]
 
 
+class LinearArgsC(ctypes.Structure):   # ce_linear_args (field order = include/chronoedit_b200.h)
+    _fields_ = [
+        ("A", c_void_p), ("lda", c_int32), ("W", c_void_p), ("ldw", c_int32), ("M", c_int32), ("N", c_int32), ("K", c_int32),
+        ("out", c_void_p), ("ldo", c_int32), ("out_f32", c_void_p), ("ld_f32", c_int32), ("bias", c_void_p), ("bias_row", c_void_p),
+        ("epilogue", c_int32), ("resid", c_void_p), ("ldr", c_int32), ("gate", c_void_p), ("gate_stride", c_int32),
+        ("rows_per_batch", c_int32), ("stats_out", c_void_p), ("stats_ld", c_int32), ("stats_mode", c_int32), ("group_m", c_int32),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/chronoedit_b200.h declares
 SIGNATURES = {
     "ce_abi_version": (c_int, []),
@@ -116,6 +125,11 @@ SIGNATURES = {
     "ce_rmsnorm_rope_bf16": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_int,
                                      c_int, c_void_p]),
     "ce_rope_table_host": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
+    "ce_linear_ex_bf16": (c_int, [POINTER(LinearArgsC), c_void_p]),
+    "ce_layernorm_stats_bf16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int,
+                                        c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "ce_rmsnorm_rope_stats_bf16": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                           c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
 }
 
 _lib = None

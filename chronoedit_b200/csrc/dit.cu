@@ -791,6 +791,26 @@ int ce_linear_bf16(const void* A, int lda, const void* W, int ldw, const void* b
   return launch_gemm_bf16(reinterpret_cast<const bf16*>(A), lda, reinterpret_cast<const bf16*>(W), ldw, g, reinterpret_cast<cudaStream_t>(stream));
 }
 
+// Test aid: one GEMM with every GemmArgs field, including the epilogue row statistics and the tile rasterisation.
+int ce_linear_ex_bf16(const ce_linear_args* a, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(a != nullptr, "ce_linear_ex_bf16: null args");
+  GemmArgs g;
+  g.M = a->M; g.N = a->N; g.K = a->K;
+  g.out = reinterpret_cast<bf16*>(a->out); g.ldo = a->ldo;
+  g.out_f32 = a->out_f32; g.ld_f32 = a->ld_f32;
+  g.bias = reinterpret_cast<const bf16*>(a->bias);
+  g.bias_row = reinterpret_cast<const bf16*>(a->bias_row);
+  g.epi = a->epilogue;
+  g.resid = reinterpret_cast<const bf16*>(a->resid); g.ldr = a->ldr;
+  g.gate = a->gate; g.gate_stride = a->gate_stride; g.rows_per_batch = a->rows_per_batch > 0 ? a->rows_per_batch : 1;
+  g.stats_out = reinterpret_cast<float2*>(a->stats_out); g.stats_ld = a->stats_ld; g.stats_mode = a->stats_mode;
+  g.group_m = a->group_m;
+  return launch_gemm_bf16(reinterpret_cast<const bf16*>(a->A), a->lda, reinterpret_cast<const bf16*>(a->W), a->ldw, g,
+                          reinterpret_cast<cudaStream_t>(stream));
+}
+
 static long long* g_attn_timing = nullptr;
 // Profiling aid: subsequent ce_attention_bf16 calls record the phase cycles of the first consumer thread of block 0 into `buf`
 // ([16] int64 on the device); pass NULL to stop.
@@ -851,6 +871,27 @@ int ce_rmsnorm_rope_bf16(void* x, int ldx, int rows, int D, float eps, const voi
   if (rc) return rc;
   return launch_rmsnorm_rope(reinterpret_cast<bf16*>(x), ldx, rows, D, eps, reinterpret_cast<const bf16*>(weight), rope_cos, rope_sin, L,
                              head_dim, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// Test aids: the two row kernels that take their statistics from GEMM epilogue partials (GemmArgs::stats_out).
+int ce_layernorm_stats_bf16(const void* x, int ldx, void* y, int ldy, int rows, int D, float eps, const float* scale, const float* shift,
+                            int mod_stride, int rows_per_batch, const float* weight, const float* bias, int scale_is_1p, const float* stats,
+                            int stats_ld, int tiles, int tile_n, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  return launch_layernorm_stats(reinterpret_cast<const bf16*>(x), ldx, reinterpret_cast<bf16*>(y), ldy, rows, D, eps, scale, shift, mod_stride,
+                                rows_per_batch, weight, bias, scale_is_1p, reinterpret_cast<const float2*>(stats), stats_ld, tiles, tile_n,
+                                reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_rmsnorm_rope_stats_bf16(void* x, int ldx, int rows, int D, float eps, const void* weight0, const void* weight1, int nmat,
+                               const float* rope_cos, const float* rope_sin, int L, int head_dim, const float* stats, int stats_ld, int tiles,
+                               void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  return launch_rmsnorm_rope_stats(reinterpret_cast<bf16*>(x), ldx, rows, D, eps, reinterpret_cast<const bf16*>(weight0),
+                                   reinterpret_cast<const bf16*>(weight1), nmat, rope_cos, rope_sin, L, head_dim,
+                                   reinterpret_cast<const float2*>(stats), stats_ld, tiles, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ce_rope_table_host(int head_dim, int frames, int height_patches, int width_patches, int max_seq_len, int temporal_skip_len, float theta,

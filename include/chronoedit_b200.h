@@ -286,6 +286,50 @@ int ce_rope_table_host(int head_dim, int frames, int height_patches, int width_p
                        int temporal_skip_len, float theta, float* cos_out_host, float* sin_out_host);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Test aids: the DiT's fused-statistics path, one operator at a time.  When D % 256 == 0 the GEMM that writes a
+ * row also writes per-(row, N tile) statistics of the values it stored, and the LayerNorm / RMSNorm that follows
+ * merges those partials instead of reducing over the row.  Not needed to run the model.
+ * ------------------------------------------------------------------------------------------------------------ */
+typedef struct ce_linear_args {
+  const void* A;           /* [M, lda] bf16 */
+  int32_t lda;
+  const void* W;           /* [N, ldw] bf16 (nn.Linear weight) */
+  int32_t ldw;
+  int32_t M, N, K;         /* N % 8 == 0 */
+  void* out;               /* [M, ldo] bf16 (may be NULL when out_f32 is given and stats_mode == 0) */
+  int32_t ldo;
+  float* out_f32;          /* optional [M, ld_f32]: acc + bias in fp32 before any rounding */
+  int32_t ld_f32;          /* 0 = N */
+  const void* bias;        /* [N] bf16 or NULL */
+  const void* bias_row;    /* [M] bf16 or NULL: added per output row */
+  int32_t epilogue;        /* as ce_linear_bf16 */
+  const void* resid;       /* [M, ldr] bf16, epilogues 3 and 4 */
+  int32_t ldr;
+  const float* gate;       /* [batches, gate_stride] fp32, epilogue 3; batch = row / rows_per_batch */
+  int32_t gate_stride;
+  int32_t rows_per_batch;
+  float* stats_out;        /* optional [M, stats_ld] pairs of floats, one per (row, N tile) of the stored bf16 output: */
+  int32_t stats_ld;        /*   stats_mode 1: (mean, M2 = sum (y - mean)^2) over the tile's columns  */
+  int32_t stats_mode;      /*   stats_mode 2: (sum y^2, 0);  tile width 256 if N >= 256, else 128 if N >= 128, else 64 */
+  int32_t group_m;         /* M tiles per rasterisation group; 0 = default.  Results do not depend on it. */
+} ce_linear_args;
+
+/* out = epilogue(A x W^T + bias) with every option of the DiT's GEMM, including the row statistics. */
+int ce_linear_ex_bf16(const ce_linear_args* args, void* stream);
+
+/* FP32LayerNorm (+ modulate or affine) like ce_layernorm_bf16, with the row statistics merged from `tiles` stats_mode-1
+ * partials of width tile_n covering [0, D) (stats [rows, stats_ld] float pairs).  scale_is_1p: `scale` holds 1 + scale. */
+int ce_layernorm_stats_bf16(const void* x, int ldx, void* y, int ldy, int rows, int D, float eps, const float* scale,
+                            const float* shift, int mod_stride, int rows_per_batch, const float* weight, const float* bias,
+                            int scale_is_1p, const float* stats, int stats_ld, int tiles, int tile_n, void* stream);
+
+/* RMSNorm across heads (+ optional RoPE) like ce_rmsnorm_rope_bf16, in place on nmat (1 or 2) matrices of width D side by
+ * side in x (q | k): matrix m starts at column m * D, uses weight m and the stats_mode-2 partials [m * tiles, (m+1) * tiles). */
+int ce_rmsnorm_rope_stats_bf16(void* x, int ldx, int rows, int D, float eps, const void* weight0, const void* weight1, int nmat,
+                               const float* rope_cos, const float* rope_sin, int L, int head_dim, const float* stats,
+                               int stats_ld, int tiles, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Sampling glue either side of the DiT call (SURVEY.md section 8(f) row 1): one launch per denoising step for
  *   noise = uncond + g*(cond - uncond)                                   chronoedit_diffusers/pipeline_chronoedit.py:736
  *   FlowUniPCMultistepScheduler.step: x0 conversion, UniC corrector, UniP predictor (solver_order 2, bh2, predict_x0,

@@ -49,6 +49,16 @@ def test_no_cpu_fallback():
     a = torch.zeros(8, 8, dtype=torch.bfloat16)
     rc = lib.ce_linear_bf16(L.ptr(a), 8, L.ptr(a), 8, None, L.ptr(a), 8, None, 8, 8, 8, 0, None, 0, None, 0, 1, None)
     assert rc != 0
+    # the fused-statistics operators: the device check comes first, whatever the arguments
+    st = torch.zeros(8, 2)
+    la = L.LinearArgsC(A=a.data_ptr(), lda=8, W=a.data_ptr(), ldw=8, M=8, N=8, K=8, out=a.data_ptr(), ldo=8, stats_out=st.data_ptr(),
+                       stats_ld=1, stats_mode=1)
+    assert lib.ce_linear_ex_bf16(ctypes.byref(la), None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    assert lib.ce_linear_ex_bf16(None, None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    assert lib.ce_layernorm_stats_bf16(L.ptr(a), 8, L.ptr(a), 8, 8, 8, 1e-6, None, None, 0, 0, None, None, 0, L.ptr(st), 1, 1, 8,
+                                       None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    assert lib.ce_rmsnorm_rope_stats_bf16(L.ptr(a), 8, 8, 8, 1e-6, L.ptr(a), None, 1, None, None, 0, 8, L.ptr(st), 1, 1,
+                                          None) == -3 and b"no CPU fallback" in lib.ce_last_error()
     # the sampler entry point: argument validation first, then the device check -- never a CPU evaluation
     args = L.UniPCStepArgsC()
     x = torch.zeros(64)

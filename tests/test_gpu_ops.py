@@ -1,5 +1,5 @@
 """Operator-level parity of the sm_90a kernels, called through the C ABI (ctypes), against a plain PyTorch fp32
-restatement of the same op on the same seeded inputs.  Tolerance: north_star's rtol=1e-3 / atol=1e-4 wherever the
+restatement of the same op on the same seeded inputs (fp64 for LayerNorm).  Tolerance: north_star's rtol=1e-3 / atol=1e-4 wherever the
 op can expose an fp32 result (GEMM accumulators); for bf16 outputs the check is "equal to the fp32 reference rounded
 to bf16, up to 1 bf16 ulp at rounding ties" expressed as rtol=2^-7 on |y|, plus a mean-error bound that a systematic
 error would break.
@@ -29,6 +29,40 @@ def _bf16_close(got: torch.Tensor, ref_f32: torch.Tensor, what: str, ulp: float 
     rel_mean = (err.mean() / ref.abs().mean().clamp_min(1e-12)).item()
     assert bad < 1e-3, f"{what}: {bad * 100:.3f}% of elements beyond {ulp} bf16 ulp (max err {err.max().item():.4g})"
     assert rel_mean < mean_tol, f"{what}: mean relative error {rel_mean:.3g}"
+
+
+ROW_KINDS = ("iid", "block_offset", "outlier", "constant", "tile_constant")
+
+
+def structured_rows(kind: str, rows: int, D: int, g: torch.Generator, block: int = 256) -> torch.Tensor:
+    """fp32 [rows, D] row data on g's device, shaped so that row statistics merged from per-block partials go visibly wrong:
+      iid            N(0.5, 3^2)
+      block_offset   N(0, 1) plus an offset ~ N(0, 2^2) per (row, block of `block` columns): the block means differ
+      outlier        N(0, 1) with +-60 on the first column of a block (the pivot of a GEMM statistics tile) and -40 elsewhere
+      constant       one value per row (LayerNorm must give exactly its shift)
+      tile_constant  one value per (row, block): all of the variance is between blocks
+    """
+    dev = g.device
+    nb = (D + block - 1) // block
+
+    def per_block(v):
+        return v.repeat_interleave(block, dim=1)[:, :D]
+
+    if kind == "iid":
+        return torch.randn(rows, D, generator=g, device=dev) * 3 + 0.5
+    if kind == "block_offset":
+        return torch.randn(rows, D, generator=g, device=dev) + per_block(torch.randn(rows, nb, generator=g, device=dev) * 2)
+    if kind == "outlier":
+        x = torch.randn(rows, D, generator=g, device=dev)
+        k = nb // 2
+        x[:, k * block] += 60 * torch.sign(torch.randn(rows, generator=g, device=dev))
+        x[:, min(D - 1, k * block + block // 2 + 13)] -= 40
+        return x
+    if kind == "constant":
+        return (torch.randn(rows, 1, generator=g, device=dev) * 3 + 0.5).expand(rows, D).contiguous()
+    if kind == "tile_constant":
+        return per_block(torch.randn(rows, nb, generator=g, device=dev) * 2 + 0.5)
+    raise ValueError(kind)
 
 
 def run_linear(M, N, K, epi, seed=0, rows_per_batch=None):
@@ -199,14 +233,30 @@ def test_attention_alternative_kernels(version):
         L.check(L.lib().ce_debug_attention_kernel(-1))
 
 
+def layer_norm_f64(x: torch.Tensor, eps: float) -> torch.Tensor:
+    """fp64 LayerNorm over the last dim of the stored x.  The mean is sum / D, which is exact for a constant row, so there
+    x - mean is exactly 0 (torch's fp32 layer_norm is off by an ulp of the mean there, which rstd = 1/sqrt(eps) magnifies)."""
+    xd = x.double()
+    d = xd - xd.sum(-1, keepdim=True) / x.shape[-1]
+    return d / torch.sqrt((d * d).mean(-1, keepdim=True) + eps)
+
+
+def _with_kinds(iid_cases, structured_cases):
+    """iid cases keep their plain ids; every structured case runs on each non-iid kind of structured_rows."""
+    return ([pytest.param(*c, "iid", id="-".join(map(str, c))) for c in iid_cases] +
+            [pytest.param(*c, k, id="-".join(map(str, c + (k,)))) for k in ROW_KINDS[1:] for c in structured_cases])
+
+
 @gpu
-@pytest.mark.parametrize("rows,D,mode", [(300, 256, "mod"), (77, 5120, "mod"), (64, 1280, "affine"), (33, 384, "plain"),
-                                         (4739, 5120, "mod"), (4736, 3072, "affine"), (5003, 5120, "plain")])   # large row counts with ragged tails
-def test_layernorm(rows, D, mode):
+@pytest.mark.parametrize("rows,D,mode,kind", _with_kinds(
+    [(300, 256, "mod"), (77, 5120, "mod"), (64, 1280, "affine"), (33, 384, "plain"),
+     (4739, 5120, "mod"), (4736, 3072, "affine"), (5003, 5120, "plain")],   # large row counts with ragged tails
+    [(300, 384, "plain"), (64, 1280, "affine"), (4739, 5120, "mod")]))
+def test_layernorm(rows, D, mode, kind):
     L = _lib()
     lib = L.lib()
     g = torch.Generator(device="cpu").manual_seed(rows)
-    x = (torch.randn(rows, D, generator=g) * 3 + 0.5).bfloat16().cuda()
+    x = structured_rows(kind, rows, D, g).bfloat16().cuda()
     rpb = 100
     nb = (rows + rpb - 1) // rpb
     mod = torch.randn(nb, 6, D, generator=g).float().cuda()
@@ -217,21 +267,25 @@ def test_layernorm(rows, D, mode):
     if mode == "mod":
         scale, shift = mod[:, 1], mod[:, 0]
         L.check(lib.ce_layernorm_bf16(L.ptr(x), D, L.ptr(y), D, rows, D, eps, L.ptr(scale), L.ptr(shift), 6 * D, rpb, None, None, L.current_stream()))
-        ln = torch.nn.functional.layer_norm(x.float(), (D,), None, None, eps)
-        ref = ln * (1 + scale.repeat_interleave(rpb, 0)[:rows]) + shift.repeat_interleave(rpb, 0)[:rows]
+        ln = layer_norm_f64(x, eps)
+        ref = ln * (1 + scale.double().repeat_interleave(rpb, 0)[:rows]) + shift.double().repeat_interleave(rpb, 0)[:rows]
     elif mode == "affine":
         L.check(lib.ce_layernorm_bf16(L.ptr(x), D, L.ptr(y), D, rows, D, eps, None, None, 0, 0, L.ptr(w), L.ptr(b), L.current_stream()))
-        ref = torch.nn.functional.layer_norm(x.float(), (D,), w, b, eps)
+        ref = layer_norm_f64(x, eps) * w.double() + b.double()
     else:
         L.check(lib.ce_layernorm_bf16(L.ptr(x), D, L.ptr(y), D, rows, D, eps, None, None, 0, 0, None, None, L.current_stream()))
-        ref = torch.nn.functional.layer_norm(x.float(), (D,), None, None, eps)
+        ref = layer_norm_f64(x, eps)
     torch.cuda.synchronize()
-    _bf16_close(y, ref, f"layernorm {mode} rows={rows} D={D}")
+    _bf16_close(y, ref, f"layernorm {mode} {kind} rows={rows} D={D}")
+    if kind == "constant":   # x - mean is exactly 0: the output is exactly the shift / bias (or 0)
+        assert torch.equal(y.float().cpu(), ref.bfloat16().float().cpu()), f"layernorm {mode} of constant rows is not exact"
 
 
 @gpu
-@pytest.mark.parametrize("rows,H,rope", [(234, 3, True), (126, 2, False), (600, 40, True), (4746, 40, True), (4740, 24, False)])   # last two: large, ragged
-def test_rmsnorm_rope(rows, H, rope):
+@pytest.mark.parametrize("rows,H,rope,kind", _with_kinds(
+    [(234, 3, True), (126, 2, False), (600, 40, True), (4746, 40, True), (4740, 24, False)],   # last two: large, ragged
+    [(600, 40, True), (126, 2, False)]))
+def test_rmsnorm_rope(rows, H, rope, kind):
     from oracle import dit_oracle as O
 
     L = _lib()
@@ -240,7 +294,10 @@ def test_rmsnorm_rope(rows, H, rope):
     D = H * hd
     g = torch.Generator(device="cpu").manual_seed(rows)
     ld = 3 * D
-    buf = torch.randn(rows, ld, generator=g).bfloat16().cuda()
+    buf = torch.randn(rows, ld, generator=g)
+    if kind != "iid":
+        buf[:, D:2 * D] = structured_rows(kind, rows, D, g)
+    buf = buf.bfloat16().cuda()
     w = (1 + 0.1 * torch.randn(D, generator=g)).bfloat16().cuda()
     before = buf.clone()
     cfg = O.DiTConfig.tiny(heads=H)
@@ -265,7 +322,7 @@ def test_rmsnorm_rope(rows, H, rope):
         yh = y.unflatten(2, (H, hd)).transpose(1, 2)
         yh = O._apply_rope(yh, O.rope_table(cfg, frames, hp * 2, wp * 2))
         y = yh.transpose(1, 2).flatten(2, 3)
-    _bf16_close(buf[:, D:2 * D], y[0].float(), f"rmsnorm_rope rows={rows} H={H} rope={rope}")
+    _bf16_close(buf[:, D:2 * D], y[0].float(), f"rmsnorm_rope {kind} rows={rows} H={H} rope={rope}")
 
 
 @gpu
