@@ -7,20 +7,20 @@
 // padding of Cin up to 64.  Stride-2 convolutions use the tensor map's element strides.  The temporal halo is real data:
 // the caller keeps the causal history frames in front of the chunk (wan2pt1.py:49-60, CACHE_T = 2).
 // Weights are pre-packed [Cout, taps, Cin_pad] so the B tile is a plain 2-D box.  Pipeline and warpgroup roles are those of
-// gemm.cu (one TMA producer warpgroup, two wgmma consumer warpgroups of 64 rows each); the epilogue adds bias, optional
-// residual, the upsample3d frame interleave and an optional planar (NCTHW) clamped store for the decoder head.
+// the GEMM (ring_gemm.cuh: one TMA producer warpgroup, two wgmma consumer warpgroups of 64 rows each); the epilogue adds bias,
+// optional residual, the upsample3d frame interleave and an optional planar (NCTHW) clamped store for the decoder head.
 //
 // Replaces cuDNN's conv3d/conv2d behind CausalConv3d / nn.Conv2d of the reference's chronoedit/_src/tokenizers/wan2pt1.py
 // (:42-60, :98-110, :186-220) plus F.pad / torch.cat cache handling and the residual add (:220).
 #include "conv.cuh"
-#include "wgmma.cuh"
+#include "ring_gemm.cuh"
 
 namespace ce {
 
 namespace {
 
-constexpr int TILE_H = 8, TILE_W = 16, BM = 128, BK = 64;
-constexpr int CONV_THREADS = 384;
+constexpr int TILE_H = 8, TILE_W = 16;
+static_assert(TILE_H * TILE_W == BM, "a tile of output pixels is one BM-row GEMM tile");
 
 struct ConvGeom {
   int tiles_w, tiles_h, tiles_n, num_tiles;
@@ -37,38 +37,10 @@ __device__ __forceinline__ void conv_tile_coords(int t, const ConvGeom& g, int& 
 }
 
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(CONV_THREADS, 1)
+__global__ void __launch_bounds__(RING_THREADS, 1)
 conv3d_cl_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_constant__ CUtensorMap tma_w, ConvArgs a, ConvGeom g) {
-  constexpr uint32_t A_BYTES = BM * BK * 2;
-  constexpr uint32_t B_BYTES = BN * BK * 2;
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));
-  uint64_t* empty = full + STAGES;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 2);  // one arrive per consumer warpgroup
-    }
-    fence_mbar_init();
-    tma_prefetch_desc(&tma_x);
-    tma_prefetch_desc(&tma_w);
-  }
-  __syncthreads();
-
-  if (warp < 4) {
-    setmaxnreg_dec<40>();
-    if (warp == 0 && elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = blockIdx.x; t < g.num_tiles; t += gridDim.x) {
+  Ring<BN, STAGES> ring;
+  if (!ring.start(&tma_x, &tma_w, g.num_tiles, [&](int t) {
         int to, th, tw, nb;
         conv_tile_coords(t, g, to, th, tw, nb);
         const int w_in0 = tw * TILE_W * a.sw - a.pw;
@@ -79,32 +51,20 @@ conv3d_cl_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_constan
           for (int dh = 0; dh < a.kh; ++dh)
             for (int dw = 0; dw < a.kw; ++dw, ++tap)
               for (int cb = 0; cb < g.cblocks; ++cb) {
-                mbar_wait(&empty[stage], phase ^ 1);
-                mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
-                tma_load_4d(sA + stage * A_BYTES, &tma_x, &full[stage], cb * BK, w_in0 + dw, h_in0 + dh, t_in0 + dt);
-                tma_load_2d(sB + stage * B_BYTES, &tma_w, &full[stage], tap * a.Cin_pad + cb * BK, nb * BN);
-                if (++stage == STAGES) {
-                  stage = 0;
-                  phase ^= 1;
-                }
+                const auto s = ring.acquire();
+                tma_load_4d(s.a, &tma_x, s.bar, cb * BK, w_in0 + dw, h_in0 + dh, t_in0 + dt);
+                tma_load_2d(s.b, &tma_w, s.bar, tap * a.Cin_pad + cb * BK, nb * BN);
               }
-      }
-    }
+      }))
     return;
-  }
-
-  setmaxnreg_inc<232>();
-  const int wg = (warp >> 2) - 1;
-  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // the thread's rows of the tile: r0 and r0 + 8
-  const int c_in_group = 2 * (lane & 3);
+  const int r0 = ring_row();   // the thread's rows of the tile: r0 and r0 + 8
+  const int c_in_group = ring_col();
   const int c_half = a.split_time ? a.Cout / 2 : a.Cout;  // channels per stored voxel
-  int stage = 0;
-  uint32_t phase = 0;
   float acc[BN / 2];
-  for (int t = blockIdx.x; t < g.num_tiles; t += gridDim.x) {
+  for (int t : RingTiles{g.num_tiles}) {
     int to, th, tw, nb;
     conv_tile_coords(t, g, to, th, tw, nb);
-    wgmma_ring_tile<BN, STAGES>(acc, smem_u32(sA) + wg * 64 * 128, smem_u32(sB), A_BYTES, B_BYTES, full, empty, g.kblocks, stage, phase);
+    ring.mma_tile(acc, g.kblocks);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = r0 + 8 * h;
@@ -161,18 +121,6 @@ conv3d_cl_kernel(const __grid_constant__ CUtensorMap tma_x, const __grid_constan
   }
 }
 
-template <int BN, int STAGES>
-int launch_conv_variant(const CUtensorMap& tx, const CUtensorMap& tw, const ConvArgs& a, ConvGeom g, cudaStream_t stream) {
-  constexpr size_t smem = (size_t)STAGES * (BM * BK * 2 + BN * BK * 2) + 1024 + 256;
-  CE_ENSURE_SMEM((conv3d_cl_kernel<BN, STAGES>), smem);
-  g.tiles_n = (a.Cout + BN - 1) / BN;
-  g.num_tiles = a.Tout * g.tiles_h * g.tiles_w * g.tiles_n;
-  const int grid = g.num_tiles < device_sm_count() ? g.num_tiles : device_sm_count();
-  conv3d_cl_kernel<BN, STAGES><<<grid, CONV_THREADS, smem, stream>>>(tx, tw, a, g);
-  CE_CHECK_CUDA(cudaGetLastError());
-  return CE_OK;
-}
-
 }  // namespace
 
 int launch_conv3d_cl(const ConvArgs& a, cudaStream_t stream) {
@@ -188,8 +136,6 @@ int launch_conv3d_cl(const ConvArgs& a, cudaStream_t stream) {
   g.taps = a.kt * a.kh * a.kw;
   g.cblocks = a.Cin_pad / 64;
   g.kblocks = g.taps * g.cblocks;
-  g.tiles_n = 0;
-  g.num_tiles = 0;
   CUtensorMap tx, tw;
   {
     uint64_t dims[4] = {(uint64_t)a.Cin, (uint64_t)a.Win, (uint64_t)a.Hin, (uint64_t)a.Tin};
@@ -207,9 +153,11 @@ int launch_conv3d_cl(const ConvArgs& a, cudaStream_t stream) {
     int rc = make_tmap_bf16(&tw, a.w, 2, dims, strides, box);
     if (rc) return rc;
   }
-  if (bn == 32) return launch_conv_variant<32, 8>(tx, tw, a, g, stream);
-  if (bn == 96) return launch_conv_variant<96, 6>(tx, tw, a, g, stream);
-  return launch_conv_variant<192, 5>(tx, tw, a, g, stream);
+  g.tiles_n = (a.Cout + bn - 1) / bn;
+  g.num_tiles = a.Tout * g.tiles_h * g.tiles_w * g.tiles_n;
+  if (bn == 32) return launch_ring_gemm<32, 8>(conv3d_cl_kernel<32, 8>, g.num_tiles, stream, tx, tw, a, g);
+  if (bn == 96) return launch_ring_gemm<96, 6>(conv3d_cl_kernel<96, 6>, g.num_tiles, stream, tx, tw, a, g);
+  return launch_ring_gemm<192, 5>(conv3d_cl_kernel<192, 5>, g.num_tiles, stream, tx, tw, a, g);
 }
 
 }  // namespace ce

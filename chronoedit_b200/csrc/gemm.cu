@@ -1,12 +1,8 @@
-// bf16 GEMM for sm_90a: TMA -> shared-memory ring -> wgmma (accumulators in registers) -> fused epilogue.
+// bf16 GEMM for sm_90a on the TMA -> shared-memory ring -> wgmma pipeline of ring_gemm.cuh, with a fused epilogue.
 //
 //   out[M,N] = epilogue( A[M,K] * W[N,K]^T )        A: activations (row-major), W: nn.Linear weight (row-major)
 //
-// Persistent, warp-specialised, one CTA per SM, 384 threads = 3 warpgroups (registers re-partitioned with setmaxnreg):
-//   warpgroup 0     TMA producer (one lane of warp 0): A tile 128x64, W tile BNx64 per k-block, 128B swizzle, STAGES-deep ring
-//   warpgroups 1,2  consumers: 64 rows x BN columns of the tile each, 4 x wgmma (M64, N=BN, K16) per k-block with both operands
-//                   read from the ring, then bias / activation / gate / residual from the accumulator registers -> global
-// While the consumers run the epilogue of tile i the producer already fills the ring for tile i+1.
+// Per k-block an A tile 128x64 and a W tile BNx64; the epilogue applies bias / activation / gate / residual / row statistics.
 // Tile order is grouped along M so that concurrently resident tiles share W column panels through L2.
 //
 // Replaces the cuBLASLt calls behind every nn.Linear of the reference DiT block
@@ -17,15 +13,11 @@
 #include <cstdlib>
 
 #include "gemm.cuh"
-#include "wgmma.cuh"
+#include "ring_gemm.cuh"
 
 namespace ce {
 
 namespace {
-
-constexpr int BM = 128;
-constexpr int BK = 64;
-constexpr int GEMM_THREADS = 384;
 
 __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int group_m, int& mb, int& nb) {
   const int per_group = group_m * tiles_n;
@@ -46,72 +38,33 @@ __device__ __forceinline__ float gelu_tanh_f(float x) {
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.7071067811865476f)); }
 
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __launch_bounds__(RING_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g) {
-  constexpr uint32_t A_BYTES = BM * BK * 2;
-  constexpr uint32_t B_BYTES = BN * BK * 2;
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));
-  uint64_t* empty = full + STAGES;
-
-  const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int tiles_m = (g.M + BM - 1) / BM;
   const int tiles_n = (g.N + BN - 1) / BN;
   const int num_tiles = tiles_m * tiles_n;
   const int kblocks = (g.K + BK - 1) / BK;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 2);  // one arrive per consumer warpgroup
-    }
-    fence_mbar_init();
-    tma_prefetch_desc(&tma_a);
-    tma_prefetch_desc(&tma_b);
-  }
-  __syncthreads();
-
-  if (warp < 4) {
-    // ------------------------------------------------------------------ TMA producer
-    setmaxnreg_dec<40>();
-    if (warp == 0 && elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+  Ring<BN, STAGES> ring;
+  if (!ring.start(&tma_a, &tma_b, num_tiles, [&](int t) {   // TMA producer
         int mb, nb;
         tile_coords(t, tiles_m, tiles_n, g.group_m, mb, nb);
         for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full[stage], A_BYTES + B_BYTES);
-          tma_load_2d(sA + stage * A_BYTES, &tma_a, &full[stage], kb * BK, mb * BM);
-          tma_load_2d(sB + stage * B_BYTES, &tma_b, &full[stage], kb * BK, nb * BN);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
+          const auto s = ring.acquire();
+          tma_load_2d(s.a, &tma_a, s.bar, kb * BK, mb * BM);
+          tma_load_2d(s.b, &tma_b, s.bar, kb * BK, nb * BN);
         }
-      }
-    }
+      }))
     return;
-  }
-
   // -------------------------------------------------------------------- consumers: main loop + epilogue
-  setmaxnreg_inc<232>();
-  const int wg = (warp >> 2) - 1;                           // rows [64 wg, 64 wg + 64) of the tile
-  const int r_in_tile = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int c_in_group = 2 * (lane & 3);
-  int stage = 0;
-  uint32_t phase = 0;
+  const int r_in_tile = ring_row();   // rows r_in_tile and r_in_tile + 8 of the tile
+  const int c_in_group = ring_col();
   float acc[BN / 2];
-  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+  for (int t : RingTiles{num_tiles}) {
     int mb, nb;
     tile_coords(t, tiles_m, tiles_n, g.group_m, mb, nb);
-    wgmma_ring_tile<BN, STAGES>(acc, smem_u32(sA) + wg * 64 * 128, smem_u32(sB), A_BYTES, B_BYTES, full, empty, kblocks, stage, phase);
+    ring.mma_tile(acc, kblocks);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {   // the thread's two rows
       const int row = mb * BM + r_in_tile + 8 * h;
@@ -194,17 +147,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
   }
 }
 
-template <int BN, int STAGES>
-int launch_variant(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& g, cudaStream_t stream) {
-  constexpr size_t smem = (size_t)STAGES * (BM * BK * 2 + BN * BK * 2) + 1024 /*align slack*/ + 256 /*barriers*/;
-  CE_ENSURE_SMEM((gemm_bf16_kernel<BN, STAGES>), smem);
-  const int tiles = ((g.M + BM - 1) / BM) * ((g.N + BN - 1) / BN);
-  const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
-  gemm_bf16_kernel<BN, STAGES><<<grid, GEMM_THREADS, smem, stream>>>(ta, tb, g);
-  CE_CHECK_CUDA(cudaGetLastError());
-  return CE_OK;
-}
-
 }  // namespace
 
 int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmArgs& g, cudaStream_t stream) {
@@ -238,9 +180,10 @@ int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmA
   if (rc) return rc;
   rc = make_tmap_2d(&tb, W, (uint64_t)a.N, (uint64_t)a.K, (uint64_t)ldw, (uint32_t)bn);
   if (rc) return rc;
-  if (bn == 256) return launch_variant<256, 4>(ta, tb, a, stream);
-  if (bn == 128) return launch_variant<128, 6>(ta, tb, a, stream);
-  return launch_variant<64, 8>(ta, tb, a, stream);
+  const int tiles = ((a.M + BM - 1) / BM) * ((a.N + bn - 1) / bn);
+  if (bn == 256) return launch_ring_gemm<256, 4>(gemm_bf16_kernel<256, 4>, tiles, stream, ta, tb, a);
+  if (bn == 128) return launch_ring_gemm<128, 6>(gemm_bf16_kernel<128, 6>, tiles, stream, ta, tb, a);
+  return launch_ring_gemm<64, 8>(gemm_bf16_kernel<64, 8>, tiles, stream, ta, tb, a);
 }
 
 }  // namespace ce

@@ -163,34 +163,4 @@ __device__ __forceinline__ void wgmma_rs<128, 1>(float (&d)[64], const uint32_t 
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
 }
 
-// Main loop of one consumer warpgroup over a TMA-fed ring of k-blocks: acc[64 x BN] = sum over `kblocks` of A[64 x 64] * B[BN x 64]^T.
-// a_smem / b_smem are the shared-memory addresses of this warpgroup's 64 A rows and of the B tile inside stage 0.  One wgmma group
-// stays in flight: stage s is handed back to the producer (one arrive per warpgroup on empty[s]) when the group after it has been
-// issued, so the tensor cores never wait for the hand-back.  `stage` / `phase` carry the ring position from tile to tile.
-template <int BN, int STAGES>
-__device__ __forceinline__ void wgmma_ring_tile(float (&acc)[BN / 2], uint32_t a_smem, uint32_t b_smem, uint32_t a_stage_bytes,
-                                                uint32_t b_stage_bytes, uint64_t* full, uint64_t* empty, int kblocks, int& stage,
-                                                uint32_t& phase) {
-  const bool signaller = (threadIdx.x & 127) == 0;
-  int prev = -1;
-  for (int kb = 0; kb < kblocks; ++kb) {
-    mbar_wait(&full[stage], phase);
-    const uint64_t da = wgmma_desc_kmajor_sw128(a_smem + stage * a_stage_bytes);
-    const uint64_t db = wgmma_desc_kmajor_sw128(b_smem + stage * b_stage_bytes);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) wgmma_ss<BN, 0>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
-    wgmma_commit();
-    wgmma_wait<1>();
-    if (prev >= 0 && signaller) mbar_arrive(&empty[prev]);
-    prev = stage;
-    if (++stage == STAGES) {
-      stage = 0;
-      phase ^= 1;
-    }
-  }
-  wgmma_wait<0>();
-  if (prev >= 0 && signaller) mbar_arrive(&empty[prev]);
-}
-
 }  // namespace ce
