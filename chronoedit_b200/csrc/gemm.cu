@@ -37,6 +37,8 @@ __device__ __forceinline__ float gelu_tanh_f(float x) {
 }
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.7071067811865476f)); }
 
+constexpr uint32_t NEG_ZERO2 = 0x80008000u;   // two bf16 -0.0
+
 template <int BN, int STAGES>
 __global__ void __launch_bounds__(RING_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g) {
@@ -58,40 +60,67 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
       }))
     return;
   // -------------------------------------------------------------------- consumers: main loop + epilogue
+  // The epilogue works in passes so that its global loads are not serialised behind its stores.  out, resid and bias are all
+  // bf16 pointers and do alias (out == resid in place in the DiT's residual GEMMs), so the compiler keeps every load behind every
+  // earlier store: with one load and one store per column group, as before, a tile waited for 64 round trips to memory.
+  //   pass 1  (no store) bias, rounding to bf16, GELU; packs the value as stored into one register per two columns, which frees
+  //           half of the accumulator registers (the kernel has 168 per thread, 128 of them accumulators at BN = 256)
+  //   pass 2  per row, chunks of CH column groups: the chunk's residual and gate loads, then its stores and row statistics
+  // A thread reads each element before it writes it, so in-place stays correct.  Arithmetic, rounding points and the order of
+  // the statistics sums are those of the single pass; the output is bit-identical.  CH = 16 spills at BN = 256.
+  constexpr int CH = BN / 8 < 8 ? BN / 8 : 8;
   const int r_in_tile = ring_row();   // rows r_in_tile and r_in_tile + 8 of the tile
   const int c_in_group = ring_col();
+  const bool resid_epi = g.epi == EPI_BIAS_GATE_RESID || g.epi == EPI_BIAS_RESID;
   float acc[BN / 2];
   for (int t : RingTiles{num_tiles}) {
     int mb, nb;
     tile_coords(t, tiles_m, tiles_n, g.group_m, mb, nb);
     ring.mma_tile(acc, kblocks);
+    const int row0 = mb * BM + r_in_tile;
+    if (g.out_f32) {   // fp32 copy of acc + bias (validation path), on its own so that pass 1 has no store
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {   // the thread's two rows
-      const int row = mb * BM + r_in_tile + 8 * h;
-      const bool row_ok = row < g.M;
-      const int batch = row_ok ? row / g.rows_per_batch : 0;
-      // row statistics of this tile (GemmArgs::stats_out): the four lanes that share a row keep partial sums about one pivot
-      float st_pivot = 0.f, st_s = 0.f, st_ss = 0.f;
-      int st_n = 0;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {   // 8-column groups, two columns per lane
+      for (int j = 0; j < BN / 8; ++j) {
         const int n = nb * BN + j * 8 + c_in_group;
-        const bool ok = row_ok && nb * BN + j * 8 < g.N;
-        float y0 = acc[4 * j + 2 * h], y1 = acc[4 * j + 2 * h + 1];
-        bool stored = false;
-        if (ok) {
-          if (g.bias) {
-            const float2 bv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(g.bias + n));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          if (row < g.M && nb * BN + j * 8 < g.N) {
+            const float2 bv = unpack_bf16x2(g.bias ? *reinterpret_cast<const uint32_t*>(g.bias + n) : NEG_ZERO2);
+            const float br = g.bias_row ? __bfloat162float(g.bias_row[row]) : -0.f;
+            *reinterpret_cast<float2*>(g.out_f32 + (size_t)row * (g.ld_f32 ? g.ld_f32 : g.N) + n) =
+                make_float2(acc[4 * j + 2 * h] + bv.x + br, acc[4 * j + 2 * h + 1] + bv.y + br);
+          }
+        }
+      }
+    }
+    uint32_t yp[BN / 8][2];   // [column group][row]: bf16(acc + bias), after GELU; raw acc where nothing is stored
+    // ---- pass 1: bias (loaded once per chunk for both rows), rounding, activation
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += CH) {
+      uint32_t bias_w[CH];
+#pragma unroll
+      for (int jj = 0; jj < CH; ++jj) {
+        const int n = nb * BN + (j0 + jj) * 8 + c_in_group;
+        bias_w[jj] = g.bias && row0 < g.M && nb * BN + (j0 + jj) * 8 < g.N ? *reinterpret_cast<const uint32_t*>(g.bias + n) : NEG_ZERO2;
+      }
+#pragma unroll
+      for (int jj = 0; jj < CH; ++jj) {
+        const int j = j0 + jj;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          float y0 = acc[4 * j + 2 * h], y1 = acc[4 * j + 2 * h + 1];
+          // The wgmma asm takes acc as "+f", so without this the values would stay live until the next tile's first wgmma
+          // (which ignores them: scale_d = 0) and pass 2 could not have their registers.
+          acc[4 * j + 2 * h] = acc[4 * j + 2 * h + 1] = 0.f;
+          if (row < g.M && nb * BN + j * 8 < g.N) {
+            const float2 bv = unpack_bf16x2(bias_w[jj]);   // -0.0 without a bias: x + -0.0 == x for every x, zeros included
             y0 += bv.x;
             y1 += bv.y;
-          }
-          if (g.bias_row) {
-            const float br = __bfloat162float(g.bias_row[row]);
+            const float br = g.bias_row ? __bfloat162float(g.bias_row[row]) : -0.f;
             y0 += br;
             y1 += br;
-          }
-          if (g.out_f32) *reinterpret_cast<float2*>(g.out_f32 + (size_t)row * (g.ld_f32 ? g.ld_f32 : g.N) + n) = make_float2(y0, y1);
-          if (g.out) {
             y0 = bf16_round(y0);  // nn.Linear returns bf16
             y1 = bf16_round(y1);
             if (g.epi == EPI_BIAS_GELU_TANH) {
@@ -100,30 +129,64 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
             } else if (g.epi == EPI_BIAS_GELU_ERF) {
               y0 = gelu_erf_f(y0);
               y1 = gelu_erf_f(y1);
-            } else if (g.epi == EPI_BIAS_GATE_RESID || g.epi == EPI_BIAS_RESID) {
-              const float2 x = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(g.resid + (size_t)row * g.ldr + n));
+            }
+          }
+          yp[j][h] = pack_bf16x2(y0, y1);   // exact except after GELU, where it is the rounding of the store
+        }
+      }
+    }
+    if (!g.out) continue;
+    // ---- pass 2: residual / gate, store, row statistics
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {   // the thread's two rows
+      const int row = row0 + 8 * h;
+      const bool row_ok = row < g.M;
+      const int batch = row_ok ? row / g.rows_per_batch : 0;
+      // row statistics of this tile (GemmArgs::stats_out): the four lanes that share a row keep partial sums about one pivot
+      float st_pivot = 0.f, st_s = 0.f, st_ss = 0.f;
+      int st_n = 0;
+#pragma unroll
+      for (int j0 = 0; j0 < BN / 8; j0 += CH) {
+        uint32_t resid_w[CH];
+        float2 gate_v[CH];
+#pragma unroll
+        for (int jj = 0; jj < CH; ++jj) {   // the chunk's loads
+          const int n = nb * BN + (j0 + jj) * 8 + c_in_group;
+          const bool ld = resid_epi && row_ok && nb * BN + (j0 + jj) * 8 < g.N;
+          resid_w[jj] = ld ? *reinterpret_cast<const uint32_t*>(g.resid + (size_t)row * g.ldr + n) : 0u;
+          gate_v[jj] = ld && g.epi == EPI_BIAS_GATE_RESID ? *reinterpret_cast<const float2*>(g.gate + (size_t)batch * g.gate_stride + n)
+                                                          : make_float2(0.f, 0.f);
+        }
+#pragma unroll
+        for (int jj = 0; jj < CH; ++jj) {   // 8-column groups, two columns per lane
+          const int j = j0 + jj;
+          const int n = nb * BN + j * 8 + c_in_group;
+          const bool ok = row_ok && nb * BN + j * 8 < g.N;
+          const float2 yv = unpack_bf16x2(yp[j][h]);
+          float y0 = yv.x, y1 = yv.y;
+          if (ok) {
+            if (resid_epi) {
+              const float2 x = unpack_bf16x2(resid_w[jj]);
               if (g.epi == EPI_BIAS_GATE_RESID) {
-                const float2 gt = *reinterpret_cast<const float2*>(g.gate + (size_t)batch * g.gate_stride + n);
-                y0 = x.x + y0 * gt.x;
-                y1 = x.y + y1 * gt.y;
+                y0 = x.x + y0 * gate_v[jj].x;
+                y1 = x.y + y1 * gate_v[jj].y;
               } else {
                 y0 = x.x + y0;
                 y1 = x.y + y1;
               }
             }
             *reinterpret_cast<uint32_t*>(g.out + (size_t)row * g.ldo + n) = pack_bf16x2(y0, y1);
-            stored = true;
           }
-        }
-        if (g.stats_mode) {   // statistics of the values as stored (bf16), pivot-shifted inside the tile
-          const float z0 = bf16_round(y0), z1 = bf16_round(y1);
-          if (j == 0) st_pivot = g.stats_mode == 1 ? __shfl_sync(0xffffffffu, z0, lane & ~3) : 0.f;  // the row's first column
-          if (stored) {
-            const float d0 = z0 - st_pivot, d1 = z1 - st_pivot;
-            st_s += d0 + d1;
-            st_ss = fmaf(d0, d0, st_ss);
-            st_ss = fmaf(d1, d1, st_ss);
-            st_n += 8;
+          if (g.stats_mode) {   // statistics of the values as stored (bf16), pivot-shifted inside the tile
+            const float z0 = bf16_round(y0), z1 = bf16_round(y1);
+            if (j == 0) st_pivot = g.stats_mode == 1 ? __shfl_sync(0xffffffffu, z0, lane & ~3) : 0.f;  // the row's first column
+            if (ok) {
+              const float d0 = z0 - st_pivot, d1 = z1 - st_pivot;
+              st_s += d0 + d1;
+              st_ss = fmaf(d0, d0, st_ss);
+              st_ss = fmaf(d1, d1, st_ss);
+              st_n += 8;
+            }
           }
         }
       }

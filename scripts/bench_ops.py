@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Operator micro-benchmarks at the 14B / 720p shapes (CUDA events, warm-up, L2-busting operand rotation).
-    python scripts/bench_ops.py [attn] [gemm] [rows] [conv]
+    python scripts/bench_ops.py [attn] [gemm [cublas]] [rows] [conv]
 Prints one JSON line per op; used to iterate on a kernel without running the whole 40-layer step."""
 import json
 import math
@@ -98,26 +98,42 @@ def bench_attn_dual(B=2, H=40, Lq=7200, Lk=512, Lk2=257):
     print(json.dumps({"op": "attention_dual", "B": B, "H": H, "Lq": Lq, "Lk": Lk, "Lk2": Lk2, "ms": round(ms, 4), "tflops": round(fl / ms / 1e9, 1)}), flush=True)
 
 
-def bench_gemm(M, N, K, epi=0, nbuf=3):
+# The six block GEMMs of the DiT at the 14B / 720p step (dit.cu), as dit.cu calls them: in-place residual (out == resid == x),
+# a batch-2 gate read from the modulation table (row stride 6 D), statistics for the LayerNorm / RMSNorm that follows.
+#   name, N, K, epilogue, stats_mode
+DIT_GEMMS = [("qkv", 15360, 5120, 0, 2), ("o_proj", 5120, 5120, 3, 1), ("cross_q", 5120, 5120, 0, 2),
+             ("cross_out", 5120, 5120, 4, 1), ("ffn_up", 13824, 5120, 1, 0), ("ffn_down", 5120, 13824, 3, 1),
+             # EPI_BIAS without statistics at the o-proj / FFN-down shapes: the difference to those rows is the epilogue's cost
+             ("o_proj_bias_only", 5120, 5120, 0, 0), ("ffn_down_bias_only", 5120, 13824, 0, 0)]
+
+
+def bench_gemm(name, N, K, epi, stats_mode, M=14400, rows_per_batch=7200, nbuf=3, cublas=True):
     A = [torch.randn(M, K, device="cuda", dtype=torch.bfloat16) for _ in range(nbuf)]
     W = [torch.randn(N, K, device="cuda", dtype=torch.bfloat16) * 0.02 for _ in range(nbuf)]
-    bias = torch.zeros(N, device="cuda", dtype=torch.bfloat16)
-    out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
-    resid = torch.randn(M, N, device="cuda", dtype=torch.bfloat16)
-    gate = torch.randn(2, N, device="cuda", dtype=torch.float32)
+    bias = (torch.randn(N, device="cuda") * 0.02).bfloat16()
+    x = torch.randn(M, N, device="cuda", dtype=torch.bfloat16)   # output, and residual in place for epilogues 3 / 4
+    mod = torch.randn(M // rows_per_batch, 6, N, device="cuda") * 0.1
+    tn = 256 if N >= 256 else (128 if N >= 128 else 64)
+    stats = torch.empty(M, (N + tn - 1) // tn, 2, device="cuda")
+    resid_epi = epi in (3, 4)
     i = [0]
 
     def fn():
         a, w = A[i[0] % nbuf], W[i[0] % nbuf]
         i[0] += 1
-        L.check(lib.ce_linear_bf16(L.ptr(a), K, L.ptr(w), K, L.ptr(bias), L.ptr(out), N, None, M, N, K, epi, L.ptr(resid), N, L.ptr(gate), N,
-                                   (M + 1) // 2, L.current_stream()))
+        args = L.LinearArgsC(A=a.data_ptr(), lda=K, W=w.data_ptr(), ldw=K, M=M, N=N, K=K, out=x.data_ptr(), ldo=N, bias=bias.data_ptr(),
+                             epilogue=epi, resid=x.data_ptr() if resid_epi else None, ldr=N if resid_epi else 0,
+                             gate=mod[:, 2].data_ptr() if epi == 3 else None, gate_stride=6 * N if epi == 3 else 0,
+                             rows_per_batch=rows_per_batch, stats_out=stats.data_ptr() if stats_mode else None,
+                             stats_ld=stats.shape[1] if stats_mode else 0, stats_mode=stats_mode)
+        L.check(lib.ce_linear_ex_bf16(args, L.current_stream()))
 
     ms = timeit(fn)
-    print(json.dumps({"op": "gemm", "M": M, "N": N, "K": K, "epi": epi, "ms": round(ms, 4), "tflops": round(2.0 * M * N * K / ms / 1e9, 1)}), flush=True)
-    # library bar: cuBLAS through torch on the same shapes
-    ms2 = timeit(lambda: torch.matmul(A[0], W[0].t()))
-    print(json.dumps({"op": "cublas_gemm", "M": M, "N": N, "K": K, "ms": round(ms2, 4), "tflops": round(2.0 * M * N * K / ms2 / 1e9, 1)}), flush=True)
+    print(json.dumps({"op": "gemm", "name": name, "M": M, "N": N, "K": K, "epi": epi, "stats_mode": stats_mode, "ms": round(ms, 4),
+                      "tflops": round(2.0 * M * N * K / ms / 1e9, 1)}), flush=True)
+    if cublas:   # library bar: cuBLAS through torch on the same shapes
+        ms2 = timeit(lambda: torch.matmul(A[0], W[0].t()))
+        print(json.dumps({"op": "cublas_gemm", "M": M, "N": N, "K": K, "ms": round(ms2, 4), "tflops": round(2.0 * M * N * K / ms2 / 1e9, 1)}), flush=True)
 
 
 def bench_rows(M=14400, D=5120):
@@ -176,8 +192,8 @@ if __name__ == "__main__":
         bench_attn(Lk=512)
         bench_attn_libs(L=7200, Lk=512)
     if "gemm" in what:
-        for (M, N, K, epi) in [(14400, 15360, 5120, 0), (14400, 5120, 5120, 3), (14400, 13824, 5120, 1), (14400, 5120, 13824, 3), (7200, 5120, 5120, 0)]:
-            bench_gemm(M, N, K, epi)
+        for case in DIT_GEMMS:
+            bench_gemm(*case, cublas="cublas" in what)
     if "rows" in what:
         bench_rows()
     if "conv" in what:
