@@ -59,6 +59,10 @@ class LinearArgsC(ctypes.Structure):   # ce_linear_args (field order = include/c
     ]
 
 
+class LinearFp8ArgsC(ctypes.Structure):   # ce_linear_fp8_args
+    _fields_ = [("base", LinearArgsC), ("a_scale", c_void_p), ("w_scale", c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/chronoedit_b200.h declares
 SIGNATURES = {
     "ce_abi_version": (c_int, []),
@@ -126,6 +130,8 @@ SIGNATURES = {
                                      c_int, c_void_p]),
     "ce_rope_table_host": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "ce_linear_ex_bf16": (c_int, [POINTER(LinearArgsC), c_void_p]),
+    "ce_linear_fp8_ex": (c_int, [POINTER(LinearFp8ArgsC), c_void_p]),
+    "ce_quantize_rows_fp8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "ce_layernorm_stats_bf16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int,
                                         c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     "ce_rmsnorm_rope_stats_bf16": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int, c_void_p, c_void_p,

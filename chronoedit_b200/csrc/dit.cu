@@ -28,7 +28,7 @@ using namespace ce;
 
 struct WeightRef {
   const void* ptr = nullptr;
-  int dtype = 0;  // 0 bf16, 1 fp32
+  int dtype = 0;  // 0 bf16, 1 fp32, 2 e4m3 (FP8 mode's block weights)
   int64_t numel = 0;
 };
 
@@ -51,6 +51,9 @@ struct ce_dit {
   std::vector<int> ev_cat;
   std::vector<double> ev_work;       // algorithmic flops (cat 0,1) or bytes (cat 2) of the launch
   size_t ev_used = 0;
+  // FP8 mode: the current forward's workspace slices for a GEMM's quantized A operand and its row scales
+  uint8_t* fp8_q = nullptr;
+  float* fp8_scale = nullptr;
 };
 
 enum { CAT_GEMM = 0, CAT_ATTN = 1, CAT_ROWS = 2, CAT_OTHER = 3, NUM_CATS = 4 };
@@ -78,10 +81,12 @@ struct Workspace {
   bf16 *temb_bf16, *tproj;
   float *sin_emb, *h1, *temb_f32, *mod, *modf;
   float2 *stats_x, *stats_qkv, *stats_q2;   // epilogue row statistics (GemmArgs::stats_out): [M, D/256], [M, 3D/256], [M, D/256]
+  uint8_t* fp8_q;     // FP8 mode only: [M, max(D, F)] e4m3, the A operand of one block GEMM at a time
+  float* fp8_scale;   //                [M] its row scales
   int64_t bytes;
 };
 
-Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li) {
+Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li, bool fp8) {
   const int64_t D = D_of(c), F = c.ffn_dim, M = (int64_t)B * L;
   const int64_t Kp = (int64_t)c.in_channels * c.patch_t * c.patch_h * c.patch_w;
   const int64_t No = (int64_t)c.out_channels * c.patch_t * c.patch_h * c.patch_w;
@@ -114,6 +119,8 @@ Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li
   w.stats_x = b.take<float2>(M * td);
   w.stats_qkv = b.take<float2>(M * 3 * td);
   w.stats_q2 = b.take<float2>(M * td);
+  w.fp8_q = fp8 ? b.take<uint8_t>(M * (D > F ? D : F)) : nullptr;
+  w.fp8_scale = fp8 ? b.take<float>(M) : nullptr;
   w.bytes = (b.off + 255) & ~int64_t(255);
   return w;
 }
@@ -124,12 +131,26 @@ struct WeightSpec {
   int64_t numel;
 };
 
-std::vector<WeightSpec> required_weights(const ce_dit_config& c) {
+// The handle holds FP8 weights when layer 0's QKV weight was registered as e4m3; ce_dit_weights_complete checks the rest.
+bool holds_fp8(const ce_dit* h) {
+  auto it = h->w.find("blocks.0.attn1.to_qkv.weight");
+  return it != h->w.end() && it->second.dtype == 2;
+}
+
+std::vector<WeightSpec> required_weights(const ce_dit_config& c, bool fp8) {
   const int64_t D = D_of(c), F = c.ffn_dim;
   const int64_t Kp = (int64_t)c.in_channels * c.patch_t * c.patch_h * c.patch_w;
   const int64_t No = (int64_t)c.out_channels * c.patch_t * c.patch_h * c.patch_w;
   std::vector<WeightSpec> v;
   auto add = [&](const std::string& n, int dt, int64_t ne) { v.push_back({n, dt, ne}); };
+  auto add_block_linear = [&](const std::string& m, int64_t N, int64_t K) {   // one of the six FP8-mode GEMMs: [N, K]
+    if (fp8) {
+      add(m + ".weight", 2, N * K);
+      add(m + ".weight_scale", 1, N);
+    } else {
+      add(m + ".weight", 0, N * K);
+    }
+  };
   add("patch_embedding.weight", 0, D * Kp);
   add("patch_embedding.bias", 0, D);
   const std::string ce_ = "condition_embedder.";
@@ -157,15 +178,15 @@ std::vector<WeightSpec> required_weights(const ce_dit_config& c) {
   add("blocks.scale_shift_table", 1, (int64_t)c.num_layers * 6 * D);
   for (int i = 0; i < c.num_layers; ++i) {
     const std::string p = "blocks." + std::to_string(i) + ".";
-    add(p + "attn1.to_qkv.weight", 0, 3 * D * D);
+    add_block_linear(p + "attn1.to_qkv", 3 * D, D);
     add(p + "attn1.to_qkv.bias", 0, 3 * D);
     add(p + "attn1.norm_q.weight", 0, D);
     add(p + "attn1.norm_k.weight", 0, D);
-    add(p + "attn1.to_out.0.weight", 0, D * D);
+    add_block_linear(p + "attn1.to_out.0", D, D);
     add(p + "attn1.to_out.0.bias", 0, D);
     add(p + "norm2.weight", 1, D);
     add(p + "norm2.bias", 1, D);
-    add(p + "attn2.to_q.weight", 0, D * D);
+    add_block_linear(p + "attn2.to_q", D, D);
     add(p + "attn2.to_q.bias", 0, D);
     add(p + "attn2.norm_q.weight", 0, D);
     add(p + "attn2.norm_k.weight", 0, D);
@@ -176,11 +197,11 @@ std::vector<WeightSpec> required_weights(const ce_dit_config& c) {
       add(p + "attn2.add_kv_proj.bias", 0, 2 * D);
       add(p + "attn2.norm_added_k.weight", 0, D);
     }
-    add(p + "attn2.to_out.0.weight", 0, D * D);
+    add_block_linear(p + "attn2.to_out.0", D, D);
     add(p + "attn2.to_out.0.bias", 0, D);
-    add(p + "ffn.net.0.proj.weight", 0, F * D);
+    add_block_linear(p + "ffn.net.0.proj", F, D);
     add(p + "ffn.net.0.proj.bias", 0, F);
-    add(p + "ffn.net.2.weight", 0, D * F);
+    add_block_linear(p + "ffn.net.2", D, F);
     add(p + "ffn.net.2.bias", 0, D);
   }
   add("scale_shift_table", 1, 2 * D);
@@ -310,8 +331,21 @@ static int linear(ce_dit* h, const bf16* A, int lda, const std::string& wname, i
   g.epi = epi;
   g.resid = resid; g.ldr = ldr;
   g.gate = gate; g.gate_stride = gate_stride; g.rows_per_batch = rows_per_batch;
+  const WeightRef& w = h->w.at(wname + ".weight");
+  if (w.dtype == 2) {   // FP8 mode: quantize A per row into the workspace, then the e4m3 GEMM (one launch more than bf16)
+    prof_begin(h, CAT_ROWS, 3.0 * M * (double)K + 4.0 * M, s);
+    int rc = launch_quantize_rows_fp8(A, lda, M, K, h->fp8_q, K, h->fp8_scale, s);
+    if (rc) return rc;
+    prof_end(h, s);
+    ++h->launches;
+    prof_begin(h, CAT_GEMM, 2.0 * M * (double)N * K, s);
+    rc = launch_gemm_fp8(reinterpret_cast<const e4m3*>(h->fp8_q), K, h->fp8_scale, reinterpret_cast<const e4m3*>(w.ptr), K,
+                         W_F32(wname + ".weight_scale"), g, s);
+    if (rc == 0) prof_end(h, s);
+    return rc;
+  }
   prof_begin(h, CAT_GEMM, 2.0 * M * (double)N * K, s);
-  int rc = launch_gemm_bf16(A, lda, W_BF16(wname + ".weight"), K, g, s);
+  int rc = launch_gemm_bf16(A, lda, reinterpret_cast<const bf16*>(w.ptr), K, g, s);
   if (rc == 0) prof_end(h, s);
   return rc;
 }
@@ -390,12 +424,16 @@ int ce_dit_set_weight(ce_dit* h, const char* name, const void* ptr, int dtype, i
 
 int ce_dit_weights_complete(const ce_dit* h) {
   CE_REQUIRE(h, "null handle");
-  for (const WeightSpec& s : required_weights(h->cfg)) {
+  const bool fp8 = holds_fp8(h);
+  for (const WeightSpec& s : required_weights(h->cfg, fp8)) {
     auto it = h->w.find(s.name);
     if (it == h->w.end()) return fail(CE_ERR_MISSING_WEIGHT, "missing weight: " + s.name);
     if (it->second.dtype != s.dtype)
       return fail(CE_ERR_MISSING_WEIGHT, "weight " + s.name + " has dtype " + std::to_string(it->second.dtype) + ", expected " +
-                                             std::to_string(s.dtype) + " (0 bf16, 1 fp32)");
+                                             std::to_string(s.dtype) + " (0 bf16, 1 fp32, 2 e4m3" +
+                                             (s.dtype == 2 || it->second.dtype == 2
+                                                  ? "; the six block GEMM weights of every layer are either all bf16 or all e4m3)"
+                                                  : ")"));
     if (it->second.numel != s.numel)
       return fail(CE_ERR_MISSING_WEIGHT, "weight " + s.name + " has " + std::to_string(it->second.numel) + " elements, expected " +
                                              std::to_string(s.numel));
@@ -406,7 +444,7 @@ int ce_dit_weights_complete(const ce_dit* h) {
 int64_t ce_dit_workspace_bytes(const ce_dit* h, int batch, int frames, int height, int width, int text_len) {
   if (!h || validate_geometry(h, batch, frames, height, width, text_len)) return -1;
   const int L = frames * (height / h->cfg.patch_h) * (width / h->cfg.patch_w);
-  return carve(h->cfg, nullptr, batch, L, text_len, 257).bytes;
+  return carve(h->cfg, nullptr, batch, L, text_len, 257, holds_fp8(h)).bytes;
 }
 
 int64_t ce_dit_last_launch_count(const ce_dit* h) { return h ? h->launches : 0; }
@@ -526,11 +564,15 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   const int L = spx ? Lfull / sp.world : Lfull, tok0 = spx ? sp.rank * L : 0, M = B * L;
   const SpLayout lay = spx ? sp_layout(B, Lfull, D, No, sp.world) : SpLayout();
   if (spx && lay.bytes > sp.region_bytes) return fail(CE_ERR_WORKSPACE, "sequence parallel: peer region too small (ce_dit_sp_region_bytes)");
-  Workspace ws = carve(c, workspace, B, L, Lt, Li);
+  const bool fp8 = holds_fp8(h);
+  CE_REQUIRE(!(spx && fp8), "sequence parallelism is not built for FP8 weights: run the FP8 mode on one GPU");
+  Workspace ws = carve(c, workspace, B, L, Lt, Li, fp8);
   if (ws.bytes > workspace_bytes)
     return fail(CE_ERR_WORKSPACE, "workspace too small: need " + std::to_string(ws.bytes) + " bytes, got " + std::to_string(workspace_bytes));
   CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
   if ((rc = ensure_rope(h, frames, hp, wp, s))) return rc;   // always the full table [Lfull, 64]
+  h->fp8_q = ws.fp8_q;
+  h->fp8_scale = ws.fp8_scale;
   // step-invariant context (text / image embedders and every block's cross-attention K/V, :52-60, :147-165): kept in the
   // caller's cache across the steps of one edit when one is given; recomputed into the workspace otherwise
   const int64_t kv_t_elems = (int64_t)B * Lt * 2 * D, kv_i_elems = c.image_dim > 0 ? (int64_t)B * Li * 2 * D : 0;
@@ -791,11 +833,7 @@ int ce_linear_bf16(const void* A, int lda, const void* W, int ldw, const void* b
   return launch_gemm_bf16(reinterpret_cast<const bf16*>(A), lda, reinterpret_cast<const bf16*>(W), ldw, g, reinterpret_cast<cudaStream_t>(stream));
 }
 
-// Test aid: one GEMM with every GemmArgs field, including the epilogue row statistics and the tile rasterisation.
-int ce_linear_ex_bf16(const ce_linear_args* a, void* stream) {
-  int rc = check_device();
-  if (rc) return rc;
-  CE_REQUIRE(a != nullptr, "ce_linear_ex_bf16: null args");
+static GemmArgs gemm_args_of(const ce_linear_args* a) {
   GemmArgs g;
   g.M = a->M; g.N = a->N; g.K = a->K;
   g.out = reinterpret_cast<bf16*>(a->out); g.ldo = a->ldo;
@@ -807,8 +845,32 @@ int ce_linear_ex_bf16(const ce_linear_args* a, void* stream) {
   g.gate = a->gate; g.gate_stride = a->gate_stride; g.rows_per_batch = a->rows_per_batch > 0 ? a->rows_per_batch : 1;
   g.stats_out = reinterpret_cast<float2*>(a->stats_out); g.stats_ld = a->stats_ld; g.stats_mode = a->stats_mode;
   g.group_m = a->group_m;
-  return launch_gemm_bf16(reinterpret_cast<const bf16*>(a->A), a->lda, reinterpret_cast<const bf16*>(a->W), a->ldw, g,
+  return g;
+}
+
+// Test aid: one GEMM with every GemmArgs field, including the epilogue row statistics and the tile rasterisation.
+int ce_linear_ex_bf16(const ce_linear_args* a, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(a != nullptr, "ce_linear_ex_bf16: null args");
+  return launch_gemm_bf16(reinterpret_cast<const bf16*>(a->A), a->lda, reinterpret_cast<const bf16*>(a->W), a->ldw, gemm_args_of(a),
                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+// Test aids of the FP8 mode: its GEMM with every epilogue option, and its row quantization.
+int ce_linear_fp8_ex(const ce_linear_fp8_args* a, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(a != nullptr, "ce_linear_fp8_ex: null args");
+  return launch_gemm_fp8(reinterpret_cast<const e4m3*>(a->base.A), a->base.lda, a->a_scale, reinterpret_cast<const e4m3*>(a->base.W),
+                         a->base.ldw, a->w_scale, gemm_args_of(&a->base), reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_quantize_rows_fp8(const void* x, int ldx, int rows, int K, void* q, int ldq, float* scale, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  return launch_quantize_rows_fp8(reinterpret_cast<const bf16*>(x), ldx, rows, K, reinterpret_cast<uint8_t*>(q), ldq, scale,
+                                  reinterpret_cast<cudaStream_t>(stream));
 }
 
 static long long* g_attn_timing = nullptr;

@@ -1,7 +1,9 @@
 // HBM-bound row kernels of the DiT path: fp32 LayerNorm + adaLN modulate, RMSNorm-across-heads + 3D RoPE,
-// patchify / unpatchify, and the tiny-M Linear layers of the time embedder.  All are coalesced 16-byte
+// patchify / unpatchify, the tiny-M Linear layers of the time embedder, and the FP8 mode's row quantisation.  All are coalesced 16-byte
 // accesses with one CTA per token row (rows >> SM count), statistics in fp32 via warp shuffles.
 #include "elementwise.cuh"
+
+#include <cuda_fp8.h>
 
 namespace ce {
 
@@ -426,7 +428,52 @@ __global__ void add_table_kernel(const float* __restrict__ table, int table_rows
   }
 }
 
+// One CTA per row: the row's absolute maximum (exact in fp32), then q = e4m3_satfinite(x / s) with s = amax / 448 (1 for a zero
+// row) as IEEE divisions, the same operations as the torch expression of the rule (DESIGN.md, "FP8 mode").  The second read of
+// the row comes from L1 / L2.
+__global__ void __launch_bounds__(ROW_THREADS)
+quantize_rows_fp8_kernel(const bf16* __restrict__ x, int ldx, int K, uint8_t* __restrict__ q, int ldq, float* __restrict__ scale) {
+  __shared__ float part[ROW_THREADS / 32];
+  const bf16* xr = x + (size_t)blockIdx.x * ldx;
+  float m = 0.f;
+  for (int c = threadIdx.x * 8; c < K; c += ROW_THREADS * 8) {
+    float f[8];
+    unpack8(*reinterpret_cast<const uint4*>(xr + c), f);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m = fmaxf(m, fabsf(f[e]));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = part[0];
+#pragma unroll
+  for (int w = 1; w < ROW_THREADS / 32; ++w) m = fmaxf(m, part[w]);
+  const float s = m == 0.f ? 1.f : __fdiv_rn(m, 448.f);
+  if (threadIdx.x == 0) scale[blockIdx.x] = s;
+  uint8_t* qr = q + (size_t)blockIdx.x * ldq;
+  for (int c = threadIdx.x * 8; c < K; c += ROW_THREADS * 8) {
+    float f[8];
+    unpack8(*reinterpret_cast<const uint4*>(xr + c), f);
+    uint32_t w[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      w[e] = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(f[2 * e], s), __fdiv_rn(f[2 * e + 1], s)), __NV_SATFINITE, __NV_E4M3);
+    *reinterpret_cast<uint2*>(qr + c) = make_uint2(w[0] | (w[1] << 16), w[2] | (w[3] << 16));
+  }
+}
+
 }  // namespace
+
+int launch_quantize_rows_fp8(const bf16* x, int ldx, int rows, int K, uint8_t* q, int ldq, float* scale, cudaStream_t stream) {
+  CE_REQUIRE(rows > 0 && K > 0 && K % 16 == 0, "quantize_rows_fp8: rows > 0 and a width that is a multiple of 16");
+  CE_REQUIRE(ldx % 8 == 0 && ldx >= K && ldq % 16 == 0 && ldq >= K, "quantize_rows_fp8: ldx % 8, ldq % 16, both >= K");
+  CE_REQUIRE(x && q && scale && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q) & 15) == 0,
+             "quantize_rows_fp8: x and q must be 16-byte aligned");
+  quantize_rows_fp8_kernel<<<rows, ROW_THREADS, 0, stream>>>(x, ldx, K, q, ldq, scale);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
 
 int launch_layernorm(const bf16* x, int ldx, bf16* y, int ldy, int rows, int D, float eps, const float* scale,
                      const float* shift, int mod_stride, int rows_per_batch, const float* weight, const float* bias,

@@ -42,6 +42,10 @@ int launch_rmsnorm_rope_stats(bf16* x, int ldx, int rows, int D, float eps, cons
                               const float* rope_cos, const float* rope_sin, int L, int head_dim, const float2* stats, int stats_ld, int tiles,
                               cudaStream_t stream, const SpScatter* sp = nullptr);
 
+// FP8 mode: per row m of x[rows, K] (K % 16 == 0), scale[m] = max_k |x[m,k]| / 448 (1 if that is 0) and
+// q[m, k] = e4m3 bits of cvt.rn.satfinite(x[m,k] / scale[m]) (IEEE fp32 divisions).  One launch, HBM-bound.
+int launch_quantize_rows_fp8(const bf16* x, int ldx, int rows, int K, uint8_t* q, int ldq, float* scale, cudaStream_t stream);
+
 // patches[(b,f,i,j), c*4 + dh*2 + dw] = x[b, c, f, 2i+dh, 2j+dw]   (im2row for the k=s=(1,2,2) patch-embedding conv, :368,429-430)
 int launch_patchify(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, cudaStream_t stream);
 // out[b, c, f, 2i+dh, 2j+dw] = y[(b,f,i,j), (dh*2+dw)*C + c]       (unpatchify permute of :463-467)

@@ -3,6 +3,8 @@
 //   out[M,N] = epilogue( A[M,K] * W[N,K]^T )        A: activations (row-major), W: nn.Linear weight (row-major)
 //
 // Per k-block an A tile 128x64 and a W tile BNx64; the epilogue applies bias / activation / gate / residual / row statistics.
+// The FP8 instantiation (gemm_fp8_kernel) reads e4m3 operands in k-blocks of 128 and multiplies the accumulator by a row scale
+// and a column scale before the same epilogue: out[M,N] = epilogue( (Aq * Wq^T) * s_a[M] * s_w[N] ).
 // Tile order is grouped along M so that concurrently resident tiles share W column panels through L2.
 //
 // Replaces the cuBLASLt calls behind every nn.Linear of the reference DiT block
@@ -39,23 +41,25 @@ __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f +
 
 constexpr uint32_t NEG_ZERO2 = 0x80008000u;   // two bf16 -0.0
 
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(RING_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g) {
+// The kernel body for operands of type T (bf16, or e4m3 with the row scales s_a[M] and column scales s_w[N]).
+template <int BN, int STAGES, class T>
+__device__ __forceinline__ void gemm_tiles(const CUtensorMap* tma_a, const CUtensorMap* tma_b, const GemmArgs& g, const float* s_a,
+                                           const float* s_w) {
+  constexpr int KB = BK_OF<T>;
   const int lane = threadIdx.x & 31;
   const int tiles_m = (g.M + BM - 1) / BM;
   const int tiles_n = (g.N + BN - 1) / BN;
   const int num_tiles = tiles_m * tiles_n;
-  const int kblocks = (g.K + BK - 1) / BK;
+  const int kblocks = (g.K + KB - 1) / KB;
 
   Ring<BN, STAGES> ring;
-  if (!ring.start(&tma_a, &tma_b, num_tiles, [&](int t) {   // TMA producer
+  if (!ring.start(tma_a, tma_b, num_tiles, [&](int t) {   // TMA producer
         int mb, nb;
         tile_coords(t, tiles_m, tiles_n, g.group_m, mb, nb);
         for (int kb = 0; kb < kblocks; ++kb) {
           const auto s = ring.acquire();
-          tma_load_2d(s.a, &tma_a, s.bar, kb * BK, mb * BM);
-          tma_load_2d(s.b, &tma_b, s.bar, kb * BK, nb * BN);
+          tma_load_2d(s.a, tma_a, s.bar, kb * KB, mb * BM);
+          tma_load_2d(s.b, tma_b, s.bar, kb * KB, nb * BN);
         }
       }))
     return;
@@ -76,8 +80,28 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
   for (int t : RingTiles{num_tiles}) {
     int mb, nb;
     tile_coords(t, tiles_m, tiles_n, g.group_m, mb, nb);
-    ring.mma_tile(acc, kblocks);
+    ring.template mma_tile<T>(acc, kblocks);
     const int row0 = mb * BM + r_in_tile;
+    if constexpr (sizeof(T) == 1) {   // y = (acc * s_a[row]) * s_w[col], before everything else reads acc (out_f32 included)
+      float sa[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) sa[h] = row0 + 8 * h < g.M ? s_a[row0 + 8 * h] : 0.f;
+#pragma unroll
+      for (int j0 = 0; j0 < BN / 8; j0 += CH) {
+#pragma unroll
+        for (int j = j0; j < j0 + CH; ++j) {
+          if (nb * BN + j * 8 < g.N) {
+            const float2 sw = *reinterpret_cast<const float2*>(s_w + nb * BN + j * 8 + c_in_group);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              acc[4 * j + 2 * h] = acc[4 * j + 2 * h] * sa[h] * sw.x;
+              acc[4 * j + 2 * h + 1] = acc[4 * j + 2 * h + 1] * sa[h] * sw.y;
+            }
+          }
+        }
+        asm volatile("" ::: "memory");   // at most CH column scales in flight: all BN / 8 at once spill at BN = 256
+      }
+    }
     if (g.out_f32) {   // fp32 copy of acc + bias (validation path), on its own so that pass 1 has no store
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
@@ -210,12 +234,26 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
   }
 }
 
-}  // namespace
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(RING_THREADS, 1)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g) {
+  gemm_tiles<BN, STAGES, bf16>(&tma_a, &tma_b, g, nullptr, nullptr);
+}
 
-int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmArgs& g, cudaStream_t stream) {
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(RING_THREADS, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g, const float* s_a,
+                const float* s_w) {
+  gemm_tiles<BN, STAGES, e4m3>(&tma_a, &tma_b, g, s_a, s_w);
+}
+
+template <class T>
+int launch_gemm(const T* A, int lda, const float* s_a, const T* W, int ldw, const float* s_w, const GemmArgs& g, cudaStream_t stream) {
+  constexpr bool fp8 = sizeof(T) == 1;
   CE_REQUIRE(g.M > 0 && g.N > 0 && g.K > 0, "gemm: empty problem");
   CE_REQUIRE(g.N % 8 == 0, "gemm: N must be a multiple of 8");
-  CE_REQUIRE(lda % 8 == 0 && ldw % 8 == 0, "gemm: lda, ldw must be multiples of 8 (16-byte TMA strides)");
+  if (fp8) CE_REQUIRE(lda % 16 == 0 && ldw % 16 == 0, "gemm: lda, ldw must be multiples of 16 (16-byte TMA strides)");
+  else CE_REQUIRE(lda % 8 == 0 && ldw % 8 == 0, "gemm: lda, ldw must be multiples of 8 (16-byte TMA strides)");
   CE_REQUIRE((g.out != nullptr && g.ldo % 8 == 0) || (g.out == nullptr && g.out_f32 != nullptr), "gemm: out / ldo");
   CE_REQUIRE((reinterpret_cast<uintptr_t>(g.out) & 15) == 0, "gemm: out must be 16-byte aligned");
   CE_REQUIRE(g.out_f32 == nullptr || ((reinterpret_cast<uintptr_t>(g.out_f32) & 15) == 0 && g.ld_f32 % 4 == 0 && (g.ld_f32 == 0 || g.ld_f32 >= g.N)),
@@ -238,15 +276,35 @@ int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmA
     if (env_gm > 0) a.group_m = env_gm;
   }
   const int bn = gemm_tile_n(a.N);
+  const auto tmap = fp8 ? make_tmap_2d_u8 : make_tmap_2d;
   CUtensorMap ta, tb;
-  int rc = make_tmap_2d(&ta, A, (uint64_t)a.M, (uint64_t)a.K, (uint64_t)lda, BM);
+  int rc = tmap(&ta, A, (uint64_t)a.M, (uint64_t)a.K, (uint64_t)lda, BM);
   if (rc) return rc;
-  rc = make_tmap_2d(&tb, W, (uint64_t)a.N, (uint64_t)a.K, (uint64_t)ldw, (uint32_t)bn);
+  rc = tmap(&tb, W, (uint64_t)a.N, (uint64_t)a.K, (uint64_t)ldw, (uint32_t)bn);
   if (rc) return rc;
   const int tiles = ((a.M + BM - 1) / BM) * ((a.N + bn - 1) / bn);
-  if (bn == 256) return launch_ring_gemm<256, 4>(gemm_bf16_kernel<256, 4>, tiles, stream, ta, tb, a);
-  if (bn == 128) return launch_ring_gemm<128, 6>(gemm_bf16_kernel<128, 6>, tiles, stream, ta, tb, a);
-  return launch_ring_gemm<64, 8>(gemm_bf16_kernel<64, 8>, tiles, stream, ta, tb, a);
+  if constexpr (fp8) {
+    if (bn == 256) return launch_ring_gemm<256, 4>(gemm_fp8_kernel<256, 4>, tiles, stream, ta, tb, a, s_a, s_w);
+    if (bn == 128) return launch_ring_gemm<128, 6>(gemm_fp8_kernel<128, 6>, tiles, stream, ta, tb, a, s_a, s_w);
+    return launch_ring_gemm<64, 8>(gemm_fp8_kernel<64, 8>, tiles, stream, ta, tb, a, s_a, s_w);
+  } else {
+    if (bn == 256) return launch_ring_gemm<256, 4>(gemm_bf16_kernel<256, 4>, tiles, stream, ta, tb, a);
+    if (bn == 128) return launch_ring_gemm<128, 6>(gemm_bf16_kernel<128, 6>, tiles, stream, ta, tb, a);
+    return launch_ring_gemm<64, 8>(gemm_bf16_kernel<64, 8>, tiles, stream, ta, tb, a);
+  }
+}
+
+}  // namespace
+
+int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmArgs& g, cudaStream_t stream) {
+  return launch_gemm<bf16>(A, lda, nullptr, W, ldw, nullptr, g, stream);
+}
+
+int launch_gemm_fp8(const e4m3* Aq, int lda, const float* s_a, const e4m3* Wq, int ldw, const float* s_w, const GemmArgs& g,
+                    cudaStream_t stream) {
+  CE_REQUIRE(s_a != nullptr && s_w != nullptr && (reinterpret_cast<uintptr_t>(s_w) & 7) == 0,
+             "gemm_fp8: a_scale and w_scale are required, w_scale 8-byte aligned");
+  return launch_gemm<e4m3>(Aq, lda, s_a, Wq, ldw, s_w, g, stream);
 }
 
 }  // namespace ce

@@ -1,9 +1,13 @@
 // Interface of the wgmma GEMM used by the DiT path (gemm.cu).
 #pragma once
 #include "host_common.h"
+#include <cuda_fp8.h>
+
 #include "ptx.cuh"
 
 namespace ce {
+
+typedef __nv_fp8_e4m3 e4m3;
 
 // Fused epilogues.  "y" is the Linear output rounded to bf16 exactly as nn.Linear returns it in the
 // reference's bf16 path; every variant keeps the reference's rounding points (SURVEY.md section 8a).
@@ -45,5 +49,10 @@ inline int gemm_tile_n(int N) { return N >= 256 ? 256 : (N >= 128 ? 128 : 64); }
 
 // out[M,N] = epilogue(A[M,K] (row-major, lda) x W[N,K]^T (row-major = nn.Linear weight, ldw)).
 int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmArgs& g, cudaStream_t stream);
+
+// The FP8 mode's GEMM: y[m,n] = (sum_k Aq[m,k] Wq[n,k] * s_a[m]) * s_w[n] with e4m3 operands (Aq row-major, lda; Wq row-major, ldw;
+// lda, ldw multiples of 16) and fp32 scales s_a[M], s_w[N]; out[M,N] = epilogue(y) exactly as launch_gemm_bf16 applies it to acc.
+int launch_gemm_fp8(const e4m3* Aq, int lda, const float* s_a, const e4m3* Wq, int ldw, const float* s_w, const GemmArgs& g,
+                    cudaStream_t stream);
 
 }  // namespace ce

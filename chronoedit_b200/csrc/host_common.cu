@@ -32,8 +32,8 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box, const uint32_t* elem_strides) {
+static int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return fail(CE_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
   cuuint64_t gdim[5];
@@ -49,11 +49,16 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail(CE_ERR_INVALID, "TMA base pointer not 16-byte aligned");
   for (int i = 0; i + 1 < rank; ++i)
     if (gstr[i] % 16 != 0) return fail(CE_ERR_INVALID, "TMA global stride not a multiple of 16 bytes");
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
+  CUresult r = fn(out, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(CE_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
   return CE_OK;
+}
+
+int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                   const uint32_t* box, const uint32_t* elem_strides) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box, elem_strides);
 }
 
 int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
@@ -61,6 +66,13 @@ int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t col
   uint64_t strides[1] = {ld * 2};
   uint32_t box[2] = {64, box_rows};
   return make_tmap_bf16(out, base, 2, dims, strides, box);
+}
+
+int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
+  uint64_t dims[2] = {cols, rows};
+  uint64_t strides[1] = {ld};
+  uint32_t box[2] = {128, box_rows};
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, 2, dims, strides, box, nullptr);
 }
 
 constexpr int kMaxDevices = 64;

@@ -1,9 +1,9 @@
-// The TMA -> shared-memory ring -> wgmma pipeline under gemm_bf16_kernel (gemm.cu) and conv3d_cl_kernel (conv.cu).
+// The TMA -> shared-memory ring -> wgmma pipeline under gemm_bf16_kernel / gemm_fp8_kernel (gemm.cu) and conv3d_cl_kernel (conv.cu).
 //
 // Persistent, warp-specialised, one CTA per SM, 384 threads = 3 warpgroups (registers re-partitioned with setmaxnreg):
 //   warpgroup 0     TMA producer (one lane of warp 0): per k-block one A tile BMxBK and one B tile BNxBK into the next stage
 //                   of a STAGES-deep ring (128B swizzle); the operation supplies the coordinates
-//   warpgroups 1,2  consumers: 64 rows x BN columns of the tile each, 4 x wgmma (M64, N=BN, K16) per k-block with both operands
+//   warpgroups 1,2  consumers: 64 rows x BN columns of the tile each, 4 x wgmma (M64, N=BN, K16 bf16 / K32 e4m3) per k-block with both operands
 //                   read from the ring, then the operation's epilogue from the accumulator registers -> global
 // Both roles walk the same tiles (RingTiles) and ring positions, so the producer fills the ring for tile i+1 while the
 // consumers run the epilogue of tile i.  A kernel calls ring.start() with its producer, then `for (int t : RingTiles{n})
@@ -16,6 +16,8 @@ namespace ce {
 
 constexpr int BM = 128;          // tile rows: two consumer warpgroups of 64
 constexpr int BK = 64;           // k-block: one 128-byte swizzled row of bf16
+template <class T>
+constexpr int BK_OF = 128 / sizeof(T);   // k-block in elements of T: 64 bf16, 128 e4m3
 constexpr int RING_THREADS = 384;
 
 // The tiles of this CTA in the order both roles walk them: blockIdx.x, blockIdx.x + gridDim.x, ... below num_tiles.
@@ -98,9 +100,11 @@ struct Ring {
     return s;
   }
 
-  // Consumer main loop of this thread's warpgroup: acc[64 x BN] = sum over `kblocks` of A[64 x 64] (its 64 rows of the tile)
-  // * B[BN x 64]^T.  One wgmma group stays in flight: a stage is handed back to the producer (one arrive per warpgroup on
-  // empty) when the group after it has been issued, so the tensor cores never wait for the hand-back.
+  // Consumer main loop of this thread's warpgroup: acc[64 x BN] = sum over `kblocks` of A[64 x BK_OF<T>] (its 64 rows of the
+  // tile) * B[BN x BK_OF<T>]^T, with T = bf16 or __nv_fp8_e4m3 (a k-block is one 128-byte row either way, 4 instructions).
+  // One wgmma group stays in flight: a stage is handed back to the producer (one arrive per warpgroup on empty) when the group
+  // after it has been issued, so the tensor cores never wait for the hand-back.
+  template <class T = bf16>
   __device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], int kblocks) {
     const int wg = (threadIdx.x >> 7) - 1;
     const uint32_t a_smem = smem_u32(sA) + wg * 64 * 128, b_smem = smem_u32(sB);
@@ -112,7 +116,10 @@ struct Ring {
       const uint64_t db = wgmma_desc_kmajor_sw128(b_smem + stage * B_BYTES);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_ss<BN, 0>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+      for (int k = 0; k < 4; ++k) {
+        if constexpr (sizeof(T) == 1) wgmma_ss_e4m3<BN>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+        else wgmma_ss<BN, 0>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+      }
       wgmma_commit();
       wgmma_wait<1>();
       if (prev >= 0 && signaller) mbar_arrive(&empty[prev]);

@@ -24,6 +24,24 @@ from ._lib import CEError, DiTConfigC, check, current_stream, ptr
 # reference `_keep_in_fp32_modules` (transformer_chronoedit.py:338)
 KEEP_FP32 = ("time_embedder", "scale_shift_table", "norm1", "norm2", "norm3")
 
+# The FP8 mode's weights: the six per-token GEMMs of every block (attn1.to_qkv is the fused to_q | to_k | to_v).  The patch
+# embedding, the condition embedders, proj_out and the step-invariant cross-attention K/V projections stay bf16.
+FP8_LINEARS = ("attn1.to_q", "attn1.to_k", "attn1.to_v", "attn1.to_out.0", "attn2.to_q", "attn2.to_out.0", "ffn.net.0.proj",
+               "ffn.net.2")
+
+
+def quantize_fp8_rows(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The FP8 mode's quantization rule, one scale per row of `x` (an output channel of a weight, a token of an activation):
+    s = max_k |x[row, k]| / 448 in fp32 (1 if that maximum is 0) and q = e4m3(clamp(x / s, -448, 448)), rounded to nearest-even.
+    Returns (q as torch.float8_e4m3fn, s as fp32).  The same on CPU and CUDA, and what the device computes for every FP8
+    GEMM's activations (ce_quantize_rows_fp8)."""
+    x = x.float()
+    amax = x.abs().amax(dim=-1)
+    # a tensor divisor: torch's CUDA division by a Python scalar multiplies by its reciprocal, which is not the IEEE quotient
+    s = torch.where(amax == 0, torch.ones_like(amax), amax / torch.full_like(amax, 448.0))
+    q = (x / s.unsqueeze(-1)).clamp(-448, 448).to(torch.float8_e4m3fn)
+    return q, s
+
 
 @dataclass
 class Transformer2DModelOutput:
@@ -190,6 +208,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._ctx_cache: list = []   # entries: dict(txt=, img=, txt_v=, img_v=, shape=, buf=)
         self._lora_adapters: Dict[str, Dict[str, torch.Tensor]] = {}
         self.last_captures: Dict[int, torch.Tensor] = {}
+        self._fp8 = False
 
     # ------------------------------------------------------------------------------------------ plumbing
     @property
@@ -209,6 +228,9 @@ class ChronoEditTransformer3DModel(nn.Module):
         return super()._apply(fn, *a, **k)
 
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
+        if self._fp8:
+            raise CEError("load_state_dict after enable_fp8(): the FP8 block weights are quantized from the bf16 ones; load the "
+                          "checkpoint (and fuse any LoRA) first, then call enable_fp8()")
         # new weights under the same prompt tensors: the cached cross-attention K/V and any captured graph are stale; with
         # assign=True the parameters are new tensors, so the fused device buffers must be rebuilt as well
         self._ctx_cache = []
@@ -238,6 +260,34 @@ class ChronoEditTransformer3DModel(nn.Module):
             check(_lib.lib().ce_dit_create(_lib.ctypes.byref(cfg), _lib.ctypes.byref(h)))
             self._handle = h
         return self._handle
+
+    # ------------------------------------------------------------------------------------------ FP8 mode
+    @property
+    def fp8_enabled(self) -> bool:
+        return self._fp8
+
+    @torch.no_grad()
+    def enable_fp8(self) -> None:
+        """Opt-in FP8 mode (DESIGN.md, "FP8 mode"): the six per-token GEMMs of every block run as e4m3 wgmma with one scale per
+        output channel (weights, quantized here by `quantize_fp8_rows`) and one per token (activations, quantized on the device
+        before each GEMM).  Each of those layers then holds buffers `weight_fp8` (float8_e4m3fn, [N, K]) and `weight_scale`
+        (fp32, [N]) instead of its bf16 `weight`, whose storage is released.  One-way; works on CPU or CUDA, and the buffers
+        follow .to() / .cpu().  Call it after loading the checkpoint and fusing any LoRA: both raise afterwards."""
+        if self._fp8:
+            return
+        for blk in self.blocks:
+            for name in FP8_LINEARS:
+                holder = blk.get_submodule(name)
+                q, s = quantize_fp8_rows(holder.weight.data)
+                del holder.weight
+                holder.register_buffer("weight_fp8", q)
+                holder.register_buffer("weight_scale", s)
+        self._fp8 = True
+        self._packed = False
+        self._pack_keepalive = {}   # the fused bf16 QKV buffers
+        self._graphs = {}
+        self._ctx_cache = []
+        self._workspaces = {}
 
     # ------------------------------------------------------------------------------------------ fp32 validation mode
     @torch.no_grad()
@@ -305,6 +355,10 @@ class ChronoEditTransformer3DModel(nn.Module):
             want = torch.float32 if any(k in n for k in KEEP_FP32) else torch.bfloat16
             if p.dtype != want:
                 p.data = p.data.to(want)
+        for n, b in self.named_buffers():
+            want = torch.float8_e4m3fn if n.endswith(".weight_fp8") else torch.float32
+            if b.dtype != want:
+                raise CEError(f"FP8 buffer {n} has dtype {b.dtype}, expected {want} (was the module cast with .to(dtype)?)")
         self._ensure_handle()
         keep: Dict[str, torch.Tensor] = {}
 
@@ -322,13 +376,19 @@ class ChronoEditTransformer3DModel(nn.Module):
         def reg(name, t):
             t = t.contiguous() if not t.is_contiguous() else t
             keep[name] = t
-            check(L.ce_dit_set_weight(self._handle, name.encode(), ptr(t), 1 if t.dtype == torch.float32 else 0, t.numel()))
+            code = {torch.bfloat16: 0, torch.float32: 1, torch.float8_e4m3fn: 2}[t.dtype]
+            check(L.ce_dit_set_weight(self._handle, name.encode(), ptr(t), code, t.numel()))
 
         fused_names = set()
         for i, blk in enumerate(self.blocks):
             p = f"blocks.{i}."
+            qkv = [blk.attn1.to_q, blk.attn1.to_k, blk.attn1.to_v]
+            if self._fp8:   # e4m3 weight under the bf16 name, scales beside it
+                reg(p + "attn1.to_qkv.weight", fuse(p + "attn1.to_qkv", qkv, "weight_fp8"))
+                reg(p + "attn1.to_qkv.weight_scale", fuse(p + "attn1.to_qkv", qkv, "weight_scale"))
             for attr in ("weight", "bias"):
-                reg(p + "attn1.to_qkv." + attr, fuse(p + "attn1.to_qkv", [blk.attn1.to_q, blk.attn1.to_k, blk.attn1.to_v], attr))
+                if attr == "bias" or not self._fp8:
+                    reg(p + "attn1.to_qkv." + attr, fuse(p + "attn1.to_qkv", qkv, attr))
                 reg(p + "attn2.to_kv." + attr, fuse(p + "attn2.to_kv", [blk.attn2.to_k, blk.attn2.to_v], attr))
                 if self.config.image_dim is not None:
                     reg(p + "attn2.add_kv_proj." + attr, fuse(p + "attn2.add_kv_proj", [blk.attn2.add_k_proj, blk.attn2.add_v_proj], attr))
@@ -342,6 +402,9 @@ class ChronoEditTransformer3DModel(nn.Module):
             if any(n.startswith(f) for f in fused_names) or (n.startswith("blocks.") and n.endswith("scale_shift_table")):
                 continue
             reg(n, p.data)
+        for n, b in self.named_buffers():   # FP8 mode: weight_fp8 / weight_scale of the unfused block GEMMs
+            if not any(n.startswith(f) for f in fused_names):
+                reg(n[: -len("_fp8")] if n.endswith(".weight_fp8") else n, b)
         check(L.ce_dit_weights_complete(self._handle))
         self._pack_keepalive = keep
         self._packed = True
@@ -659,6 +722,8 @@ class ChronoEditTransformer3DModel(nn.Module):
         chronoedit/_src/models/utils.py:66-290, wan_t2v_model.py:385-391).  `diff` / `diff_b` entries (norm / bias deltas the
         reference converter drops or treats as lora_bias) are rejected.  Everything is validated BEFORE the first weight is
         touched.  One-time weight preparation with torch matmuls; not on the per-step path.  Returns the number of weights updated."""
+        if self._fp8:
+            raise CEError("fuse_lora after enable_fp8(): fuse the LoRA into the bf16 weights first, then call enable_fp8()")
         lora_state_dict = kwargs.pop("lora_state_dict", None)
         if args and isinstance(args[0], dict):        # fuse_lora(state_dict[, lora_scale])
             lora_state_dict, args = args[0], args[1:]

@@ -67,12 +67,18 @@ void ce_dit_destroy(ce_dit* h);
  *   blocks.scale_shift_table                 [num_layers,6,D] fp32 (stack of blocks.N.scale_shift_table)
  *   patch_embedding.weight                   [D, Cin*pt*ph*pw] (the Conv3d weight, flattened)
  * dtype: 0 = bf16, 1 = fp32.  fp32 is required for (and only for) the reference's `_keep_in_fp32_modules`
- * (time_embedder, scale_shift_table, norm1/norm2/norm3 affine parameters, :338). */
+ * (time_embedder, scale_shift_table, norm1/norm2/norm3 affine parameters, :338).
+ * FP8 mode: dtype 2 = e4m3 (torch.float8_e4m3fn) for the six per-token block weights attn1.to_qkv, attn1.to_out.0,
+ * attn2.to_q, attn2.to_out.0, ffn.net.0.proj and ffn.net.2, each with its fp32 per-output-channel scale registered as
+ * "<name>.weight_scale" [N] (dtype 1): W ~ weight * weight_scale[n].  Either all six of every layer are e4m3 or none is;
+ * ce_dit_weights_complete rejects a mixture.  Such a handle quantizes each of those GEMMs' activations per row on the
+ * device (DESIGN.md, "FP8 mode"); sequence parallelism is not built for it. */
 int ce_dit_set_weight(ce_dit* h, const char* name, const void* ptr, int dtype, int64_t numel);
 /* 0 when every parameter the configuration needs has been registered; otherwise fails and names the first missing. */
 int ce_dit_weights_complete(const ce_dit* h);
 
-/* Scratch bytes one forward needs for `batch` samples of latent geometry (frames, height, width) and text_len tokens. */
+/* Scratch bytes one forward needs for `batch` samples of latent geometry (frames, height, width) and text_len tokens.
+ * A handle holding FP8 weights needs M * max(D, ffn_dim) bytes + M floats more (M = batch * tokens): the quantized rows. */
 int64_t ce_dit_workspace_bytes(const ce_dit* h, int batch, int frames, int height, int width, int text_len);
 
 /* ChronoEditTransformer3DModel.forward (:397-476).
@@ -316,6 +322,20 @@ typedef struct ce_linear_args {
 
 /* out = epilogue(A x W^T + bias) with every option of the DiT's GEMM, including the row statistics. */
 int ce_linear_ex_bf16(const ce_linear_args* args, void* stream);
+
+/* FP8 mode's GEMM: base.A [M, lda] and base.W [N, ldw] hold e4m3 (lda, ldw, K multiples of 16); the accumulator is
+ * y = (sum_k A W) * a_scale[m] * w_scale[n] (fp32 [M] and [N], w_scale 8-byte aligned), then every epilogue option of
+ * `base` applies to y as ce_linear_ex_bf16 applies it to A x W^T (out_f32 receives y + bias). */
+typedef struct ce_linear_fp8_args {
+  ce_linear_args base;
+  const float* a_scale;
+  const float* w_scale;
+} ce_linear_fp8_args;
+int ce_linear_fp8_ex(const ce_linear_fp8_args* args, void* stream);
+
+/* Per-row e4m3 quantization of x [rows, K] bf16 (K % 16 == 0, ldx % 8 == 0, ldq % 16 == 0): scale[m] = max_k |x| / 448
+ * (1 for a zero row), q[m, k] = e4m3 bits of cvt.rn.satfinite(x / scale[m]), the division in IEEE fp32. */
+int ce_quantize_rows_fp8(const void* x, int ldx, int rows, int K, void* q, int ldq, float* scale, void* stream);
 
 /* FP32LayerNorm (+ modulate or affine) like ce_layernorm_bf16, with the row statistics merged from `tiles` stats_mode-1
  * partials of width tile_n covering [0, D) (stats [rows, stats_ld] float pairs).  scale_is_1p: `scale` holds 1 + scale. */

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Operator micro-benchmarks at the 14B / 720p shapes (CUDA events, warm-up, L2-busting operand rotation).
     python scripts/bench_ops.py [attn] [gemm [cublas]] [rows] [conv]
+`gemm` times each block GEMM in bf16 and, in the fp8_* fields, as the FP8 mode runs it (quantization and e4m3 GEMM).
 Prints one JSON line per op; used to iterate on a kernel without running the whole 40-layer step."""
 import json
 import math
@@ -129,8 +130,37 @@ def bench_gemm(name, N, K, epi, stats_mode, M=14400, rows_per_batch=7200, nbuf=3
         L.check(lib.ce_linear_ex_bf16(args, L.current_stream()))
 
     ms = timeit(fn)
-    print(json.dumps({"op": "gemm", "name": name, "M": M, "N": N, "K": K, "epi": epi, "stats_mode": stats_mode, "ms": round(ms, 4),
-                      "tflops": round(2.0 * M * N * K / ms / 1e9, 1)}), flush=True)
+    row = {"op": "gemm", "name": name, "M": M, "N": N, "K": K, "epi": epi, "stats_mode": stats_mode, "ms": round(ms, 4),
+           "tflops": round(2.0 * M * N * K / ms / 1e9, 1)}
+    # FP8 column: the same GEMM as the FP8 mode runs it (ce_linear_fp8_ex on e4m3 operands), and the row quantization of A
+    # that precedes it in dit.cu (ce_quantize_rows_fp8, one launch per GEMM)
+    from chronoedit_b200.transformer import quantize_fp8_rows
+
+    Aq = [torch.empty(M, K, device="cuda", dtype=torch.uint8) for _ in range(nbuf)]
+    sa = [torch.empty(M, device="cuda") for _ in range(nbuf)]
+    Wq, sw = zip(*[quantize_fp8_rows(w) for w in W])
+
+    def quant():
+        j = i[0] % nbuf
+        i[0] += 1
+        L.check(lib.ce_quantize_rows_fp8(L.ptr(A[j]), K, M, K, L.ptr(Aq[j]), K, L.ptr(sa[j]), L.current_stream()))
+
+    def fn8():
+        j = i[0] % nbuf
+        i[0] += 1
+        base = L.LinearArgsC(A=Aq[j].data_ptr(), lda=K, W=Wq[j].data_ptr(), ldw=K, M=M, N=N, K=K, out=x.data_ptr(), ldo=N,
+                             bias=bias.data_ptr(), epilogue=epi, resid=x.data_ptr() if resid_epi else None, ldr=N if resid_epi else 0,
+                             gate=mod[:, 2].data_ptr() if epi == 3 else None, gate_stride=6 * N if epi == 3 else 0,
+                             rows_per_batch=rows_per_batch, stats_out=stats.data_ptr() if stats_mode else None,
+                             stats_ld=stats.shape[1] if stats_mode else 0, stats_mode=stats_mode)
+        args = L.LinearFp8ArgsC(base=base, a_scale=sa[j].data_ptr(), w_scale=sw[j].data_ptr())
+        L.check(lib.ce_linear_fp8_ex(args, L.current_stream()))
+
+    msq = timeit(quant)
+    ms8 = timeit(fn8)
+    row.update(fp8_ms=round(ms8, 4), fp8_tflops=round(2.0 * M * N * K / ms8 / 1e9, 1), fp8_quant_ms=round(msq, 4),
+               fp8_quant_GBps=round(3.0 * M * K / msq / 1e6, 1))
+    print(json.dumps(row), flush=True)
     if cublas:   # library bar: cuBLAS through torch on the same shapes
         ms2 = timeit(lambda: torch.matmul(A[0], W[0].t()))
         print(json.dumps({"op": "cublas_gemm", "M": M, "N": N, "K": K, "ms": round(ms2, 4), "tflops": round(2.0 * M * N * K / ms2 / 1e9, 1)}), flush=True)
