@@ -3,12 +3,13 @@
 // Mirrors ChronoEditTransformer3DModel.forward (/root/reference/chronoedit_diffusers/transformer_chronoedit.py:397-476)
 // with every rounding point of the reference's bf16 path kept (SURVEY.md section 8a).  Per block
 // (ChronoEditTransformerBlock.forward, :267-295) the launches are:
-//   LN+modulate -> QKV GEMM (one launch, N=3D) -> RMSNorm+RoPE(q), RMSNorm+RoPE(k) -> attention -> out-proj GEMM with
-//   gate*y+x epilogue -> LN(affine) -> q GEMM -> RMSNorm(q) -> [text k|v GEMM, RMSNorm(k)] [image k|v GEMM, RMSNorm(k)]
-//   -> attention(text) -> attention(image, += ) -> out-proj GEMM with y+x epilogue -> LN+modulate -> FFN-1 GEMM with
-//   bias+GELU epilogue -> FFN-2 GEMM with gate*y+x epilogue.
+//   LN+modulate -> QKV GEMM (one launch, N=3D) -> RMSNorm+RoPE(q|k) -> attention -> out-proj GEMM with gate*y+x epilogue
+//   -> LN(affine) -> q GEMM -> RMSNorm(q) -> [text k|v GEMM, RMSNorm(k)] [image k|v GEMM, RMSNorm(k)] -> attention(text +
+//   image, one launch) -> out-proj GEMM with y+x epilogue -> LN+modulate -> FFN-1 GEMM with bias+GELU epilogue -> FFN-2 GEMM
+//   with gate*y+x epilogue.
+// When D % 256 == 0 the GEMM before each LN / RMSNorm also writes that norm's row statistics, and RMSNorm+RoPE(q|k) is one
+// launch; other widths take row kernels that reduce over the row themselves, and two RMSNorm+RoPE launches.
 #include <math.h>
-#include <stdlib.h>
 
 #include <map>
 #include <string>
@@ -62,19 +63,6 @@ namespace {
 
 int D_of(const ce_dit_config& c) { return c.num_attention_heads * c.attention_head_dim; }
 
-struct Bump {
-  uint8_t* base;
-  int64_t off = 0;
-  explicit Bump(void* b) : base(reinterpret_cast<uint8_t*>(b)) {}
-  template <typename T>
-  T* take(int64_t n) {
-    off = (off + 255) & ~int64_t(255);
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += n * (int64_t)sizeof(T);
-    return p;
-  }
-};
-
 struct Workspace {
   bf16 *x, *xn, *qkv, *attn, *hbuf, *patches, *yout;
   bf16 *text1, *ctx_text, *img0, *img1, *img2, *ctx_img, *kv_text, *kv_img;
@@ -121,93 +109,155 @@ Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li
   w.stats_q2 = b.take<float2>(M * td);
   w.fp8_q = fp8 ? b.take<uint8_t>(M * (D > F ? D : F)) : nullptr;
   w.fp8_scale = fp8 ? b.take<float>(M) : nullptr;
-  w.bytes = (b.off + 255) & ~int64_t(255);
+  w.bytes = b.bytes();
   return w;
 }
 
-struct WeightSpec {
-  std::string name;
-  int dtype;
-  int64_t numel;
+// The device staging buffer of ce_dit_forward_host_ex: the inputs, then the sample (left there for the caller at sample_offset).
+struct Staging {
+  int64_t n_x, n_t, n_i, n_o;   // elements of hidden_states, encoder_hidden_states, encoder_hidden_states_image, sample
+  bf16 *x, *text, *image, *sample;
+  float* timestep;
+  int64_t sample_offset, bytes;
 };
 
-// The handle holds FP8 weights when layer 0's QKV weight was registered as e4m3; ce_dit_weights_complete checks the rest.
-bool holds_fp8(const ce_dit* h) {
-  auto it = h->w.find("blocks.0.attn1.to_qkv.weight");
-  return it != h->w.end() && it->second.dtype == 2;
+Staging carve_staging(const ce_dit_config& c, void* base, int batch, int frames, int height, int width, int text_len) {
+  Staging st;
+  st.n_x = (int64_t)batch * c.in_channels * frames * height * width;
+  st.n_t = (int64_t)batch * text_len * c.text_dim;
+  st.n_i = (int64_t)batch * 257 * c.image_dim;
+  st.n_o = (int64_t)batch * c.out_channels * frames * height * width;
+  Bump b(base);
+  st.x = b.take<bf16>(st.n_x);
+  st.timestep = b.take<float>(batch);
+  st.text = b.take<bf16>(st.n_t);
+  st.image = b.take<bf16>(st.n_i > 0 ? st.n_i : 8);
+  st.sample_offset = b.bytes();
+  st.sample = b.take<bf16>(st.n_o);
+  st.bytes = b.bytes();
+  return st;
 }
 
-std::vector<WeightSpec> required_weights(const ce_dit_config& c, bool fp8) {
+// One GEMM weight [N, K] of the forward with its bias [N]: bf16, or e4m3 with fp32 per-output-channel scales [N] (FP8 mode).
+struct Linear {
+  const void* weight = nullptr;
+  int dtype = 0;   // 0 bf16, 2 e4m3
+  const bf16* bias = nullptr;
+  const float* weight_scale = nullptr;
+};
+
+struct LayerWeights {
+  Linear qkv, out1, q2, kv, add_kv, out2, ffn1, ffn2;   // attn1.to_qkv, attn1.to_out.0, attn2.to_q, attn2.to_kv, attn2.add_kv_proj,
+                                                        // attn2.to_out.0, ffn.net.0.proj, ffn.net.2
+  const bf16 *norm_q1{}, *norm_k1{}, *norm_q2{}, *norm_k2{}, *norm_added_k{};
+  const float *norm2_w{}, *norm2_b{};
+};
+
+// Every parameter the forward reads, resolved from the names registered with ce_dit_set_weight.
+struct Weights {
+  bool fp8 = false;   // the six block GEMM weights of every layer are e4m3: chosen by layer 0's attn1.to_qkv.weight
+  Linear patch, text1, text2, img_ff0, img_ff2, proj_out;
+  const float *time1_w{}, *time1_b{}, *time2_w{}, *time2_b{};
+  const bf16 *time_proj_w{}, *time_proj_b{};
+  const float *img_norm1_w{}, *img_norm1_b{}, *img_norm2_w{}, *img_norm2_b{};
+  const float *block_table{}, *head_table{};   // blocks.scale_shift_table [layers, 6, D], scale_shift_table [2, D]
+  std::vector<LayerWeights> layers;
+};
+
+// Looks weights up one at a time, checking dtype and element count; the first one that is missing or wrong records
+// CE_ERR_MISSING_WEIGHT with its name, and every lookup after it returns null.
+struct WeightLookup {
+  const std::map<std::string, WeightRef>& w;
+  int rc = CE_OK;
+
+  const void* get(const std::string& name, int dtype, int64_t numel) {
+    if (rc) return nullptr;
+    auto it = w.find(name);
+    if (it == w.end()) {
+      rc = fail(CE_ERR_MISSING_WEIGHT, "missing weight: " + name);
+      return nullptr;
+    }
+    if (it->second.dtype != dtype) {
+      rc = fail(CE_ERR_MISSING_WEIGHT, "weight " + name + " has dtype " + std::to_string(it->second.dtype) + ", expected " +
+                                           std::to_string(dtype) + " (0 bf16, 1 fp32, 2 e4m3" +
+                                           (dtype == 2 || it->second.dtype == 2
+                                                ? "; the six block GEMM weights of every layer are either all bf16 or all e4m3)"
+                                                : ")"));
+      return nullptr;
+    }
+    if (it->second.numel != numel) {
+      rc = fail(CE_ERR_MISSING_WEIGHT, "weight " + name + " has " + std::to_string(it->second.numel) + " elements, expected " +
+                                           std::to_string(numel));
+      return nullptr;
+    }
+    return it->second.ptr;
+  }
+  const bf16* b16(const std::string& name, int64_t numel) { return static_cast<const bf16*>(get(name, 0, numel)); }
+  const float* f32(const std::string& name, int64_t numel) { return static_cast<const float*>(get(name, 1, numel)); }
+  // module `m` of shape [N, K]: "<m>.weight", for e4m3 "<m>.weight_scale", then "<m>.bias"
+  Linear linear(const std::string& m, int64_t N, int64_t K, bool e4m3 = false) {
+    Linear l;
+    l.dtype = e4m3 ? 2 : 0;
+    l.weight = get(m + ".weight", l.dtype, N * K);
+    if (e4m3) l.weight_scale = f32(m + ".weight_scale", N);
+    l.bias = b16(m + ".bias", N);
+    return l;
+  }
+};
+
+int resolve_weights(const ce_dit* h, Weights& w) {
+  const ce_dit_config& c = h->cfg;
   const int64_t D = D_of(c), F = c.ffn_dim;
   const int64_t Kp = (int64_t)c.in_channels * c.patch_t * c.patch_h * c.patch_w;
   const int64_t No = (int64_t)c.out_channels * c.patch_t * c.patch_h * c.patch_w;
-  std::vector<WeightSpec> v;
-  auto add = [&](const std::string& n, int dt, int64_t ne) { v.push_back({n, dt, ne}); };
-  auto add_block_linear = [&](const std::string& m, int64_t N, int64_t K) {   // one of the six FP8-mode GEMMs: [N, K]
-    if (fp8) {
-      add(m + ".weight", 2, N * K);
-      add(m + ".weight_scale", 1, N);
-    } else {
-      add(m + ".weight", 0, N * K);
-    }
-  };
-  add("patch_embedding.weight", 0, D * Kp);
-  add("patch_embedding.bias", 0, D);
+  auto qkv0 = h->w.find("blocks.0.attn1.to_qkv.weight");
+  w.fp8 = qkv0 != h->w.end() && qkv0->second.dtype == 2;
+  WeightLookup r{h->w};
+  w.patch = r.linear("patch_embedding", D, Kp);
   const std::string ce_ = "condition_embedder.";
-  add(ce_ + "time_embedder.linear_1.weight", 1, D * c.freq_dim);
-  add(ce_ + "time_embedder.linear_1.bias", 1, D);
-  add(ce_ + "time_embedder.linear_2.weight", 1, D * D);
-  add(ce_ + "time_embedder.linear_2.bias", 1, D);
-  add(ce_ + "time_proj.weight", 0, 6 * D * D);
-  add(ce_ + "time_proj.bias", 0, 6 * D);
-  add(ce_ + "text_embedder.linear_1.weight", 0, D * c.text_dim);
-  add(ce_ + "text_embedder.linear_1.bias", 0, D);
-  add(ce_ + "text_embedder.linear_2.weight", 0, D * D);
-  add(ce_ + "text_embedder.linear_2.bias", 0, D);
+  w.time1_w = r.f32(ce_ + "time_embedder.linear_1.weight", D * c.freq_dim);
+  w.time1_b = r.f32(ce_ + "time_embedder.linear_1.bias", D);
+  w.time2_w = r.f32(ce_ + "time_embedder.linear_2.weight", D * D);
+  w.time2_b = r.f32(ce_ + "time_embedder.linear_2.bias", D);
+  w.time_proj_w = r.b16(ce_ + "time_proj.weight", 6 * D * D);
+  w.time_proj_b = r.b16(ce_ + "time_proj.bias", 6 * D);
+  w.text1 = r.linear(ce_ + "text_embedder.linear_1", D, c.text_dim);
+  w.text2 = r.linear(ce_ + "text_embedder.linear_2", D, D);
   if (c.image_dim > 0) {
     const int64_t I = c.image_dim;
-    add(ce_ + "image_embedder.norm1.weight", 1, I);
-    add(ce_ + "image_embedder.norm1.bias", 1, I);
-    add(ce_ + "image_embedder.ff.net.0.proj.weight", 0, I * I);
-    add(ce_ + "image_embedder.ff.net.0.proj.bias", 0, I);
-    add(ce_ + "image_embedder.ff.net.2.weight", 0, D * I);
-    add(ce_ + "image_embedder.ff.net.2.bias", 0, D);
-    add(ce_ + "image_embedder.norm2.weight", 1, D);
-    add(ce_ + "image_embedder.norm2.bias", 1, D);
+    w.img_norm1_w = r.f32(ce_ + "image_embedder.norm1.weight", I);
+    w.img_norm1_b = r.f32(ce_ + "image_embedder.norm1.bias", I);
+    w.img_ff0 = r.linear(ce_ + "image_embedder.ff.net.0.proj", I, I);
+    w.img_ff2 = r.linear(ce_ + "image_embedder.ff.net.2", D, I);
+    w.img_norm2_w = r.f32(ce_ + "image_embedder.norm2.weight", D);
+    w.img_norm2_b = r.f32(ce_ + "image_embedder.norm2.bias", D);
   }
-  add("blocks.scale_shift_table", 1, (int64_t)c.num_layers * 6 * D);
+  w.block_table = r.f32("blocks.scale_shift_table", (int64_t)c.num_layers * 6 * D);
+  w.layers.resize(c.num_layers);
   for (int i = 0; i < c.num_layers; ++i) {
     const std::string p = "blocks." + std::to_string(i) + ".";
-    add_block_linear(p + "attn1.to_qkv", 3 * D, D);
-    add(p + "attn1.to_qkv.bias", 0, 3 * D);
-    add(p + "attn1.norm_q.weight", 0, D);
-    add(p + "attn1.norm_k.weight", 0, D);
-    add_block_linear(p + "attn1.to_out.0", D, D);
-    add(p + "attn1.to_out.0.bias", 0, D);
-    add(p + "norm2.weight", 1, D);
-    add(p + "norm2.bias", 1, D);
-    add_block_linear(p + "attn2.to_q", D, D);
-    add(p + "attn2.to_q.bias", 0, D);
-    add(p + "attn2.norm_q.weight", 0, D);
-    add(p + "attn2.norm_k.weight", 0, D);
-    add(p + "attn2.to_kv.weight", 0, 2 * D * D);
-    add(p + "attn2.to_kv.bias", 0, 2 * D);
+    LayerWeights& l = w.layers[i];
+    l.qkv = r.linear(p + "attn1.to_qkv", 3 * D, D, w.fp8);
+    l.norm_q1 = r.b16(p + "attn1.norm_q.weight", D);
+    l.norm_k1 = r.b16(p + "attn1.norm_k.weight", D);
+    l.out1 = r.linear(p + "attn1.to_out.0", D, D, w.fp8);
+    l.norm2_w = r.f32(p + "norm2.weight", D);
+    l.norm2_b = r.f32(p + "norm2.bias", D);
+    l.q2 = r.linear(p + "attn2.to_q", D, D, w.fp8);
+    l.norm_q2 = r.b16(p + "attn2.norm_q.weight", D);
+    l.norm_k2 = r.b16(p + "attn2.norm_k.weight", D);
+    l.kv = r.linear(p + "attn2.to_kv", 2 * D, D);
     if (c.image_dim > 0) {
-      add(p + "attn2.add_kv_proj.weight", 0, 2 * D * (int64_t)c.added_kv_proj_dim);
-      add(p + "attn2.add_kv_proj.bias", 0, 2 * D);
-      add(p + "attn2.norm_added_k.weight", 0, D);
+      l.add_kv = r.linear(p + "attn2.add_kv_proj", 2 * D, c.added_kv_proj_dim);
+      l.norm_added_k = r.b16(p + "attn2.norm_added_k.weight", D);
     }
-    add_block_linear(p + "attn2.to_out.0", D, D);
-    add(p + "attn2.to_out.0.bias", 0, D);
-    add_block_linear(p + "ffn.net.0.proj", F, D);
-    add(p + "ffn.net.0.proj.bias", 0, F);
-    add_block_linear(p + "ffn.net.2", D, F);
-    add(p + "ffn.net.2.bias", 0, D);
+    l.out2 = r.linear(p + "attn2.to_out.0", D, D, w.fp8);
+    l.ffn1 = r.linear(p + "ffn.net.0.proj", F, D, w.fp8);
+    l.ffn2 = r.linear(p + "ffn.net.2", D, F, w.fp8);
   }
-  add("scale_shift_table", 1, 2 * D);
-  add("proj_out.weight", 0, No * D);
-  add("proj_out.bias", 0, No);
-  return v;
+  w.head_table = r.f32("scale_shift_table", 2 * D);
+  w.proj_out = r.linear("proj_out", No, D);
+  return r.rc;
 }
 
 int validate_geometry(const ce_dit* h, int batch, int frames, int height, int width, int text_len) {
@@ -287,73 +337,52 @@ int ensure_rope(ce_dit* h, int frames, int hp, int wp, cudaStream_t stream) {
 
 }  // namespace
 
-#define W_BF16(name) reinterpret_cast<const bf16*>(h->w.at(name).ptr)
-#define W_F32(name) reinterpret_cast<const float*>(h->w.at(name).ptr)
-static inline void prof_begin(ce_dit* h, int cat, double work, cudaStream_t s) {
-  if (!h->profiling || h->ev_used + 2 > h->ev.size()) return;
-  cudaEventRecord(h->ev[h->ev_used], s);
-  h->ev_cat[h->ev_used / 2] = cat;
-  h->ev_work[h->ev_used / 2] = work;
+// Every launch of the forward goes through run(): under ce_dit_profile_begin it records a (begin, end) event pair around the
+// launch with its category and work (algorithmic flops for GEMM and attention, bytes for the row kernels), and it counts the
+// launch once it is enqueued.
+template <class Launch>
+static int run(ce_dit* h, cudaStream_t s, int cat, double work, Launch&& launch) {
+  const bool prof = h->profiling && h->ev_used + 2 <= h->ev.size();
+  if (prof) {
+    cudaEventRecord(h->ev[h->ev_used], s);
+    h->ev_cat[h->ev_used / 2] = cat;
+    h->ev_work[h->ev_used / 2] = work;
+  }
+  const int rc = launch();
+  if (rc) return rc;
+  if (prof) {
+    cudaEventRecord(h->ev[h->ev_used + 1], s);
+    h->ev_used += 2;
+  }
+  ++h->launches;
+  return CE_OK;
 }
-static inline void prof_end(ce_dit* h, cudaStream_t s) {
-  if (!h->profiling || h->ev_used + 2 > h->ev.size()) return;
-  cudaEventRecord(h->ev[h->ev_used + 1], s);
-  h->ev_used += 2;
-}
-#define RUNC(cat, work, call)          \
-  do {                                 \
-    prof_begin(h, (cat), (work), s);   \
-    int _rc = (call);                  \
-    if (_rc) return _rc;               \
-    prof_end(h, s);                    \
-    ++h->launches;                     \
-  } while (0)
-#define RUN(call) RUNC(CAT_OTHER, 0.0, call)
-#define RUN2(call)           \
-  do {                       \
-    int _rc = (call);        \
-    if (_rc) return _rc;     \
-    ++h->launches;           \
+#define LAUNCH(cat, work, call)                                              \
+  do {                                                                       \
+    const int _rc = run(h, s, (cat), (work), [&] { return (call); });       \
+    if (_rc) return _rc;                                                     \
   } while (0)
 
-static int linear(ce_dit* h, const bf16* A, int lda, const std::string& wname, int M, int N, int K, bf16* out, int ldo, int epi,
-                  const bf16* resid, int ldr, const float* gate, int gate_stride, int rows_per_batch, cudaStream_t s,
-                  float2* stats_out = nullptr, int stats_mode = 0) {
-  GemmArgs g;
-  if (stats_out) {
-    g.stats_out = stats_out;
-    g.stats_mode = stats_mode;
-    g.stats_ld = (N + gemm_tile_n(N) - 1) / gemm_tile_n(N);
-  }
+static double attention_flops(const AttnArgs& a) { return 4.0 * a.B * a.H * (double)a.Lq * (a.Lk + a.Lk2) * a.head_dim; }
+
+// out[M, N] = epilogue(A[M, K] x W^T + bias) with A and out dense.  `e` brings the epilogue fields (epi, resid, gate,
+// stats_out / stats_mode); the statistics come one per N tile of gemm_tile_n(N).  An e4m3 weight takes two launches: the
+// per-row quantization of A into the workspace, then the FP8 GEMM.
+static int linear(ce_dit* h, cudaStream_t s, const Linear& w, const bf16* A, int M, int N, int K, bf16* out, GemmArgs e) {
+  GemmArgs g = e;
   g.M = M; g.N = N; g.K = K;
-  g.out = out; g.ldo = ldo;
-  g.bias = W_BF16(wname + ".bias");
-  g.epi = epi;
-  g.resid = resid; g.ldr = ldr;
-  g.gate = gate; g.gate_stride = gate_stride; g.rows_per_batch = rows_per_batch;
-  const WeightRef& w = h->w.at(wname + ".weight");
-  if (w.dtype == 2) {   // FP8 mode: quantize A per row into the workspace, then the e4m3 GEMM (one launch more than bf16)
-    prof_begin(h, CAT_ROWS, 3.0 * M * (double)K + 4.0 * M, s);
-    int rc = launch_quantize_rows_fp8(A, lda, M, K, h->fp8_q, K, h->fp8_scale, s);
-    if (rc) return rc;
-    prof_end(h, s);
-    ++h->launches;
-    prof_begin(h, CAT_GEMM, 2.0 * M * (double)N * K, s);
-    rc = launch_gemm_fp8(reinterpret_cast<const e4m3*>(h->fp8_q), K, h->fp8_scale, reinterpret_cast<const e4m3*>(w.ptr), K,
-                         W_F32(wname + ".weight_scale"), g, s);
-    if (rc == 0) prof_end(h, s);
-    return rc;
+  g.out = out; g.ldo = N;
+  g.bias = w.bias;
+  if (g.stats_out) g.stats_ld = (N + gemm_tile_n(N) - 1) / gemm_tile_n(N);
+  if (w.dtype == 2) {
+    LAUNCH(CAT_ROWS, 3.0 * M * (double)K + 4.0 * M, launch_quantize_rows_fp8(A, K, M, K, h->fp8_q, K, h->fp8_scale, s));
+    LAUNCH(CAT_GEMM, 2.0 * M * (double)N * K,
+           launch_gemm_fp8(reinterpret_cast<const e4m3*>(h->fp8_q), K, h->fp8_scale, static_cast<const e4m3*>(w.weight), K,
+                           w.weight_scale, g, s));
+  } else {
+    LAUNCH(CAT_GEMM, 2.0 * M * (double)N * K, launch_gemm_bf16(A, K, static_cast<const bf16*>(w.weight), K, g, s));
   }
-  prof_begin(h, CAT_GEMM, 2.0 * M * (double)N * K, s);
-  int rc = launch_gemm_bf16(A, lda, reinterpret_cast<const bf16*>(w.ptr), K, g, s);
-  if (rc == 0) prof_end(h, s);
-  return rc;
-}
-static int attention(ce_dit* h, const AttnArgs& a, cudaStream_t s) {
-  prof_begin(h, CAT_ATTN, 4.0 * a.B * a.H * (double)a.Lq * (a.Lk + a.Lk2) * a.head_dim, s);
-  int rc = launch_attention(a, s);
-  if (rc == 0) prof_end(h, s);
-  return rc;
+  return CE_OK;
 }
 
 // ---- internals shared with dit_fp32.cu
@@ -424,27 +453,16 @@ int ce_dit_set_weight(ce_dit* h, const char* name, const void* ptr, int dtype, i
 
 int ce_dit_weights_complete(const ce_dit* h) {
   CE_REQUIRE(h, "null handle");
-  const bool fp8 = holds_fp8(h);
-  for (const WeightSpec& s : required_weights(h->cfg, fp8)) {
-    auto it = h->w.find(s.name);
-    if (it == h->w.end()) return fail(CE_ERR_MISSING_WEIGHT, "missing weight: " + s.name);
-    if (it->second.dtype != s.dtype)
-      return fail(CE_ERR_MISSING_WEIGHT, "weight " + s.name + " has dtype " + std::to_string(it->second.dtype) + ", expected " +
-                                             std::to_string(s.dtype) + " (0 bf16, 1 fp32, 2 e4m3" +
-                                             (s.dtype == 2 || it->second.dtype == 2
-                                                  ? "; the six block GEMM weights of every layer are either all bf16 or all e4m3)"
-                                                  : ")"));
-    if (it->second.numel != s.numel)
-      return fail(CE_ERR_MISSING_WEIGHT, "weight " + s.name + " has " + std::to_string(it->second.numel) + " elements, expected " +
-                                             std::to_string(s.numel));
-  }
-  return CE_OK;
+  Weights w;
+  return resolve_weights(h, w);
 }
 
 int64_t ce_dit_workspace_bytes(const ce_dit* h, int batch, int frames, int height, int width, int text_len) {
   if (!h || validate_geometry(h, batch, frames, height, width, text_len)) return -1;
+  Weights w;
+  resolve_weights(h, w);   // only w.fp8 is read here, and it is set even before every weight has been registered
   const int L = frames * (height / h->cfg.patch_h) * (width / h->cfg.patch_w);
-  return carve(h->cfg, nullptr, batch, L, text_len, 257, holds_fp8(h)).bytes;
+  return carve(h->cfg, nullptr, batch, L, text_len, 257, w.fp8).bytes;
 }
 
 int64_t ce_dit_last_launch_count(const ce_dit* h) { return h ? h->launches : 0; }
@@ -545,7 +563,8 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   int rc = check_device();
   if (rc) return rc;
   if ((rc = validate_geometry(h, batch, frames, height, width, text_len))) return rc;
-  if ((rc = ce_dit_weights_complete(h))) return rc;
+  Weights W;
+  if ((rc = resolve_weights(h, W))) return rc;
   const ce_dit_config& c = h->cfg;
   CE_REQUIRE((c.image_dim > 0) == (encoder_hidden_states_image != nullptr),
              "ce_dit_forward: encoder_hidden_states_image must be given iff the model has an image embedder");
@@ -564,9 +583,8 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   const int L = spx ? Lfull / sp.world : Lfull, tok0 = spx ? sp.rank * L : 0, M = B * L;
   const SpLayout lay = spx ? sp_layout(B, Lfull, D, No, sp.world) : SpLayout();
   if (spx && lay.bytes > sp.region_bytes) return fail(CE_ERR_WORKSPACE, "sequence parallel: peer region too small (ce_dit_sp_region_bytes)");
-  const bool fp8 = holds_fp8(h);
-  CE_REQUIRE(!(spx && fp8), "sequence parallelism is not built for FP8 weights: run the FP8 mode on one GPU");
-  Workspace ws = carve(c, workspace, B, L, Lt, Li, fp8);
+  CE_REQUIRE(!(spx && W.fp8), "sequence parallelism is not built for FP8 weights: run the FP8 mode on one GPU");
+  Workspace ws = carve(c, workspace, B, L, Lt, Li, W.fp8);
   if (ws.bytes > workspace_bytes)
     return fail(CE_ERR_WORKSPACE, "workspace too small: need " + std::to_string(ws.bytes) + " bytes, got " + std::to_string(workspace_bytes));
   CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
@@ -584,61 +602,71 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   auto kv_text_of = [&](int layer) { return ctx_cache ? reinterpret_cast<bf16*>(reinterpret_cast<uint8_t*>(ctx_cache) + layer * ctx_layer_bytes) : ws.kv_text; };
   auto kv_img_of = [&](int layer) { return ctx_cache ? kv_text_of(layer) + kv_t_elems : ws.kv_img; };
   const bool ctx_compute = !(ctx_cache && ctx_reuse);
-  // Row statistics for the LayerNorms / RMSNorms come from the epilogue of the GEMM that wrote the row whenever the N tiles (256 wide)
-  // line up with the q | k | v boundaries; the row kernels are then streaming passes (elementwise.cuh).  CE_DIT_STATS=0: the
-  // round-1 kernels that reduce over the row themselves (A/B, and the path for widths that are not a multiple of 256).
-  static const bool stats_env = [] {
-    const char* e = getenv("CE_DIT_STATS");
-    return !(e && e[0] == '0');
-  }();
-  const bool st = stats_env && D % 256 == 0 && D / 256 <= 32;
+  // Row statistics for the LayerNorms / RMSNorms inside the blocks come from the epilogue of the GEMM that wrote the row whenever
+  // the N tiles (256 wide) line up with the q | k | v boundaries; the row kernels are then streaming passes (elementwise.cuh).
+  // Other widths take the kernels that reduce over the row themselves.  The row kernels of both kinds take D <= 8192.
+  const bool st = D % 256 == 0;
   const int tD = D / 256;
   auto ln = [&](const bf16* x, bf16* y, const float* scale, const float* shift, int mod_stride, int rpb, const float* w, const float* b, int is1p) {
     return st ? launch_layernorm_stats(x, D, y, D, M, D, c.eps, scale, shift, mod_stride, rpb, w, b, is1p, ws.stats_x, tD, tD, 256, s)
               : launch_layernorm(x, D, y, D, M, D, c.eps, scale, shift, mod_stride, rpb, w, b, s, is1p);
   };
+  // linear() epilogues: `stats` receives the output's row statistics (mode 1 for a LayerNorm, 2 for an RMSNorm) on the
+  // statistics path; the residual ones update the residual stream ws.x in place, gated by a modulation chunk [B, 6D] or not
+  auto epi = [&](int e, float2* stats = nullptr, int mode = 0) {
+    GemmArgs g;
+    g.epi = e;
+    if (st && stats) {
+      g.stats_out = stats;
+      g.stats_mode = mode;
+    }
+    return g;
+  };
+  auto resid_epi = [&](const float* gate) {
+    GemmArgs g = epi(gate ? EPI_BIAS_GATE_RESID : EPI_BIAS_RESID, ws.stats_x, 1);
+    g.resid = ws.x; g.ldr = D;
+    if (gate) {
+      g.gate = gate; g.gate_stride = 6 * D; g.rows_per_batch = L;
+    }
+    return g;
+  };
   h->launches = 0;
   const float attn_scale = 1.0f / sqrtf((float)c.attention_head_dim);
-  const std::string ce_ = "condition_embedder.";
 
   // ---- patch embedding (Conv3d k=s=(1,2,2) as im2row + GEMM, :429-430)
-  if (spx) RUN(launch_patchify_range(reinterpret_cast<const bf16*>(hidden_states), ws.patches, B, c.in_channels, frames, height, width, tok0, L, s));
-  else RUN(launch_patchify(reinterpret_cast<const bf16*>(hidden_states), ws.patches, B, c.in_channels, frames, height, width, s));
-  RUN2(linear(h, ws.patches, Kp, "patch_embedding", M, D, Kp, ws.x, D, EPI_BIAS, nullptr, 0, nullptr, 0, 1, s, st ? ws.stats_x : nullptr, 1));
+  if (spx) LAUNCH(CAT_OTHER, 0.0, launch_patchify_range(reinterpret_cast<const bf16*>(hidden_states), ws.patches, B, c.in_channels, frames, height, width, tok0, L, s));
+  else LAUNCH(CAT_OTHER, 0.0, launch_patchify(reinterpret_cast<const bf16*>(hidden_states), ws.patches, B, c.in_channels, frames, height, width, s));
+  if ((rc = linear(h, s, W.patch, ws.patches, M, D, Kp, ws.x, epi(EPI_BIAS, ws.stats_x, 1)))) return rc;
 
   // ---- condition embedder (:147-165)
-  RUN(launch_timestep_sinusoid(timestep, ws.sin_emb, B, c.freq_dim, s));
-  RUN(launch_small_linear(ws.sin_emb, c.freq_dim, W_F32(ce_ + "time_embedder.linear_1.weight"), W_F32(ce_ + "time_embedder.linear_1.bias"),
-                          0, D, B, /*act=*/1, 0, ws.h1, nullptr, s));
-  RUN(launch_small_linear(ws.h1, D, W_F32(ce_ + "time_embedder.linear_2.weight"), W_F32(ce_ + "time_embedder.linear_2.bias"), 0, D, B, 0, 0,
-                          ws.temb_f32, ws.temb_bf16, s));  // temb = (...).type_as(bf16)
-  RUN(launch_small_linear(ws.temb_f32, D, W_BF16(ce_ + "time_proj.weight"), W_BF16(ce_ + "time_proj.bias"), 1, 6 * D, B, 0, /*in_silu_bf16=*/1,
-                          nullptr, ws.tproj, s));
-  RUN(launch_add_table(W_F32("blocks.scale_shift_table"), c.num_layers, ws.tproj, 6 * D, ws.mod, B, D, 6, s, /*scale chunks 1,4 -> 1+scale*/ 0x12u));
-  RUN(launch_add_table(W_F32("scale_shift_table"), 1, ws.temb_bf16, D, ws.modf, B, D, 2, s, /*chunk 1 = scale*/ 0x2u));
+  LAUNCH(CAT_OTHER, 0.0, launch_timestep_sinusoid(timestep, ws.sin_emb, B, c.freq_dim, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_small_linear(ws.sin_emb, c.freq_dim, W.time1_w, W.time1_b, 0, D, B, /*act=*/1, 0, ws.h1, nullptr, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_small_linear(ws.h1, D, W.time2_w, W.time2_b, 0, D, B, 0, 0, ws.temb_f32, ws.temb_bf16, s));  // temb = (...).type_as(bf16)
+  LAUNCH(CAT_OTHER, 0.0, launch_small_linear(ws.temb_f32, D, W.time_proj_w, W.time_proj_b, 1, 6 * D, B, 0, /*in_silu_bf16=*/1, nullptr, ws.tproj, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_add_table(W.block_table, c.num_layers, ws.tproj, 6 * D, ws.mod, B, D, 6, s, /*scale chunks 1,4 -> 1+scale*/ 0x12u));
+  LAUNCH(CAT_OTHER, 0.0, launch_add_table(W.head_table, 1, ws.temb_bf16, D, ws.modf, B, D, 2, s, /*chunk 1 = scale*/ 0x2u));
   // text: Linear -> GELU(tanh) -> Linear
   if (ctx_compute) {
-  RUN2(linear(h, reinterpret_cast<const bf16*>(encoder_hidden_states), c.text_dim, ce_ + "text_embedder.linear_1", B * Lt, D, c.text_dim,
-             ws.text1, D, EPI_BIAS_GELU_TANH, nullptr, 0, nullptr, 0, 1, s));
-  RUN2(linear(h, ws.text1, D, ce_ + "text_embedder.linear_2", B * Lt, D, D, ws.ctx_text, D, EPI_BIAS, nullptr, 0, nullptr, 0, 1, s));
+    const bf16* text = reinterpret_cast<const bf16*>(encoder_hidden_states);
+    if ((rc = linear(h, s, W.text1, text, B * Lt, D, c.text_dim, ws.text1, epi(EPI_BIAS_GELU_TANH)))) return rc;
+    if ((rc = linear(h, s, W.text2, ws.text1, B * Lt, D, D, ws.ctx_text, epi(EPI_BIAS)))) return rc;
   }
   if (ctx_compute && c.image_dim > 0) {  // image: FP32LayerNorm -> Linear -> GELU(erf) -> Linear -> FP32LayerNorm (:111-123)
     const int I = c.image_dim;
-    RUN(launch_layernorm(reinterpret_cast<const bf16*>(encoder_hidden_states_image), I, ws.img0, I, B * Li, I, 1e-5f, nullptr, nullptr, 0, 0,
-                         W_F32(ce_ + "image_embedder.norm1.weight"), W_F32(ce_ + "image_embedder.norm1.bias"), s));
-    RUN2(linear(h, ws.img0, I, ce_ + "image_embedder.ff.net.0.proj", B * Li, I, I, ws.img1, I, EPI_BIAS_GELU_ERF, nullptr, 0, nullptr, 0, 1, s));
-    RUN2(linear(h, ws.img1, I, ce_ + "image_embedder.ff.net.2", B * Li, D, I, ws.img2, D, EPI_BIAS, nullptr, 0, nullptr, 0, 1, s));
-    RUN(launch_layernorm(ws.img2, D, ws.ctx_img, D, B * Li, D, 1e-5f, nullptr, nullptr, 0, 0, W_F32(ce_ + "image_embedder.norm2.weight"),
-                         W_F32(ce_ + "image_embedder.norm2.bias"), s));
+    LAUNCH(CAT_OTHER, 0.0, launch_layernorm(reinterpret_cast<const bf16*>(encoder_hidden_states_image), I, ws.img0, I, B * Li, I, 1e-5f, nullptr, nullptr, 0, 0,
+                                            W.img_norm1_w, W.img_norm1_b, s));
+    if ((rc = linear(h, s, W.img_ff0, ws.img0, B * Li, I, I, ws.img1, epi(EPI_BIAS_GELU_ERF)))) return rc;
+    if ((rc = linear(h, s, W.img_ff2, ws.img1, B * Li, D, I, ws.img2, epi(EPI_BIAS)))) return rc;
+    LAUNCH(CAT_OTHER, 0.0, launch_layernorm(ws.img2, D, ws.ctx_img, D, B * Li, D, 1e-5f, nullptr, nullptr, 0, 0, W.img_norm2_w, W.img_norm2_b, s));
   }
 
   // ---- transformer blocks (:447-448)
   for (int i = 0; i < c.num_layers; ++i) {
-    const std::string p = "blocks." + std::to_string(i) + ".";
+    const LayerWeights& lw = W.layers[i];
     const float* mod = ws.mod + (size_t)i * B * 6 * D;  // [B, 6, D]: shift, scale, gate, c_shift, c_scale, c_gate
     // 1. self-attention
-    RUNC(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, mod + 1 * D, mod + 0 * D, 6 * D, L, nullptr, nullptr, 1));
-    RUN2(linear(h, ws.xn, D, p + "attn1.to_qkv", M, 3 * D, D, ws.qkv, 3 * D, EPI_BIAS, nullptr, 0, nullptr, 0, 1, s, st ? ws.stats_qkv : nullptr, 2));
+    LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, mod + 1 * D, mod + 0 * D, 6 * D, L, nullptr, nullptr, 1));
+    if ((rc = linear(h, s, lw.qkv, ws.xn, M, 3 * D, D, ws.qkv, epi(EPI_BIAS, ws.stats_qkv, 2)))) return rc;
     const bf16* attn_in = ws.attn;
     if (spx) {
       // heads <-> tokens exchange by peer stores: q | k normalised + rotated and scattered by head, v scattered by head, barrier,
@@ -652,10 +680,10 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
         sc.dst[1][w] = reinterpret_cast<bf16*>(sp.region[w] + lay.k);
         vdst[w] = reinterpret_cast<bf16*>(sp.region[w] + lay.v);
       }
-      RUN(launch_rmsnorm_rope_stats(ws.qkv, 3 * D, M, D, c.eps, W_BF16(p + "attn1.norm_q.weight"), W_BF16(p + "attn1.norm_k.weight"), 2, h->rope_cos,
-                                    h->rope_sin, Lfull, c.attention_head_dim, ws.stats_qkv, 3 * tD, tD, s, &sc));
-      RUN(launch_sp_scatter_cols(ws.qkv + 2 * D, 3 * D, B, L, D, vdst, sp.world, Dl, Lfull, tok0, s));
-      RUN(launch_sp_barrier(sp, lay, s));
+      LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope_stats(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, Lfull,
+                                                       c.attention_head_dim, ws.stats_qkv, 3 * tD, tD, s, &sc));
+      LAUNCH(CAT_OTHER, 0.0, launch_sp_scatter_cols(ws.qkv + 2 * D, 3 * D, B, L, D, vdst, sp.world, Dl, Lfull, tok0, s));
+      LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));
       AttnArgs a;
       a.B = B; a.H = Hl; a.Lq = Lfull; a.Lk = Lfull;
       a.q = reinterpret_cast<const bf16*>(sp.region[sp.rank] + lay.q); a.ldq = Dl;
@@ -666,18 +694,17 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
       a.peer_rows = L;
       a.out_col0 = sp.rank * Dl;
       a.scale = attn_scale;
-      RUN2(attention(h, a, s));
-      RUN(launch_sp_barrier(sp, lay, s));
+      LAUNCH(CAT_ATTN, attention_flops(a), launch_attention(a, s));
+      LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));
       attn_in = reinterpret_cast<const bf16*>(sp.region[sp.rank] + lay.attn);
     } else {
-    if (st) {
-      RUNC(CAT_ROWS, 8.0 * M * D, launch_rmsnorm_rope_stats(ws.qkv, 3 * D, M, D, c.eps, W_BF16(p + "attn1.norm_q.weight"), W_BF16(p + "attn1.norm_k.weight"), 2,
-                                                             h->rope_cos, h->rope_sin, L, c.attention_head_dim, ws.stats_qkv, 3 * tD, tD, s));
-    } else {
-      RUNC(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(ws.qkv, 3 * D, M, D, c.eps, W_BF16(p + "attn1.norm_q.weight"), h->rope_cos, h->rope_sin, L, c.attention_head_dim, s));
-      RUNC(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(ws.qkv + D, 3 * D, M, D, c.eps, W_BF16(p + "attn1.norm_k.weight"), h->rope_cos, h->rope_sin, L, c.attention_head_dim, s));
-    }
-    {
+      if (st) {
+        LAUNCH(CAT_ROWS, 8.0 * M * D, launch_rmsnorm_rope_stats(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, L,
+                                                                c.attention_head_dim, ws.stats_qkv, 3 * tD, tD, s));
+      } else {
+        LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, h->rope_cos, h->rope_sin, L, c.attention_head_dim, s));
+        LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(ws.qkv + D, 3 * D, M, D, c.eps, lw.norm_k1, h->rope_cos, h->rope_sin, L, c.attention_head_dim, s));
+      }
       AttnArgs a;
       a.B = B; a.H = H; a.Lq = L; a.Lk = L;
       a.q = ws.qkv; a.ldq = 3 * D;
@@ -685,28 +712,27 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
       a.v = ws.qkv + 2 * D; a.ldv = 3 * D;
       a.out = ws.attn; a.ldo = D;
       a.scale = attn_scale;
-      RUN2(attention(h, a, s));
+      LAUNCH(CAT_ATTN, attention_flops(a), launch_attention(a, s));
     }
-    }
-    RUN2(linear(h, attn_in, D, p + "attn1.to_out.0", M, D, D, ws.x, D, EPI_BIAS_GATE_RESID, ws.x, D, mod + 2 * D, 6 * D, L, s, st ? ws.stats_x : nullptr, 1));
+    if ((rc = linear(h, s, lw.out1, attn_in, M, D, D, ws.x, resid_epi(mod + 2 * D)))) return rc;
     // 2. cross-attention
-    RUNC(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, nullptr, nullptr, 0, 0, W_F32(p + "norm2.weight"), W_F32(p + "norm2.bias"), 0));
+    LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, nullptr, nullptr, 0, 0, lw.norm2_w, lw.norm2_b, 0));
     bf16* q2 = ws.qkv;  // [M, D]
-    RUN2(linear(h, ws.xn, D, p + "attn2.to_q", M, D, D, q2, D, EPI_BIAS, nullptr, 0, nullptr, 0, 1, s, st ? ws.stats_q2 : nullptr, 2));
+    if ((rc = linear(h, s, lw.q2, ws.xn, M, D, D, q2, epi(EPI_BIAS, ws.stats_q2, 2)))) return rc;
     if (st) {
-      RUNC(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope_stats(q2, D, M, D, c.eps, W_BF16(p + "attn2.norm_q.weight"), nullptr, 1, nullptr, nullptr, 0,
-                                                             c.attention_head_dim, ws.stats_q2, tD, tD, s));
+      LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope_stats(q2, D, M, D, c.eps, lw.norm_q2, nullptr, 1, nullptr, nullptr, 0, c.attention_head_dim,
+                                                              ws.stats_q2, tD, tD, s));
     } else {
-      RUNC(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(q2, D, M, D, c.eps, W_BF16(p + "attn2.norm_q.weight"), nullptr, nullptr, 0, c.attention_head_dim, s));
+      LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(q2, D, M, D, c.eps, lw.norm_q2, nullptr, nullptr, 0, c.attention_head_dim, s));
     }
     bf16* kv_text = kv_text_of(i);
     bf16* kv_img = kv_img_of(i);
     if (ctx_compute) {
-      RUN2(linear(h, ws.ctx_text, D, p + "attn2.to_kv", B * Lt, 2 * D, D, kv_text, 2 * D, EPI_BIAS, nullptr, 0, nullptr, 0, 1, s));
-      RUN(launch_rmsnorm_rope(kv_text, 2 * D, B * Lt, D, c.eps, W_BF16(p + "attn2.norm_k.weight"), nullptr, nullptr, 0, c.attention_head_dim, s));
+      if ((rc = linear(h, s, lw.kv, ws.ctx_text, B * Lt, 2 * D, D, kv_text, epi(EPI_BIAS)))) return rc;
+      LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(kv_text, 2 * D, B * Lt, D, c.eps, lw.norm_k2, nullptr, nullptr, 0, c.attention_head_dim, s));
       if (c.image_dim > 0) {
-        RUN2(linear(h, ws.ctx_img, D, p + "attn2.add_kv_proj", B * Li, 2 * D, D, kv_img, 2 * D, EPI_BIAS, nullptr, 0, nullptr, 0, 1, s));
-        RUN(launch_rmsnorm_rope(kv_img, 2 * D, B * Li, D, c.eps, W_BF16(p + "attn2.norm_added_k.weight"), nullptr, nullptr, 0, c.attention_head_dim, s));
+        if ((rc = linear(h, s, lw.add_kv, ws.ctx_img, B * Li, 2 * D, D, kv_img, epi(EPI_BIAS)))) return rc;
+        LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(kv_img, 2 * D, B * Li, D, c.eps, lw.norm_added_k, nullptr, nullptr, 0, c.attention_head_dim, s));
       }
     }
     {  // text and image cross-attention in ONE launch: two key/value sources, two softmaxes, results added (:84-104)
@@ -722,13 +748,13 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
       }
       a.out = ws.attn; a.ldo = D;
       a.scale = attn_scale;
-      RUN2(attention(h, a, s));
+      LAUNCH(CAT_ATTN, attention_flops(a), launch_attention(a, s));
     }
-    RUN2(linear(h, ws.attn, D, p + "attn2.to_out.0", M, D, D, ws.x, D, EPI_BIAS_RESID, ws.x, D, nullptr, 0, 1, s, st ? ws.stats_x : nullptr, 1));
+    if ((rc = linear(h, s, lw.out2, ws.attn, M, D, D, ws.x, resid_epi(nullptr)))) return rc;
     // 3. feed-forward
-    RUNC(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, mod + 4 * D, mod + 3 * D, 6 * D, L, nullptr, nullptr, 1));
-    RUN2(linear(h, ws.xn, D, p + "ffn.net.0.proj", M, F, D, ws.hbuf, F, EPI_BIAS_GELU_TANH, nullptr, 0, nullptr, 0, 1, s));
-    RUN2(linear(h, ws.hbuf, F, p + "ffn.net.2", M, D, F, ws.x, D, EPI_BIAS_GATE_RESID, ws.x, D, mod + 5 * D, 6 * D, L, s, st ? ws.stats_x : nullptr, 1));
+    LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, mod + 4 * D, mod + 3 * D, 6 * D, L, nullptr, nullptr, 1));
+    if ((rc = linear(h, s, lw.ffn1, ws.xn, M, F, D, ws.hbuf, epi(EPI_BIAS_GELU_TANH)))) return rc;
+    if ((rc = linear(h, s, lw.ffn2, ws.hbuf, M, D, F, ws.x, resid_epi(mod + 5 * D)))) return rc;
     if (i == 0 && block0_out)
       CE_CHECK_CUDA(cudaMemcpyAsync(block0_out, ws.x, (size_t)M * D * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
     for (const auto& cap : h->capture)
@@ -736,46 +762,30 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   }
 
   // ---- output head (:451-467): modf = [B, 2, D] with shift = chunk 0, scale = chunk 1
-  RUNC(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, ws.modf + D, ws.modf, 2 * D, L, nullptr, nullptr, 1));
-  RUN2(linear(h, ws.xn, D, "proj_out", M, No, D, ws.yout, No, EPI_BIAS, nullptr, 0, nullptr, 0, 1, s));
+  LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, ws.modf + D, ws.modf, 2 * D, L, nullptr, nullptr, 1));
+  if ((rc = linear(h, s, W.proj_out, ws.xn, M, No, D, ws.yout, epi(EPI_BIAS)))) return rc;
   if (spx) {   // every rank gets the whole head output (rows all-gathered by peer stores), then un-patchifies the full sample
     bf16* ydst[8];
     for (int w = 0; w < sp.world; ++w) ydst[w] = reinterpret_cast<bf16*>(sp.region[w] + lay.yout);
-    RUN(launch_sp_broadcast_rows(ws.yout, B, L, No, ydst, sp.world, Lfull, tok0, s));
-    RUN(launch_sp_barrier(sp, lay, s));
-    RUN(launch_unpatchify(reinterpret_cast<const bf16*>(sp.region[sp.rank] + lay.yout), No, reinterpret_cast<bf16*>(sample), B, c.out_channels, frames,
-                          height, width, s));
-    RUN(launch_sp_barrier(sp, lay, s));   // nobody overwrites a peer's yout (next forward) before it has been read
+    LAUNCH(CAT_OTHER, 0.0, launch_sp_broadcast_rows(ws.yout, B, L, No, ydst, sp.world, Lfull, tok0, s));
+    LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));
+    LAUNCH(CAT_OTHER, 0.0, launch_unpatchify(reinterpret_cast<const bf16*>(sp.region[sp.rank] + lay.yout), No, reinterpret_cast<bf16*>(sample), B,
+                                             c.out_channels, frames, height, width, s));
+    LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));   // nobody overwrites a peer's yout (next forward) before it has been read
     return CE_OK;
   }
-  RUN(launch_unpatchify(ws.yout, No, reinterpret_cast<bf16*>(sample), B, c.out_channels, frames, height, width, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_unpatchify(ws.yout, No, reinterpret_cast<bf16*>(sample), B, c.out_channels, frames, height, width, s));
   return CE_OK;
 }
 
 int64_t ce_dit_host_staging_bytes(const ce_dit* h, int batch, int frames, int height, int width, int text_len) {
   if (!h) return -1;
-  const ce_dit_config& c = h->cfg;
-  int64_t b = 0;
-  auto al = [](int64_t v) { return (v + 255) & ~int64_t(255); };
-  b += al((int64_t)batch * c.in_channels * frames * height * width * 2);
-  b += al((int64_t)batch * 4);
-  b += al((int64_t)batch * text_len * c.text_dim * 2);
-  b += al((int64_t)batch * 257 * (c.image_dim > 0 ? c.image_dim : 8) * 2);
-  b += al((int64_t)batch * c.out_channels * frames * height * width * 2);
-  return b;
+  return carve_staging(h->cfg, nullptr, batch, frames, height, width, text_len).bytes;
 }
 
 int64_t ce_dit_host_staging_sample_offset(const ce_dit* h, int batch, int frames, int height, int width, int text_len) {
   if (!h) return -1;
-  const ce_dit_config& c = h->cfg;
-  Bump b(nullptr);
-  b.take<bf16>((int64_t)batch * c.in_channels * frames * height * width);
-  b.take<float>(batch);
-  b.take<bf16>((int64_t)batch * text_len * c.text_dim);
-  const int64_t n_i = (int64_t)batch * 257 * c.image_dim;
-  b.take<bf16>(n_i > 0 ? n_i : 8);
-  b.off = (b.off + 255) & ~int64_t(255);
-  return b.off;
+  return carve_staging(h->cfg, nullptr, batch, frames, height, width, text_len).sample_offset;
 }
 
 int ce_dit_forward_host(ce_dit* h, const void* hidden_states_host, const float* timestep_host, const void* encoder_hidden_states_host,
@@ -790,29 +800,19 @@ int ce_dit_forward_host_ex(ce_dit* h, const void* hidden_states_host, const floa
                            int text_len, void* staging, int64_t staging_bytes, void* workspace, int64_t workspace_bytes, void* ctx_cache,
                            int64_t ctx_cache_bytes, int ctx_reuse, void* stream_v) {
   CE_REQUIRE(h && hidden_states_host && timestep_host && encoder_hidden_states_host && sample_host && staging, "ce_dit_forward_host: null argument");
-  const ce_dit_config& c = h->cfg;
-  CE_REQUIRE(staging_bytes >= ce_dit_host_staging_bytes(h, batch, frames, height, width, text_len), "ce_dit_forward_host: staging too small");
+  const Staging st = carve_staging(h->cfg, staging, batch, frames, height, width, text_len);
+  CE_REQUIRE(staging_bytes >= st.bytes, "ce_dit_forward_host: staging too small");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
-  Bump b(staging);
-  const int64_t n_x = (int64_t)batch * c.in_channels * frames * height * width;
-  const int64_t n_t = (int64_t)batch * text_len * c.text_dim;
-  const int64_t n_i = (int64_t)batch * 257 * c.image_dim;
-  const int64_t n_o = (int64_t)batch * c.out_channels * frames * height * width;
-  bf16* d_x = b.take<bf16>(n_x);
-  float* d_ts = b.take<float>(batch);
-  bf16* d_t = b.take<bf16>(n_t);
-  bf16* d_i = b.take<bf16>(n_i > 0 ? n_i : 8);
-  bf16* d_o = b.take<bf16>(n_o);
-  CE_CHECK_CUDA(cudaMemcpyAsync(d_x, hidden_states_host, n_x * 2, cudaMemcpyHostToDevice, s));
-  CE_CHECK_CUDA(cudaMemcpyAsync(d_ts, timestep_host, batch * 4, cudaMemcpyHostToDevice, s));
+  CE_CHECK_CUDA(cudaMemcpyAsync(st.x, hidden_states_host, st.n_x * 2, cudaMemcpyHostToDevice, s));
+  CE_CHECK_CUDA(cudaMemcpyAsync(st.timestep, timestep_host, batch * 4, cudaMemcpyHostToDevice, s));
   // the encoder states are copied every call (they are part of the call's inputs); with ctx_reuse the kernels do not read them
-  CE_CHECK_CUDA(cudaMemcpyAsync(d_t, encoder_hidden_states_host, n_t * 2, cudaMemcpyHostToDevice, s));
-  if (encoder_hidden_states_image_host && n_i > 0)
-    CE_CHECK_CUDA(cudaMemcpyAsync(d_i, encoder_hidden_states_image_host, n_i * 2, cudaMemcpyHostToDevice, s));
-  int rc = ce_dit_forward_ex(h, d_x, d_ts, d_t, (encoder_hidden_states_image_host && n_i > 0) ? d_i : nullptr, d_o, batch, frames, height, width,
+  CE_CHECK_CUDA(cudaMemcpyAsync(st.text, encoder_hidden_states_host, st.n_t * 2, cudaMemcpyHostToDevice, s));
+  const bool image = encoder_hidden_states_image_host && st.n_i > 0;
+  if (image) CE_CHECK_CUDA(cudaMemcpyAsync(st.image, encoder_hidden_states_image_host, st.n_i * 2, cudaMemcpyHostToDevice, s));
+  int rc = ce_dit_forward_ex(h, st.x, st.timestep, st.text, image ? st.image : nullptr, st.sample, batch, frames, height, width,
                              text_len, workspace, workspace_bytes, nullptr, ctx_cache, ctx_cache_bytes, ctx_reuse, stream_v);
   if (rc) return rc;
-  CE_CHECK_CUDA(cudaMemcpyAsync(sample_host, d_o, n_o * 2, cudaMemcpyDeviceToHost, s));
+  CE_CHECK_CUDA(cudaMemcpyAsync(sample_host, st.sample, st.n_o * 2, cudaMemcpyDeviceToHost, s));
   CE_CHECK_CUDA(cudaStreamSynchronize(s));
   return CE_OK;
 }
@@ -820,17 +820,17 @@ int ce_dit_forward_host_ex(ce_dit* h, const void* hidden_states_host, const floa
 // ---------------------------------------------------------------------------------------------- operator exports
 int ce_linear_bf16(const void* A, int lda, const void* W, int ldw, const void* bias, void* out, int ldo, float* out_f32, int M, int N,
                    int K, int epilogue, const void* resid, int ldr, const float* gate, int gate_stride, int rows_per_batch, void* stream) {
-  int rc = check_device();
-  if (rc) return rc;
-  GemmArgs g;
-  g.M = M; g.N = N; g.K = K;
-  g.out = reinterpret_cast<bf16*>(out); g.ldo = ldo;
-  g.out_f32 = out_f32;
-  g.bias = reinterpret_cast<const bf16*>(bias);
-  g.epi = epilogue;
-  g.resid = reinterpret_cast<const bf16*>(resid); g.ldr = ldr;
-  g.gate = gate; g.gate_stride = gate_stride; g.rows_per_batch = rows_per_batch > 0 ? rows_per_batch : 1;
-  return launch_gemm_bf16(reinterpret_cast<const bf16*>(A), lda, reinterpret_cast<const bf16*>(W), ldw, g, reinterpret_cast<cudaStream_t>(stream));
+  ce_linear_args a = {};
+  a.A = A; a.lda = lda;
+  a.W = W; a.ldw = ldw;
+  a.M = M; a.N = N; a.K = K;
+  a.out = out; a.ldo = ldo;
+  a.out_f32 = out_f32;
+  a.bias = bias;
+  a.epilogue = epilogue;
+  a.resid = resid; a.ldr = ldr;
+  a.gate = gate; a.gate_stride = gate_stride; a.rows_per_batch = rows_per_batch;
+  return ce_linear_ex_bf16(&a, stream);
 }
 
 static GemmArgs gemm_args_of(const ce_linear_args* a) {

@@ -22,12 +22,6 @@ using namespace ce;
 
 namespace {
 
-constexpr int TPB = 256;
-inline int grid_for(size_t n) {
-  size_t g = (n + TPB - 1) / TPB;
-  return (int)(g < device_sm_count() * 16 ? (g ? g : 1) : device_sm_count() * 16);
-}
-
 // out[r, :] (bf16, 3*Kp wide) from x[r, 0:K] fp32 (leading dim ldx); A layout [hi | lo | hi], W layout [hi | hi | lo]; columns
 // K..Kp-1 of each third are zero
 __global__ void split3_kernel(const float* __restrict__ x, int ldx, int rows, int K, int Kp, bf16* __restrict__ out, int w_layout) {
@@ -201,20 +195,6 @@ __global__ void add_inplace_kernel(float* __restrict__ a, const float* __restric
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) a[i] += b[i];
 }
 
-struct Bump32 {
-  uint8_t* base;
-  int64_t off = 0;
-  explicit Bump32(void* b) : base(reinterpret_cast<uint8_t*>(b)) {}
-  template <typename T>
-  T* take(int64_t n) {
-    off = (off + 255) & ~int64_t(255);
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += n * (int64_t)sizeof(T);
-    return p;
-  }
-};
-inline int up8(int v) { return (v + 7) & ~7; }
-
 struct Ws32 {
   float *x, *xn, *q, *k, *v, *attn, *attn2, *h, *patches, *yout, *text1, *ctx_text, *img0, *img1, *img2, *ctx_img, *kt, *vt, *ki, *vi;
   float *sin_emb, *h1, *temb, *tproj, *mod, *modf, *S, *P;
@@ -225,7 +205,7 @@ struct Ws32 {
 Ws32 carve32(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li) {
   const int64_t D = (int64_t)c.num_attention_heads * c.attention_head_dim, F = c.ffn_dim, M = (int64_t)B * L;
   const int64_t Kp = (int64_t)c.in_channels * 4, No = (int64_t)c.out_channels * 4, I = c.image_dim > 0 ? c.image_dim : 8;
-  Bump32 b(base);
+  Bump b(base);
   Ws32 w;
   w.x = b.take<float>(M * D); w.xn = b.take<float>(M * D); w.q = b.take<float>(M * D); w.k = b.take<float>(M * D); w.v = b.take<float>(M * D);
   w.attn = b.take<float>(M * D); w.attn2 = b.take<float>(M * D); w.h = b.take<float>(M * F);
@@ -244,7 +224,7 @@ Ws32 carve32(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li) {
   const int64_t a_elems = std::max<int64_t>(M, (int64_t)B * std::max(Lt, Li)) * 3 * up8((int)kmax);
   const int64_t w_elems = std::max<int64_t>(std::max<int64_t>(F, 6 * D), Lmax) * 3 * up8((int)kmax);
   w.Ap = b.take<bf16>(a_elems); w.Wp = b.take<bf16>(w_elems);
-  w.bytes = (b.off + 255) & ~int64_t(255);
+  w.bytes = b.bytes();
   return w;
 }
 

@@ -30,13 +30,6 @@ struct ce_encoder {
 
 namespace {
 
-constexpr int TPB = 256;
-inline int grid_for(size_t n) {
-  size_t g = (n + TPB - 1) / TPB;
-  return (int)(g < device_sm_count() * 16 ? (g ? g : 1) : device_sm_count() * 16);
-}
-inline int up8(int v) { return (v + 7) & ~7; }
-
 __global__ void embedding_kernel(const int64_t* __restrict__ ids, const bf16* __restrict__ table, bf16* __restrict__ out, int n, int D, int64_t vocab) {
   const size_t total = (size_t)n * (D / 8);
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -128,19 +121,6 @@ __global__ void clip_patchify_kernel(const bf16* __restrict__ px, bf16* __restri
   }
 }
 
-struct Bump {
-  uint8_t* base;
-  int64_t off = 0;
-  explicit Bump(void* b) : base(reinterpret_cast<uint8_t*>(b)) {}
-  template <typename T>
-  T* take(int64_t n) {
-    off = (off + 255) & ~int64_t(255);
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += n * (int64_t)sizeof(T);
-    return p;
-  }
-};
-
 struct EncWs {
   bf16 *x, *xn, *qk, *vT, *attn, *h0, *h1, *P, *patches, *pe;
   float* S;
@@ -162,7 +142,7 @@ EncWs carve(const ce_encoder_config& c, void* base, int B, int L) {
   const int64_t Kp = up8(3 * c.patch_size * c.patch_size);
   w.patches = b.take<bf16>(c.kind == 1 ? (int64_t)B * (L - 1) * Kp : 8);
   w.pe = b.take<bf16>(c.kind == 1 ? (int64_t)B * (L - 1) * D : 8);
-  w.bytes = (b.off + 255) & ~int64_t(255);
+  w.bytes = b.bytes();
   return w;
 }
 

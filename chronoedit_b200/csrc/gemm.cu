@@ -10,10 +10,6 @@
 // Replaces the cuBLASLt calls behind every nn.Linear of the reference DiT block
 // (chronoedit_diffusers/transformer_chronoedit.py:58-60, 84-87, 106, 292) plus the elementwise
 // launches that follow them (:281, :286, :293).
-#include <stdlib.h>
-
-#include <cstdlib>
-
 #include "gemm.cuh"
 #include "ring_gemm.cuh"
 
@@ -268,13 +264,6 @@ int launch_gemm(const T* A, int lda, const float* s_a, const T* W, int ldw, cons
   // Tiles are rasterised in groups of group_m M-tiles x all N-tiles so that the A panel of a group stays in L2 while the W
   // panels stream past it (16 M-tiles x 128 rows x K = 5120 is 20 MB of A, inside the H100's 50 MB L2).
   if (a.group_m <= 0) a.group_m = 16;
-  {
-    static const int env_gm = [] {   // developer knob (A/B)
-      const char* e = getenv("CE_GEMM_GROUP_M");
-      return e ? atoi(e) : 0;
-    }();
-    if (env_gm > 0) a.group_m = env_gm;
-  }
   const int bn = gemm_tile_n(a.N);
   const auto tmap = fp8 ? make_tmap_2d_u8 : make_tmap_2d;
   CUtensorMap ta, tb;

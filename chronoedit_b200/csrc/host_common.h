@@ -60,4 +60,30 @@ int ensure_dynamic_smem(const void* kernel, int bytes);
     if (_rc) return _rc;                                                                           \
   } while (0)  // CE_OK iff the current device is compute capability 9.x
 
+// ---- workspace carving and launch sizing -------------------------------------------------------
+// Hands out consecutive 256-byte aligned slices of one caller-owned buffer.  With a null base it only measures: every pointer
+// is null and `off` is the size so far, so one carve function serves both the size query and the forward.
+struct Bump {
+  uint8_t* base;
+  int64_t off = 0;
+  explicit Bump(void* b) : base(reinterpret_cast<uint8_t*>(b)) {}
+  template <typename T>
+  T* take(int64_t n) {
+    off = (off + 255) & ~int64_t(255);
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += n * (int64_t)sizeof(T);
+    return p;
+  }
+  int64_t bytes() const { return (off + 255) & ~int64_t(255); }
+};
+
+inline int up8(int v) { return (v + 7) & ~7; }
+
+// Blocks of TPB threads for a grid-stride loop over n elements: one per TPB elements, at most 16 per SM.
+constexpr int TPB = 256;
+inline int grid_for(size_t n) {
+  const size_t g = (n + TPB - 1) / TPB, cap = (size_t)device_sm_count() * 16;
+  return (int)(g < cap ? (g ? g : 1) : cap);
+}
+
 }  // namespace ce

@@ -76,11 +76,6 @@ __global__ void patchify_range_kernel(const bf16* __restrict__ x, bf16* __restri
   }
 }
 
-inline int grid_for(size_t n) {
-  size_t g = (n + 255) / 256;
-  return (int)(g < device_sm_count() * 16 ? (g ? g : 1) : device_sm_count() * 16);
-}
-
 }  // namespace
 
 SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world) {
