@@ -27,16 +27,10 @@ const std::string& last_error();
 
 using namespace ce;
 
-struct WeightRef {
-  const void* ptr = nullptr;
-  int dtype = 0;  // 0 bf16, 1 fp32, 2 e4m3 (FP8 mode's block weights)
-  int64_t numel = 0;
-};
-
 struct ce_dit {
   ce_dit_config cfg;
-  std::map<std::string, WeightRef> w;
-  std::map<std::string, WeightRef> w32;   // fp32 validation mode: every parameter in fp32 under its reference name
+  WeightMap w;     // dtype 2 (e4m3) for FP8 mode's block weights
+  WeightMap w32;   // fp32 validation mode: every parameter in fp32 under its reference name
   // RoPE tables, cached per latent geometry
   int rope_f = 0, rope_h = 0, rope_w = 0, rope_dev = -1;
   float* rope_cos = nullptr;
@@ -164,46 +158,15 @@ struct Weights {
   std::vector<LayerWeights> layers;
 };
 
-// Looks weights up one at a time, checking dtype and element count; the first one that is missing or wrong records
-// CE_ERR_MISSING_WEIGHT with its name, and every lookup after it returns null.
-struct WeightLookup {
-  const std::map<std::string, WeightRef>& w;
-  int rc = CE_OK;
-
-  const void* get(const std::string& name, int dtype, int64_t numel) {
-    if (rc) return nullptr;
-    auto it = w.find(name);
-    if (it == w.end()) {
-      rc = fail(CE_ERR_MISSING_WEIGHT, "missing weight: " + name);
-      return nullptr;
-    }
-    if (it->second.dtype != dtype) {
-      rc = fail(CE_ERR_MISSING_WEIGHT, "weight " + name + " has dtype " + std::to_string(it->second.dtype) + ", expected " +
-                                           std::to_string(dtype) + " (0 bf16, 1 fp32, 2 e4m3" +
-                                           (dtype == 2 || it->second.dtype == 2
-                                                ? "; the six block GEMM weights of every layer are either all bf16 or all e4m3)"
-                                                : ")"));
-      return nullptr;
-    }
-    if (it->second.numel != numel) {
-      rc = fail(CE_ERR_MISSING_WEIGHT, "weight " + name + " has " + std::to_string(it->second.numel) + " elements, expected " +
-                                           std::to_string(numel));
-      return nullptr;
-    }
-    return it->second.ptr;
-  }
-  const bf16* b16(const std::string& name, int64_t numel) { return static_cast<const bf16*>(get(name, 0, numel)); }
-  const float* f32(const std::string& name, int64_t numel) { return static_cast<const float*>(get(name, 1, numel)); }
-  // module `m` of shape [N, K]: "<m>.weight", for e4m3 "<m>.weight_scale", then "<m>.bias"
-  Linear linear(const std::string& m, int64_t N, int64_t K, bool e4m3 = false) {
-    Linear l;
-    l.dtype = e4m3 ? 2 : 0;
-    l.weight = get(m + ".weight", l.dtype, N * K);
-    if (e4m3) l.weight_scale = f32(m + ".weight_scale", N);
-    l.bias = b16(m + ".bias", N);
-    return l;
-  }
-};
+// module `m` of shape [N, K]: "<m>.weight", for e4m3 "<m>.weight_scale", then "<m>.bias"
+Linear lookup_linear(WeightLookup& r, const std::string& m, int64_t N, int64_t K, bool e4m3 = false) {
+  Linear l;
+  l.dtype = e4m3 ? 2 : 0;
+  l.weight = r.get(m + ".weight", l.dtype, N * K);
+  if (e4m3) l.weight_scale = r.f32(m + ".weight_scale", N);
+  l.bias = r.b16(m + ".bias", N);
+  return l;
+}
 
 int resolve_weights(const ce_dit* h, Weights& w) {
   const ce_dit_config& c = h->cfg;
@@ -213,7 +176,7 @@ int resolve_weights(const ce_dit* h, Weights& w) {
   auto qkv0 = h->w.find("blocks.0.attn1.to_qkv.weight");
   w.fp8 = qkv0 != h->w.end() && qkv0->second.dtype == 2;
   WeightLookup r{h->w};
-  w.patch = r.linear("patch_embedding", D, Kp);
+  w.patch = lookup_linear(r, "patch_embedding", D, Kp);
   const std::string ce_ = "condition_embedder.";
   w.time1_w = r.f32(ce_ + "time_embedder.linear_1.weight", D * c.freq_dim);
   w.time1_b = r.f32(ce_ + "time_embedder.linear_1.bias", D);
@@ -221,14 +184,14 @@ int resolve_weights(const ce_dit* h, Weights& w) {
   w.time2_b = r.f32(ce_ + "time_embedder.linear_2.bias", D);
   w.time_proj_w = r.b16(ce_ + "time_proj.weight", 6 * D * D);
   w.time_proj_b = r.b16(ce_ + "time_proj.bias", 6 * D);
-  w.text1 = r.linear(ce_ + "text_embedder.linear_1", D, c.text_dim);
-  w.text2 = r.linear(ce_ + "text_embedder.linear_2", D, D);
+  w.text1 = lookup_linear(r, ce_ + "text_embedder.linear_1", D, c.text_dim);
+  w.text2 = lookup_linear(r, ce_ + "text_embedder.linear_2", D, D);
   if (c.image_dim > 0) {
     const int64_t I = c.image_dim;
     w.img_norm1_w = r.f32(ce_ + "image_embedder.norm1.weight", I);
     w.img_norm1_b = r.f32(ce_ + "image_embedder.norm1.bias", I);
-    w.img_ff0 = r.linear(ce_ + "image_embedder.ff.net.0.proj", I, I);
-    w.img_ff2 = r.linear(ce_ + "image_embedder.ff.net.2", D, I);
+    w.img_ff0 = lookup_linear(r, ce_ + "image_embedder.ff.net.0.proj", I, I);
+    w.img_ff2 = lookup_linear(r, ce_ + "image_embedder.ff.net.2", D, I);
     w.img_norm2_w = r.f32(ce_ + "image_embedder.norm2.weight", D);
     w.img_norm2_b = r.f32(ce_ + "image_embedder.norm2.bias", D);
   }
@@ -237,26 +200,26 @@ int resolve_weights(const ce_dit* h, Weights& w) {
   for (int i = 0; i < c.num_layers; ++i) {
     const std::string p = "blocks." + std::to_string(i) + ".";
     LayerWeights& l = w.layers[i];
-    l.qkv = r.linear(p + "attn1.to_qkv", 3 * D, D, w.fp8);
+    l.qkv = lookup_linear(r, p + "attn1.to_qkv", 3 * D, D, w.fp8);
     l.norm_q1 = r.b16(p + "attn1.norm_q.weight", D);
     l.norm_k1 = r.b16(p + "attn1.norm_k.weight", D);
-    l.out1 = r.linear(p + "attn1.to_out.0", D, D, w.fp8);
+    l.out1 = lookup_linear(r, p + "attn1.to_out.0", D, D, w.fp8);
     l.norm2_w = r.f32(p + "norm2.weight", D);
     l.norm2_b = r.f32(p + "norm2.bias", D);
-    l.q2 = r.linear(p + "attn2.to_q", D, D, w.fp8);
+    l.q2 = lookup_linear(r, p + "attn2.to_q", D, D, w.fp8);
     l.norm_q2 = r.b16(p + "attn2.norm_q.weight", D);
     l.norm_k2 = r.b16(p + "attn2.norm_k.weight", D);
-    l.kv = r.linear(p + "attn2.to_kv", 2 * D, D);
+    l.kv = lookup_linear(r, p + "attn2.to_kv", 2 * D, D);
     if (c.image_dim > 0) {
-      l.add_kv = r.linear(p + "attn2.add_kv_proj", 2 * D, c.added_kv_proj_dim);
+      l.add_kv = lookup_linear(r, p + "attn2.add_kv_proj", 2 * D, c.added_kv_proj_dim);
       l.norm_added_k = r.b16(p + "attn2.norm_added_k.weight", D);
     }
-    l.out2 = r.linear(p + "attn2.to_out.0", D, D, w.fp8);
-    l.ffn1 = r.linear(p + "ffn.net.0.proj", F, D, w.fp8);
-    l.ffn2 = r.linear(p + "ffn.net.2", D, F, w.fp8);
+    l.out2 = lookup_linear(r, p + "attn2.to_out.0", D, D, w.fp8);
+    l.ffn1 = lookup_linear(r, p + "ffn.net.0.proj", F, D, w.fp8);
+    l.ffn2 = lookup_linear(r, p + "ffn.net.2", D, F, w.fp8);
   }
   w.head_table = r.f32("scale_shift_table", 2 * D);
-  w.proj_out = r.linear("proj_out", No, D);
+  w.proj_out = lookup_linear(r, "proj_out", No, D);
   return r.rc;
 }
 
@@ -386,11 +349,7 @@ static int linear(ce_dit* h, cudaStream_t s, const Linear& w, const bf16* A, int
 }
 
 // ---- internals shared with dit_fp32.cu
-const float* ce_dit_internal_weight_f32(const ce_dit* h, const std::string& name, int64_t expect_numel) {
-  auto it = h->w32.find(name);
-  if (it == h->w32.end() || it->second.numel != expect_numel) return nullptr;
-  return reinterpret_cast<const float*>(it->second.ptr);
-}
+const WeightMap& ce_dit_internal_weights_f32(const ce_dit* h) { return h->w32; }
 int ce_dit_internal_rope(ce_dit* h, int frames, int hp, int wp, cudaStream_t s, const float** cos_out, const float** sin_out) {
   int rc = ensure_rope(h, frames, hp, wp, s);
   if (rc) return rc;
@@ -405,14 +364,8 @@ extern "C" {
 int ce_abi_version(void) { return CE_ABI_VERSION; }
 
 int ce_dit_set_weight_fp32(ce_dit* h, const char* name, const float* ptr, int64_t numel) {
-  CE_REQUIRE(h && name && ptr, "ce_dit_set_weight_fp32: null argument");
-  CE_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "ce_dit_set_weight_fp32: pointer must be 16-byte aligned");
-  WeightRef r;
-  r.ptr = ptr;
-  r.dtype = 1;
-  r.numel = numel;
-  h->w32[name] = r;
-  return CE_OK;
+  CE_REQUIRE(h, "ce_dit_set_weight_fp32: null handle");
+  return register_weight(h->w32, "ce_dit_set_weight_fp32", name, ptr, 1, numel);
 }
 const char* ce_last_error(void) { return ce::last_error().c_str(); }
 int ce_device_check(void) { return check_device(); }
@@ -441,14 +394,8 @@ void ce_dit_destroy(ce_dit* h) {
 }
 
 int ce_dit_set_weight(ce_dit* h, const char* name, const void* ptr, int dtype, int64_t numel) {
-  CE_REQUIRE(h && name && ptr, "ce_dit_set_weight: null argument");
-  CE_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "ce_dit_set_weight: pointer must be 16-byte aligned");
-  WeightRef r;
-  r.ptr = ptr;
-  r.dtype = dtype;
-  r.numel = numel;
-  h->w[name] = r;
-  return CE_OK;
+  CE_REQUIRE(h, "ce_dit_set_weight: null handle");
+  return register_weight(h->w, "ce_dit_set_weight", name, ptr, dtype, numel);
 }
 
 int ce_dit_weights_complete(const ce_dit* h) {

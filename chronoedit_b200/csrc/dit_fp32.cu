@@ -13,6 +13,7 @@
 #include <math.h>
 
 #include <string>
+#include <vector>
 
 #include "../../include/chronoedit_b200.h"
 #include "elementwise.cuh"
@@ -130,27 +131,6 @@ __global__ void rmsnorm_rope_f32_kernel(float* __restrict__ x, int ldx, int rows
     xr[2 * p + 1] = im;
   }
 }
-// P[r, c] = softmax_c(S[r, c] * scale) over c < cols, 0 for cols <= c < ldp   (one block per row, fp32)
-__global__ void softmax_rows_f32_kernel(const float* __restrict__ S, int lds, float* __restrict__ P, int ldp, int cols, float scale) {
-  __shared__ float red[32];
-  const float* s = S + (size_t)blockIdx.x * lds;
-  float* p = P + (size_t)blockIdx.x * ldp;
-  float mx = -INFINITY;
-  for (int i = threadIdx.x; i < cols; i += blockDim.x) mx = fmaxf(mx, s[i]);
-  mx = warp_max(mx);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
-  __syncthreads();
-  mx = warp_max((threadIdx.x & 31) < (blockDim.x >> 5) ? red[threadIdx.x & 31] : -INFINITY);
-  __syncthreads();
-  float sum = 0.f;
-  for (int i = threadIdx.x; i < cols; i += blockDim.x) sum += expf((s[i] - mx) * scale);
-  sum = warp_sum(sum);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sum;
-  __syncthreads();
-  sum = warp_sum((threadIdx.x & 31) < (blockDim.x >> 5) ? red[threadIdx.x & 31] : 0.f);
-  const float inv = 1.0f / sum;
-  for (int i = threadIdx.x; i < ldp; i += blockDim.x) p[i] = i < cols ? expf((s[i] - mx) * scale) * inv : 0.f;
-}
 __global__ void patchify_f32_kernel(const float* __restrict__ x, float* __restrict__ patches, int B, int C, int T, int H, int W) {
   const int hp = H >> 1, wp = W >> 1, K = C * 4;
   const size_t total = (size_t)B * T * hp * wp * K;
@@ -228,65 +208,96 @@ Ws32 carve32(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li) {
   return w;
 }
 
-}  // namespace
+// One Linear of the fp32 model: weight [N, K], bias [N].
+struct Lin32 {
+  const float *w = nullptr, *b = nullptr;
+};
+struct Layer32 {
+  const float* table;   // scale_shift_table [6, D]
+  Lin32 q, k, v, out1, q2, k2, v2, add_k, add_v, out2, ffn1, ffn2;
+  const float *norm_q, *norm_k, *norm2_w, *norm2_b, *norm_q2, *norm_k2, *norm_added_k;
+};
+// Every fp32 parameter ce_dit_forward_fp32 reads, under its reference name.
+struct Weights32 {
+  Lin32 patch, time1, time2, time_proj, text1, text2, img_ff0, img_ff2, proj_out;
+  const float *img_norm1_w{}, *img_norm1_b{}, *img_norm2_w{}, *img_norm2_b{}, *head_table{};
+  std::vector<Layer32> layers;
+};
 
-// handle internals (dit.cu)
-const float* ce_dit_internal_weight_f32(const ce_dit* h, const std::string& name, int64_t expect_numel);
-int ce_dit_internal_rope(ce_dit* h, int frames, int hp, int wp, cudaStream_t s, const float** cos_out, const float** sin_out);
-const ce_dit_config* ce_dit_internal_config(const ce_dit* h);
+int resolve_weights32(const WeightMap& map, const ce_dit_config& c, Weights32& w) {
+  const int64_t D = (int64_t)c.num_attention_heads * c.attention_head_dim, F = c.ffn_dim, I = c.image_dim;
+  WeightLookup r{map};
+  auto lin = [&](const std::string& m, int64_t N, int64_t K) { return Lin32{r.f32(m + ".weight", N * K), r.f32(m + ".bias", N)}; };
+  const std::string ce_ = "condition_embedder.";
+  w.patch = lin("patch_embedding", D, (int64_t)c.in_channels * 4);
+  w.time1 = lin(ce_ + "time_embedder.linear_1", D, c.freq_dim);
+  w.time2 = lin(ce_ + "time_embedder.linear_2", D, D);
+  w.time_proj = lin(ce_ + "time_proj", 6 * D, D);
+  w.text1 = lin(ce_ + "text_embedder.linear_1", D, c.text_dim);
+  w.text2 = lin(ce_ + "text_embedder.linear_2", D, D);
+  if (I > 0) {
+    w.img_norm1_w = r.f32(ce_ + "image_embedder.norm1.weight", I);
+    w.img_norm1_b = r.f32(ce_ + "image_embedder.norm1.bias", I);
+    w.img_ff0 = lin(ce_ + "image_embedder.ff.net.0.proj", I, I);
+    w.img_ff2 = lin(ce_ + "image_embedder.ff.net.2", D, I);
+    w.img_norm2_w = r.f32(ce_ + "image_embedder.norm2.weight", D);
+    w.img_norm2_b = r.f32(ce_ + "image_embedder.norm2.bias", D);
+  }
+  for (int i = 0; i < c.num_layers; ++i) {
+    const std::string p = "blocks." + std::to_string(i) + ".";
+    Layer32 l{};
+    l.table = r.f32(p + "scale_shift_table", 6 * D);
+    l.q = lin(p + "attn1.to_q", D, D);
+    l.k = lin(p + "attn1.to_k", D, D);
+    l.v = lin(p + "attn1.to_v", D, D);
+    l.norm_q = r.f32(p + "attn1.norm_q.weight", D);
+    l.norm_k = r.f32(p + "attn1.norm_k.weight", D);
+    l.out1 = lin(p + "attn1.to_out.0", D, D);
+    l.norm2_w = r.f32(p + "norm2.weight", D);
+    l.norm2_b = r.f32(p + "norm2.bias", D);
+    l.q2 = lin(p + "attn2.to_q", D, D);
+    l.norm_q2 = r.f32(p + "attn2.norm_q.weight", D);
+    l.k2 = lin(p + "attn2.to_k", D, D);
+    l.v2 = lin(p + "attn2.to_v", D, D);
+    l.norm_k2 = r.f32(p + "attn2.norm_k.weight", D);
+    if (I > 0) {
+      l.add_k = lin(p + "attn2.add_k_proj", D, D);
+      l.add_v = lin(p + "attn2.add_v_proj", D, D);
+      l.norm_added_k = r.f32(p + "attn2.norm_added_k.weight", D);
+    }
+    l.out2 = lin(p + "attn2.to_out.0", D, D);
+    l.ffn1 = lin(p + "ffn.net.0.proj", F, D);
+    l.ffn2 = lin(p + "ffn.net.2", D, F);
+    w.layers.push_back(l);
+  }
+  w.head_table = r.f32("scale_shift_table", 2 * D);
+  w.proj_out = lin("proj_out", (int64_t)c.out_channels * 4, D);
+  return r.rc;
+}
 
-#define RUN32(call)      \
-  do {                   \
-    int _rc = (call);    \
-    if (_rc) return _rc; \
-  } while (0)
-#define KCHECK() CE_CHECK_CUDA(cudaGetLastError())
-
-namespace {
-
+// The launches of the fp32 forward.  They are not counted: ce_dit_last_launch_count reports the last bf16 forward.
 struct Ctx32 {
-  ce_dit* h;
   Ws32 ws;
-  cudaStream_t s;
-  int rc = 0;
-  const float* W(const std::string& n, int64_t numel) {
-    const float* p = ce_dit_internal_weight_f32(h, n, numel);
-    if (!p && !rc) rc = fail(CE_ERR_MISSING_WEIGHT, "fp32 validation mode: missing fp32 weight " + n);
-    return p;
-  }
+  Launcher run;
   // out[M, ldo] (fp32) = act(A[M, K] (lda) . W[N, K]^T + bias)
-  int linear(const float* A, int lda, int M, int K, const std::string& wname, int N, float* out, int ldo, int act) {
-    const float* Wt = W(wname + ".weight", (int64_t)N * K);
-    const float* bias = W(wname + ".bias", N);
-    if (rc) return rc;
-    return matmul(A, lda, M, K, Wt, K, N, out, ldo, bias, act);
-  }
-  int matmul(const float* A, int lda, int M, int K, const float* Wt, int ldw, int N, float* out, int ldo, const float* bias, int act) {
+  int linear(const float* A, int lda, int M, int K, const Lin32& w, int N, float* out, int ldo, int act) {
     const int Kp = up8(K);
-    split3_kernel<<<grid_for((size_t)M * Kp), TPB, 0, s>>>(A, lda, M, K, Kp, ws.Ap, 0);
-    split3_kernel<<<grid_for((size_t)N * Kp), TPB, 0, s>>>(Wt, ldw, N, K, Kp, ws.Wp, 1);
-    KCHECK();
+    CE_TRY(run.kernel(split3_kernel, grid_for((size_t)M * Kp), TPB, A, lda, M, K, Kp, ws.Ap, 0));
+    CE_TRY(run.kernel(split3_kernel, grid_for((size_t)N * Kp), TPB, w.w, K, N, K, Kp, ws.Wp, 1));
     GemmArgs g;
     g.M = M; g.N = N; g.K = 3 * Kp;
     g.out = nullptr; g.ldo = 0; g.out_f32 = out; g.ld_f32 = ldo;
     g.bias = nullptr; g.epi = EPI_BIAS;
-    RUN32(launch_gemm_bf16(ws.Ap, 3 * Kp, ws.Wp, 3 * Kp, g, s));
-    if (bias || act) {
-      bias_act_kernel<<<grid_for((size_t)M * N), TPB, 0, s>>>(out, ldo, M, N, bias, act);
-      KCHECK();
-    }
+    CE_TRY(run([&] { return launch_gemm_bf16(ws.Ap, 3 * Kp, ws.Wp, 3 * Kp, g, run.s); }));
+    if (w.b || act) CE_TRY(run.kernel(bias_act_kernel, grid_for((size_t)M * N), TPB, out, ldo, M, N, w.b, act));
     return CE_OK;
   }
   int layernorm(const float* x, float* y, int rows, int D, float eps, const float* scale, const float* shift, int mod_stride, int rpb,
                 const float* w, const float* b) {
-    layernorm_f32_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, y, rows, D, eps, scale, shift, mod_stride, rpb > 0 ? rpb : rows, w, b);
-    KCHECK();
-    return CE_OK;
+    return run.kernel(layernorm_f32_kernel, (rows + 7) / 8, 256, x, y, rows, D, eps, scale, shift, mod_stride, rpb > 0 ? rpb : rows, w, b);
   }
   int rms(float* x, int ldx, int rows, int D, float eps, const float* w, const float* rc_, const float* rs_, int L, int hd) {
-    rmsnorm_rope_f32_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, ldx, rows, D, eps, w, rc_, rs_, L, hd);
-    KCHECK();
-    return CE_OK;
+    return run.kernel(rmsnorm_rope_f32_kernel, (rows + 7) / 8, 256, x, ldx, rows, D, eps, w, rc_, rs_, L, hd);
   }
   // out[b, i, h*hd:(h+1)*hd] = softmax(q k^T * scale) v   for every (b, h); q [B*Lq, D], k / v [B*Lk, D]
   int attention(const float* q, const float* k, const float* v, float* out, int B, int H, int Lq, int Lk, int D, int hd, float scale) {
@@ -297,25 +308,22 @@ struct Ctx32 {
         const float* kh = k + (size_t)b * Lk * D + hh * hd;
         const float* vh = v + (size_t)b * Lk * D + hh * hd;
         // S[Lq, Lk8]: rows Lk..Lk8-1 of the "weight" operand are zero-padded by giving split3 rows = Lk8 over a zeroed tail
-        CE_CHECK_CUDA(cudaMemsetAsync(ws.Wp, 0, (size_t)Lk8 * 3 * up8(hd) * sizeof(bf16), s));
+        CE_CHECK_CUDA(cudaMemsetAsync(ws.Wp, 0, (size_t)Lk8 * 3 * up8(hd) * sizeof(bf16), run.s));
         {
           const int Kp = up8(hd);
-          split3_kernel<<<grid_for((size_t)Lq * Kp), TPB, 0, s>>>(qh, D, Lq, hd, Kp, ws.Ap, 0);
-          split3_kernel<<<grid_for((size_t)Lk * Kp), TPB, 0, s>>>(kh, D, Lk, hd, Kp, ws.Wp, 1);
-          KCHECK();
+          CE_TRY(run.kernel(split3_kernel, grid_for((size_t)Lq * Kp), TPB, qh, D, Lq, hd, Kp, ws.Ap, 0));
+          CE_TRY(run.kernel(split3_kernel, grid_for((size_t)Lk * Kp), TPB, kh, D, Lk, hd, Kp, ws.Wp, 1));
           GemmArgs g;
           g.M = Lq; g.N = Lk8; g.K = 3 * Kp; g.out_f32 = ws.S; g.ld_f32 = Lk8;
-          RUN32(launch_gemm_bf16(ws.Ap, 3 * Kp, ws.Wp, 3 * Kp, g, s));
+          CE_TRY(run([&] { return launch_gemm_bf16(ws.Ap, 3 * Kp, ws.Wp, 3 * Kp, g, run.s); }));
         }
-        softmax_rows_f32_kernel<<<Lq, 256, 0, s>>>(ws.S, Lk8, ws.P, Lk8, Lk, scale);
-        KCHECK();
+        CE_TRY(run([&] { return launch_softmax_rows_f32(ws.S, Lk8, ws.P, Lk8, Lq, Lk, scale, run.s); }));
         {  // O = P . V : P [Lq, Lk8] (padded columns are 0), V^T as the "weight" operand [hd, Lk8] (keys >= Lk zero-filled)
-          split3_kernel<<<grid_for((size_t)Lq * Lk8), TPB, 0, s>>>(ws.P, Lk8, Lq, Lk8, Lk8, ws.Ap, 0);
-          split3_transposed_kernel<<<grid_for((size_t)hd * Lk8), TPB, 0, s>>>(vh, D, Lk, Lk8, hd, ws.Wp);
-          KCHECK();
+          CE_TRY(run.kernel(split3_kernel, grid_for((size_t)Lq * Lk8), TPB, ws.P, Lk8, Lq, Lk8, Lk8, ws.Ap, 0));
+          CE_TRY(run.kernel(split3_transposed_kernel, grid_for((size_t)hd * Lk8), TPB, vh, D, Lk, Lk8, hd, ws.Wp));
           GemmArgs g;
           g.M = Lq; g.N = hd; g.K = 3 * Lk8; g.out_f32 = out + (size_t)b * Lq * D + hh * hd; g.ld_f32 = D;
-          RUN32(launch_gemm_bf16(ws.Ap, 3 * Lk8, ws.Wp, 3 * Lk8, g, s));
+          CE_TRY(run([&] { return launch_gemm_bf16(ws.Ap, 3 * Lk8, ws.Wp, 3 * Lk8, g, run.s); }));
         }
       }
     return CE_OK;
@@ -323,6 +331,11 @@ struct Ctx32 {
 };
 
 }  // namespace
+
+// handle internals (dit.cu)
+const WeightMap& ce_dit_internal_weights_f32(const ce_dit* h);
+int ce_dit_internal_rope(ce_dit* h, int frames, int hp, int wp, cudaStream_t s, const float** cos_out, const float** sin_out);
+const ce_dit_config* ce_dit_internal_config(const ce_dit* h);
 
 extern "C" {
 
@@ -337,106 +350,89 @@ int ce_dit_forward_fp32(ce_dit* h, const float* hidden_states, const float* time
                         const float* encoder_hidden_states_image, float* sample, int batch, int frames, int height, int width, int text_len,
                         void* workspace, int64_t workspace_bytes, float* block_out, void* stream_v) {
   CE_REQUIRE(h && hidden_states && timestep && encoder_hidden_states && sample && workspace, "ce_dit_forward_fp32: null argument");
-  int rc = check_device();
-  if (rc) return rc;
   const ce_dit_config& c = *ce_dit_internal_config(h);
   CE_REQUIRE(batch >= 1 && batch <= 8 && (frames == 2 || frames == c.rope_temporal_skip_len) && height % c.patch_h == 0 && width % c.patch_w == 0,
              "ce_dit_forward_fp32: geometry (same rules as ce_dit_forward)");
   CE_REQUIRE((c.image_dim > 0) == (encoder_hidden_states_image != nullptr), "ce_dit_forward_fp32: image states iff image_dim");
+  Weights32 W;
+  CE_TRY(resolve_weights32(ce_dit_internal_weights_f32(h), c, W));
+  CE_TRY(check_device());
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
   const int B = batch, hp = height / c.patch_h, wp = width / c.patch_w, L = frames * hp * wp, M = B * L;
   const int H = c.num_attention_heads, hd = c.attention_head_dim, D = H * hd, F = c.ffn_dim, Lt = text_len, Li = 257;
   const int Kp = c.in_channels * 4, No = c.out_channels * 4;
-  Ctx32 X{h, carve32(c, workspace, B, L, Lt, Li), s};
+  Ctx32 X{carve32(c, workspace, B, L, Lt, Li), Launcher{s, nullptr}};
   Ws32& ws = X.ws;
   if (ws.bytes > workspace_bytes) return fail(CE_ERR_WORKSPACE, "fp32 validation workspace too small: need " + std::to_string(ws.bytes));
   CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
   const float *rope_c, *rope_s;
-  RUN32(ce_dit_internal_rope(h, frames, hp, wp, s, &rope_c, &rope_s));
+  CE_TRY(ce_dit_internal_rope(h, frames, hp, wp, s, &rope_c, &rope_s));
   const float scale = 1.0f / sqrtf((float)hd);
-  const std::string ce_ = "condition_embedder.";
 
   // patch embedding (:429-430)
-  patchify_f32_kernel<<<grid_for((size_t)M * Kp), TPB, 0, s>>>(hidden_states, ws.patches, B, c.in_channels, frames, height, width);
-  KCHECK();
-  RUN32(X.linear(ws.patches, Kp, M, Kp, "patch_embedding", D, ws.x, D, 0));
+  CE_TRY(X.run.kernel(patchify_f32_kernel, grid_for((size_t)M * Kp), TPB, hidden_states, ws.patches, B, c.in_channels, frames, height, width));
+  CE_TRY(X.linear(ws.patches, Kp, M, Kp, W.patch, D, ws.x, D, 0));
   // condition embedder (:147-165): everything fp32, no bf16 rounding anywhere
-  RUN32(launch_timestep_sinusoid(timestep, ws.sin_emb, B, c.freq_dim, s));
-  RUN32(X.linear(ws.sin_emb, c.freq_dim, B, c.freq_dim, ce_ + "time_embedder.linear_1", D, ws.h1, D, 3));
-  RUN32(X.linear(ws.h1, D, B, D, ce_ + "time_embedder.linear_2", D, ws.temb, D, 0));
+  CE_TRY(X.run([&] { return launch_timestep_sinusoid(timestep, ws.sin_emb, B, c.freq_dim, s); }));
+  CE_TRY(X.linear(ws.sin_emb, c.freq_dim, B, c.freq_dim, W.time1, D, ws.h1, D, 3));
+  CE_TRY(X.linear(ws.h1, D, B, D, W.time2, D, ws.temb, D, 0));
   CE_CHECK_CUDA(cudaMemcpyAsync(ws.h1, ws.temb, (size_t)B * D * 4, cudaMemcpyDeviceToDevice, s));
-  bias_act_kernel<<<grid_for((size_t)B * D), TPB, 0, s>>>(ws.h1, D, B, D, nullptr, 3);   // act_fn(temb)
-  KCHECK();
-  RUN32(X.linear(ws.h1, D, B, D, ce_ + "time_proj", 6 * D, ws.tproj, 6 * D, 0));
-  RUN32(X.linear(encoder_hidden_states, c.text_dim, B * Lt, c.text_dim, ce_ + "text_embedder.linear_1", D, ws.text1, D, 1));
-  RUN32(X.linear(ws.text1, D, B * Lt, D, ce_ + "text_embedder.linear_2", D, ws.ctx_text, D, 0));
+  CE_TRY(X.run.kernel(bias_act_kernel, grid_for((size_t)B * D), TPB, ws.h1, D, B, D, nullptr, 3));   // act_fn(temb)
+  CE_TRY(X.linear(ws.h1, D, B, D, W.time_proj, 6 * D, ws.tproj, 6 * D, 0));
+  CE_TRY(X.linear(encoder_hidden_states, c.text_dim, B * Lt, c.text_dim, W.text1, D, ws.text1, D, 1));
+  CE_TRY(X.linear(ws.text1, D, B * Lt, D, W.text2, D, ws.ctx_text, D, 0));
   if (c.image_dim > 0) {
     const int I = c.image_dim;
-    RUN32(X.layernorm(encoder_hidden_states_image, ws.img0, B * Li, I, 1e-5f, nullptr, nullptr, 0, 0, X.W(ce_ + "image_embedder.norm1.weight", I),
-                      X.W(ce_ + "image_embedder.norm1.bias", I)));
-    RUN32(X.linear(ws.img0, I, B * Li, I, ce_ + "image_embedder.ff.net.0.proj", I, ws.img1, I, 2));
-    RUN32(X.linear(ws.img1, I, B * Li, I, ce_ + "image_embedder.ff.net.2", D, ws.img2, D, 0));
-    RUN32(X.layernorm(ws.img2, ws.ctx_img, B * Li, D, 1e-5f, nullptr, nullptr, 0, 0, X.W(ce_ + "image_embedder.norm2.weight", D),
-                      X.W(ce_ + "image_embedder.norm2.bias", D)));
+    CE_TRY(X.layernorm(encoder_hidden_states_image, ws.img0, B * Li, I, 1e-5f, nullptr, nullptr, 0, 0, W.img_norm1_w, W.img_norm1_b));
+    CE_TRY(X.linear(ws.img0, I, B * Li, I, W.img_ff0, I, ws.img1, I, 2));
+    CE_TRY(X.linear(ws.img1, I, B * Li, I, W.img_ff2, D, ws.img2, D, 0));
+    CE_TRY(X.layernorm(ws.img2, ws.ctx_img, B * Li, D, 1e-5f, nullptr, nullptr, 0, 0, W.img_norm2_w, W.img_norm2_b));
   }
-  if (X.rc) return X.rc;
 
   for (int i = 0; i < c.num_layers; ++i) {
-    const std::string p = "blocks." + std::to_string(i) + ".";
-    const float* table = X.W(p + "scale_shift_table", 6 * (int64_t)D);
-    if (X.rc) return X.rc;
-    add_table_f32_kernel<<<grid_for((size_t)B * 6 * D), TPB, 0, s>>>(table, ws.tproj, 6 * D, 1, ws.mod, B, D, 6);   // [B, 6, D]
-    KCHECK();
+    const Layer32& l = W.layers[i];
+    CE_TRY(X.run.kernel(add_table_f32_kernel, grid_for((size_t)B * 6 * D), TPB, l.table, ws.tproj, 6 * D, 1, ws.mod, B, D, 6));   // [B, 6, D]
     const float* mod = ws.mod;
     // 1. self-attention (:279-281)
-    RUN32(X.layernorm(ws.x, ws.xn, M, D, c.eps, mod + 1 * D, mod + 0 * D, 6 * D, L, nullptr, nullptr));
-    RUN32(X.linear(ws.xn, D, M, D, p + "attn1.to_q", D, ws.q, D, 0));
-    RUN32(X.linear(ws.xn, D, M, D, p + "attn1.to_k", D, ws.k, D, 0));
-    RUN32(X.linear(ws.xn, D, M, D, p + "attn1.to_v", D, ws.v, D, 0));
-    RUN32(X.rms(ws.q, D, M, D, c.eps, X.W(p + "attn1.norm_q.weight", D), rope_c, rope_s, L, hd));
-    RUN32(X.rms(ws.k, D, M, D, c.eps, X.W(p + "attn1.norm_k.weight", D), rope_c, rope_s, L, hd));
-    RUN32(X.attention(ws.q, ws.k, ws.v, ws.attn, B, H, L, L, D, hd, scale));
-    RUN32(X.linear(ws.attn, D, M, D, p + "attn1.to_out.0", D, ws.xn, D, 0));
-    resid_kernel<<<grid_for((size_t)M * D), TPB, 0, s>>>(ws.x, ws.xn, M, D, mod + 2 * D, 6 * D, L);
-    KCHECK();
+    CE_TRY(X.layernorm(ws.x, ws.xn, M, D, c.eps, mod + 1 * D, mod + 0 * D, 6 * D, L, nullptr, nullptr));
+    CE_TRY(X.linear(ws.xn, D, M, D, l.q, D, ws.q, D, 0));
+    CE_TRY(X.linear(ws.xn, D, M, D, l.k, D, ws.k, D, 0));
+    CE_TRY(X.linear(ws.xn, D, M, D, l.v, D, ws.v, D, 0));
+    CE_TRY(X.rms(ws.q, D, M, D, c.eps, l.norm_q, rope_c, rope_s, L, hd));
+    CE_TRY(X.rms(ws.k, D, M, D, c.eps, l.norm_k, rope_c, rope_s, L, hd));
+    CE_TRY(X.attention(ws.q, ws.k, ws.v, ws.attn, B, H, L, L, D, hd, scale));
+    CE_TRY(X.linear(ws.attn, D, M, D, l.out1, D, ws.xn, D, 0));
+    CE_TRY(X.run.kernel(resid_kernel, grid_for((size_t)M * D), TPB, ws.x, ws.xn, M, D, mod + 2 * D, 6 * D, L));
     // 2. cross-attention (:284-286)
-    RUN32(X.layernorm(ws.x, ws.xn, M, D, c.eps, nullptr, nullptr, 0, 0, X.W(p + "norm2.weight", D), X.W(p + "norm2.bias", D)));
-    RUN32(X.linear(ws.xn, D, M, D, p + "attn2.to_q", D, ws.q, D, 0));
-    RUN32(X.rms(ws.q, D, M, D, c.eps, X.W(p + "attn2.norm_q.weight", D), nullptr, nullptr, 0, hd));
-    RUN32(X.linear(ws.ctx_text, D, B * Lt, D, p + "attn2.to_k", D, ws.kt, D, 0));
-    RUN32(X.linear(ws.ctx_text, D, B * Lt, D, p + "attn2.to_v", D, ws.vt, D, 0));
-    RUN32(X.rms(ws.kt, D, B * Lt, D, c.eps, X.W(p + "attn2.norm_k.weight", D), nullptr, nullptr, 0, hd));
-    RUN32(X.attention(ws.q, ws.kt, ws.vt, ws.attn, B, H, L, Lt, D, hd, scale));
+    CE_TRY(X.layernorm(ws.x, ws.xn, M, D, c.eps, nullptr, nullptr, 0, 0, l.norm2_w, l.norm2_b));
+    CE_TRY(X.linear(ws.xn, D, M, D, l.q2, D, ws.q, D, 0));
+    CE_TRY(X.rms(ws.q, D, M, D, c.eps, l.norm_q2, nullptr, nullptr, 0, hd));
+    CE_TRY(X.linear(ws.ctx_text, D, B * Lt, D, l.k2, D, ws.kt, D, 0));
+    CE_TRY(X.linear(ws.ctx_text, D, B * Lt, D, l.v2, D, ws.vt, D, 0));
+    CE_TRY(X.rms(ws.kt, D, B * Lt, D, c.eps, l.norm_k2, nullptr, nullptr, 0, hd));
+    CE_TRY(X.attention(ws.q, ws.kt, ws.vt, ws.attn, B, H, L, Lt, D, hd, scale));
     if (c.image_dim > 0) {
-      RUN32(X.linear(ws.ctx_img, D, B * Li, D, p + "attn2.add_k_proj", D, ws.ki, D, 0));
-      RUN32(X.linear(ws.ctx_img, D, B * Li, D, p + "attn2.add_v_proj", D, ws.vi, D, 0));
-      RUN32(X.rms(ws.ki, D, B * Li, D, c.eps, X.W(p + "attn2.norm_added_k.weight", D), nullptr, nullptr, 0, hd));
-      RUN32(X.attention(ws.q, ws.ki, ws.vi, ws.attn2, B, H, L, Li, D, hd, scale));
-      add_inplace_kernel<<<grid_for((size_t)M * D), TPB, 0, s>>>(ws.attn, ws.attn2, (size_t)M * D);
-      KCHECK();
+      CE_TRY(X.linear(ws.ctx_img, D, B * Li, D, l.add_k, D, ws.ki, D, 0));
+      CE_TRY(X.linear(ws.ctx_img, D, B * Li, D, l.add_v, D, ws.vi, D, 0));
+      CE_TRY(X.rms(ws.ki, D, B * Li, D, c.eps, l.norm_added_k, nullptr, nullptr, 0, hd));
+      CE_TRY(X.attention(ws.q, ws.ki, ws.vi, ws.attn2, B, H, L, Li, D, hd, scale));
+      CE_TRY(X.run.kernel(add_inplace_kernel, grid_for((size_t)M * D), TPB, ws.attn, ws.attn2, (size_t)M * D));
     }
-    RUN32(X.linear(ws.attn, D, M, D, p + "attn2.to_out.0", D, ws.xn, D, 0));
-    resid_kernel<<<grid_for((size_t)M * D), TPB, 0, s>>>(ws.x, ws.xn, M, D, nullptr, 0, 1);
-    KCHECK();
+    CE_TRY(X.linear(ws.attn, D, M, D, l.out2, D, ws.xn, D, 0));
+    CE_TRY(X.run.kernel(resid_kernel, grid_for((size_t)M * D), TPB, ws.x, ws.xn, M, D, nullptr, 0, 1));
     // 3. feed-forward (:289-293)
-    RUN32(X.layernorm(ws.x, ws.xn, M, D, c.eps, mod + 4 * D, mod + 3 * D, 6 * D, L, nullptr, nullptr));
-    RUN32(X.linear(ws.xn, D, M, D, p + "ffn.net.0.proj", F, ws.h, F, 1));
-    RUN32(X.linear(ws.h, F, M, F, p + "ffn.net.2", D, ws.xn, D, 0));
-    resid_kernel<<<grid_for((size_t)M * D), TPB, 0, s>>>(ws.x, ws.xn, M, D, mod + 5 * D, 6 * D, L);
-    KCHECK();
-    if (X.rc) return X.rc;
+    CE_TRY(X.layernorm(ws.x, ws.xn, M, D, c.eps, mod + 4 * D, mod + 3 * D, 6 * D, L, nullptr, nullptr));
+    CE_TRY(X.linear(ws.xn, D, M, D, l.ffn1, F, ws.h, F, 1));
+    CE_TRY(X.linear(ws.h, F, M, F, l.ffn2, D, ws.xn, D, 0));
+    CE_TRY(X.run.kernel(resid_kernel, grid_for((size_t)M * D), TPB, ws.x, ws.xn, M, D, mod + 5 * D, 6 * D, L));
     if (i == 0 && block_out) CE_CHECK_CUDA(cudaMemcpyAsync(block_out, ws.x, (size_t)M * D * 4, cudaMemcpyDeviceToDevice, s));
   }
   // head (:451-467)
-  add_table_f32_kernel<<<grid_for((size_t)B * 2 * D), TPB, 0, s>>>(X.W("scale_shift_table", 2 * (int64_t)D), ws.temb, D, 0, ws.modf, B, D, 2);
-  KCHECK();
-  if (X.rc) return X.rc;
-  RUN32(X.layernorm(ws.x, ws.xn, M, D, c.eps, ws.modf + D, ws.modf, 2 * D, L, nullptr, nullptr));
-  RUN32(X.linear(ws.xn, D, M, D, "proj_out", No, ws.yout, No, 0));
-  unpatchify_f32_kernel<<<grid_for((size_t)B * c.out_channels * frames * height * width), TPB, 0, s>>>(ws.yout, No, sample, B, c.out_channels, frames,
-                                                                                                       height, width);
-  KCHECK();
-  return X.rc;
+  CE_TRY(X.run.kernel(add_table_f32_kernel, grid_for((size_t)B * 2 * D), TPB, W.head_table, ws.temb, D, 0, ws.modf, B, D, 2));
+  CE_TRY(X.layernorm(ws.x, ws.xn, M, D, c.eps, ws.modf + D, ws.modf, 2 * D, L, nullptr, nullptr));
+  CE_TRY(X.linear(ws.xn, D, M, D, W.proj_out, No, ws.yout, No, 0));
+  return X.run.kernel(unpatchify_f32_kernel, grid_for((size_t)B * c.out_channels * frames * height * width), TPB, ws.yout, No, sample, B,
+                      c.out_channels, frames, height, width);
 }
 
 }  // extern "C"

@@ -463,7 +463,84 @@ quantize_rows_fp8_kernel(const bf16* __restrict__ x, int ldx, int K, uint8_t* __
   }
 }
 
+// Score rules of softmax_rows_kernel: which keys of a row count, the score of key j from the GEMM accumulators s, and the
+// exponential of (score - row max).
+template <bool FAST>
+struct ScaledScore {
+  float scale;
+  __device__ int keys(int cols) const { return cols; }
+  __device__ float operator()(const float* s, int, int j) const { return s[j]; }
+  __device__ float exp(float d) const { return FAST ? __expf(d * scale) : expf(d * scale); }
+};
+struct T5Score {
+  const bf16* bias;
+  int bias_ld, Lq, valid;
+  __device__ int keys(int cols) const { return valid < cols ? valid : cols; }
+  __device__ float operator()(const float* s, int row, int j) const {
+    const bf16* bh = bias + (size_t)(row / Lq) * bias_ld + (Lq - 1 - row % Lq);
+    return bf16_round(bf16_round(s[j]) + __bfloat162float(bh[j]));
+  }
+  __device__ float exp(float d) const { return expf(d); }
+};
+struct ClipScore {
+  float scale;
+  __device__ int keys(int cols) const { return cols; }
+  __device__ float operator()(const float* s, int, int j) const { return bf16_round(bf16_round(s[j]) * scale); }
+  __device__ float exp(float d) const { return expf(d); }
+};
+
+__device__ __forceinline__ void store_prob(float* p, float v) { *p = v; }
+__device__ __forceinline__ void store_prob(bf16* p, float v) { *p = __float2bfloat16_rn(v); }
+
+// One block per row: two-pass block reduction (max, then sum of exponentials), then p = exp(score - max) / sum.
+template <class Score, class Out>
+__global__ void __launch_bounds__(256)
+softmax_rows_kernel(const float* __restrict__ S, int lds, Out* __restrict__ P, int ldp, int cols, Score score) {
+  __shared__ float red[32];
+  const int row = blockIdx.x;
+  const float* s = S + (size_t)row * lds;
+  Out* p = P + (size_t)row * ldp;
+  const int nk = score.keys(cols);
+  float mx = -INFINITY;
+  for (int j = threadIdx.x; j < nk; j += blockDim.x) mx = fmaxf(mx, score(s, row, j));
+  mx = warp_max(mx);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  mx = warp_max((threadIdx.x & 31) < (blockDim.x >> 5) ? red[threadIdx.x & 31] : -INFINITY);
+  __syncthreads();
+  float sum = 0.f;
+  for (int j = threadIdx.x; j < nk; j += blockDim.x) sum += score.exp(score(s, row, j) - mx);
+  sum = warp_sum(sum);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sum;
+  __syncthreads();
+  sum = warp_sum((threadIdx.x & 31) < (blockDim.x >> 5) ? red[threadIdx.x & 31] : 0.f);
+  const float inv = 1.0f / sum;
+  for (int j = threadIdx.x; j < ldp; j += blockDim.x) store_prob(p + j, j < nk ? score.exp(score(s, row, j) - mx) * inv : 0.f);
+}
+
 }  // namespace
+
+int launch_softmax_rows(const float* S, int lds, bf16* P, int ldp, int rows, int cols, const SoftmaxScores& sc, cudaStream_t stream) {
+  switch (sc.rule) {
+    case SOFTMAX_SCALED:
+      softmax_rows_kernel<<<rows, 256, 0, stream>>>(S, lds, P, ldp, cols, ScaledScore<true>{sc.scale});
+      break;
+    case SOFTMAX_T5:
+      softmax_rows_kernel<<<rows, 256, 0, stream>>>(S, lds, P, ldp, cols, T5Score{sc.bias, sc.bias_ld, sc.Lq, sc.valid});
+      break;
+    case SOFTMAX_CLIP:
+      softmax_rows_kernel<<<rows, 256, 0, stream>>>(S, lds, P, ldp, cols, ClipScore{sc.scale});
+      break;
+  }
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
+
+int launch_softmax_rows_f32(const float* S, int lds, float* P, int ldp, int rows, int cols, float scale, cudaStream_t stream) {
+  softmax_rows_kernel<<<rows, 256, 0, stream>>>(S, lds, P, ldp, cols, ScaledScore<false>{scale});
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
 
 int launch_quantize_rows_fp8(const bf16* x, int ldx, int rows, int K, uint8_t* q, int ldq, float* scale, cudaStream_t stream) {
   CE_REQUIRE(rows > 0 && K > 0 && K % 16 == 0, "quantize_rows_fp8: rows > 0 and a width that is a multiple of 16");

@@ -46,6 +46,23 @@ int launch_rmsnorm_rope_stats(bf16* x, int ldx, int rows, int D, float eps, cons
 // q[m, k] = e4m3 bits of cvt.rn.satfinite(x[m,k] / scale[m]) (IEEE fp32 divisions).  One launch, HBM-bound.
 int launch_quantize_rows_fp8(const bf16* x, int ldx, int rows, int K, uint8_t* q, int ldq, float* scale, cudaStream_t stream);
 
+// Row softmax of the fp32 GEMM accumulators S [rows, lds] (rows = heads x Lq queries) into P [rows, ldp]: p = bf16(softmax_fp32(
+// score)) over the keys j < cols, and 0 for the other columns up to ldp.  The score of key j in query row i of head h:
+//   SOFTMAX_SCALED (VAE):  s * scale, exponentials with __expf
+//   SOFTMAX_T5:    bf16(bf16(s) + bias[h, (j - i) + Lq - 1]); keys j >= valid are masked out (probability 0, as adding
+//                  finfo(bf16).min does in the reference)
+//   SOFTMAX_CLIP:  bf16(bf16(s) * scale)
+enum SoftmaxRule { SOFTMAX_SCALED, SOFTMAX_T5, SOFTMAX_CLIP };
+struct SoftmaxScores {
+  SoftmaxRule rule = SOFTMAX_SCALED;
+  float scale = 1.f;
+  const bf16* bias = nullptr;   // T5: [heads, bias_ld]
+  int bias_ld = 0, Lq = 0, valid = 0;
+};
+int launch_softmax_rows(const float* S, int lds, bf16* P, int ldp, int rows, int cols, const SoftmaxScores& sc, cudaStream_t stream);
+// The fp32 validation forward's: P fp32 = softmax(s * scale) with expf.
+int launch_softmax_rows_f32(const float* S, int lds, float* P, int ldp, int rows, int cols, float scale, cudaStream_t stream);
+
 // patches[(b,f,i,j), c*4 + dh*2 + dw] = x[b, c, f, 2i+dh, 2j+dw]   (im2row for the k=s=(1,2,2) patch-embedding conv, :368,429-430)
 int launch_patchify(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, cudaStream_t stream);
 // out[b, c, f, 2i+dh, 2j+dw] = y[(b,f,i,j), (dh*2+dw)*C + c]       (unpatchify permute of :463-467)

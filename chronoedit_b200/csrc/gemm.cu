@@ -296,4 +296,29 @@ int launch_gemm_fp8(const e4m3* Aq, int lda, const float* s_a, const e4m3* Wq, i
   return launch_gemm<e4m3>(Aq, lda, s_a, Wq, ldw, s_w, g, stream);
 }
 
+int run_gemm(Launcher& run, const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K, bf16* out, int ldo, const bf16* bias, int epi,
+             const bf16* resid, int ldr) {
+  GemmArgs g;
+  g.M = M; g.N = N; g.K = K; g.out = out; g.ldo = ldo; g.bias = bias;
+  g.epi = epi; g.resid = resid; g.ldr = ldr;
+  return run([&] { return launch_gemm_bf16(A, lda, W, ldw, g, run.s); });
+}
+
+int gemm_attention(Launcher& run, const GemmAttention& a) {
+  const int I = a.H * a.dk, L8 = up8(a.L);
+  CE_TRY(run_gemm(run, a.x, a.D, a.wqk, a.D, a.L, 2 * I, a.D, a.qk, 2 * I, a.bqk));
+  GemmArgs g;
+  g.M = I; g.N = L8; g.K = a.D; g.out = a.vT; g.ldo = L8; g.bias_row = a.bv;
+  CE_TRY(run([&] { return launch_gemm_bf16(a.wv, a.D, a.x, a.D, g, run.s); }));
+  for (int h = 0; h < a.H; ++h) {
+    g = GemmArgs();
+    g.M = a.L; g.N = L8; g.K = a.dk; g.out_f32 = a.S + (size_t)h * a.L * L8; g.ld_f32 = L8;
+    CE_TRY(run([&] { return launch_gemm_bf16(a.qk + h * a.dk, 2 * I, a.qk + I + h * a.dk, 2 * I, g, run.s); }));
+  }
+  CE_TRY(run([&] { return launch_softmax_rows(a.S, L8, a.P, L8, a.H * a.L, a.L, a.sc, run.s); }));
+  for (int h = 0; h < a.H; ++h)
+    CE_TRY(run_gemm(run, a.P + (size_t)h * a.L * L8, L8, a.vT + (size_t)h * a.dk * L8, L8, a.L, a.dk, a.kpv, a.out + h * a.dk, a.ldo));
+  return CE_OK;
+}
+
 }  // namespace ce

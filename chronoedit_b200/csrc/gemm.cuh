@@ -3,6 +3,7 @@
 #include "host_common.h"
 #include <cuda_fp8.h>
 
+#include "elementwise.cuh"
 #include "ptx.cuh"
 
 namespace ce {
@@ -54,5 +55,30 @@ int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmA
 // lda, ldw multiples of 16) and fp32 scales s_a[M], s_w[N]; out[M,N] = epilogue(y) exactly as launch_gemm_bf16 applies it to acc.
 int launch_gemm_fp8(const e4m3* Aq, int lda, const float* s_a, const e4m3* Wq, int ldw, const float* s_w, const GemmArgs& g,
                     cudaStream_t stream);
+
+// One launch_gemm_bf16 through `run`, with only the epilogue fields bias / epi / resid.
+int run_gemm(Launcher& run, const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K, bf16* out, int ldo, const bf16* bias = nullptr,
+             int epi = EPI_BIAS, const bf16* resid = nullptr, int ldr = 0);
+
+// Multi-head attention built from GEMMs over one sequence of L tokens, I = heads * dk, L8 = up8(L):
+//   q|k = x [Wq;Wk]^T + bqk                -> qk [L, 2I]
+//   V^T = Wv x^T + bv (per row)            -> vT [I, L8]   (x rows L..L8-1 are read: finite or not, they only reach columns
+//                                                           of V^T that P.V does not sum over, or multiply zeros of P)
+//   per head: S_h = q_h k_h^T (fp32)       -> S [H, L, L8]   (k rows L..L8-1 of qk are read but never written here: whatever
+//                                                           they hold only reaches columns L..L8-1 of S, which the softmax
+//                                                           does not read)
+//   P = one row-softmax launch (rule sc)   -> P [H, L, L8]
+//   per head: O_h = P_h[:, 0:kpv] V_h      -> out [L, I] (ld ldo)
+// x [L8, D] (ld D), Wqk [2I, D], Wv [I, D]; bqk / bv may be null.  Every launch goes through `run`.
+struct GemmAttention {
+  const bf16 *x, *wqk, *bqk, *wv, *bv;
+  int L, D, H, dk;
+  int kpv;   // keys P.V sums over: L, or L8 when P's padding columns are zero and V^T's are finite
+  SoftmaxScores sc;
+  bf16 *qk, *vT, *P, *out;
+  float* S;
+  int ldo;
+};
+int gemm_attention(Launcher& run, const GemmAttention& a);
 
 }  // namespace ce

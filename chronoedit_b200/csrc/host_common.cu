@@ -15,6 +15,36 @@ int fail(int code, const std::string& msg) {
 }
 const std::string& last_error() { return g_last_error; }
 
+int register_weight(WeightMap& w, const char* fn, const char* name, const void* ptr, int dtype, int64_t numel) {
+  CE_REQUIRE(name && ptr, std::string(fn) + ": null argument");
+  CE_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, std::string(fn) + ": pointer must be 16-byte aligned");
+  w[name] = WeightRef{ptr, dtype, numel};
+  return CE_OK;
+}
+
+const void* WeightLookup::get(const std::string& name, int dtype, int64_t numel) {
+  if (rc) return nullptr;
+  auto it = w.find(name);
+  if (it == w.end()) {
+    rc = fail(CE_ERR_MISSING_WEIGHT, "missing weight: " + name);
+    return nullptr;
+  }
+  if (dtype >= 0 && it->second.dtype != dtype) {
+    rc = fail(CE_ERR_MISSING_WEIGHT, "weight " + name + " has dtype " + std::to_string(it->second.dtype) + ", expected " +
+                                         std::to_string(dtype) + " (0 bf16, 1 fp32, 2 e4m3" +
+                                         (dtype == 2 || it->second.dtype == 2
+                                              ? "; the six block GEMM weights of every layer are either all bf16 or all e4m3)"
+                                              : ")"));
+    return nullptr;
+  }
+  if (it->second.numel != numel) {
+    rc = fail(CE_ERR_MISSING_WEIGHT, "weight " + name + " has " + std::to_string(it->second.numel) + " elements, expected " +
+                                         std::to_string(numel));
+    return nullptr;
+  }
+  return it->second.ptr;
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);

@@ -3,12 +3,16 @@
 // link-time dependency on libcuda and builds on a GPU-less box).
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <map>
 #include <string>
 
 namespace ce {
+
+typedef __nv_bfloat16 bf16;
 
 // ---- error plumbing ------------------------------------------------------------------------
 // Every extern "C" entry point returns 0 on success or a negative code and records a message
@@ -85,5 +89,60 @@ inline int grid_for(size_t n) {
   const size_t g = (n + TPB - 1) / TPB, cap = (size_t)device_sm_count() * 16;
   return (int)(g < cap ? (g ? g : 1) : cap);
 }
+
+#define CE_TRY(expr)        \
+  do {                      \
+    const int _rc = (expr); \
+    if (_rc) return _rc;    \
+  } while (0)
+
+// ---- weights ----------------------------------------------------------------------------------
+// A weight registered with a handle: the caller's pointer, its dtype (0 bf16, 1 fp32, 2 e4m3; -1 where the handle's set_weight
+// takes none) and its element count.
+struct WeightRef {
+  const void* ptr = nullptr;
+  int dtype = -1;
+  int64_t numel = 0;
+};
+using WeightMap = std::map<std::string, WeightRef>;
+
+// The body of every *_set_weight entry point: `fn` names it in the error message.
+int register_weight(WeightMap& w, const char* fn, const char* name, const void* ptr, int dtype, int64_t numel);
+
+// Looks weights up one at a time, checking the element count and the dtype (unless dtype < 0: handles whose set_weight takes
+// none); the first one that is missing or wrong records CE_ERR_MISSING_WEIGHT with its name, and every lookup after it returns
+// null.
+struct WeightLookup {
+  const WeightMap& w;
+  int rc = CE_OK;
+
+  const void* get(const std::string& name, int dtype, int64_t numel);
+  template <class T>
+  const T* any(const std::string& name, int64_t numel) { return static_cast<const T*>(get(name, -1, numel)); }
+  const bf16* b16(const std::string& name, int64_t numel) { return static_cast<const bf16*>(get(name, 0, numel)); }
+  const float* f32(const std::string& name, int64_t numel) { return static_cast<const float*>(get(name, 1, numel)); }
+};
+
+// ---- launches ---------------------------------------------------------------------------------
+// Every launch of the VAE, encoder and fp32 validation chains: a launch_* call, or a __global__ function launched here and
+// checked with cudaGetLastError.  A launch that was enqueued is counted in *launches (when given).
+struct Launcher {
+  cudaStream_t s;
+  int64_t* launches;
+
+  template <class Launch>
+  int operator()(Launch&& launch) {
+    const int rc = launch();
+    if (!rc && launches) ++*launches;
+    return rc;
+  }
+  template <class... P, class... A>
+  int kernel(void (*k)(P...), int grid, int block, A... args) {
+    k<<<grid, block, 0, s>>>(args...);
+    CE_CHECK_CUDA(cudaGetLastError());
+    if (launches) ++*launches;
+    return CE_OK;
+  }
+};
 
 }  // namespace ce

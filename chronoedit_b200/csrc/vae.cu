@@ -5,10 +5,9 @@
 // streaming (frame 0 alone, then 4-frame chunks when encoding; one latent frame per iteration when decoding) with a
 // 2-frame history per causal convolution.  Activations are channels-last bf16; every convolution with Cin >= 64 is the
 // wgmma implicit GEMM of conv.cu reading its input (history frames + chunk) in place; the three small-Cin convolutions
-// (3->dim, z->top, 2z->2z) go through im2row + the wgmma GEMM; RMS_norm+SiLU / upsample / softmax are the row kernels
-// of vae_kernels.cu; the single-head mid attention is GEMM (QK^T, fp32) -> row softmax -> GEMM (P V).
+// (3->dim, z->top, 2z->2z) go through im2row + the wgmma GEMM; RMS_norm+SiLU / upsample are the row kernels of
+// vae_kernels.cu; the single-head mid attention is gemm_attention (gemm.cu) with H = 1.
 #include <math.h>
-#include <stdlib.h>
 
 #include <map>
 #include <string>
@@ -21,26 +20,9 @@
 
 using namespace ce;
 
-// CE_VAE_DEBUG=1: after every op, synchronise and print non-finite count / mean |x| of its output (debug only).
-__global__ void vae_debug_stats_kernel(const bf16* x, size_t n, unsigned long long* bad, float* sum) {
-  float s = 0.f;
-  unsigned long long b = 0;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float v = __bfloat162float(x[i]);
-    if (!isfinite(v)) ++b; else s += fabsf(v);
-  }
-  atomicAdd(sum, s);
-  if (b) atomicAdd(bad, b);
-}
-
-struct VWeight {
-  const void* ptr = nullptr;
-  int64_t numel = 0;
-};
-
 struct ce_vae {
   ce_vae_config cfg;
-  std::map<std::string, VWeight> w;
+  WeightMap w;
   int64_t launches = 0;
 };
 
@@ -62,70 +44,40 @@ struct StreamBuf {  // input buffer of one streaming (causal) convolution: `hist
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
-// One encode or decode call.  `dry` = planning pass: same walk, no launches, only the two bump allocators advance.
+// One encode or decode call.  `dry` = planning pass: the same walk without launches, in which the two bump allocators measure the
+// workspace and every weight is looked up with its packed element count before anything is launched.
 struct Run {
   ce_vae* h;
   cudaStream_t s;
   bool dry;
-  uint8_t* base;
-  int64_t persist_off = 0;   // persistent region grows from the front (stream buffers, collected outputs)
-  int64_t scratch_base = 0;  // scratch region starts after the persistent plan
-  int64_t scratch_off = 0, scratch_max = 0;
+  Bump persist;   // from the front of the workspace: stream buffers, collected outputs
+  Bump scratch;   // after the persistent region; reset per chunk
+  int64_t scratch_max = 0;
   std::map<std::string, StreamBuf> streams;
+  WeightLookup weights{h->w};
+  Launcher run{s, &h->launches};
   int rc = 0;
 
-  bf16* take_persist(size_t elems, size_t elem_size = 2) {
-    persist_off = (persist_off + 255) & ~int64_t(255);
-    bf16* p = dry ? nullptr : reinterpret_cast<bf16*>(base + persist_off);
-    persist_off += (int64_t)(elems * elem_size);
-    return p;
-  }
+  Run(ce_vae* h_, cudaStream_t s_, uint8_t* persist_base, uint8_t* scratch_base)
+      : h(h_), s(s_), dry(persist_base == nullptr), persist(persist_base), scratch(scratch_base) {}
+
   void* take_scratch_bytes(size_t bytes) {
-    scratch_off = (scratch_off + 255) & ~int64_t(255);
-    void* p = dry ? nullptr : reinterpret_cast<void*>(base + scratch_base + scratch_off);
-    scratch_off += (int64_t)bytes;
-    if (scratch_off > scratch_max) scratch_max = scratch_off;
+    void* p = scratch.take<uint8_t>((int64_t)bytes);
+    if (scratch.off > scratch_max) scratch_max = scratch.off;
     return p;
   }
-  Act scratch(int T, int H, int W, int C) {
+  Act scratch_act(int T, int H, int W, int C) {
     Act a;
     a.T = T; a.H = H; a.W = W; a.C = C;
     a.p = reinterpret_cast<bf16*>(take_scratch_bytes(a.numel() * 2));
     return a;
   }
-  void reset_scratch() { scratch_off = 0; }
+  void reset_scratch() { scratch.off = 0; }
+  int64_t workspace_bytes() const { return persist.bytes() + ((scratch_max + 255) & ~int64_t(255)) + 256; }
 
-  const bf16* W(const std::string& name) {
-    auto it = h->w.find(name);
-    if (it == h->w.end()) {
-      if (!rc) rc = fail(CE_ERR_MISSING_WEIGHT, "vae: missing weight " + name);
-      return nullptr;
-    }
-    return reinterpret_cast<const bf16*>(it->second.ptr);
-  }
-  void ok(int r) {
-    if (r && !rc) rc = r;
-    if (!r) ++h->launches;
-  }
-  void debug(const std::string& what, const bf16* p, size_t n) {
-    static const bool on = getenv("CE_VAE_DEBUG") != nullptr;
-    if (!on || dry || rc || !p) return;
-    unsigned long long* bad;
-    float* sum;
-    cudaMalloc(&bad, 8);
-    cudaMalloc(&sum, 4);
-    cudaMemsetAsync(bad, 0, 8, s);
-    cudaMemsetAsync(sum, 0, 4, s);
-    vae_debug_stats_kernel<<<256, 256, 0, s>>>(p, n, bad, sum);
-    unsigned long long hb = 0;
-    float hs = 0;
-    cudaMemcpyAsync(&hb, bad, 8, cudaMemcpyDeviceToHost, s);
-    cudaMemcpyAsync(&hs, sum, 4, cudaMemcpyDeviceToHost, s);
-    cudaError_t e = cudaStreamSynchronize(s);
-    printf("[vae-debug] %-44s n=%-10zu nonfinite=%-8llu mean|x|=%.5f %s\n", what.c_str(), n, hb, hs / (double)n, e == cudaSuccess ? "" : cudaGetErrorString(e));
-    fflush(stdout);
-    cudaFree(bad);
-    cudaFree(sum);
+  template <class Launch>
+  void launch(Launch&& l) {
+    if (!dry && !rc) rc = run(l);
   }
 
   // ---- streaming conv input buffers
@@ -135,7 +87,7 @@ struct Run {
     StreamBuf b;
     b.hist = hist; b.tcap = tcap; b.H = H; b.W = W_; b.C = C;
     const size_t elems = (size_t)(hist + tcap) * H * W_ * C;
-    b.p = take_persist(elems);
+    b.p = persist.take<bf16>((int64_t)elems);
     if (!dry && hist > 0) {
       cudaError_t e = cudaMemsetAsync(b.p, 0, (size_t)hist * H * W_ * C * 2, s);  // zero history = causal zero padding
       if (e != cudaSuccess && !rc) rc = fail(CE_ERR_CUDA, cudaGetErrorString(e));
@@ -168,26 +120,22 @@ struct Run {
 
   // ---- primitive ops
   void rms(const Act& x, const std::string& gamma_name, bf16* y, bool silu) {
-    const bf16* g = W(gamma_name);
-    if (dry || rc) return;
-    ok(launch_rms_silu_cl(x.p, g, y, x.pixels(), x.C, silu ? 1 : 0, s));
-    debug("rms " + gamma_name, y, x.numel());
+    const bf16* g = weights.any<bf16>(gamma_name, x.C);
+    launch([&] { return launch_rms_silu_cl(x.p, g, y, x.pixels(), x.C, silu ? 1 : 0, s); });
   }
   // implicit-GEMM conv reading `in` = [Tin frames] (history included) -> out
   void conv(const std::string& name, const bf16* in, int Tin, int Hin, int Win, int Cin, Act& out, int kt, int kh, int kw, int st, int sh,
             int sw, int ph, int pw, const bf16* resid = nullptr, int split_time = 0) {
-    const bf16* w = W(name + ".weight");
-    const bf16* b = W(name + ".bias");
-    if (dry || rc) return;
     ConvArgs a;
+    a.Cout = split_time ? out.C * 2 : out.C; a.Cin_pad = round_up(Cin, 64);
+    a.w = weights.any<bf16>(name + ".weight", (int64_t)a.Cout * kt * kh * kw * a.Cin_pad);
+    a.bias = weights.any<bf16>(name + ".bias", a.Cout);
     a.x = in; a.Tin = Tin; a.Hin = Hin; a.Win = Win; a.Cin = Cin;
-    a.w = w; a.bias = b; a.Cout = split_time ? out.C * 2 : out.C; a.Cin_pad = round_up(Cin, 64);
     a.kt = kt; a.kh = kh; a.kw = kw; a.st = st; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw;
     a.t_base = 0;
     a.y = out.p; a.Tout = split_time ? out.T / 2 : out.T; a.Hout = out.H; a.Wout = out.W;
     a.resid = resid; a.split_time = split_time;
-    ok(launch_conv3d_cl(a, s));
-    debug("conv " + name, out.p, out.numel());
+    launch([&] { return launch_conv3d_cl(a, s); });
   }
   // streaming causal conv (kt = 3): x is already in the stream buffer's chunk region
   void causal_conv(const std::string& name, StreamBuf& b, int T, Act& out, int kh, const bf16* resid = nullptr, int split_time = 0) {
@@ -195,14 +143,9 @@ struct Run {
     push_history(b, T);
     b.primed = true;
   }
-  void gemm(const bf16* A, int lda, const bf16* Wt, int ldw, int M, int N, int K, bf16* out, int ldo, const bf16* bias, const bf16* bias_row,
-            float* out_f32, int epi = EPI_BIAS, const bf16* resid = nullptr, int ldr = 0) {
-    if (dry || rc) return;
-    GemmArgs g;
-    g.M = M; g.N = N; g.K = K; g.out = out; g.ldo = ldo; g.out_f32 = out_f32; g.bias = bias; g.bias_row = bias_row;
-    g.epi = epi; g.resid = resid; g.ldr = ldr;
-    ok(launch_gemm_bf16(A, lda, Wt, ldw, g, s));
-    if (out) debug("gemm M=" + std::to_string(M) + " N=" + std::to_string(N) + " K=" + std::to_string(K), out, (size_t)M * ldo);
+  void gemm(const bf16* A, int lda, const bf16* Wt, int ldw, int M, int N, int K, bf16* out, int ldo, const bf16* bias, int epi = EPI_BIAS,
+            const bf16* resid = nullptr, int ldr = 0) {
+    if (!dry && !rc) rc = run_gemm(run, A, lda, Wt, ldw, M, N, K, out, ldo, bias, epi, resid, ldr);
   }
 
   // ---- blocks
@@ -211,18 +154,18 @@ struct Run {
     StreamBuf& sa = stream(n + ".residual.2", 2, tcap, x.H, x.W, x.C);
     Act a_in = chunk_of(sa, x.T);
     rms(x, n + ".residual.0.gamma", a_in.p, true);
-    Act t1 = scratch(x.T, x.H, x.W, Cout);
+    Act t1 = scratch_act(x.T, x.H, x.W, Cout);
     causal_conv(n + ".residual.2", sa, x.T, t1, 3);
     StreamBuf& sb = stream(n + ".residual.6", 2, tcap, x.H, x.W, Cout);
     Act b_in = chunk_of(sb, x.T);
     rms(t1, n + ".residual.3.gamma", b_in.p, true);
     const bf16* hres = x.p;
     if (x.C != Cout) {
-      Act sc = scratch(x.T, x.H, x.W, Cout);
+      Act sc = scratch_act(x.T, x.H, x.W, Cout);
       conv(n + ".shortcut", x.p, x.T, x.H, x.W, x.C, sc, 1, 1, 1, 1, 1, 1, 0, 0);
       hres = sc.p;
     }
-    Act out = scratch(x.T, x.H, x.W, Cout);
+    Act out = scratch_act(x.T, x.H, x.W, Cout);
     causal_conv(n + ".residual.6", sb, x.T, out, 3, hres);
     return out;
   }
@@ -230,27 +173,29 @@ struct Run {
   // AttentionBlock.forward (wan2pt1.py:240-259): per frame, single head of width C over H*W tokens
   Act attn_block(const std::string& n, const Act& x) {
     const int C = x.C, P = x.H * x.W, Ppad = round_up(P, 8);
-    Act xn = scratch(x.T, x.H, x.W, C);
+    Act xn = scratch_act(x.T, x.H, x.W, C);
     rms(x, n + ".norm.gamma", xn.p, false);
-    Act out = scratch(x.T, x.H, x.W, C);
-    const bf16* wqkv = W(n + ".to_qkv.weight");
-    const bf16* bqkv = W(n + ".to_qkv.bias");
-    const bf16* wproj = W(n + ".proj.weight");
-    const bf16* bproj = W(n + ".proj.bias");
-    bf16* qk = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * 2 * C * 2));
-    bf16* vT = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)C * Ppad * 2));
-    float* S = reinterpret_cast<float*>(take_scratch_bytes((size_t)P * Ppad * 4));
-    bf16* Pm = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * Ppad * 2));
-    bf16* O = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * C * 2));
-    for (int f = 0; f < x.T && !rc; ++f) {
-      const bf16* xf = dry ? nullptr : xn.p + (size_t)f * P * C;
-      gemm(xf, C, wqkv, C, P, 2 * C, C, qk, 2 * C, bqkv, nullptr, nullptr);                                      // q | k
-      gemm(wqkv ? wqkv + (size_t)2 * C * C : nullptr, C, xf, C, C, Ppad, C, vT, Ppad, nullptr, bqkv ? bqkv + 2 * C : nullptr, nullptr);  // V^T (+ b_v per row)
-      gemm(qk, 2 * C, qk ? qk + C : nullptr, 2 * C, P, Ppad, C, nullptr, 0, nullptr, nullptr, S);              // S = q k^T (fp32)
-      if (!dry && !rc) ok(launch_softmax_rows(S, Ppad, Pm, Ppad, P, P, 1.0f / sqrtf((float)C), s));
-      gemm(Pm, Ppad, vT, Ppad, P, C, P, O, C, nullptr, nullptr, nullptr);                                       // O = P V
-      gemm(O, C, wproj, C, P, C, C, dry ? nullptr : out.p + (size_t)f * P * C, C, bproj, nullptr, nullptr, EPI_BIAS_RESID,
-           dry ? nullptr : x.p + (size_t)f * P * C, C);                                                         // proj + identity
+    Act out = scratch_act(x.T, x.H, x.W, C);
+    GemmAttention a;
+    a.wqk = weights.any<bf16>(n + ".to_qkv.weight", (int64_t)3 * C * C);
+    a.bqk = weights.any<bf16>(n + ".to_qkv.bias", 3 * C);
+    a.wv = a.wqk ? a.wqk + (size_t)2 * C * C : nullptr;
+    a.bv = a.bqk ? a.bqk + 2 * C : nullptr;
+    const bf16* wproj = weights.any<bf16>(n + ".proj.weight", (int64_t)C * C);
+    const bf16* bproj = weights.any<bf16>(n + ".proj.bias", C);
+    a.L = P; a.D = C; a.H = 1; a.dk = C; a.kpv = P;
+    a.sc.rule = SOFTMAX_SCALED;
+    a.sc.scale = 1.0f / sqrtf((float)C);
+    a.qk = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * 2 * C * 2));
+    a.vT = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)C * Ppad * 2));
+    a.S = reinterpret_cast<float*>(take_scratch_bytes((size_t)P * Ppad * 4));
+    a.P = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * Ppad * 2));
+    a.out = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * C * 2));
+    a.ldo = C;
+    for (int f = 0; f < x.T && !dry && !rc; ++f) {
+      a.x = xn.p + (size_t)f * P * C;
+      rc = gemm_attention(run, a);
+      gemm(a.out, C, wproj, C, P, C, C, out.p + (size_t)f * P * C, C, bproj, EPI_BIAS_RESID, x.p + (size_t)f * P * C, C);   // proj + identity
     }
     return out;
   }
@@ -265,14 +210,14 @@ struct Run {
       } else {
         Act in = chunk_of(st, x.T);
         copy(x, in.p);
-        Act y = scratch(2 * x.T, x.H, x.W, C);
+        Act y = scratch_act(2 * x.T, x.H, x.W, C);
         causal_conv(n + ".time_conv", st, x.T, y, 1, nullptr, /*split_time=*/1);
         x = y;
       }
     }
-    Act up = scratch(x.T, 2 * x.H, 2 * x.W, C);
-    if (!dry && !rc) ok(launch_upsample2x_cl(x.p, up.p, x.T, x.H, x.W, C, s));
-    Act out = scratch(x.T, 2 * x.H, 2 * x.W, C / 2);
+    Act up = scratch_act(x.T, 2 * x.H, 2 * x.W, C);
+    launch([&] { return launch_upsample2x_cl(x.p, up.p, x.T, x.H, x.W, C, s); });
+    Act out = scratch_act(x.T, 2 * x.H, 2 * x.W, C / 2);
     conv(n + ".resample.1", up.p, up.T, up.H, up.W, C, out, 1, 3, 3, 1, 1, 1, 1, 1);
     return out;
   }
@@ -282,7 +227,7 @@ struct Run {
     const int C = x.C;
     const int Ho = (x.H + 1 - 3) / 2 + 1, Wo = (x.W + 1 - 3) / 2 + 1;
     if (!temporal) {
-      Act out = scratch(x.T, Ho, Wo, C);
+      Act out = scratch_act(x.T, Ho, Wo, C);
       conv(n + ".resample.1", x.p, x.T, x.H, x.W, C, out, 1, 3, 3, 1, 2, 2, 0, 0);  // ZeroPad2d(0,1,0,1) = OOB zero fill
       return out;
     }
@@ -291,13 +236,13 @@ struct Run {
     conv(n + ".resample.1", x.p, x.T, x.H, x.W, C, sp, 1, 3, 3, 1, 2, 2, 0, 0);
     if (!st.primed) {  // first chunk passes through and becomes the history (:147-150)
       st.primed = true;
-      Act out = scratch(x.T, Ho, Wo, C);
+      Act out = scratch_act(x.T, Ho, Wo, C);
       copy(sp, out.p);
       push_history(st, x.T);
       return out;
     }
     const int To = (1 + x.T - 3) / 2 + 1;
-    Act out = scratch(To, Ho, Wo, C);
+    Act out = scratch_act(To, Ho, Wo, C);
     conv(n + ".time_conv", st.p, 1 + x.T, Ho, Wo, C, out, 3, 1, 1, 2, 1, 1, 0, 0);
     push_history(st, x.T);
     return out;
@@ -308,11 +253,10 @@ struct Run {
                   int t_base, int kt, int kh, bf16* out, int ldo, int Tout, int Cout) {
     const int K = kt * kh * kh * Cin, Kpad = round_up(K, 8);
     bf16* A = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)Tout * Hin * Win * Kpad * 2));
-    const bf16* w = W(name + ".weight");
-    const bf16* b = W(name + ".bias");
-    if (dry || rc) return;
-    ok(launch_im2row(x, sc, st_, sh, sw, Tin, Hin, Win, Cin, A, Kpad, Tout, Hin, Win, kt, kh, kh, kh / 2, kh / 2, t_base, s));
-    gemm(A, Kpad, w, Kpad, Tout * Hin * Win, Cout, Kpad, out, ldo, b, nullptr, nullptr);
+    const bf16* w = weights.any<bf16>(name + ".weight", (int64_t)Cout * Kpad);
+    const bf16* b = weights.any<bf16>(name + ".bias", Cout);
+    launch([&] { return launch_im2row(x, sc, st_, sh, sw, Tin, Hin, Win, Cin, A, Kpad, Tout, Hin, Win, kt, kh, kh, kh / 2, kh / 2, t_base, s); });
+    gemm(A, Kpad, w, Kpad, Tout * Hin * Win, Cout, Kpad, out, ldo, b);
   }
 };
 
@@ -371,7 +315,7 @@ int run_decode(Run& R, const bf16* z, bf16* video, int Tl, int h, int w, int cla
     Act x0 = R.chunk_of(s1, 1);
     R.small_conv("conv2", z, zplane, (size_t)h * w, (size_t)w, 1, Tl, h, w, zc, /*t_base=*/i, 1, 1, x0.p, zc, 1, zc);
     // decoder.conv1: 3x3x3 causal with Cin = z_dim: im2row over [history ; chunk] (channels-last) + GEMM
-    Act x = R.scratch(1, h, w, top);
+    Act x = R.scratch_act(1, h, w, top);
     R.small_conv("decoder.conv1", s1.p, 1, (size_t)h * w * zc, (size_t)w * zc, (size_t)zc, s1.hist + 1, h, w, zc, 0, 3, 3, x.p, top, 1, top);
     R.push_history(s1, 1);
     x = R.res_block("decoder.middle.0", x, top, cap);
@@ -392,17 +336,15 @@ int run_decode(Run& R, const bf16* z, bf16* video, int Tl, int h, int w, int cla
     Act hin = R.chunk_of(sh, x.T);
     R.rms(x, "decoder.head.0.gamma", hin.p, true);
     {
-      const bf16* wgt = R.W("decoder.head.2.weight");
-      const bf16* b = R.W("decoder.head.2.bias");
-      if (!R.dry && !R.rc) {
-        ConvArgs a;
-        a.x = sh.p; a.Tin = sh.hist + x.T; a.Hin = x.H; a.Win = x.W; a.Cin = x.C;
-        a.w = wgt; a.bias = b; a.Cout = 3; a.Cin_pad = round_up(x.C, 64);
-        a.kt = 3; a.kh = 3; a.kw = 3; a.ph = 1; a.pw = 1;
-        a.y = video; a.Tout = x.T; a.Hout = x.H; a.Wout = x.W;
-        a.planar_out = 1; a.clamp = clamp; a.planar_T = T_px; a.planar_t0 = t_out;
-        R.ok(launch_conv3d_cl(a, R.s));
-      }
+      ConvArgs a;
+      a.x = sh.p; a.Tin = sh.hist + x.T; a.Hin = x.H; a.Win = x.W; a.Cin = x.C;
+      a.Cout = 3; a.Cin_pad = round_up(x.C, 64);
+      a.w = R.weights.any<bf16>("decoder.head.2.weight", (int64_t)3 * 27 * a.Cin_pad);
+      a.bias = R.weights.any<bf16>("decoder.head.2.bias", 3);
+      a.kt = 3; a.kh = 3; a.kw = 3; a.ph = 1; a.pw = 1;
+      a.y = video; a.Tout = x.T; a.Hout = x.H; a.Wout = x.W;
+      a.planar_out = 1; a.clamp = clamp; a.planar_T = T_px; a.planar_t0 = t_out;
+      R.launch([&] { return launch_conv3d_cl(a, R.s); });
       R.push_history(sh, x.T);
     }
     t_out += x.T;
@@ -418,13 +360,13 @@ int run_encode(Run& R, const bf16* video, bf16* mu, int T, int H, int Wd) {
   const int top = top_dim(c), zc = c.z_dim;
   const int Tl = 1 + (T - 1) / 4, h = H / 8, w = Wd / 8;
   std::vector<LayerSpec> layers = encoder_layers(c);
-  bf16* enc_out = R.take_persist((size_t)Tl * h * w * 2 * zc);  // head outputs of every chunk, channels-last
+  bf16* enc_out = R.persist.take<bf16>((int64_t)Tl * h * w * 2 * zc);  // head outputs of every chunk, channels-last
   int t_lat = 0;
   for (int f0 = 0; f0 < T && !R.rc;) {
     const int Tc = f0 == 0 ? 1 : 4;
     R.reset_scratch();
     int cap = 4;
-    Act x = R.scratch(Tc, H, Wd, c.dim);
+    Act x = R.scratch_act(Tc, H, Wd, c.dim);
     // encoder.conv1: 3x3x3 causal with Cin = 3 straight from the planar video (its own past frames are the history)
     R.small_conv("encoder.conv1", video, (size_t)T * H * Wd, (size_t)H * Wd, (size_t)Wd, 1, T, H, Wd, 3, /*t_base=*/f0 - 2, 3, 3, x.p, c.dim, Tc,
                  c.dim);
@@ -457,8 +399,9 @@ int run_encode(Run& R, const bf16* video, bf16* mu, int T, int H, int Wd) {
   R.reset_scratch();
   const size_t P = (size_t)Tl * h * w;
   bf16* q = reinterpret_cast<bf16*>(R.take_scratch_bytes(P * 2 * zc * 2));
-  R.gemm(enc_out, 2 * zc, R.W("conv1.weight"), 2 * zc, (int)P, 2 * zc, 2 * zc, q, 2 * zc, R.W("conv1.bias"), nullptr, nullptr);
-  if (!R.dry && !R.rc) R.ok(launch_cl_to_planar(q, 2 * zc, mu, P, 2 * zc, R.s));  // moments = mean | logvar
+  const bf16* w1 = R.weights.any<bf16>("conv1.weight", (int64_t)4 * zc * zc);
+  R.gemm(enc_out, 2 * zc, w1, 2 * zc, (int)P, 2 * zc, 2 * zc, q, 2 * zc, R.weights.any<bf16>("conv1.bias", 2 * zc));
+  R.launch([&] { return launch_cl_to_planar(q, 2 * zc, mu, P, 2 * zc, R.s); });  // moments = mean | logvar
   return R.rc;
 }
 
@@ -491,22 +434,15 @@ int ce_vae_create(const ce_vae_config* cfg, ce_vae** out) {
 void ce_vae_destroy(ce_vae* h) { delete h; }
 
 int ce_vae_set_weight(ce_vae* h, const char* name, const void* ptr, int64_t numel) {
-  CE_REQUIRE(h && name && ptr, "ce_vae_set_weight: null argument");
-  CE_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "ce_vae_set_weight: pointer must be 16-byte aligned");
-  VWeight w;
-  w.ptr = ptr;
-  w.numel = numel;
-  h->w[name] = w;
-  return CE_OK;
+  CE_REQUIRE(h, "ce_vae_set_weight: null handle");
+  return register_weight(h->w, "ce_vae_set_weight", name, ptr, -1, numel);
 }
 
 int64_t ce_vae_workspace_bytes(ce_vae* h, int decode, int frames, int height, int width) {
   if (check_geometry(h, frames, height, width, decode != 0)) return -1;
-  Run plan{h, nullptr, true, nullptr};
+  Run plan(h, nullptr, nullptr, nullptr);
   int rc = decode ? run_decode(plan, nullptr, nullptr, frames, height, width, 0) : run_encode(plan, nullptr, nullptr, frames, height, width);
-  if (rc) return -1;
-  const int64_t persist = (plan.persist_off + 255) & ~int64_t(255);
-  return persist + ((plan.scratch_max + 255) & ~int64_t(255)) + 256;
+  return rc || plan.weights.rc ? -1 : plan.workspace_bytes();
 }
 
 static int run(ce_vae* h, bool decode, const void* in, void* out, int frames, int height, int width, int clamp, void* workspace,
@@ -517,15 +453,14 @@ static int run(ce_vae* h, bool decode, const void* in, void* out, int frames, in
   CE_REQUIRE(in && out && workspace, "vae: null argument");
   CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "vae: workspace must be 256-byte aligned");
   // plan first: sizes of the persistent region (stream buffers) and of the per-chunk scratch
-  Run plan{h, nullptr, true, nullptr};
+  Run plan(h, nullptr, nullptr, nullptr);
   rc = decode ? run_decode(plan, nullptr, nullptr, frames, height, width, 0) : run_encode(plan, nullptr, nullptr, frames, height, width);
-  if (rc) return rc;
-  const int64_t persist = (plan.persist_off + 255) & ~int64_t(255);
-  const int64_t need = persist + ((plan.scratch_max + 255) & ~int64_t(255)) + 256;
+  if (rc || (rc = plan.weights.rc)) return rc;
+  const int64_t need = plan.workspace_bytes();
   if (need > workspace_bytes)
     return fail(CE_ERR_WORKSPACE, "vae: workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(workspace_bytes));
-  Run R{h, reinterpret_cast<cudaStream_t>(stream), false, reinterpret_cast<uint8_t*>(workspace)};
-  R.scratch_base = persist;
+  uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
+  Run R(h, reinterpret_cast<cudaStream_t>(stream), base, base + plan.persist.bytes());
   h->launches = 0;
   return decode ? run_decode(R, reinterpret_cast<const bf16*>(in), reinterpret_cast<bf16*>(out), frames, height, width, clamp)
                 : run_encode(R, reinterpret_cast<const bf16*>(in), reinterpret_cast<bf16*>(out), frames, height, width);

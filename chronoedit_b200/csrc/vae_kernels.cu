@@ -1,5 +1,5 @@
 // HBM-bound kernels of the Wan VAE path (channels-last bf16): RMS_norm(+SiLU), nearest 2x upsample, im2row for the
-// few small-Cin convolutions, row softmax for the single-head mid attention, layout conversion.
+// few small-Cin convolutions, layout conversion.
 #include "vae_kernels.cuh"
 
 namespace ce {
@@ -117,29 +117,6 @@ im2row_kernel(const bf16* __restrict__ x, size_t sc, size_t st, size_t sh, size_
   }
 }
 
-// P[r, :] = softmax(S[r, :] * scale) in fp32, stored bf16.
-__global__ void __launch_bounds__(256)
-softmax_rows_kernel(const float* __restrict__ S, int lds, bf16* __restrict__ P, int ldp, int cols, float scale) {
-  __shared__ float red[32];
-  const float* s = S + (size_t)blockIdx.x * lds;
-  bf16* p = P + (size_t)blockIdx.x * ldp;
-  float mx = -INFINITY;
-  for (int i = threadIdx.x; i < cols; i += blockDim.x) mx = fmaxf(mx, s[i]);
-  mx = warp_max(mx);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
-  __syncthreads();
-  mx = warp_max((threadIdx.x & 31) < (blockDim.x >> 5) ? red[threadIdx.x & 31] : -INFINITY);
-  __syncthreads();
-  float sum = 0.f;
-  for (int i = threadIdx.x; i < cols; i += blockDim.x) sum += __expf((s[i] - mx) * scale);
-  sum = warp_sum(sum);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sum;
-  __syncthreads();
-  sum = warp_sum((threadIdx.x & 31) < (blockDim.x >> 5) ? red[threadIdx.x & 31] : 0.f);
-  const float inv = 1.0f / sum;
-  for (int i = threadIdx.x; i < cols; i += blockDim.x) p[i] = __float2bfloat16_rn(__expf((s[i] - mx) * scale) * inv);
-}
-
 // planar[c, p] = cl[p, c] for c < Cout (posterior mean = first z_dim channels of conv1's output)
 __global__ void cl_to_planar_kernel(const bf16* __restrict__ cl, int C, bf16* __restrict__ planar, size_t pixels, int Cout) {
   const size_t total = pixels * Cout;
@@ -150,22 +127,16 @@ __global__ void cl_to_planar_kernel(const bf16* __restrict__ cl, int C, bf16* __
   }
 }
 
-int grid_for(size_t total, int block) {
-  size_t g = (total + block - 1) / block;
-  const size_t cap = (size_t)device_sm_count() * 16;
-  return (int)(g < cap ? (g == 0 ? 1 : g) : cap);
-}
-
 }  // namespace
 
 int launch_rms_silu_cl(const bf16* x, const bf16* gamma, bf16* y, size_t pixels, int C, int apply_silu, cudaStream_t stream) {
   CE_REQUIRE(C % 8 == 0 && C <= 512, "rms_silu: C % 8, C <= 512");
   if (C <= 256 / 2) {
     const size_t threads = pixels * 16;
-    rms_silu_cl_kernel<16><<<grid_for(threads, 256), 256, 0, stream>>>(x, gamma, y, pixels, C, apply_silu);
+    rms_silu_cl_kernel<16><<<grid_for(threads), TPB, 0, stream>>>(x, gamma, y, pixels, C, apply_silu);
   } else {
     const size_t threads = pixels * 32;
-    rms_silu_cl_kernel<32><<<grid_for(threads, 256), 256, 0, stream>>>(x, gamma, y, pixels, C, apply_silu);
+    rms_silu_cl_kernel<32><<<grid_for(threads), TPB, 0, stream>>>(x, gamma, y, pixels, C, apply_silu);
   }
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
@@ -174,7 +145,7 @@ int launch_rms_silu_cl(const bf16* x, const bf16* gamma, bf16* y, size_t pixels,
 int launch_upsample2x_cl(const bf16* in, bf16* out, int T, int H, int W, int C, cudaStream_t stream) {
   CE_REQUIRE(C % 8 == 0, "upsample: C % 8");
   const size_t total = (size_t)T * 4 * H * W * (C / 8);
-  upsample2x_cl_kernel<<<grid_for(total, 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out), T, H, W, C / 8);
+  upsample2x_cl_kernel<<<grid_for(total), TPB, 0, stream>>>(reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out), T, H, W, C / 8);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }
@@ -184,19 +155,13 @@ int launch_im2row(const bf16* x, size_t sc, size_t st, size_t sh, size_t sw, int
   CE_REQUIRE(Kpad % 8 == 0 && Kpad >= kt * kh * kw * Cin, "im2row: Kpad");
   CE_REQUIRE((size_t)Tout * Hout * Wout < (size_t(1) << 31) && (reinterpret_cast<uintptr_t>(A) & 15) == 0, "im2row: pixel count / alignment");
   const size_t total = (size_t)Tout * Hout * Wout * (Kpad / 8);
-  im2row_kernel<<<grid_for(total, 256), 256, 0, stream>>>(x, sc, st, sh, sw, Tin, Hin, Win, Cin, A, Kpad, Tout, Hout, Wout, kt, kh, kw, ph, pw, t_base);
-  CE_CHECK_CUDA(cudaGetLastError());
-  return CE_OK;
-}
-
-int launch_softmax_rows(const float* S, int lds, bf16* P, int ldp, int rows, int cols, float scale, cudaStream_t stream) {
-  softmax_rows_kernel<<<rows, 256, 0, stream>>>(S, lds, P, ldp, cols, scale);
+  im2row_kernel<<<grid_for(total), TPB, 0, stream>>>(x, sc, st, sh, sw, Tin, Hin, Win, Cin, A, Kpad, Tout, Hout, Wout, kt, kh, kw, ph, pw, t_base);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }
 
 int launch_cl_to_planar(const bf16* cl, int C, bf16* planar, size_t pixels, int Cout, cudaStream_t stream) {
-  cl_to_planar_kernel<<<grid_for(pixels * Cout, 256), 256, 0, stream>>>(cl, C, planar, pixels, Cout);
+  cl_to_planar_kernel<<<grid_for(pixels * Cout), TPB, 0, stream>>>(cl, C, planar, pixels, Cout);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }

@@ -187,8 +187,10 @@ int ce_vae_create(const ce_vae_config* cfg, ce_vae** out);
 void ce_vae_destroy(ce_vae* h);
 /* Parameters by the in-tree twin's names (e.g. "decoder.upsamples.3.time_conv.weight"), all bf16, PRE-PACKED by the caller:
  *   convolution weights [Cout, Cin, kt, kh, kw] -> [Cout, taps, Cin_pad] with taps ordered (dt, dh, dw), Cin_pad = Cin rounded
- *     up to 64 (zero filled) when Cin >= 64; for Cin < 64 -> [Cout, Kpad] with K = taps*Cin rounded up to 8;
- *   "*.gamma" [C]; attention "to_qkv.weight" [3C, C], "proj.weight" [C, C]; biases [Cout]. */
+ *     up to 64 (zero filled); the four small convolutions (encoder.conv1, decoder.conv1, conv1, conv2) -> [Cout, Kpad] with
+ *     K = taps*Cin rounded up to 8;
+ *   "*.gamma" [C]; attention "to_qkv.weight" [3C, C], "proj.weight" [C, C]; biases [Cout].
+ * numel is checked against these sizes before anything is launched (ce_vae_workspace_bytes fails on a missing or mis-sized weight). */
 int ce_vae_set_weight(ce_vae* h, const char* name, const void* ptr, int64_t numel);
 /* decode != 0: (frames, height, width) is the LATENT geometry; else the PIXEL geometry. */
 int64_t ce_vae_workspace_bytes(ce_vae* h, int decode, int frames, int height, int width);
