@@ -2,15 +2,19 @@
 //
 // Persistent, warp-specialised, one CTA per SM, 384 threads = 3 warpgroups (registers re-partitioned with setmaxnreg):
 //   warpgroup 0     TMA producer (one lane of warp 0): per k-block one A tile BMxBK and one B tile BNxBK into the next stage
-//                   of a STAGES-deep ring (128B swizzle); the operation supplies the coordinates
+//                   of a STAGES-deep ring (128B swizzle); the operation supplies the coordinates.  Given epilogue_warps, its
+//                   warps 1-3 are the operation's epilogue warps (the GEMM's: they take the rounded tile from the consumers
+//                   through shared memory and finish it while the consumers run the next tile's main loop); otherwise they idle
 //   warpgroups 1,2  consumers: 64 rows x BN columns of the tile each, 4 x wgmma (M64, N=BN, K16 bf16 / K32 e4m3) per k-block with both operands
-//                   read from the ring, then the operation's epilogue from the accumulator registers -> global
-// Both roles walk the same tiles (RingTiles) and ring positions, so the producer fills the ring for tile i+1 while the
+//                   read from the ring, then the operation's epilogue from the accumulator registers
+// All roles walk the same tiles (RingTiles) and ring positions, so the producer fills the ring for tile i+1 while the
 // consumers run the epilogue of tile i.  A kernel calls ring.start() with its producer, then `for (int t : RingTiles{n})
 // { ring.mma_tile(acc, kblocks); epilogue }` in its own body (a lambda epilogue ran the BN = 192 conv 10 % slower, H100 700 W).
 #pragma once
 #include "host_common.h"
 #include "wgmma.cuh"
+
+#include <type_traits>
 
 namespace ce {
 
@@ -37,7 +41,13 @@ struct RingTiles {
 __device__ __forceinline__ int ring_row() { return ((threadIdx.x >> 5) - 4) * 16 + ((threadIdx.x & 31) >> 2); }
 __device__ __forceinline__ int ring_col() { return 2 * (threadIdx.x & 3); }
 
-// Shared memory, from a 1024-byte aligned base (the 128B swizzle atom): A ring, B ring, full[STAGES], empty[STAGES].
+// Ring::start()'s default for a kernel without epilogue warps.
+struct NoEpilogueWarps {
+  __device__ __forceinline__ void operator()() const {}
+};
+
+// Shared memory, from a 1024-byte aligned base (the 128B swizzle atom): A ring, B ring, then 256 bytes of barriers: full[STAGES],
+// empty[STAGES] and, from empty + STAGES, room for the operation's own; the operation's shared memory starts at tail().
 // `stage` / `phase` are one role's position in the ring; each role keeps its own copy and carries it from tile to tile.
 template <int BN, int STAGES>
 struct Ring {
@@ -59,10 +69,17 @@ struct Ring {
     empty = full + STAGES;
   }
 
-  // Barrier init and role split.  Warpgroup 0 gives its registers up, runs produce(t) on one lane for every tile t of this
-  // CTA and returns false; the consumer warpgroups take the registers and return true.
-  template <class Produce>
-  __device__ __forceinline__ bool start(const CUtensorMap* tma_a, const CUtensorMap* tma_b, int num_tiles, Produce&& produce) {
+  __device__ __forceinline__ uint8_t* tail() const { return reinterpret_cast<uint8_t*>(full) + 256; }
+
+  // Barrier init and role split.  Warpgroup 0 gives registers up, runs produce(t) on one lane for every tile t of this CTA and,
+  // given epilogue_warps, runs it on its warps 1-3; then it returns false.  The consumer warpgroups take the registers and
+  // return true.  Registers per thread: 40 / 232 / 232, or with epilogue warps, which need more than the producer,
+  // 88 / 208 / 208 (the kernel itself is compiled to 168, the 384-thread bound).  The epilogue warps run in here, as the
+  // producer does: when the kernel picked the role after start() returned, ptxas dropped both setmaxnreg (C7507).
+  template <class Produce, class EpilogueWarps = NoEpilogueWarps>
+  __device__ __forceinline__ bool start(const CUtensorMap* tma_a, const CUtensorMap* tma_b, int num_tiles, Produce&& produce,
+                                        EpilogueWarps&& epilogue_warps = EpilogueWarps()) {
+    constexpr bool EPI = !std::is_same<std::decay_t<EpilogueWarps>, NoEpilogueWarps>::value;
     if (threadIdx.x == 0) {
       for (int i = 0; i < STAGES; ++i) {
         mbar_init(&full[i], 1);
@@ -74,12 +91,15 @@ struct Ring {
     }
     __syncthreads();
     if (threadIdx.x < 128) {
-      setmaxnreg_dec<40>();
+      setmaxnreg_dec<EPI ? 88 : 40>();
       if (threadIdx.x < 32 && elect_one_sync())
         for (int t : RingTiles{num_tiles}) produce(t);
+      if constexpr (EPI) {
+        if (threadIdx.x >= 32) epilogue_warps();
+      }
       return false;
     }
-    setmaxnreg_inc<232>();
+    setmaxnreg_inc<EPI ? 208 : 232>();
     return true;
   }
 
@@ -131,10 +151,11 @@ struct Ring {
   }
 };
 
-// Persistent launch of a ring kernel: min(tiles, SM count) CTAs of RING_THREADS threads, one per SM.
-template <int BN, int STAGES, class... Params>
+// Persistent launch of a ring kernel: min(tiles, SM count) CTAs of RING_THREADS threads, one per SM, with EXTRA bytes of
+// shared memory after the ring for the operation (Ring::tail()).
+template <int BN, int STAGES, size_t EXTRA = 0, class... Params>
 int launch_ring_gemm(void (*kernel)(Params...), int tiles, cudaStream_t stream, Params... params) {
-  constexpr size_t smem = Ring<BN, STAGES>::SMEM_BYTES;
+  constexpr size_t smem = Ring<BN, STAGES>::SMEM_BYTES + EXTRA;
   CE_ENSURE_SMEM(kernel, smem);
   const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
   kernel<<<grid, RING_THREADS, smem, stream>>>(params...);

@@ -1,7 +1,9 @@
 #!/usr/bin/env python
 """Operator micro-benchmarks at the 14B / 720p shapes (CUDA events, warm-up, L2-busting operand rotation).
-    python scripts/bench_ops.py [attn] [gemm [cublas]] [rows] [conv]
+    python scripts/bench_ops.py [attn] [gemm [cublas]] [gemmk] [rows] [conv]
 `gemm` times each block GEMM in bf16 and, in the fp8_* fields, as the FP8 mode runs it (quantization and e4m3 GEMM).
+`gemmk` times the bf16 o-proj GEMM over K and fits the time per wave of tiles to a + b K: `a` is the per-tile cost that does not
+scale with K (epilogue, hand-overs), `b` the main loop, printed as the TFLOP/s of all SMs while it runs.
 Prints one JSON line per op; used to iterate on a kernel without running the whole 40-layer step."""
 import json
 import math
@@ -105,10 +107,14 @@ def bench_attn_dual(B=2, H=40, Lq=7200, Lk=512, Lk2=257):
 DIT_GEMMS = [("qkv", 15360, 5120, 0, 2), ("o_proj", 5120, 5120, 3, 1), ("cross_q", 5120, 5120, 0, 2),
              ("cross_out", 5120, 5120, 4, 1), ("ffn_up", 13824, 5120, 1, 0), ("ffn_down", 5120, 13824, 3, 1),
              # EPI_BIAS without statistics at the o-proj / FFN-down shapes: the difference to those rows is the epilogue's cost
-             ("o_proj_bias_only", 5120, 5120, 0, 0), ("ffn_down_bias_only", 5120, 13824, 0, 0)]
+             ("o_proj_bias_only", 5120, 5120, 0, 0), ("ffn_down_bias_only", 5120, 13824, 0, 0),
+             # FFN up without GELU: the difference to the ffn_up row is GELU's cost
+             ("ffn_up_bias_only", 13824, 5120, 0, 0),
+             # the qkv shape at K = 64: one k-block per tile, so the time is nearly all epilogue
+             ("qkv_k64", 15360, 64, 0, 2)]
 
 
-def bench_gemm(name, N, K, epi, stats_mode, M=14400, rows_per_batch=7200, nbuf=3, cublas=True):
+def bench_gemm(name, N, K, epi, stats_mode, M=14400, rows_per_batch=7200, nbuf=3, cublas=True, fp8=True):
     A = [torch.randn(M, K, device="cuda", dtype=torch.bfloat16) for _ in range(nbuf)]
     W = [torch.randn(N, K, device="cuda", dtype=torch.bfloat16) * 0.02 for _ in range(nbuf)]
     bias = (torch.randn(N, device="cuda") * 0.02).bfloat16()
@@ -132,6 +138,9 @@ def bench_gemm(name, N, K, epi, stats_mode, M=14400, rows_per_batch=7200, nbuf=3
     ms = timeit(fn)
     row = {"op": "gemm", "name": name, "M": M, "N": N, "K": K, "epi": epi, "stats_mode": stats_mode, "ms": round(ms, 4),
            "tflops": round(2.0 * M * N * K / ms / 1e9, 1)}
+    if not fp8:
+        print(json.dumps(row), flush=True)
+        return ms
     # FP8 column: the same GEMM as the FP8 mode runs it (ce_linear_fp8_ex on e4m3 operands), and the row quantization of A
     # that precedes it in dit.cu (ce_quantize_rows_fp8, one launch per GEMM)
     from chronoedit_b200.transformer import quantize_fp8_rows
@@ -164,6 +173,20 @@ def bench_gemm(name, N, K, epi, stats_mode, M=14400, rows_per_batch=7200, nbuf=3
     if cublas:   # library bar: cuBLAS through torch on the same shapes
         ms2 = timeit(lambda: torch.matmul(A[0], W[0].t()))
         print(json.dumps({"op": "cublas_gemm", "M": M, "N": N, "K": K, "ms": round(ms2, 4), "tflops": round(2.0 * M * N * K / ms2 / 1e9, 1)}), flush=True)
+
+
+def bench_gemm_k(Ks=(1280, 2560, 5120, 10240, 13824), M=14400, N=5120):
+    """The o-proj GEMM (gate * residual + statistics) at several K: least-squares fit of ms per wave = a + b K."""
+    import numpy as np
+
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    tiles = ((M + 127) // 128) * ((N + 255) // 256)
+    waves = (tiles + sms - 1) // sms
+    per_wave = [bench_gemm(f"o_proj_k{K}", N, K, 3, 1, M=M, cublas=False, fp8=False) / waves for K in Ks]
+    b, a = np.polyfit(np.array(Ks, dtype=float), np.array(per_wave), 1)
+    print(json.dumps({"op": "gemmk_fit", "M": M, "N": N, "tiles": tiles, "waves": waves, "sms": sms,
+                      "a_us_per_tile": round(a * 1e3, 2), "b_ns_per_k": round(b * 1e6, 3),
+                      "main_loop_tflops": round(sms * 2.0 * 128 * 256 / (b * 1e-3) / 1e12, 1)}), flush=True)
 
 
 def bench_rows(M=14400, D=5120):
@@ -224,6 +247,8 @@ if __name__ == "__main__":
     if "gemm" in what:
         for case in DIT_GEMMS:
             bench_gemm(*case, cublas="cublas" in what)
+    if "gemmk" in what:
+        bench_gemm_k()
     if "rows" in what:
         bench_rows()
     if "conv" in what:
