@@ -7,8 +7,8 @@
 //   -> LN(affine) -> q GEMM -> RMSNorm(q) -> [text k|v GEMM, RMSNorm(k)] [image k|v GEMM, RMSNorm(k)] -> attention(text +
 //   image, one launch) -> out-proj GEMM with y+x epilogue -> LN+modulate -> FFN-1 GEMM with bias+GELU epilogue -> FFN-2 GEMM
 //   with gate*y+x epilogue.
-// When D % 256 == 0 the GEMM before each LN / RMSNorm also writes that norm's row statistics, and RMSNorm+RoPE(q|k) is one
-// launch; other widths take row kernels that reduce over the row themselves, and two RMSNorm+RoPE launches.
+// When D % 256 == 0 the GEMM before each LN / RMSNorm also writes that norm's row statistics; other widths take row kernels
+// that reduce over the row themselves.  RMSNorm+RoPE(q|k) is one launch either way.
 #include <math.h>
 
 #include <map>
@@ -551,12 +551,12 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   const bool ctx_compute = !(ctx_cache && ctx_reuse);
   // Row statistics for the LayerNorms / RMSNorms inside the blocks come from the epilogue of the GEMM that wrote the row whenever
   // the N tiles (256 wide) line up with the q | k | v boundaries; the row kernels are then streaming passes (elementwise.cuh).
-  // Other widths take the kernels that reduce over the row themselves.  The row kernels of both kinds take D <= 8192.
+  // Other widths get no partials, and the row kernels reduce over the row themselves.  The row kernels take D <= 8192.
   const bool st = D % 256 == 0;
   const int tD = D / 256;
+  auto partials = [&](const float2* stats, int ld) { return st ? RowPartials{stats, ld, tD, 256} : RowPartials{}; };
   auto ln = [&](const bf16* x, bf16* y, const float* scale, const float* shift, int mod_stride, int rpb, const float* w, const float* b, int is1p) {
-    return st ? launch_layernorm_stats(x, D, y, D, M, D, c.eps, scale, shift, mod_stride, rpb, w, b, is1p, ws.stats_x, tD, tD, 256, s)
-              : launch_layernorm(x, D, y, D, M, D, c.eps, scale, shift, mod_stride, rpb, w, b, s, is1p);
+    return launch_layernorm(x, D, y, D, M, D, c.eps, scale, shift, mod_stride, rpb, w, b, is1p, partials(ws.stats_x, tD), s);
   };
   // linear() epilogues: `stats` receives the output's row statistics (mode 1 for a LayerNorm, 2 for an RMSNorm) on the
   // statistics path; the residual ones update the residual stream ws.x in place, gated by a modulation chunk [B, 6D] or not
@@ -601,10 +601,11 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   if (ctx_compute && c.image_dim > 0) {  // image: FP32LayerNorm -> Linear -> GELU(erf) -> Linear -> FP32LayerNorm (:111-123)
     const int I = c.image_dim;
     LAUNCH(CAT_OTHER, 0.0, launch_layernorm(reinterpret_cast<const bf16*>(encoder_hidden_states_image), I, ws.img0, I, B * Li, I, 1e-5f, nullptr, nullptr, 0, 0,
-                                            W.img_norm1_w, W.img_norm1_b, s));
+                                            W.img_norm1_w, W.img_norm1_b, 0, RowPartials{}, s));
     if ((rc = linear(h, s, W.img_ff0, ws.img0, B * Li, I, I, ws.img1, epi(EPI_BIAS_GELU_ERF)))) return rc;
     if ((rc = linear(h, s, W.img_ff2, ws.img1, B * Li, D, I, ws.img2, epi(EPI_BIAS)))) return rc;
-    LAUNCH(CAT_OTHER, 0.0, launch_layernorm(ws.img2, D, ws.ctx_img, D, B * Li, D, 1e-5f, nullptr, nullptr, 0, 0, W.img_norm2_w, W.img_norm2_b, s));
+    LAUNCH(CAT_OTHER, 0.0, launch_layernorm(ws.img2, D, ws.ctx_img, D, B * Li, D, 1e-5f, nullptr, nullptr, 0, 0, W.img_norm2_w, W.img_norm2_b, 0,
+                                            RowPartials{}, s));
   }
 
   // ---- transformer blocks (:447-448)
@@ -627,8 +628,8 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
         sc.dst[1][w] = reinterpret_cast<bf16*>(sp.region[w] + lay.k);
         vdst[w] = reinterpret_cast<bf16*>(sp.region[w] + lay.v);
       }
-      LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope_stats(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, Lfull,
-                                                       c.attention_head_dim, ws.stats_qkv, 3 * tD, tD, s, &sc));
+      LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, Lfull,
+                                                 c.attention_head_dim, partials(ws.stats_qkv, 3 * tD), s, &sc));
       LAUNCH(CAT_OTHER, 0.0, launch_sp_scatter_cols(ws.qkv + 2 * D, 3 * D, B, L, D, vdst, sp.world, Dl, Lfull, tok0, s));
       LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));
       AttnArgs a;
@@ -645,13 +646,8 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
       LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));
       attn_in = reinterpret_cast<const bf16*>(sp.region[sp.rank] + lay.attn);
     } else {
-      if (st) {
-        LAUNCH(CAT_ROWS, 8.0 * M * D, launch_rmsnorm_rope_stats(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, L,
-                                                                c.attention_head_dim, ws.stats_qkv, 3 * tD, tD, s));
-      } else {
-        LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, h->rope_cos, h->rope_sin, L, c.attention_head_dim, s));
-        LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(ws.qkv + D, 3 * D, M, D, c.eps, lw.norm_k1, h->rope_cos, h->rope_sin, L, c.attention_head_dim, s));
-      }
+      LAUNCH(CAT_ROWS, 8.0 * M * D, launch_rmsnorm_rope(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, L,
+                                                        c.attention_head_dim, partials(ws.stats_qkv, 3 * tD), s));
       AttnArgs a;
       a.B = B; a.H = H; a.Lq = L; a.Lk = L;
       a.q = ws.qkv; a.ldq = 3 * D;
@@ -666,20 +662,18 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
     LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, nullptr, nullptr, 0, 0, lw.norm2_w, lw.norm2_b, 0));
     bf16* q2 = ws.qkv;  // [M, D]
     if ((rc = linear(h, s, lw.q2, ws.xn, M, D, D, q2, epi(EPI_BIAS, ws.stats_q2, 2)))) return rc;
-    if (st) {
-      LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope_stats(q2, D, M, D, c.eps, lw.norm_q2, nullptr, 1, nullptr, nullptr, 0, c.attention_head_dim,
-                                                              ws.stats_q2, tD, tD, s));
-    } else {
-      LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(q2, D, M, D, c.eps, lw.norm_q2, nullptr, nullptr, 0, c.attention_head_dim, s));
-    }
+    LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(q2, D, M, D, c.eps, lw.norm_q2, nullptr, 1, nullptr, nullptr, 0, c.attention_head_dim,
+                                                      partials(ws.stats_q2, tD), s));
     bf16* kv_text = kv_text_of(i);
     bf16* kv_img = kv_img_of(i);
     if (ctx_compute) {
       if ((rc = linear(h, s, lw.kv, ws.ctx_text, B * Lt, 2 * D, D, kv_text, epi(EPI_BIAS)))) return rc;
-      LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(kv_text, 2 * D, B * Lt, D, c.eps, lw.norm_k2, nullptr, nullptr, 0, c.attention_head_dim, s));
+      LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(kv_text, 2 * D, B * Lt, D, c.eps, lw.norm_k2, nullptr, 1, nullptr, nullptr, 0, c.attention_head_dim,
+                                                     RowPartials{}, s));
       if (c.image_dim > 0) {
         if ((rc = linear(h, s, lw.add_kv, ws.ctx_img, B * Li, 2 * D, D, kv_img, epi(EPI_BIAS)))) return rc;
-        LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(kv_img, 2 * D, B * Li, D, c.eps, lw.norm_added_k, nullptr, nullptr, 0, c.attention_head_dim, s));
+        LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(kv_img, 2 * D, B * Li, D, c.eps, lw.norm_added_k, nullptr, 1, nullptr, nullptr, 0, c.attention_head_dim,
+                                                       RowPartials{}, s));
       }
     }
     {  // text and image cross-attention in ONE launch: two key/value sources, two softmaxes, results added (:84-104)
@@ -871,26 +865,27 @@ int ce_layernorm_bf16(const void* x, int ldx, void* y, int ldy, int rows, int D,
   int rc = check_device();
   if (rc) return rc;
   return launch_layernorm(reinterpret_cast<const bf16*>(x), ldx, reinterpret_cast<bf16*>(y), ldy, rows, D, eps, scale, shift, mod_stride,
-                          rows_per_batch, weight, bias, reinterpret_cast<cudaStream_t>(stream));
+                          rows_per_batch, weight, bias, 0, RowPartials{}, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ce_rmsnorm_rope_bf16(void* x, int ldx, int rows, int D, float eps, const void* weight, const float* rope_cos, const float* rope_sin,
                          int L, int head_dim, void* stream) {
   int rc = check_device();
   if (rc) return rc;
-  return launch_rmsnorm_rope(reinterpret_cast<bf16*>(x), ldx, rows, D, eps, reinterpret_cast<const bf16*>(weight), rope_cos, rope_sin, L,
-                             head_dim, reinterpret_cast<cudaStream_t>(stream));
+  return launch_rmsnorm_rope(reinterpret_cast<bf16*>(x), ldx, rows, D, eps, reinterpret_cast<const bf16*>(weight), nullptr, 1, rope_cos,
+                             rope_sin, L, head_dim, RowPartials{}, reinterpret_cast<cudaStream_t>(stream));
 }
 
-// Test aids: the two row kernels that take their statistics from GEMM epilogue partials (GemmArgs::stats_out).
+// Test aids: the two row kernels with their statistics from GEMM epilogue partials (GemmArgs::stats_out), or reduced in the kernel
+// when stats is null.
 int ce_layernorm_stats_bf16(const void* x, int ldx, void* y, int ldy, int rows, int D, float eps, const float* scale, const float* shift,
                             int mod_stride, int rows_per_batch, const float* weight, const float* bias, int scale_is_1p, const float* stats,
                             int stats_ld, int tiles, int tile_n, void* stream) {
   int rc = check_device();
   if (rc) return rc;
-  return launch_layernorm_stats(reinterpret_cast<const bf16*>(x), ldx, reinterpret_cast<bf16*>(y), ldy, rows, D, eps, scale, shift, mod_stride,
-                                rows_per_batch, weight, bias, scale_is_1p, reinterpret_cast<const float2*>(stats), stats_ld, tiles, tile_n,
-                                reinterpret_cast<cudaStream_t>(stream));
+  return launch_layernorm(reinterpret_cast<const bf16*>(x), ldx, reinterpret_cast<bf16*>(y), ldy, rows, D, eps, scale, shift, mod_stride,
+                          rows_per_batch, weight, bias, scale_is_1p, RowPartials{reinterpret_cast<const float2*>(stats), stats_ld, tiles, tile_n},
+                          reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ce_rmsnorm_rope_stats_bf16(void* x, int ldx, int rows, int D, float eps, const void* weight0, const void* weight1, int nmat,
@@ -898,9 +893,9 @@ int ce_rmsnorm_rope_stats_bf16(void* x, int ldx, int rows, int D, float eps, con
                                void* stream) {
   int rc = check_device();
   if (rc) return rc;
-  return launch_rmsnorm_rope_stats(reinterpret_cast<bf16*>(x), ldx, rows, D, eps, reinterpret_cast<const bf16*>(weight0),
-                                   reinterpret_cast<const bf16*>(weight1), nmat, rope_cos, rope_sin, L, head_dim,
-                                   reinterpret_cast<const float2*>(stats), stats_ld, tiles, reinterpret_cast<cudaStream_t>(stream));
+  return launch_rmsnorm_rope(reinterpret_cast<bf16*>(x), ldx, rows, D, eps, reinterpret_cast<const bf16*>(weight0),
+                             reinterpret_cast<const bf16*>(weight1), nmat, rope_cos, rope_sin, L, head_dim,
+                             RowPartials{reinterpret_cast<const float2*>(stats), stats_ld, tiles, 0}, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ce_rope_table_host(int head_dim, int frames, int height_patches, int width_patches, int max_seq_len, int temporal_skip_len, float theta,

@@ -5,6 +5,8 @@
 
 #include <cuda_fp8.h>
 
+#include <type_traits>
+
 namespace ce {
 
 namespace {
@@ -21,9 +23,14 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// One WARP PAIR per token row (4 rows per 256-thread CTA): each lane keeps HV 16-byte vectors of the row in registers,
-// all of them loaded before anything consumes them; statistics = warp shuffles + one 64-thread named barrier.
-// ~100 registers/thread -> 16+ resident warps per SM, so one row's arithmetic overlaps other rows' loads.
+// LayerNorm and RMSNorm: one WARP PAIR per token row (4 rows per 256-thread CTA), 16-byte vectors.  The row statistics come from
+// one of two sources, chosen at compile time (FromPartials); the rest of each kernel is the same for both:
+//   - reduced in the kernel: each lane keeps HV 16-byte vectors of the row in registers, all of them loaded before anything consumes
+//     them; statistics = warp shuffles + one 64-thread named barrier.  ~100 registers/thread -> 16+ resident warps per SM, so one
+//     row's arithmetic overlaps other rows' loads.
+//   - per-(row, N tile) partials from the epilogue of the GEMM that produced the row (GemmArgs::stats_out): each warp merges them with
+//     shuffles and the row kernel becomes a pure streaming pass: no reduction over the data, no barrier, loads and stores of different
+//     vectors independent of each other.  The row is read from global memory where it is consumed, not held in registers.
 __device__ __forceinline__ float2 pair_sum(float a, float b, float2* part) {
   a = warp_sum(a);
   b = warp_sum(b);
@@ -34,11 +41,8 @@ __device__ __forceinline__ float2 pair_sum(float a, float b, float2* part) {
   return make_float2(a + o.x, b + o.y);
 }
 
-// ---------------------------------------------------------------------------------------------
-// Row statistics that arrive as per-(row, N tile) partials from the epilogue of the GEMM that produced the row (GemmArgs::stats_out):
-// each warp merges them with shuffles -- Chan's pairwise update for (mean, M2), always (lower lane, higher lane) so that every lane
-// ends with bit-identical values -- and the row kernel becomes a pure streaming pass: no reduction over the data, no barrier, loads
-// and stores of different vectors independent of each other.
+// Merge of the LayerNorm partials: Chan's pairwise update for (mean, M2), always (lower lane, higher lane) so that every lane ends with
+// bit-identical values.
 struct RowStat {
   float n, mean, m2;
 };
@@ -73,151 +77,69 @@ __device__ __forceinline__ RowStat warp_merge_stats(const float2* __restrict__ p
   return s;
 }
 
-template <int HV>
-__global__ void __launch_bounds__(ROW_THREADS, 2)
-layernorm_stats_kernel(const bf16* __restrict__ x, int ldx, bf16* __restrict__ y, int ldy, int rows, int D, float eps,
-                       const float* __restrict__ scale, const float* __restrict__ shift, int mod_stride, int rows_per_batch,
-                       const float* __restrict__ weight, const float* __restrict__ bias, int scale_is_1p,
-                       const float2* __restrict__ stats, int stats_ld, int tiles, int tile_n) {
-  const int lane64 = threadIdx.x & 63;
-  const int row = blockIdx.x * (ROW_THREADS / 64) + (threadIdx.x >> 6);
-  if (row >= rows) return;
-  const RowStat st = warp_merge_stats(stats + (size_t)row * stats_ld, tiles, tile_n, D);
-  const float mean = st.mean;
-  const float rstd = rsqrtf(st.m2 / (float)D + eps);
-  const float nmr = -mean * rstd;
-  const int nvec = D >> 3;
-  const int b = row / rows_per_batch;
-  const uint4* xr = reinterpret_cast<const uint4*>(x + (size_t)row * ldx);
-  uint4* yr = reinterpret_cast<uint4*>(y + (size_t)row * ldy);
-  const float* pa = scale ? scale + (size_t)b * mod_stride : weight;
-  const float* pb = scale ? shift + (size_t)b * mod_stride : bias;
+// This lane's vector lane64 + i * 64 (i < HV) of a row: from registers filled up front (zero past the row's end) when the kernel
+// reduces over the row, from global memory where it is consumed when the statistics come from partials.
+template <int HV, bool FromPartials>
+struct RowVecs {
+  const uint4* xr;
+  int lane64;
+  uint4 v[FromPartials ? 1 : HV];
+  __device__ __forceinline__ RowVecs(const uint4* xr_, int lane64_, int nvec) : xr(xr_), lane64(lane64_) {
+    if constexpr (!FromPartials) {
 #pragma unroll
-  for (int i = 0; i < HV; ++i) {
-    const int idx = lane64 + i * 64;
-    if (idx < nvec) {
-      float f[8], o[8];
-      unpack8(xr[idx], f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = fmaf(f[j], rstd, nmr);
-      if (pa) {
-        const float4* qa = reinterpret_cast<const float4*>(pa + idx * 8);
-        const float4* qb = reinterpret_cast<const float4*>(pb + idx * 8);
-        const float4 a0 = qa[0], a1 = qa[1], b0 = qb[0], b1 = qb[1];
-        const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-        const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-        if (scale && !scale_is_1p) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) o[j] = fmaf(o[j], 1.0f + av[j], bv[j]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) o[j] = fmaf(o[j], av[j], bv[j]);
-        }
-      }
-      yr[idx] = pack8(o);
+      for (int i = 0; i < HV; ++i) v[i] = lane64 + i * 64 < nvec ? xr[lane64 + i * 64] : make_uint4(0u, 0u, 0u, 0u);
     }
   }
-}
+  __device__ __forceinline__ uint4 operator[](int i) const { return FromPartials ? xr[lane64 + i * 64] : v[i]; }
+};
 
-// RMSNorm across heads (+ RoPE) from epilogue partial sums of squares; `nmat` matrices side by side in one row (q | k of the fused
-// QKV output): blockIdx.y selects the matrix (column offset y * D, its own weight and its own tile range)
-template <int HV>
-__global__ void __launch_bounds__(ROW_THREADS, 2)
-rmsnorm_rope_stats_kernel(bf16* __restrict__ x, int ldx, int rows, int D, float eps, const bf16* __restrict__ weight0,
-                          const bf16* __restrict__ weight1, const float* __restrict__ rope_cos, const float* __restrict__ rope_sin, int L,
-                          int head_dim, const float2* __restrict__ stats, int stats_ld, int tiles, SpScatter sp) {
-  const int lane64 = threadIdx.x & 63;
-  const int lane = threadIdx.x & 31;
-  const int row = blockIdx.x * (ROW_THREADS / 64) + (threadIdx.x >> 6);
-  if (row >= rows) return;
-  const int mat = blockIdx.y;
-  float ss = lane < tiles ? stats[(size_t)row * stats_ld + mat * tiles + lane].x : 0.f;
-  ss = warp_sum(ss);   // butterfly of commutative adds: identical in every lane
-  const float rstd = rsqrtf(ss / (float)D + eps);
-  const int nvec = D >> 3;
-  uint4* xr = reinterpret_cast<uint4*>(x + (size_t)row * ldx + (size_t)mat * D);
-  const uint4* wr = reinterpret_cast<const uint4*>(mat ? weight1 : weight0);
-  const int tok = sp.world ? sp.tok0 + row % sp.rows_per_batch : (rope_cos ? row % L : 0);   // global token (RoPE position)
-  const int half = head_dim >> 1;
-#pragma unroll
-  for (int i = 0; i < HV; ++i) {
-    const int idx = lane64 + i * 64;
-    if (idx < nvec) {
-      float f[8], w[8], o[8];
-      unpack8(xr[idx], f);
-      unpack8(wr[idx], w);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = bf16_round(bf16_round(f[j] * rstd) * w[j]);
-      const int c = idx * 8;
-      if (rope_cos) {
-        const int pair0 = (c % head_dim) >> 1;
-        const float4 cs = *reinterpret_cast<const float4*>(rope_cos + (size_t)tok * half + pair0);
-        const float4 sn = *reinterpret_cast<const float4*>(rope_sin + (size_t)tok * half + pair0);
-        const float cv[4] = {cs.x, cs.y, cs.z, cs.w};
-        const float sv[4] = {sn.x, sn.y, sn.z, sn.w};
-#pragma unroll
-        for (int p = 0; p < 4; ++p) {
-          const float re = o[2 * p], im = o[2 * p + 1];
-          o[2 * p] = re * cv[p] - im * sv[p];
-          o[2 * p + 1] = re * sv[p] + im * cv[p];
-        }
-      }
-      if (sp.world) {   // to the rank that owns this head (peer store)
-        const int head = c / head_dim, dr = head / sp.heads_per_rank, bi = row / sp.rows_per_batch;
-        bf16* d = sp.dst[mat][dr] + ((size_t)bi * sp.L_total + tok) * ((size_t)sp.heads_per_rank * head_dim) +
-                  (size_t)(head % sp.heads_per_rank) * head_dim + c % head_dim;
-        *reinterpret_cast<uint4*>(d) = pack8(o);
-      } else {
-        xr[idx] = pack8(o);
-      }
-    }
-  }
-}
-
-template <int HV>
+template <int HV, bool FromPartials>
 __global__ void __launch_bounds__(ROW_THREADS, 2)
 layernorm_kernel(const bf16* __restrict__ x, int ldx, bf16* __restrict__ y, int ldy, int rows, int D, float eps,
                  const float* __restrict__ scale, const float* __restrict__ shift, int mod_stride, int rows_per_batch,
-                 const float* __restrict__ weight, const float* __restrict__ bias, int scale_is_1p) {
-  __shared__ float2 part[ROW_THREADS / 32];
+                 const float* __restrict__ weight, const float* __restrict__ bias, int scale_is_1p, RowPartials ps) {
   const int lane64 = threadIdx.x & 63;
-  int row = blockIdx.x * (ROW_THREADS / 64) + (threadIdx.x >> 6);
-  const bool live = row < rows;
-  if (!live) row = rows - 1;  // keep the pair barrier balanced; results are not stored
+  const int row0 = blockIdx.x * (ROW_THREADS / 64) + (threadIdx.x >> 6);
+  const int row = min(row0, rows - 1);  // a pair past the last row joins the pair barrier, then leaves without storing
   const int nvec = D >> 3;
-  const uint4* xr = reinterpret_cast<const uint4*>(x + (size_t)row * ldx);
-  uint4 v[HV];
+  const RowVecs<HV, FromPartials> v(reinterpret_cast<const uint4*>(x + (size_t)row * ldx), lane64, nvec);
+  float mean, rstd;
+  if constexpr (FromPartials) {
+    const RowStat st = warp_merge_stats(ps.p + (size_t)row * ps.ld, ps.tiles, ps.tile_n, D);
+    mean = st.mean;
+    rstd = rsqrtf(st.m2 / (float)D + eps);
+  } else {
+    __shared__ float2 part[ROW_THREADS / 32];
+    // single statistics pass on pivot-shifted data d = x - x[row, 0]:  mean = pivot + E[d],  var = E[d^2] - E[d]^2
+    const float pivot = __bfloat162float(x[(size_t)row * ldx]);
+    float s = 0.f, ss = 0.f;
 #pragma unroll
-  for (int i = 0; i < HV; ++i) {
-    const int idx = lane64 + i * 64;
-    v[i] = idx < nvec ? xr[idx] : make_uint4(0u, 0u, 0u, 0u);
-  }
-  // single statistics pass on pivot-shifted data d = x - x[row, 0]:  mean = pivot + E[d],  var = E[d^2] - E[d]^2
-  const float pivot = __bfloat162float(x[(size_t)row * ldx]);
-  float s = 0.f, ss = 0.f;
+    for (int i = 0; i < HV; ++i) {
+      if (lane64 + i * 64 < nvec) {
+        float f[8];
+        unpack8(v[i], f);
 #pragma unroll
-  for (int i = 0; i < HV; ++i) {
-    if (lane64 + i * 64 < nvec) {
-      float f[8];
-      unpack8(v[i], f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float d = f[j] - pivot;
-        s += d;
-        ss = fmaf(d, d, ss);
+        for (int j = 0; j < 8; ++j) {
+          const float d = f[j] - pivot;
+          s += d;
+          ss = fmaf(d, d, ss);
+        }
       }
     }
+    const float2 tot = pair_sum(s, ss, part);
+    const float md = tot.x / (float)D;
+    mean = pivot + md;
+    rstd = rsqrtf(fmaxf(tot.y / (float)D - md * md, 0.f) + eps);
   }
-  const float2 tot = pair_sum(s, ss, part);
-  const float md = tot.x / (float)D;
-  const float mean = pivot + md;
-  const float rstd = rsqrtf(fmaxf(tot.y / (float)D - md * md, 0.f) + eps);
+  if (row0 >= rows) return;
   const float nmr = -mean * rstd;
   const int b = row / rows_per_batch;
   uint4* yr = reinterpret_cast<uint4*>(y + (size_t)row * ldy);
   const float* pa = scale ? scale + (size_t)b * mod_stride : weight;  // multiplier: (1 + scale) / scale / affine weight
   const float* pb = scale ? shift + (size_t)b * mod_stride : bias;
-  constexpr int G = 2;  // vectors per batch: their parameter loads are in flight together
+  // vectors per batch: their parameter loads are in flight together.  Batching pays when the row is already in registers; when it is
+  // streamed, a batch of one is faster (M = 14400, D = 5120 on an H100 80GB HBM3 at 700 W: 0.116 ms against 0.123 ms with 2).
+  constexpr int G = FromPartials ? 1 : 2;
 #pragma unroll
   for (int i0 = 0; i0 < HV; i0 += G) {
     float4 ta[G][2], tb[G][2];
@@ -252,70 +174,105 @@ layernorm_kernel(const bf16* __restrict__ x, int ldx, bf16* __restrict__ y, int 
             for (int j = 0; j < 8; ++j) o[j] = fmaf(o[j], av[j], bv[j]);
           }
         }
-        if (live) yr[idx] = pack8(o);
+        yr[idx] = pack8(o);
       }
     }
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-template <int HV>
+// RMSNorm across heads (+ RoPE) on `nmat` matrices side by side in one row (q | k of the fused QKV output): blockIdx.y selects the
+// matrix (column offset y * D, its own weight and, from partials, its own tile range)
+template <int HV, bool FromPartials>
 __global__ void __launch_bounds__(ROW_THREADS, 2)
-rmsnorm_rope_kernel(bf16* __restrict__ x, int ldx, int rows, int D, float eps, const bf16* __restrict__ weight,
-                    const float* __restrict__ rope_cos, const float* __restrict__ rope_sin, int L, int head_dim) {
-  __shared__ float2 part[ROW_THREADS / 32];
+rmsnorm_rope_kernel(bf16* __restrict__ x, int ldx, int rows, int D, float eps, const bf16* __restrict__ weight0,
+                    const bf16* __restrict__ weight1, const float* __restrict__ rope_cos, const float* __restrict__ rope_sin, int L,
+                    int head_dim, RowPartials ps, SpScatter sp) {
   const int lane64 = threadIdx.x & 63;
-  int row = blockIdx.x * (ROW_THREADS / 64) + (threadIdx.x >> 6);
-  const bool live = row < rows;
-  if (!live) row = rows - 1;
+  const int row0 = blockIdx.x * (ROW_THREADS / 64) + (threadIdx.x >> 6);
+  const int row = min(row0, rows - 1);  // a pair past the last row joins the pair barrier, then leaves without storing
+  const int mat = blockIdx.y;
   const int nvec = D >> 3;
-  uint4* xr = reinterpret_cast<uint4*>(x + (size_t)row * ldx);
-  const uint4* wr = reinterpret_cast<const uint4*>(weight);
-  uint4 v[HV];
+  uint4* xr = reinterpret_cast<uint4*>(x + (size_t)row * ldx + (size_t)mat * D);
+  const RowVecs<HV, FromPartials> v(xr, lane64, nvec);
+  float rstd;
+  if constexpr (FromPartials) {
+    const int lane = threadIdx.x & 31;
+    float ss = lane < ps.tiles ? ps.p[(size_t)row * ps.ld + mat * ps.tiles + lane].x : 0.f;
+    ss = warp_sum(ss);   // butterfly of commutative adds: identical in every lane
+    rstd = rsqrtf(ss / (float)D + eps);
+  } else {
+    __shared__ float2 part[ROW_THREADS / 32];
+    float ss = 0.f;
 #pragma unroll
-  for (int i = 0; i < HV; ++i) {
-    const int idx = lane64 + i * 64;
-    v[i] = idx < nvec ? xr[idx] : make_uint4(0u, 0u, 0u, 0u);
-  }
-  float ss = 0.f;
-#pragma unroll
-  for (int i = 0; i < HV; ++i) {
-    float f[8];
-    unpack8(v[i], f);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) ss = fmaf(f[j], f[j], ss);
-  }
-  const float2 tot = pair_sum(ss, 0.f, part);
-  const float rstd = rsqrtf(tot.x / (float)D + eps);
-  const int tok = rope_cos ? row % L : 0;
-  const int half = head_dim >> 1;
-#pragma unroll
-  for (int i = 0; i < HV; ++i) {
-    const int idx = lane64 + i * 64;
-    if (idx < nvec) {
-      float f[8], w[8], o[8];
+    for (int i = 0; i < HV; ++i) {
+      float f[8];
       unpack8(v[i], f);
-      unpack8(wr[idx], w);
-      // diffusers RMSNorm with a bf16 weight: (x * rstd) rounded to bf16, then * weight (bf16 multiply)
 #pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = bf16_round(bf16_round(f[j] * rstd) * w[j]);
-      if (rope_cos) {
-        const int c = idx * 8;
-        const int pair0 = (c % head_dim) >> 1;  // 4 consecutive (even, odd) pairs of one head
-        const float4 cs = *reinterpret_cast<const float4*>(rope_cos + (size_t)tok * half + pair0);
-        const float4 sn = *reinterpret_cast<const float4*>(rope_sin + (size_t)tok * half + pair0);
-        const float cv[4] = {cs.x, cs.y, cs.z, cs.w};
-        const float sv[4] = {sn.x, sn.y, sn.z, sn.w};
-#pragma unroll
-        for (int p = 0; p < 4; ++p) {
-          const float re = o[2 * p], im = o[2 * p + 1];
-          o[2 * p] = re * cv[p] - im * sv[p];
-          o[2 * p + 1] = re * sv[p] + im * cv[p];
-        }
-      }
-      if (live) xr[idx] = pack8(o);
+      for (int j = 0; j < 8; ++j) ss = fmaf(f[j], f[j], ss);
     }
+    const float2 tot = pair_sum(ss, 0.f, part);
+    rstd = rsqrtf(tot.x / (float)D + eps);
   }
+  if (row0 >= rows) return;
+  const uint4* wr = reinterpret_cast<const uint4*>(mat ? weight1 : weight0);
+  // the sequence-parallel scatter runs only with partials: it requires D % 256 == 0, where the GEMM writes them (launcher check)
+  const bool scatter = FromPartials && sp.world;
+  const int tok = scatter ? sp.tok0 + row % sp.rows_per_batch : (rope_cos ? row % L : 0);   // global token (RoPE position)
+  const int half = head_dim >> 1;
+  // One body, instantiated for each store: neither copy branches between vectors, so loads can move ahead of earlier stores.
+  auto normalise = [&](auto store) {
+#pragma unroll
+    for (int i = 0; i < HV; ++i) {
+      const int idx = lane64 + i * 64;
+      if (idx < nvec) {
+        float f[8], w[8], o[8];
+        unpack8(v[i], f);
+        unpack8(wr[idx], w);
+        // diffusers RMSNorm with a bf16 weight: (x * rstd) rounded to bf16, then * weight (bf16 multiply)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = bf16_round(bf16_round(f[j] * rstd) * w[j]);
+        if (rope_cos) {
+          const int pair0 = (idx * 8 % head_dim) >> 1;  // 4 consecutive (even, odd) pairs of one head
+          const float4 cs = *reinterpret_cast<const float4*>(rope_cos + (size_t)tok * half + pair0);
+          const float4 sn = *reinterpret_cast<const float4*>(rope_sin + (size_t)tok * half + pair0);
+          const float cv[4] = {cs.x, cs.y, cs.z, cs.w};
+          const float sv[4] = {sn.x, sn.y, sn.z, sn.w};
+#pragma unroll
+          for (int p = 0; p < 4; ++p) {
+            const float re = o[2 * p], im = o[2 * p + 1];
+            o[2 * p] = re * cv[p] - im * sv[p];
+            o[2 * p + 1] = re * sv[p] + im * cv[p];
+          }
+        }
+        store(idx, pack8(o));
+      }
+    }
+  };
+  if (scatter) {
+    normalise([&](int idx, uint4 o) {   // to the rank that owns this head (peer store)
+      const int c = idx * 8, head = c / head_dim, dr = head / sp.heads_per_rank, bi = row / sp.rows_per_batch;
+      bf16* d = sp.dst[mat][dr] + ((size_t)bi * sp.L_total + tok) * ((size_t)sp.heads_per_rank * head_dim) +
+                (size_t)(head % sp.heads_per_rank) * head_dim + c % head_dim;
+      *reinterpret_cast<uint4*>(d) = o;
+    });
+  } else {
+    normalise([&](int idx, uint4 o) { xr[idx] = o; });
+  }
+}
+
+// Launches kernel<HV, FromPartials> (through `launch`, given both as integral constants) with the smallest HV -- 16-byte vectors
+// per lane, 64 lanes per row -- that covers D.
+template <class Launch>
+void dispatch_row_kernel(int D, bool from_partials, Launch&& launch) {
+  const int nvec = D / 8;
+  auto by_hv = [&](auto from_partials_c) {
+    if (nvec <= 128) launch(std::integral_constant<int, 2>(), from_partials_c);
+    else if (nvec <= 256) launch(std::integral_constant<int, 4>(), from_partials_c);
+    else if (nvec <= 640) launch(std::integral_constant<int, 10>(), from_partials_c);
+    else launch(std::integral_constant<int, 16>(), from_partials_c);
+  };
+  if (from_partials) by_hv(std::true_type());
+  else by_hv(std::false_type());
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -552,81 +509,44 @@ int launch_quantize_rows_fp8(const bf16* x, int ldx, int rows, int K, uint8_t* q
   return CE_OK;
 }
 
-int launch_layernorm(const bf16* x, int ldx, bf16* y, int ldy, int rows, int D, float eps, const float* scale,
-                     const float* shift, int mod_stride, int rows_per_batch, const float* weight, const float* bias,
-                     cudaStream_t stream, int scale_is_1p) {
+int launch_layernorm(const bf16* x, int ldx, bf16* y, int ldy, int rows, int D, float eps, const float* scale, const float* shift,
+                     int mod_stride, int rows_per_batch, const float* weight, const float* bias, int scale_is_1p, const RowPartials& ps,
+                     cudaStream_t stream) {
   CE_REQUIRE(rows > 0 && D % 8 == 0 && D <= MAX_D, "layernorm: D must be a multiple of 8 and <= 8192");
   CE_REQUIRE(ldx % 8 == 0 && ldy % 8 == 0, "layernorm: leading dims % 8");
   CE_REQUIRE((scale == nullptr) == (shift == nullptr), "layernorm: scale and shift come together");
   CE_REQUIRE((weight == nullptr) == (bias == nullptr), "layernorm: weight and bias come together");
+  if (ps.p)
+    CE_REQUIRE(ps.tiles >= 1 && ps.tiles <= 32 && ps.ld >= ps.tiles && ps.tile_n > 0 && (ps.tiles - 1) * ps.tile_n < D && ps.tiles * ps.tile_n >= D,
+               "layernorm(stats): the tile partials must cover exactly [0, D) in at most 32 tiles");
   if (rows_per_batch <= 0) rows_per_batch = rows;
   const int grid = (rows + ROW_THREADS / 64 - 1) / (ROW_THREADS / 64);
-  const int nvec = D / 8;
-#define CE_LN(V) layernorm_kernel<V><<<grid, ROW_THREADS, 0, stream>>>(x, ldx, y, ldy, rows, D, eps, scale, shift, mod_stride, rows_per_batch, weight, bias, scale_is_1p)
-  if (nvec <= 128) CE_LN(2);
-  else if (nvec <= 256) CE_LN(4);
-  else if (nvec <= 640) CE_LN(10);
-  else CE_LN(16);
-#undef CE_LN
+  dispatch_row_kernel(D, ps.p != nullptr, [&](auto hv, auto from_partials) {
+    layernorm_kernel<hv, from_partials><<<grid, ROW_THREADS, 0, stream>>>(x, ldx, y, ldy, rows, D, eps, scale, shift, mod_stride,
+                                                                          rows_per_batch, weight, bias, scale_is_1p, ps);
+  });
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }
 
-int launch_rmsnorm_rope(bf16* x, int ldx, int rows, int D, float eps, const bf16* weight, const float* rope_cos,
-                        const float* rope_sin, int L, int head_dim, cudaStream_t stream) {
+int launch_rmsnorm_rope(bf16* x, int ldx, int rows, int D, float eps, const bf16* weight0, const bf16* weight1, int nmat,
+                        const float* rope_cos, const float* rope_sin, int L, int head_dim, const RowPartials& ps, cudaStream_t stream,
+                        const SpScatter* sp) {
   CE_REQUIRE(rows > 0 && D % 8 == 0 && D <= MAX_D, "rmsnorm: D must be a multiple of 8 and <= 8192");
-  CE_REQUIRE(ldx % 8 == 0 && weight != nullptr, "rmsnorm: ldx % 8, weight");
+  CE_REQUIRE(ldx % 8 == 0 && weight0 != nullptr, "rmsnorm: ldx % 8, weight");
+  CE_REQUIRE(nmat == 1 || (nmat == 2 && weight1 != nullptr), "rmsnorm: one or two matrices");
+  if (ps.p) CE_REQUIRE(ps.tiles >= 1 && ps.tiles <= 32 && ps.ld >= nmat * ps.tiles, "rmsnorm(stats): tile partials");
   if (rope_cos) CE_REQUIRE(rope_sin && L > 0 && head_dim % 8 == 0 && D % head_dim == 0, "rmsnorm: rope table / head_dim");
-  const int grid = (rows + ROW_THREADS / 64 - 1) / (ROW_THREADS / 64);
-  const int nvec = D / 8;
-#define CE_RMS(V) rmsnorm_rope_kernel<V><<<grid, ROW_THREADS, 0, stream>>>(x, ldx, rows, D, eps, weight, rope_cos, rope_sin, L, head_dim)
-  if (nvec <= 128) CE_RMS(2);
-  else if (nvec <= 256) CE_RMS(4);
-  else if (nvec <= 640) CE_RMS(10);
-  else CE_RMS(16);
-#undef CE_RMS
-  CE_CHECK_CUDA(cudaGetLastError());
-  return CE_OK;
-}
-
-int launch_layernorm_stats(const bf16* x, int ldx, bf16* y, int ldy, int rows, int D, float eps, const float* scale, const float* shift,
-                           int mod_stride, int rows_per_batch, const float* weight, const float* bias, int scale_is_1p, const float2* stats,
-                           int stats_ld, int tiles, int tile_n, cudaStream_t stream) {
-  CE_REQUIRE(rows > 0 && D % 8 == 0 && D <= MAX_D && ldx % 8 == 0 && ldy % 8 == 0, "layernorm(stats): shapes");
-  CE_REQUIRE(stats != nullptr && tiles >= 1 && tiles <= 32 && stats_ld >= tiles && tile_n > 0 && (tiles - 1) * tile_n < D && tiles * tile_n >= D,
-             "layernorm(stats): the tile partials must cover exactly [0, D) in at most 32 tiles");
-  CE_REQUIRE((scale == nullptr) == (shift == nullptr) && (weight == nullptr) == (bias == nullptr), "layernorm(stats): parameter pairs");
-  if (rows_per_batch <= 0) rows_per_batch = rows;
-  const int grid = (rows + ROW_THREADS / 64 - 1) / (ROW_THREADS / 64);
-  const int nvec = D / 8;
-#define CE_LNS(V) layernorm_stats_kernel<V><<<grid, ROW_THREADS, 0, stream>>>(x, ldx, y, ldy, rows, D, eps, scale, shift, mod_stride, rows_per_batch, weight, bias, scale_is_1p, stats, stats_ld, tiles, tile_n)
-  if (nvec <= 128) CE_LNS(2);
-  else if (nvec <= 256) CE_LNS(4);
-  else if (nvec <= 640) CE_LNS(10);
-  else CE_LNS(16);
-#undef CE_LNS
-  CE_CHECK_CUDA(cudaGetLastError());
-  return CE_OK;
-}
-
-int launch_rmsnorm_rope_stats(bf16* x, int ldx, int rows, int D, float eps, const bf16* weight0, const bf16* weight1, int nmat,
-                              const float* rope_cos, const float* rope_sin, int L, int head_dim, const float2* stats, int stats_ld, int tiles,
-                              cudaStream_t stream, const SpScatter* sp) {
-  CE_REQUIRE(rows > 0 && D % 8 == 0 && D <= MAX_D && ldx % 8 == 0 && weight0 != nullptr, "rmsnorm(stats): shapes");
-  CE_REQUIRE(nmat == 1 || (nmat == 2 && weight1 != nullptr), "rmsnorm(stats): one or two matrices");
-  CE_REQUIRE(stats != nullptr && tiles >= 1 && tiles <= 32 && stats_ld >= nmat * tiles, "rmsnorm(stats): tile partials");
-  if (rope_cos) CE_REQUIRE(rope_sin && L > 0 && head_dim % 8 == 0 && D % head_dim == 0, "rmsnorm(stats): rope table / head_dim");
-  dim3 grid((rows + ROW_THREADS / 64 - 1) / (ROW_THREADS / 64), nmat);
-  const int nvec = D / 8;
   SpScatter spv;
   if (sp) spv = *sp;
-  if (spv.world) CE_REQUIRE(spv.world <= 8 && spv.heads_per_rank > 0 && spv.rows_per_batch > 0 && rows % spv.rows_per_batch == 0, "rmsnorm(stats): scatter");
-#define CE_RMSS(V) rmsnorm_rope_stats_kernel<V><<<grid, ROW_THREADS, 0, stream>>>(x, ldx, rows, D, eps, weight0, weight1, rope_cos, rope_sin, L, head_dim, stats, stats_ld, tiles, spv)
-  if (nvec <= 128) CE_RMSS(2);
-  else if (nvec <= 256) CE_RMSS(4);
-  else if (nvec <= 640) CE_RMSS(10);
-  else CE_RMSS(16);
-#undef CE_RMSS
+  if (spv.world)
+    CE_REQUIRE(ps.p && spv.world <= 8 && spv.heads_per_rank > 0 && spv.rows_per_batch > 0 && rows % spv.rows_per_batch == 0,
+               "rmsnorm: scatter (with partials only)");
+  const dim3 grid((rows + ROW_THREADS / 64 - 1) / (ROW_THREADS / 64), nmat);
+  dispatch_row_kernel(D, ps.p != nullptr, [&](auto hv, auto from_partials) {
+    rmsnorm_rope_kernel<hv, from_partials><<<grid, ROW_THREADS, 0, stream>>>(x, ldx, rows, D, eps, weight0, weight1, rope_cos, rope_sin,
+                                                                             L, head_dim, ps, spv);
+  });
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }

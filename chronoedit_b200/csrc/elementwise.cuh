@@ -5,31 +5,28 @@
 
 namespace ce {
 
+// Where the row kernels below take each row's statistics from.  p == nullptr: they reduce over the row themselves.  Otherwise from the
+// epilogue of the GEMM that produced x (GemmArgs::stats_out, per-(row, N tile) partials, row r's at p + r * ld): `tiles` partials of
+// width tile_n cover [0, D) of each matrix, and the kernels become streaming passes without a reduction or a barrier.  The RMSNorm
+// reads only sums of squares (stats_mode 2) and does not use tile_n; the LayerNorm merges (mean, M2) pairs (stats_mode 1).
+struct RowPartials {
+  const float2* p = nullptr;
+  int ld = 0, tiles = 0, tile_n = 0;
+};
+
 // y[row, :] = bf16( LN_fp32(x[row, :]) * (1 + scale[b, :]) + shift[b, :] )     (b = row / rows_per_batch)
 //   scale/shift: fp32 [batches, mod_stride] or null (then the optional affine weight/bias, fp32 [D], is applied)
 // FP32LayerNorm + adaLN modulate of transformer_chronoedit.py:279, 289, 460 and the affine norm2 of :284.
 //   scale_is_1p: the `scale` table already holds (1 + scale) (ce_dit stores its modulation tables that way)
-int launch_layernorm(const bf16* x, int ldx, bf16* y, int ldy, int rows, int D, float eps, const float* scale,
-                     const float* shift, int mod_stride, int rows_per_batch, const float* weight, const float* bias,
-                     cudaStream_t stream, int scale_is_1p = 0);
+int launch_layernorm(const bf16* x, int ldx, bf16* y, int ldy, int rows, int D, float eps, const float* scale, const float* shift,
+                     int mod_stride, int rows_per_batch, const float* weight, const float* bias, int scale_is_1p, const RowPartials& ps,
+                     cudaStream_t stream);
 
-// In place on x[rows, D] (leading dim ldx): diffusers RMSNorm across all heads (fp32 variance over D,
-// y = bf16(bf16(x * rstd) * w)), then optionally interleaved-pair RoPE with cos/sin tables [L, hd/2] fp32
-// (token = row % L).  transformer_chronoedit.py:62-65 and :71-79.
-int launch_rmsnorm_rope(bf16* x, int ldx, int rows, int D, float eps, const bf16* weight, const float* rope_cos,
-                        const float* rope_sin, int L, int head_dim, cudaStream_t stream);
-
-// The same two operators when the row statistics come from the epilogue of the GEMM that produced x (GemmArgs::stats_out,
-// per-(row, N tile) partials): streaming kernels without a reduction or a barrier.  `tiles` partials of width tile_n cover [0, D).
-// The RMSNorm variant handles `nmat` (1 or 2) matrices lying side by side in a row (q | k of the fused QKV output): matrix m starts
-// at column m * D, uses weight m and partials [m * tiles, (m + 1) * tiles).
-int launch_layernorm_stats(const bf16* x, int ldx, bf16* y, int ldy, int rows, int D, float eps, const float* scale, const float* shift,
-                           int mod_stride, int rows_per_batch, const float* weight, const float* bias, int scale_is_1p, const float2* stats,
-                           int stats_ld, int tiles, int tile_n, cudaStream_t stream);
 // Sequence-parallel scatter of the normalised q | k (csrc/seqpar.cu): rows are the LOCAL tokens of this rank (rows_per_batch each,
 // global token = tok0 + local index), RoPE uses the global token, and instead of being written back in place the vector of head h
 // goes to the rank that owns head h:  dst[mat][h / heads_per_rank] + ((b * L_total + token) * (heads_per_rank * head_dim)
 // + (h % heads_per_rank) * head_dim + offset inside the head).
+// Only with partials: sequence parallelism requires D % 256 == 0, where the GEMM writes them.
 struct SpScatter {
   bf16* dst[2][8];
   int world = 0;            // 0 = no scatter (in place)
@@ -38,9 +35,14 @@ struct SpScatter {
   int rows_per_batch = 0;   // local tokens per sample
   int tok0 = 0;             // first global token of this rank
 };
-int launch_rmsnorm_rope_stats(bf16* x, int ldx, int rows, int D, float eps, const bf16* weight0, const bf16* weight1, int nmat,
-                              const float* rope_cos, const float* rope_sin, int L, int head_dim, const float2* stats, int stats_ld, int tiles,
-                              cudaStream_t stream, const SpScatter* sp = nullptr);
+// In place on x[rows, D] (leading dim ldx): diffusers RMSNorm across all heads (fp32 variance over D,
+// y = bf16(bf16(x * rstd) * w)), then optionally interleaved-pair RoPE with cos/sin tables [L, hd/2] fp32
+// (token = row % L).  transformer_chronoedit.py:62-65 and :71-79.
+// `nmat` (1 or 2) matrices lie side by side in a row (q | k of the fused QKV output): matrix m starts at column m * D, uses weight m
+// and, from partials, partials [m * tiles, (m + 1) * tiles).
+int launch_rmsnorm_rope(bf16* x, int ldx, int rows, int D, float eps, const bf16* weight0, const bf16* weight1, int nmat,
+                        const float* rope_cos, const float* rope_sin, int L, int head_dim, const RowPartials& ps, cudaStream_t stream,
+                        const SpScatter* sp = nullptr);
 
 // FP8 mode: per row m of x[rows, K] (K % 16 == 0), scale[m] = max_k |x[m,k]| / 448 (1 if that is 0) and
 // q[m, k] = e4m3 bits of cvt.rn.satfinite(x[m,k] / scale[m]) (IEEE fp32 divisions).  One launch, HBM-bound.

@@ -232,7 +232,7 @@ int ce_umt5_encode(ce_encoder* h, const int64_t* input_ids, const int32_t* valid
     const Umt5Layer& lw = W.umt5[l];
     // self-attention sub-layer: x = x + o(attn(T5LayerNorm(x)))
     CE_CHECK_CUDA(cudaMemcpyAsync(ws.xn, ws.x, (size_t)B * L * D * 2, cudaMemcpyDeviceToDevice, s));
-    CE_TRY(run([&] { return launch_rmsnorm_rope(ws.xn, D, B * L, D, c.eps, lw.ln0, nullptr, nullptr, 0, 128, s); }));
+    CE_TRY(run([&] { return launch_rmsnorm_rope(ws.xn, D, B * L, D, c.eps, lw.ln0, nullptr, 1, nullptr, nullptr, 0, 128, RowPartials{}, s); }));
     for (int b = 0; b < B; ++b) {
       GemmAttention a = attention_of(ws, c, b, L, lw.qk, nullptr, lw.v, nullptr);
       a.sc.rule = SOFTMAX_T5;
@@ -245,7 +245,7 @@ int ce_umt5_encode(ce_encoder* h, const int64_t* input_ids, const int32_t* valid
     CE_TRY(run_gemm(run, ws.attn, I, lw.o, I, B * L, D, I, ws.x, D, nullptr, EPI_BIAS_RESID, ws.x, D));
     // feed-forward sub-layer: x = x + wo(gelu_new(wi_0(n)) * wi_1(n))
     CE_CHECK_CUDA(cudaMemcpyAsync(ws.xn, ws.x, (size_t)B * L * D * 2, cudaMemcpyDeviceToDevice, s));
-    CE_TRY(run([&] { return launch_rmsnorm_rope(ws.xn, D, B * L, D, c.eps, lw.ln1, nullptr, nullptr, 0, 128, s); }));
+    CE_TRY(run([&] { return launch_rmsnorm_rope(ws.xn, D, B * L, D, c.eps, lw.ln1, nullptr, 1, nullptr, nullptr, 0, 128, RowPartials{}, s); }));
     CE_TRY(run_gemm(run, ws.xn, D, lw.wi0, D, B * L, F, D, ws.h0, F, nullptr, EPI_BIAS_GELU_TANH));
     CE_TRY(run_gemm(run, ws.xn, D, lw.wi1, D, B * L, F, D, ws.h1, F, nullptr, EPI_BIAS));
     CE_TRY(run.kernel(mul_kernel, grid_for((size_t)B * L * F), TPB, ws.h0, ws.h1, (size_t)B * L * F));
@@ -253,7 +253,7 @@ int ce_umt5_encode(ce_encoder* h, const int64_t* input_ids, const int32_t* valid
   }
   CE_CHECK_CUDA(cudaMemcpyAsync(last_hidden_state, ws.x, (size_t)B * L * D * 2, cudaMemcpyDeviceToDevice, s));
   return run([&] {
-    return launch_rmsnorm_rope(reinterpret_cast<bf16*>(last_hidden_state), D, B * L, D, c.eps, W.final_ln, nullptr, nullptr, 0, 128, s);
+    return launch_rmsnorm_rope(reinterpret_cast<bf16*>(last_hidden_state), D, B * L, D, c.eps, W.final_ln, nullptr, 1, nullptr, nullptr, 0, 128, RowPartials{}, s);
   });
 }
 
@@ -288,7 +288,7 @@ int ce_clip_vision_encode(ce_encoder* h, const void* pixel_values, void* out, in
                       D));
   auto ln = [&](const bf16* src, bf16* dst, const float* w, const float* bb) -> int {   // LayerNorm(eps) per sample
     for (int b = 0; b < B; ++b)
-      CE_TRY(run([&] { return launch_layernorm(src + (size_t)b * L8 * D, D, dst + (size_t)b * L8 * D, D, L, D, c.eps, nullptr, nullptr, 0, 0, w, bb, s); }));
+      CE_TRY(run([&] { return launch_layernorm(src + (size_t)b * L8 * D, D, dst + (size_t)b * L8 * D, D, L, D, c.eps, nullptr, nullptr, 0, 0, w, bb, 0, RowPartials{}, s); }));
     return CE_OK;
   };
   CE_TRY(ln(ws.xn, ws.x, W.pre_ln_w, W.pre_ln_b));

@@ -340,13 +340,16 @@ int ce_linear_fp8_ex(const ce_linear_fp8_args* args, void* stream);
 int ce_quantize_rows_fp8(const void* x, int ldx, int rows, int K, void* q, int ldq, float* scale, void* stream);
 
 /* FP32LayerNorm (+ modulate or affine) like ce_layernorm_bf16, with the row statistics merged from `tiles` stats_mode-1
- * partials of width tile_n covering [0, D) (stats [rows, stats_ld] float pairs).  scale_is_1p: `scale` holds 1 + scale. */
+ * partials of width tile_n covering [0, D) (stats [rows, stats_ld] float pairs).  scale_is_1p: `scale` holds 1 + scale.
+ * stats == NULL: the kernel reduces over each row itself, as ce_layernorm_bf16 does (stats_ld, tiles, tile_n are ignored). */
 int ce_layernorm_stats_bf16(const void* x, int ldx, void* y, int ldy, int rows, int D, float eps, const float* scale,
                             const float* shift, int mod_stride, int rows_per_batch, const float* weight, const float* bias,
                             int scale_is_1p, const float* stats, int stats_ld, int tiles, int tile_n, void* stream);
 
 /* RMSNorm across heads (+ optional RoPE) like ce_rmsnorm_rope_bf16, in place on nmat (1 or 2) matrices of width D side by
- * side in x (q | k): matrix m starts at column m * D, uses weight m and the stats_mode-2 partials [m * tiles, (m+1) * tiles). */
+ * side in x (q | k): matrix m starts at column m * D, uses weight m and the stats_mode-2 partials [m * tiles, (m+1) * tiles).
+ * stats == NULL: the kernel reduces over each row of each matrix itself, as ce_rmsnorm_rope_bf16 does (stats_ld and tiles
+ * are ignored). */
 int ce_rmsnorm_rope_stats_bf16(void* x, int ldx, int rows, int D, float eps, const void* weight0, const void* weight1, int nmat,
                                const float* rope_cos, const float* rope_sin, int L, int head_dim, const float* stats,
                                int stats_ld, int tiles, void* stream);

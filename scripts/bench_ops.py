@@ -200,6 +200,31 @@ def bench_rows(M=14400, D=5120):
     cos = torch.randn(M // 2, 64, device="cuda")
     ms = timeit(lambda: L.check(lib.ce_rmsnorm_rope_bf16(L.ptr(x), D, M, D, 1e-6, L.ptr(w), L.ptr(cos), L.ptr(cos), M // 2, 128, L.current_stream())))
     print(json.dumps({"op": "rmsnorm_rope", "M": M, "D": D, "ms": round(ms, 4), "GBps": round(4.0 * M * D / ms / 1e6, 1)}), flush=True)
+    # the same two operators with their row statistics from the epilogue of the GEMM that wrote the rows, as the DiT runs them at
+    # D % 256 == 0: the (1 + scale) modulation, and q | k of the fused QKV output in one launch.  Outputs of the GEMM have rms ~ 1, so
+    # the in-place RMSNorm, which keeps the GEMM's statistics over its repeats, stays in range.
+    def gemm_with_stats(N, mode, K=256):
+        out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+        st = torch.empty(M, N // 256, 2, device="cuda")
+        a = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
+        wt = (torch.randn(N, K, device="cuda") / math.sqrt(K)).bfloat16()
+        args = L.LinearArgsC(A=a.data_ptr(), lda=K, W=wt.data_ptr(), ldw=K, M=M, N=N, K=K, out=out.data_ptr(), ldo=N,
+                             stats_out=st.data_ptr(), stats_ld=N // 256, stats_mode=mode)
+        L.check(lib.ce_linear_ex_bf16(args, L.current_stream()))
+        return out, st
+
+    x, st = gemm_with_stats(D, 1)
+    mod1p = mod.clone()
+    mod1p[:, 1] += 1
+    ms = timeit(lambda: L.check(lib.ce_layernorm_stats_bf16(L.ptr(x), D, L.ptr(y), D, M, D, 1e-6, L.ptr(mod1p[:, 1]), L.ptr(mod1p[:, 0]), 6 * D,
+                                                            M // 2, None, None, 1, L.ptr(st), D // 256, D // 256, 256, L.current_stream())))
+    print(json.dumps({"op": "layernorm_mod_stats", "M": M, "D": D, "ms": round(ms, 4), "GBps": round(4.0 * M * D / ms / 1e6, 1)}), flush=True)
+    qkv, st = gemm_with_stats(3 * D, 2)
+    ang = torch.rand(M // 2, 64, device="cuda") * (2 * math.pi)   # a true rotation: the repeats keep the norm
+    cos, sin = ang.cos(), ang.sin()
+    ms = timeit(lambda: L.check(lib.ce_rmsnorm_rope_stats_bf16(L.ptr(qkv), 3 * D, M, D, 1e-6, L.ptr(w), L.ptr(w), 2, L.ptr(cos), L.ptr(sin), M // 2,
+                                                               128, L.ptr(st), 3 * D // 256, D // 256, L.current_stream())))
+    print(json.dumps({"op": "rmsnorm_rope_qk_stats", "M": M, "D": D, "ms": round(ms, 4), "GBps": round(8.0 * M * D / ms / 1e6, 1)}), flush=True)
 
 
 def bench_conv(Cin=96, Cout=96, T=4, H=720, W=1280):

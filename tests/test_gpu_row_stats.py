@@ -236,7 +236,9 @@ def test_layernorm_stats_after_gemm(rows, D, mode):
     """GEMM (stats_mode 1, residual epilogue, as the DiT's out-projections) -> ce_layernorm_stats_bf16, against fp64 LayerNorm of
     the stored x, and against the row-reducing ce_layernorm_bf16 on the same x (2 ulp: both are within 1 ulp of the reference).
     Catches a merge without Chan's between-tile term (block offsets, tile-constant rows), a partial last tile weighted as a full
-    one (D = 640), and an ignored scale_is_1p (mod0 vs mod1).  rows_per_batch does not divide the row count."""
+    one (D = 640), and an ignored scale_is_1p (mod0 vs mod1).  rows_per_batch does not divide the row count.  In mode mod1 the
+    call is also made with stats = NULL (the kernel reduces over the row): with the (1 + scale) table added in fp32 by torch it must
+    give ce_layernorm_bf16's bits for the plain scale."""
     L = _lib()
     lib = L.lib()
     rpb = 97 if rows == 300 else 1200
@@ -256,10 +258,16 @@ def test_layernorm_stats_after_gemm(rows, D, mode):
         y_row = torch.empty_like(x)
         s0, h0, ms0, _, _, _ = _ln_args("mod0" if mode.startswith("mod") else mode, mod, mod1p, w, b, D)
         L.check(lib.ce_layernorm_bf16(L.ptr(x), D, L.ptr(y_row), D, rows, D, EPS, s0, h0, ms0, rpb, wp, bp, L.current_stream()))
+        if mode == "mod1":
+            y_null = torch.empty_like(x)
+            L.check(lib.ce_layernorm_stats_bf16(L.ptr(x), D, L.ptr(y_null), D, rows, D, EPS, scale, shift, ms, rpb, wp, bp, is1p, None, 0, 0,
+                                                0, L.current_stream()))
         torch.cuda.synchronize()
         what = f"layernorm(stats) {mode} {kind} rows={rows} D={D}"
         _check_ln(y, _ln_ref(x, mode, mod, w, b, rpb), what, kind)
         _bf16_close(y, y_row.float(), what + " vs ce_layernorm_bf16", ulp=2.0)
+        if mode == "mod1":
+            assert torch.equal(y_null, y_row), what + ": stats = NULL with (1 + scale) differs from ce_layernorm_bf16 with scale"
 
 
 @gpu
@@ -317,7 +325,8 @@ def _rms_ref(x, w, H, freqs=None, B=1):
 def test_rmsnorm_rope_stats_qkv(H):
     """The self-attention q | k path: a [M, 3D] QKV buffer written by the GEMM with stats_mode 2, then nmat = 2 with different q and
     k weights (and k twice the scale of q, so reading q's partials for k fails), RoPE from ce_rope_table_host, B = 2 so the token
-    is row % L.  v must stay bit-untouched.  Rule of test_rmsnorm_rope (1 bf16 ulp of the oracle)."""
+    is row % L.  v must stay bit-untouched.  Rule of test_rmsnorm_rope (1 bf16 ulp of the oracle).  The same call with stats = NULL
+    (the kernel reduces over each row) must give the bits of two ce_rmsnorm_rope_bf16 launches, on q and on k, and leave v alone."""
     from oracle import dit_oracle as O
 
     L = _lib()
@@ -341,9 +350,16 @@ def test_rmsnorm_rope_stats_qkv(H):
         before = qkv.clone()
         L.check(L.lib().ce_rmsnorm_rope_stats_bf16(L.ptr(qkv), 3 * D, M, D, EPS, L.ptr(wq), L.ptr(wk), 2, L.ptr(cos), L.ptr(sin), Lt, 128,
                                                    L.ptr(st), 3 * tiles + 1, tiles, L.current_stream()))
+        in_kernel, two = before.clone(), before.clone()
+        L.check(L.lib().ce_rmsnorm_rope_stats_bf16(L.ptr(in_kernel), 3 * D, M, D, EPS, L.ptr(wq), L.ptr(wk), 2, L.ptr(cos), L.ptr(sin), Lt,
+                                                   128, None, 0, 0, L.current_stream()))
+        for m, wm in ((0, wq), (1, wk)):
+            L.check(L.lib().ce_rmsnorm_rope_bf16(L.ptr(two[:, m * D:]), 3 * D, M, D, EPS, L.ptr(wm), L.ptr(cos), L.ptr(sin), Lt, 128,
+                                                 L.current_stream()))
         torch.cuda.synchronize()
         what = f"rmsnorm_rope(stats) {kind} H={H}"
         assert torch.equal(qkv[:, 2 * D:], before[:, 2 * D:]), what + ": v columns were written"
+        assert torch.equal(in_kernel, two), what + ": stats = NULL differs from two ce_rmsnorm_rope_bf16 launches"
         _bf16_close(qkv[:, :D], _rms_ref(before[:, :D], wq, H, freqs, B=2), what + " q")
         _bf16_close(qkv[:, D:2 * D], _rms_ref(before[:, D:2 * D], wk, H, freqs, B=2), what + " k")
 
