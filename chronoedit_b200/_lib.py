@@ -132,6 +132,11 @@ SIGNATURES = {
     "ce_linear_ex_bf16": (c_int, [POINTER(LinearArgsC), c_void_p]),
     "ce_linear_fp8_ex": (c_int, [POINTER(LinearFp8ArgsC), c_void_p]),
     "ce_quantize_rows_fp8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "ce_dit_set_attention_fp8": (c_int, [c_void_p, c_int]),
+    "ce_quantize_heads_fp8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "ce_quantize_v_fp8": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "ce_attention_fp8": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int,
+                                 c_int, c_int, c_int, c_float, c_void_p]),
     "ce_layernorm_stats_bf16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int,
                                         c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     "ce_rmsnorm_rope_stats_bf16": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int, c_void_p, c_void_p,

@@ -35,4 +35,23 @@ struct AttnArgs {
 
 int launch_attention(const AttnArgs& a, cudaStream_t stream);
 
+// The FP8 self-attention (attention_fp8.cu, DESIGN.md "FP8 attention"): Lq = Lk = L, head_dim 128, quantized operands.
+struct AttnFp8Args {
+  int B = 0, H = 0, L = 0;
+  const uint8_t* q = nullptr;   // e4m3 q[b, i, h*128 + d] at q + (b*L + i)*ldqk + h*128 + d
+  const uint8_t* k = nullptr;   // e4m3 k, same layout
+  int ldqk = 0;                 // bytes, multiple of 16
+  const float* q_scale = nullptr;   // q_scale[(b*L + i)*lds + h], one per (token, head)
+  const float* k_scale = nullptr;   // the same for k
+  int lds = 0;
+  const uint8_t* vt = nullptr;  // e4m3 V^T [B, H, 128, Lpad]: channel rows, keys permuted within each 32-key group
+  int Lpad = 0;                 // >= L, multiple of 32; keys [L, Lpad) are zero
+  const float* v_scale = nullptr;   // [B, H*128], one per (sample, channel)
+  bf16* out = nullptr;          // out[b, i, h*128 + c] at out + (b*L + i)*ldo + h*128 + c
+  int ldo = 0;
+  float scale = 0.f;            // 1/sqrt(head_dim)
+};
+
+int launch_attention_fp8(const AttnFp8Args& a, cudaStream_t stream);
+
 }  // namespace ce

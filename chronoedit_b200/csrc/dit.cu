@@ -9,6 +9,7 @@
 //   with gate*y+x epilogue.
 // When D % 256 == 0 the GEMM before each LN / RMSNorm also writes that norm's row statistics; other widths take row kernels
 // that reduce over the row themselves.  RMSNorm+RoPE(q|k) is one launch either way.
+// With FP8 attention on (ce_dit_set_attention_fp8) the self-attention becomes quantize(q|k) -> quantize(v) -> attention_fp8.
 #include <math.h>
 
 #include <map>
@@ -49,6 +50,8 @@ struct ce_dit {
   // FP8 mode: the current forward's workspace slices for a GEMM's quantized A operand and its row scales
   uint8_t* fp8_q = nullptr;
   float* fp8_scale = nullptr;
+  // FP8 self-attention (ce_dit_set_attention_fp8): independent of the weights' dtype
+  bool attn_fp8 = false;
 };
 
 enum { CAT_GEMM = 0, CAT_ATTN = 1, CAT_ROWS = 2, CAT_OTHER = 3, NUM_CATS = 4 };
@@ -65,10 +68,17 @@ struct Workspace {
   float2 *stats_x, *stats_qkv, *stats_q2;   // epilogue row statistics (GemmArgs::stats_out): [M, D/256], [M, 3D/256], [M, D/256]
   uint8_t* fp8_q;     // FP8 mode only: [M, max(D, F)] e4m3, the A operand of one block GEMM at a time
   float* fp8_scale;   //                [M] its row scales
+  uint8_t* qk8;       // FP8 attention only: [M, 2D] e4m3 q | k of the self-attention
+  float* qk_scale;    //                     [M, 2H] their (token, head) scales
+  uint8_t* vt8;       //                     [B, H, 128, Lpad] e4m3 V^T
+  float* v_scale;     //                     [B, D] its (sample, channel) scales
   int64_t bytes;
 };
 
-Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li, bool fp8) {
+// Keys of the FP8 attention's V^T rows: L rounded up to the 32-key groups of its layout.
+int vt_keys(int L) { return (L + 31) / 32 * 32; }
+
+Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li, bool fp8, bool attn_fp8) {
   const int64_t D = D_of(c), F = c.ffn_dim, M = (int64_t)B * L;
   const int64_t Kp = (int64_t)c.in_channels * c.patch_t * c.patch_h * c.patch_w;
   const int64_t No = (int64_t)c.out_channels * c.patch_t * c.patch_h * c.patch_w;
@@ -103,6 +113,11 @@ Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li
   w.stats_q2 = b.take<float2>(M * td);
   w.fp8_q = fp8 ? b.take<uint8_t>(M * (D > F ? D : F)) : nullptr;
   w.fp8_scale = fp8 ? b.take<float>(M) : nullptr;
+  const int64_t H = c.num_attention_heads;
+  w.qk8 = attn_fp8 ? b.take<uint8_t>(M * 2 * D) : nullptr;
+  w.qk_scale = attn_fp8 ? b.take<float>(M * 2 * H) : nullptr;
+  w.vt8 = attn_fp8 ? b.take<uint8_t>((int64_t)B * D * vt_keys(L)) : nullptr;
+  w.v_scale = attn_fp8 ? b.take<float>((int64_t)B * D) : nullptr;
   w.bytes = b.bytes();
   return w;
 }
@@ -409,7 +424,7 @@ int64_t ce_dit_workspace_bytes(const ce_dit* h, int batch, int frames, int heigh
   Weights w;
   resolve_weights(h, w);   // only w.fp8 is read here, and it is set even before every weight has been registered
   const int L = frames * (height / h->cfg.patch_h) * (width / h->cfg.patch_w);
-  return carve(h->cfg, nullptr, batch, L, text_len, 257, w.fp8).bytes;
+  return carve(h->cfg, nullptr, batch, L, text_len, 257, w.fp8, h->attn_fp8).bytes;
 }
 
 int64_t ce_dit_last_launch_count(const ce_dit* h) { return h ? h->launches : 0; }
@@ -523,6 +538,7 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   SeqPar& sp = h->sp;
   const bool spx = sp.world > 1;
   if (spx) {
+    CE_REQUIRE(!h->attn_fp8, "sequence parallelism is not built for FP8 attention: run it on one GPU or switch it off (ce_dit_set_attention_fp8)");
     CE_REQUIRE(Lfull % sp.world == 0 && D % 256 == 0, "sequence parallel: tokens must divide by the rank count and the width by 256");
     CE_REQUIRE(Lfull >= 256, "sequence parallel: at least 256 tokens (the self-attention kernel with the output scatter)");
     CE_REQUIRE(!h->profiling && h->capture.empty() && block0_out == nullptr, "sequence parallel: no per-launch profiling / block capture");
@@ -531,7 +547,7 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   const SpLayout lay = spx ? sp_layout(B, Lfull, D, No, sp.world) : SpLayout();
   if (spx && lay.bytes > sp.region_bytes) return fail(CE_ERR_WORKSPACE, "sequence parallel: peer region too small (ce_dit_sp_region_bytes)");
   CE_REQUIRE(!(spx && W.fp8), "sequence parallelism is not built for FP8 weights: run the FP8 mode on one GPU");
-  Workspace ws = carve(c, workspace, B, L, Lt, Li, W.fp8);
+  Workspace ws = carve(c, workspace, B, L, Lt, Li, W.fp8, h->attn_fp8);
   if (ws.bytes > workspace_bytes)
     return fail(CE_ERR_WORKSPACE, "workspace too small: need " + std::to_string(ws.bytes) + " bytes, got " + std::to_string(workspace_bytes));
   CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
@@ -648,14 +664,29 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
     } else {
       LAUNCH(CAT_ROWS, 8.0 * M * D, launch_rmsnorm_rope(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, L,
                                                         c.attention_head_dim, partials(ws.stats_qkv, 3 * tD), s));
-      AttnArgs a;
-      a.B = B; a.H = H; a.Lq = L; a.Lk = L;
-      a.q = ws.qkv; a.ldq = 3 * D;
-      a.k = ws.qkv + D; a.ldk = 3 * D;
-      a.v = ws.qkv + 2 * D; a.ldv = 3 * D;
-      a.out = ws.attn; a.ldo = D;
-      a.scale = attn_scale;
-      LAUNCH(CAT_ATTN, attention_flops(a), launch_attention(a, s));
+      if (h->attn_fp8) {   // quantize q | k per (token, head) and v per (sample, channel), then the e4m3 attention
+        const int Lpad = vt_keys(L);
+        LAUNCH(CAT_ROWS, 6.0 * M * D + 8.0 * M * H, launch_quantize_heads_fp8(ws.qkv, 3 * D, M, 2 * H, ws.qk8, 2 * D, ws.qk_scale, s));
+        LAUNCH(CAT_ROWS, 4.0 * M * D + 1.0 * B * Lpad * D + 4.0 * B * D,
+               launch_quantize_v_fp8(ws.qkv + 2 * D, 3 * D, B, L, H, ws.vt8, Lpad, ws.v_scale, s));
+        AttnFp8Args a;
+        a.B = B; a.H = H; a.L = L;
+        a.q = ws.qk8; a.k = ws.qk8 + D; a.ldqk = 2 * D;
+        a.q_scale = ws.qk_scale; a.k_scale = ws.qk_scale + H; a.lds = 2 * H;
+        a.vt = ws.vt8; a.Lpad = Lpad; a.v_scale = ws.v_scale;
+        a.out = ws.attn; a.ldo = D;
+        a.scale = attn_scale;
+        LAUNCH(CAT_ATTN, 4.0 * B * H * (double)L * L * c.attention_head_dim, launch_attention_fp8(a, s));
+      } else {
+        AttnArgs a;
+        a.B = B; a.H = H; a.Lq = L; a.Lk = L;
+        a.q = ws.qkv; a.ldq = 3 * D;
+        a.k = ws.qkv + D; a.ldk = 3 * D;
+        a.v = ws.qkv + 2 * D; a.ldv = 3 * D;
+        a.out = ws.attn; a.ldo = D;
+        a.scale = attn_scale;
+        LAUNCH(CAT_ATTN, attention_flops(a), launch_attention(a, s));
+      }
     }
     if ((rc = linear(h, s, lw.out1, attn_in, M, D, D, ws.x, resid_epi(mod + 2 * D)))) return rc;
     // 2. cross-attention
@@ -805,6 +836,41 @@ int ce_linear_fp8_ex(const ce_linear_fp8_args* a, void* stream) {
   CE_REQUIRE(a != nullptr, "ce_linear_fp8_ex: null args");
   return launch_gemm_fp8(reinterpret_cast<const e4m3*>(a->base.A), a->base.lda, a->a_scale, reinterpret_cast<const e4m3*>(a->base.W),
                          a->base.ldw, a->w_scale, gemm_args_of(&a->base), reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_dit_set_attention_fp8(ce_dit* h, int enabled) {
+  CE_REQUIRE(h, "ce_dit_set_attention_fp8: null handle");
+  h->attn_fp8 = enabled != 0;
+  return CE_OK;
+}
+
+// Test aids of the FP8 self-attention: its two quantizers and the attention on their outputs.
+int ce_quantize_heads_fp8(const void* x, int ldx, int rows, int heads, void* q, int ldq, float* scale, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  return launch_quantize_heads_fp8(reinterpret_cast<const bf16*>(x), ldx, rows, heads, reinterpret_cast<uint8_t*>(q), ldq, scale,
+                                   reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_quantize_v_fp8(const void* v, int ldv, int B, int L, int H, void* vt, int Lpad, float* scale, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  return launch_quantize_v_fp8(reinterpret_cast<const bf16*>(v), ldv, B, L, H, reinterpret_cast<uint8_t*>(vt), Lpad, scale,
+                               reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_attention_fp8(const void* q, const void* k, int ldqk, const float* q_scale, const float* k_scale, int lds, const void* vt, int Lpad,
+                     const float* v_scale, void* out, int ldo, int B, int H, int L, float scale, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  AttnFp8Args a;
+  a.B = B; a.H = H; a.L = L;
+  a.q = reinterpret_cast<const uint8_t*>(q); a.k = reinterpret_cast<const uint8_t*>(k); a.ldqk = ldqk;
+  a.q_scale = q_scale; a.k_scale = k_scale; a.lds = lds;
+  a.vt = reinterpret_cast<const uint8_t*>(vt); a.Lpad = Lpad; a.v_scale = v_scale;
+  a.out = reinterpret_cast<bf16*>(out); a.ldo = ldo;
+  a.scale = scale;
+  return launch_attention_fp8(a, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ce_quantize_rows_fp8(const void* x, int ldx, int rows, int K, void* q, int ldq, float* scale, void* stream) {

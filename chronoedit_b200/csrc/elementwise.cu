@@ -1,5 +1,6 @@
 // HBM-bound row kernels of the DiT path: fp32 LayerNorm + adaLN modulate, RMSNorm-across-heads + 3D RoPE,
-// patchify / unpatchify, the tiny-M Linear layers of the time embedder, and the FP8 mode's row quantisation.  All are coalesced 16-byte
+// patchify / unpatchify, the tiny-M Linear layers of the time embedder, the FP8 mode's row quantisation and the FP8
+// self-attention's q | k and v quantisation.  All are coalesced 16-byte
 // accesses with one CTA per token row (rows >> SM count), statistics in fp32 via warp shuffles.
 #include "elementwise.cuh"
 
@@ -420,6 +421,89 @@ quantize_rows_fp8_kernel(const bf16* __restrict__ x, int ldx, int K, uint8_t* __
   }
 }
 
+// FP8 self-attention, q | k: one warp per (row, head); lane l holds values 4l .. 4l+3 of the head's 128.  Same operations as
+// quantize_rows_fp8_kernel.
+__global__ void __launch_bounds__(ROW_THREADS)
+quantize_heads_fp8_kernel(const bf16* __restrict__ x, int ldx, int rows, int nh, uint8_t* __restrict__ q, int ldq, float* __restrict__ scale) {
+  const int gw = blockIdx.x * (ROW_THREADS / 32) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (gw >= rows * nh) return;
+  const int row = gw / nh, hd = gw - row * nh;
+  const uint2 u = *reinterpret_cast<const uint2*>(x + (size_t)row * ldx + hd * 128 + lane * 4);
+  const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
+  const float m = warp_max(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(b.x), fabsf(b.y))));
+  const float s = m == 0.f ? 1.f : __fdiv_rn(m, 448.f);
+  if (lane == 0) scale[(size_t)row * nh + hd] = s;
+  const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(a.x, s), __fdiv_rn(a.y, s)), __NV_SATFINITE, __NV_E4M3);
+  const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(b.x, s), __fdiv_rn(b.y, s)), __NV_SATFINITE, __NV_E4M3);
+  *reinterpret_cast<uint32_t*>(q + (size_t)row * ldq + hd * 128 + lane * 4) = lo | (hi << 16);
+}
+
+// FP8 self-attention, v pass 1: the channel maxima over a sample's tokens.  CTA (32 channels, sample b): 64 row groups x 4 lanes of
+// 8 channels (16-byte loads) walk the tokens, then one smem reduction per channel.
+constexpr int VMAX_COLS = 32;
+__global__ void __launch_bounds__(ROW_THREADS)
+v_channel_scale_kernel(const bf16* __restrict__ v, int ldv, int L, int D, float* __restrict__ scale) {
+  __shared__ float part[ROW_THREADS / 4][VMAX_COLS + 1];
+  const int b = blockIdx.y;
+  const int sub = threadIdx.x & 3, rg = threadIdx.x >> 2;
+  const int c0 = blockIdx.x * VMAX_COLS + sub * 8;
+  float m[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  const bf16* base = v + (size_t)b * L * ldv + c0;
+#pragma unroll 4
+  for (int r = rg; r < L; r += ROW_THREADS / 4) {
+    float f[8];
+    unpack8(*reinterpret_cast<const uint4*>(base + (size_t)r * ldv), f);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m[e] = fmaxf(m[e], fabsf(f[e]));
+  }
+#pragma unroll
+  for (int e = 0; e < 8; ++e) part[rg][sub * 8 + e] = m[e];
+  __syncthreads();
+  if (threadIdx.x < VMAX_COLS) {
+    float mx = 0.f;
+    for (int r = 0; r < ROW_THREADS / 4; ++r) mx = fmaxf(mx, part[r][threadIdx.x]);
+    scale[(size_t)b * D + blockIdx.x * VMAX_COLS + threadIdx.x] = mx == 0.f ? 1.f : __fdiv_rn(mx, 448.f);
+  }
+}
+
+// Key at stored position p of a 32-key group of V^T.  The S accumulator gives a thread keys 8c + 2 (lane % 4) + {0, 1}; the 8-bit
+// A fragment of a K32 step wants keys 4 (lane % 4) + {0..3} (+ 16) in one register: packing the accumulator pairs c = 2j, 2j + 1
+// into register j of the fragment makes fragment position p hold this key, so V^T is stored in the same order.
+__device__ __forceinline__ int vt_key_of(int p) { return 16 * (p >> 4) + 8 * ((p & 3) >> 1) + 2 * ((p & 15) >> 2) + (p & 1); }
+
+// FP8 self-attention, v pass 2: CTA (32-key group g, head h, sample b) stages the [32 keys x 128 channels] bf16 block in shared
+// memory, then thread (channel c, half) writes stored positions 16 half .. 16 half + 15 of channel c's row (16 bytes).
+__global__ void __launch_bounds__(ROW_THREADS)
+quantize_vt_fp8_kernel(const bf16* __restrict__ v, int ldv, int L, int H, const float* __restrict__ scale, uint8_t* __restrict__ vt,
+                       int Lpad) {
+  __shared__ __align__(16) bf16 tile[32][128];
+  const int g = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  for (int i = threadIdx.x; i < 32 * 16; i += ROW_THREADS) {
+    const int r = i >> 4, ch = (i & 15) * 8, key = g * 32 + r;
+    uint4 u = make_uint4(0, 0, 0, 0);
+    if (key < L) u = *reinterpret_cast<const uint4*>(v + ((size_t)b * L + key) * ldv + h * 128 + ch);
+    *reinterpret_cast<uint4*>(&tile[r][ch]) = u;
+  }
+  __syncthreads();
+  const int c = threadIdx.x >> 1, half = threadIdx.x & 1;
+  const float s = scale[(size_t)b * H * 128 + h * 128 + c];
+  uint32_t w[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    uint32_t word = 0;
+#pragma unroll
+    for (int e = 0; e < 4; e += 2) {
+      const int p = 16 * half + 4 * j + e;
+      const float x0 = __bfloat162float(tile[vt_key_of(p)][c]), x1 = __bfloat162float(tile[vt_key_of(p + 1)][c]);
+      const uint32_t pair = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(x0, s), __fdiv_rn(x1, s)), __NV_SATFINITE, __NV_E4M3);
+      word |= pair << (8 * e);
+    }
+    w[j] = word;
+  }
+  *reinterpret_cast<uint4*>(vt + (((size_t)b * H + h) * 128 + c) * Lpad + g * 32 + 16 * half) = make_uint4(w[0], w[1], w[2], w[3]);
+}
+
 // Score rules of softmax_rows_kernel: which keys of a row count, the score of key j from the GEMM accumulators s, and the
 // exponential of (score - row max).
 template <bool FAST>
@@ -505,6 +589,30 @@ int launch_quantize_rows_fp8(const bf16* x, int ldx, int rows, int K, uint8_t* q
   CE_REQUIRE(x && q && scale && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q) & 15) == 0,
              "quantize_rows_fp8: x and q must be 16-byte aligned");
   quantize_rows_fp8_kernel<<<rows, ROW_THREADS, 0, stream>>>(x, ldx, K, q, ldq, scale);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
+
+int launch_quantize_heads_fp8(const bf16* x, int ldx, int rows, int nh, uint8_t* q, int ldq, float* scale, cudaStream_t stream) {
+  CE_REQUIRE(rows > 0 && nh > 0, "quantize_heads_fp8: rows > 0 and at least one head");
+  CE_REQUIRE(ldx % 8 == 0 && ldx >= nh * 128 && ldq % 16 == 0 && ldq >= nh * 128, "quantize_heads_fp8: ldx % 8, ldq % 16, both >= nh * 128");
+  CE_REQUIRE(x && q && scale && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q) & 15) == 0,
+             "quantize_heads_fp8: x and q must be 16-byte aligned");
+  const int64_t warps = (int64_t)rows * nh;
+  quantize_heads_fp8_kernel<<<(unsigned)((warps + ROW_THREADS / 32 - 1) / (ROW_THREADS / 32)), ROW_THREADS, 0, stream>>>(x, ldx, rows, nh, q,
+                                                                                                                        ldq, scale);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
+
+int launch_quantize_v_fp8(const bf16* v, int ldv, int B, int L, int H, uint8_t* vt, int Lpad, float* scale, cudaStream_t stream) {
+  CE_REQUIRE(B > 0 && L > 0 && H > 0 && Lpad >= L && Lpad % 32 == 0, "quantize_v_fp8: B, L, H > 0 and Lpad >= L a multiple of 32");
+  CE_REQUIRE(ldv % 8 == 0 && ldv >= H * 128, "quantize_v_fp8: ldv % 8 and >= H * 128");
+  CE_REQUIRE(v && vt && scale && (reinterpret_cast<uintptr_t>(v) & 15) == 0 && (reinterpret_cast<uintptr_t>(vt) & 15) == 0,
+             "quantize_v_fp8: v and vt must be 16-byte aligned");
+  v_channel_scale_kernel<<<dim3(H * 128 / VMAX_COLS, B), ROW_THREADS, 0, stream>>>(v, ldv, L, H * 128, scale);
+  CE_CHECK_CUDA(cudaGetLastError());
+  quantize_vt_fp8_kernel<<<dim3(Lpad / 32, H, B), ROW_THREADS, 0, stream>>>(v, ldv, L, H, scale, vt, Lpad);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }

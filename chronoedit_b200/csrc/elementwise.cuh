@@ -48,6 +48,15 @@ int launch_rmsnorm_rope(bf16* x, int ldx, int rows, int D, float eps, const bf16
 // q[m, k] = e4m3 bits of cvt.rn.satfinite(x[m,k] / scale[m]) (IEEE fp32 divisions).  One launch, HBM-bound.
 int launch_quantize_rows_fp8(const bf16* x, int ldx, int rows, int K, uint8_t* q, int ldq, float* scale, cudaStream_t stream);
 
+// FP8 self-attention, q | k: the same rule per (row, head) over 128 values.  x[rows, nh * 128] (leading dim ldx) -> q[rows, nh * 128]
+// (ldq bytes) and scale[rows, nh].  For the fused QKV buffer nh = 2H covers q and k.  One warp per (row, head), HBM-bound.
+int launch_quantize_heads_fp8(const bf16* x, int ldx, int rows, int nh, uint8_t* q, int ldq, float* scale, cudaStream_t stream);
+// FP8 self-attention, v: one scale per (sample, channel), scale[b, c] = max_i |v[b, i, c]| / 448 (1 if that is 0), and
+// vt[b, c / 128, c % 128, :] = e4m3(v[b, :, c] / scale[b, c]) transposed to keys-contiguous rows of Lpad bytes, the keys of each
+// 32-key group at the positions the P V wgmma's A fragment wants (fp8_attention_key_order in transformer.py), keys >= L zero.
+// v[b, i, c] at v + (b * L + i) * ldv + c, c < H * 128.  Two launches: the channel maxima, then transpose + quantize.
+int launch_quantize_v_fp8(const bf16* v, int ldv, int B, int L, int H, uint8_t* vt, int Lpad, float* scale, cudaStream_t stream);
+
 // Row softmax of the fp32 GEMM accumulators S [rows, lds] (rows = heads x Lq queries) into P [rows, ldp]: p = bf16(softmax_fp32(
 // score)) over the keys j < cols, and 0 for the other columns up to ldp.  The score of key j in query row i of head h:
 //   SOFTMAX_SCALED (VAE):  s * scale, exponentials with __expf

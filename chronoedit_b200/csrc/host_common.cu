@@ -98,6 +98,10 @@ int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t col
   return make_tmap_bf16(out, base, 2, dims, strides, box);
 }
 
+int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box, nullptr);
+}
+
 int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
   uint64_t dims[2] = {cols, rows};
   uint64_t strides[1] = {ld};

@@ -52,6 +52,8 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows);
 // The same for a 1-byte element type (e4m3 GEMM operands); box = [box_rows, 128 cols], still one 128-byte swizzled row.
 int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows);
+// A 1-byte tensor of any rank, as make_tmap_bf16 (the FP8 attention's q, k and V^T tiles).
+int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box);
 
 int device_sm_count();   // of the CURRENT device (cached per device index)
 int check_device();

@@ -43,6 +43,30 @@ def quantize_fp8_rows(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     return q, s
 
 
+def quantize_fp8_heads(x: torch.Tensor, head_dim: int = 128) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The FP8 attention's rule for q and k: `quantize_fp8_rows` per (token, head), over the head_dim values of each head.
+    x [..., heads * head_dim] -> (q [..., heads * head_dim] float8_e4m3fn, s [..., heads] fp32).  What ce_quantize_heads_fp8
+    computes, bit for bit."""
+    *lead, n = x.shape
+    q, s = quantize_fp8_rows(x.reshape(-1, head_dim))
+    return q.reshape(*lead, n), s.reshape(*lead, n // head_dim)
+
+
+def quantize_fp8_channels(v: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The FP8 attention's rule for v [B, L, C]: one scale per (sample, channel) over the sample's tokens, i.e.
+    `quantize_fp8_rows(v[b].T)` for every sample.  Returns (v^T [B, C, L] float8_e4m3fn, keys in order, and s [B, C] fp32).
+    One sample's scales never depend on another sample."""
+    return quantize_fp8_rows(v.transpose(1, 2))
+
+
+def fp8_attention_key_order() -> torch.Tensor:
+    """Key (0..31) held at position p of every 32-key group of the device's V^T rows (ce_quantize_v_fp8): the order in which the
+    S accumulator's registers already are the 8-bit A fragment of the P V wgmma (DESIGN.md, "FP8 attention").
+    `stored[..., 32 g + p] = vt[..., 32 g + order[p]]`."""
+    p = torch.arange(32)
+    return 16 * (p // 16) + 8 * ((p % 4) // 2) + 2 * ((p % 16) // 4) + p % 2
+
+
 @dataclass
 class Transformer2DModelOutput:
     """Same shape as diffusers.models.modeling_outputs.Transformer2DModelOutput."""
@@ -209,6 +233,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._lora_adapters: Dict[str, Dict[str, torch.Tensor]] = {}
         self.last_captures: Dict[int, torch.Tensor] = {}
         self._fp8 = False
+        self._fp8_attention = False
 
     # ------------------------------------------------------------------------------------------ plumbing
     @property
@@ -258,6 +283,7 @@ class ChronoEditTransformer3DModel(nn.Module):
             h = _lib.c_void_p()
             cfg = self._cfg_c()
             check(_lib.lib().ce_dit_create(_lib.ctypes.byref(cfg), _lib.ctypes.byref(h)))
+            check(_lib.lib().ce_dit_set_attention_fp8(h, int(self._fp8_attention)))
             self._handle = h
         return self._handle
 
@@ -287,6 +313,24 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._pack_keepalive = {}   # the fused bf16 QKV buffers
         self._graphs = {}
         self._ctx_cache = []
+        self._workspaces = {}
+
+    @property
+    def fp8_attention_enabled(self) -> bool:
+        return self._fp8_attention
+
+    def enable_fp8_attention(self, enabled: bool = True) -> None:
+        """Opt-in FP8 self-attention (DESIGN.md, "FP8 attention"): every block's self-attention quantizes q and k per (token, head)
+        and v per (sample, channel) to e4m3 on the device and runs on e4m3 wgmma.  Cross-attention stays bf16.  Reversible
+        (`enable_fp8_attention(False)`), touches no weight, independent of `enable_fp8()`; it survives .to(), load_state_dict
+        and fuse_lora.  Toggling drops captured CUDA graphs and workspaces; the context cache stays valid."""
+        enabled = bool(enabled)
+        if enabled == self._fp8_attention:
+            return
+        if self._handle is not None:
+            check(_lib.lib().ce_dit_set_attention_fp8(self._handle, int(enabled)))
+        self._fp8_attention = enabled
+        self._graphs = {}
         self._workspaces = {}
 
     # ------------------------------------------------------------------------------------------ fp32 validation mode

@@ -77,8 +77,16 @@ int ce_dit_set_weight(ce_dit* h, const char* name, const void* ptr, int dtype, i
 /* 0 when every parameter the configuration needs has been registered; otherwise fails and names the first missing. */
 int ce_dit_weights_complete(const ce_dit* h);
 
+/* FP8 self-attention (DESIGN.md, "FP8 attention"), off by default: with enabled != 0 every block's self-attention quantizes q
+ * and k per (token, head) and v per (sample, channel) to e4m3 on the device and runs on e4m3 wgmma.  Cross-attention, the
+ * context cache and the weights are untouched; it works with bf16 and with FP8 weights.  ce_dit_workspace_bytes follows the
+ * flag, so query it after setting it.  Sequence parallelism is refused while it is on. */
+int ce_dit_set_attention_fp8(ce_dit* h, int enabled);
+
 /* Scratch bytes one forward needs for `batch` samples of latent geometry (frames, height, width) and text_len tokens.
- * A handle holding FP8 weights needs M * max(D, ffn_dim) bytes + M floats more (M = batch * tokens): the quantized rows. */
+ * A handle holding FP8 weights needs M * max(D, ffn_dim) bytes + M floats more (M = batch * tokens): the quantized rows.
+ * With FP8 attention on: M * 2D bytes + M * 2H floats (q | k and their scales) + batch * D * Lpad bytes + batch * D floats
+ * (V^T and its scales; Lpad = tokens rounded up to 32). */
 int64_t ce_dit_workspace_bytes(const ce_dit* h, int batch, int frames, int height, int width, int text_len);
 
 /* ChronoEditTransformer3DModel.forward (:397-476).
@@ -338,6 +346,19 @@ int ce_linear_fp8_ex(const ce_linear_fp8_args* args, void* stream);
 /* Per-row e4m3 quantization of x [rows, K] bf16 (K % 16 == 0, ldx % 8 == 0, ldq % 16 == 0): scale[m] = max_k |x| / 448
  * (1 for a zero row), q[m, k] = e4m3 bits of cvt.rn.satfinite(x / scale[m]), the division in IEEE fp32. */
 int ce_quantize_rows_fp8(const void* x, int ldx, int rows, int K, void* q, int ldq, float* scale, void* stream);
+
+/* FP8 attention, q | k: the rule of ce_quantize_rows_fp8 per (row, head) over 128 values.  x [rows, heads * 128] bf16 (ldx % 8)
+ * -> q [rows, heads * 128] e4m3 (ldq bytes, % 16) and scale [rows, heads] fp32. */
+int ce_quantize_heads_fp8(const void* x, int ldx, int rows, int heads, void* q, int ldq, float* scale, void* stream);
+/* FP8 attention, v [B, L, H * 128] bf16 (row stride ldv): scale [B, H * 128] = max over the sample's tokens |v| / 448 (1 if 0);
+ * vt [B, H, 128, Lpad] e4m3 = v / scale transposed, keys contiguous (Lpad >= L, % 32), the keys of every 32-key group stored in
+ * the order fp8_attention_key_order() of chronoedit_b200/transformer.py gives, keys >= L zero.  Two launches. */
+int ce_quantize_v_fp8(const void* v, int ldv, int B, int L, int H, void* vt, int Lpad, float* scale, void* stream);
+/* FP8 self-attention on the quantizers' outputs: q, k [B*L, ldqk bytes] e4m3 (head h at column h * 128), q_scale / k_scale
+ * [(b*L + i) * lds + h], vt / v_scale as ce_quantize_v_fp8 writes them; out [B*L, ldo] bf16, head h at column h * 128.
+ * out = bf16((sum_j P^ v^) v_scale / sum_j P^) with P^ = e4m3(256 exp2((q^ k^ q_scale k_scale) scale log2e - running max)). */
+int ce_attention_fp8(const void* q, const void* k, int ldqk, const float* q_scale, const float* k_scale, int lds, const void* vt, int Lpad,
+                     const float* v_scale, void* out, int ldo, int B, int H, int L, float scale, void* stream);
 
 /* FP32LayerNorm (+ modulate or affine) like ce_layernorm_bf16, with the row statistics merged from `tiles` stats_mode-1
  * partials of width tile_n covering [0, D) (stats [rows, stats_ld] float pairs).  scale_is_1p: `scale` holds 1 + scale.

@@ -2,7 +2,9 @@
 """bench.py's flagship configuration (14B, 720p, 2 latent frames, batch-2 CFG DiT call + fused UniPC step per denoising step) in
 one numeric mode per invocation, for comparing the opt-in FP8 mode against bf16:
 
-    python scripts/bench_fp8.py --mode bf16|fp8 [--steps 4] [--warmup 2] [--layers 40]
+    python scripts/bench_fp8.py --mode bf16|fp8 [--attention bf16|fp8] [--steps 4] [--warmup 2] [--layers 40]
+
+--attention fp8 also switches the self-attention to FP8 (enable_fp8_attention); its quantizers count as row kernels.
 
 Prints one JSON line: steps/s (CUDA events over the timed steps), the ce_dit_profile split by class from a separate profiled
 pass (GEMM / attention / row kernels, the FP8 row quantization counted as row kernels), the device bytes of the DiT's
@@ -34,6 +36,7 @@ def gpu_info():
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--mode", choices=("bf16", "fp8"), required=True)
+    ap.add_argument("--attention", choices=("bf16", "fp8"), default="bf16")
     ap.add_argument("--steps", type=int, default=4)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--layers", type=int, default=40)
@@ -53,6 +56,8 @@ def main():
     bench.init_weights_(model, seed=0)
     if args.mode == "fp8":
         model.enable_fp8()
+    if args.attention == "fp8":
+        model.enable_fp8_attention()
     model.pack_weights()
     torch.cuda.synchronize()
     weight_bytes = sum(t.numel() * t.element_size() for t in list(model.parameters()) + list(model.buffers()))
@@ -106,7 +111,8 @@ def main():
              for i, c in enumerate(CLASSES)}
     split["gemm"]["tflops"] = round(work[0] / (pms[0] / 1000.0) / 1e12, 1) if pms[0] else None
     split["rows"]["GBps"] = round(work[2] / (pms[2] / 1000.0) / 1e9, 1) if pms[2] else None
-    print(json.dumps({"mode": args.mode, "layers": args.layers, "steps": args.steps, "steps_per_s": round(args.steps / (ms / 1000.0), 4),
+    attn = {"attention": args.attention} if args.attention != "bf16" else {}
+    print(json.dumps({"mode": args.mode, **attn, "layers": args.layers, "steps": args.steps, "steps_per_s": round(args.steps / (ms / 1000.0), 4),
                       "ms_per_step": round(ms / args.steps, 1), "profile": split, "device_weight_bytes": weight_bytes, **info}), flush=True)
 
 

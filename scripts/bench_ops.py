@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Operator micro-benchmarks at the 14B / 720p shapes (CUDA events, warm-up, L2-busting operand rotation).
-    python scripts/bench_ops.py [attn] [gemm [cublas]] [gemmk] [rows] [conv]
+    python scripts/bench_ops.py [attn] [attn8] [gemm [cublas]] [gemmk] [rows] [conv]
+`attn8` times the self-attention in bf16 and as the FP8 attention runs it: the q | k and v quantizers and the e4m3 kernel.
 `gemm` times each block GEMM in bf16 and, in the fp8_* fields, as the FP8 mode runs it (quantization and e4m3 GEMM).
 `gemmk` times the bf16 o-proj GEMM over K and fits the time per wave of tiles to a + b K: `a` is the per-tile cost that does not
 scale with K (epilogue, hand-overs), `b` the main loop, printed as the TFLOP/s of all SMs while it runs.
@@ -53,6 +54,56 @@ def bench_attn(B=2, H=40, Lq=7200, Lk=7200, nbuf=3):
     ms = timeit(fn)
     fl = 4.0 * B * H * Lq * Lk * 128
     print(json.dumps({"op": "attention", "B": B, "H": H, "Lq": Lq, "Lk": Lk, "ms": round(ms, 4), "tflops": round(fl / ms / 1e9, 1)}), flush=True)
+
+
+def bench_attn8(B=2, H=40, Lk=7200, nbuf=2):
+    """Self-attention at [B, Lk, H x 128]: the bf16 kernel, then the FP8 path's three parts on the same fused QKV buffers."""
+    D = H * 128
+    bufs = [torch.randn(B, Lk, 3 * D, device="cuda", dtype=torch.bfloat16) for _ in range(nbuf)]
+    out = torch.empty(B, Lk, D, device="cuda", dtype=torch.bfloat16)
+    Lpad = (Lk + 31) // 32 * 32
+    qk8 = torch.empty(B * Lk, 2 * D, device="cuda", dtype=torch.uint8)
+    qks = torch.empty(B * Lk, 2 * H, device="cuda")
+    vt8 = torch.empty(B, D, Lpad, device="cuda", dtype=torch.uint8)
+    vs = torch.empty(B, D, device="cuda")
+    i = [0]
+    s = L.current_stream()
+
+    def nxt():
+        x = bufs[i[0] % nbuf]
+        i[0] += 1
+        return x
+
+    def bf16():
+        x = nxt()
+        L.check(lib.ce_attention_bf16(L.ptr(x), 3 * D, L.ptr(x[..., D:]), 3 * D, L.ptr(x[..., 2 * D:]), 3 * D, L.ptr(out), D, B, H, Lk, Lk,
+                                      1 / math.sqrt(128), 0, s))
+
+    def quant_qk():
+        L.check(lib.ce_quantize_heads_fp8(L.ptr(nxt()), 3 * D, B * Lk, 2 * H, L.ptr(qk8), 2 * D, L.ptr(qks), s))
+
+    def quant_v():
+        L.check(lib.ce_quantize_v_fp8(L.ptr(nxt()[..., 2 * D:]), 3 * D, B, Lk, H, L.ptr(vt8), Lpad, L.ptr(vs), s))
+
+    def fp8():
+        L.check(lib.ce_attention_fp8(L.ptr(qk8), L.ptr(qk8[:, D:]), 2 * D, L.ptr(qks), L.ptr(qks[:, H:]), 2 * H, L.ptr(vt8), Lpad, L.ptr(vs),
+                                     L.ptr(out), D, B, H, Lk, 1 / math.sqrt(128), s))
+
+    quant_qk()
+    quant_v()
+    fl = 4.0 * B * H * Lk * Lk * 128
+    res = {}
+    for name, fn in (("bf16", bf16), ("fp8", fp8), ("quant_qk", quant_qk), ("quant_v", quant_v), ("bf16_again", bf16), ("fp8_again", fp8)):
+        res[name] = timeit(fn)
+    qk_bytes, v_bytes = B * Lk * 2 * D * 3 + B * Lk * 2 * H * 4, B * Lk * D * 2 * 2 + B * D * Lpad + B * D * 4
+    print(json.dumps({"op": "attention_fp8", "B": B, "H": H, "Lk": Lk,
+                      "bf16_ms": [round(res["bf16"], 3), round(res["bf16_again"], 3)],
+                      "fp8_ms": [round(res["fp8"], 3), round(res["fp8_again"], 3)],
+                      "bf16_tflops": round(fl / min(res["bf16"], res["bf16_again"]) / 1e9, 1),
+                      "fp8_tflops": round(fl / min(res["fp8"], res["fp8_again"]) / 1e9, 1),
+                      "quant_qk_ms": round(res["quant_qk"], 3), "quant_qk_GBps": round(qk_bytes / res["quant_qk"] / 1e6, 1),
+                      "quant_v_ms": round(res["quant_v"], 3), "quant_v_GBps": round(v_bytes / res["quant_v"] / 1e6, 1),
+                      "fp8_total_ms": round(min(res["fp8"], res["fp8_again"]) + res["quant_qk"] + res["quant_v"], 3)}), flush=True)
 
 
 def bench_attn_libs(B=2, H=40, L=7200, Lk=None):
@@ -255,6 +306,9 @@ if __name__ == "__main__":
         bench_attn(Lk=512)
         bench_attn(Lk=257)
         bench_attn_dual()
+    if "attn8" in what:
+        bench_attn8()
+        bench_attn8(B=2, Lk=28800)
     if "attnself" in what:
         bench_attn()
         bench_attn(B=1, Lq=28800, Lk=28800, nbuf=2)
