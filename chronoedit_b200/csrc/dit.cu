@@ -12,6 +12,7 @@
 // With FP8 attention on (ce_dit_set_attention_fp8) the self-attention becomes quantize(q|k) -> quantize(v) -> attention_fp8.
 #include <math.h>
 
+#include <atomic>
 #include <map>
 #include <string>
 #include <vector>
@@ -446,13 +447,16 @@ int64_t ce_dit_sp_region_bytes(const ce_dit* h, int batch, int frames, int heigh
 
 int ce_dit_sp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes) {
   CE_REQUIRE(h, "ce_dit_sp_configure: null handle");
+  const int host_barrier_ms = h->sp.host_barrier_ms;
   if (world <= 1) {
     h->sp = SeqPar();
+    h->sp.host_barrier_ms = host_barrier_ms;
     return CE_OK;
   }
   CE_REQUIRE(world <= 8 && rank >= 0 && rank < world && region_ptrs && region_bytes > 0, "ce_dit_sp_configure: arguments");
   CE_REQUIRE(h->cfg.num_attention_heads % world == 0, "ce_dit_sp_configure: the head count must be divisible by the number of ranks");
   h->sp = SeqPar();
+  h->sp.host_barrier_ms = host_barrier_ms;
   h->sp.rank = rank;
   h->sp.world = world;
   h->sp.region_bytes = region_bytes;
@@ -460,6 +464,13 @@ int ce_dit_sp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs
     CE_REQUIRE(region_ptrs[w] != nullptr, "ce_dit_sp_configure: null region pointer");
     h->sp.region[w] = reinterpret_cast<uint8_t*>(region_ptrs[w]);
   }
+  return CE_OK;
+}
+
+int ce_dit_sp_host_barrier(ce_dit* h, int timeout_ms) {
+  CE_REQUIRE(h && timeout_ms >= 0, "ce_dit_sp_host_barrier: arguments");
+  h->sp.host_barrier_ms = timeout_ms;
+  h->sp.host.reset();   // the next barrier joins the rendezvous afresh
   return CE_OK;
 }
 
@@ -539,7 +550,8 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   const bool spx = sp.world > 1;
   if (spx) {
     CE_REQUIRE(!h->attn_fp8, "sequence parallelism is not built for FP8 attention: run it on one GPU or switch it off (ce_dit_set_attention_fp8)");
-    CE_REQUIRE(Lfull % sp.world == 0 && D % 256 == 0, "sequence parallel: tokens must divide by the rank count and the width by 256");
+    CE_REQUIRE(Lfull % sp.world == 0, "sequence parallel: the tokens must divide by the rank count");
+    CE_REQUIRE(D % 256 == 0, "sequence parallel: the width must be a multiple of 256 (the q | k scatter needs the GEMM's row statistics)");
     CE_REQUIRE(Lfull >= 256, "sequence parallel: at least 256 tokens (the self-attention kernel with the output scatter)");
     CE_REQUIRE(!h->profiling && h->capture.empty() && block0_out == nullptr, "sequence parallel: no per-launch profiling / block capture");
   }
@@ -880,11 +892,11 @@ int ce_quantize_rows_fp8(const void* x, int ldx, int rows, int K, void* q, int l
                                   reinterpret_cast<cudaStream_t>(stream));
 }
 
-static long long* g_attn_timing = nullptr;
+static std::atomic<long long*> g_attn_timing{nullptr};   // process-wide; read by calls from any host thread
 // Profiling aid: subsequent ce_attention_bf16 calls record the phase cycles of the first consumer thread of block 0 into `buf`
 // ([16] int64 on the device); pass NULL to stop.
 int ce_debug_attention_timing(long long* buf) {
-  g_attn_timing = buf;
+  g_attn_timing.store(buf);
   return CE_OK;
 }
 
@@ -906,7 +918,7 @@ int ce_attention_bf16(const void* q, int ldq, const void* k, int ldk, const void
   a.out = reinterpret_cast<bf16*>(out); a.ldo = ldo;
   a.scale = scale;
   a.accumulate = accumulate;
-  a.timing = g_attn_timing;
+  a.timing = g_attn_timing.load();
   return launch_attention(a, reinterpret_cast<cudaStream_t>(stream));
 }
 

@@ -1,5 +1,6 @@
 #include "host_common.h"
 
+#include <atomic>
 #include <map>
 #include <mutex>
 #include <utility>
@@ -112,15 +113,15 @@ int make_tmap_2d_u8(CUtensorMap* out, const void* base, uint64_t rows, uint64_t 
 constexpr int kMaxDevices = 64;
 
 int device_sm_count() {
-  static int n[kMaxDevices] = {0};
+  static std::atomic<int> n[kMaxDevices] = {};   // handles driven from several host threads fill it concurrently
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return 0;
-  if (n[dev] == 0) {
-    int v = 0;
+  int v = n[dev].load(std::memory_order_relaxed);
+  if (v == 0) {
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    n[dev] = v;
+    n[dev].store(v, std::memory_order_relaxed);
   }
-  return n[dev];
+  return v;
 }
 
 int ensure_dynamic_smem(const void* kernel, int bytes) {

@@ -2,6 +2,12 @@
 
 #include <string.h>
 
+#include <chrono>
+#include <condition_variable>
+#include <map>
+#include <mutex>
+#include <string>
+
 #include "../../include/chronoedit_b200.h"
 
 namespace ce {
@@ -92,10 +98,78 @@ SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world) {
   return l;
 }
 
+// The host barrier's rendezvous: one per region table (keyed on region[0]) among the handles of this process.
+struct HostRendezvous {
+  std::mutex mu;
+  std::condition_variable cv;
+  int world = 0;
+  uint32_t arrived = 0;     // bit r: rank r has arrived at the current barrier
+  uint32_t epoch = 0;       // the epoch of the current barrier (every rank's handle counts its barriers the same way)
+  uint64_t generation = 0;  // completed barriers
+  std::string poisoned;     // non-empty: a barrier timed out or a rank fell out of step; every later barrier fails with this
+
+  int arrive(int rank, uint32_t ep, int timeout_ms) {
+    std::unique_lock<std::mutex> lock(mu);
+    if (!poisoned.empty()) return fail(CE_ERR_INVALID, "sequence-parallel host barrier: rank " + std::to_string(rank) + " at barrier " +
+                                                           std::to_string(ep) + ": the group failed earlier (" + poisoned + ")");
+    if (arrived == 0) epoch = ep;
+    if (ep != epoch || (arrived >> rank & 1u)) {
+      poisoned = "rank " + std::to_string(rank) + " arrived at barrier " + std::to_string(ep) + " while the group waits at barrier " +
+                 std::to_string(epoch) + ((arrived >> rank & 1u) ? " (twice)" : "");
+      cv.notify_all();
+      return fail(CE_ERR_INVALID, "sequence-parallel host barrier: ranks out of step: " + poisoned);
+    }
+    arrived |= 1u << rank;
+    if (arrived == (1u << world) - 1) {
+      arrived = 0;
+      ++generation;
+      cv.notify_all();
+      return CE_OK;
+    }
+    const uint64_t gen = generation;
+    const bool done = cv.wait_for(lock, std::chrono::milliseconds(timeout_ms), [&] { return generation != gen || !poisoned.empty(); });
+    if (generation != gen) return CE_OK;
+    if (!done) {
+      std::string missing;
+      for (int w = 0; w < world; ++w)
+        if (!(arrived >> w & 1u)) missing += (missing.empty() ? "" : ", ") + std::to_string(w);
+      poisoned = "rank " + std::to_string(rank) + " timed out after " + std::to_string(timeout_ms) + " ms at barrier " + std::to_string(ep) +
+                 " waiting for rank(s) " + missing;
+      cv.notify_all();
+      return fail(CE_ERR_INVALID, "sequence-parallel host barrier: " + poisoned);
+    }
+    return fail(CE_ERR_INVALID, "sequence-parallel host barrier: rank " + std::to_string(rank) + " at barrier " + std::to_string(ep) +
+                                    ": the group failed (" + poisoned + ")");
+  }
+};
+
+static int host_barrier(SeqPar& sp, cudaStream_t stream) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CE_CHECK_CUDA(cudaStreamIsCapturing(stream, &cs));
+  CE_REQUIRE(cs == cudaStreamCaptureStatusNone, "sequence-parallel host barrier: the stream is capturing (a host wait cannot be captured)");
+  CE_CHECK_CUDA(cudaStreamSynchronize(stream));
+  if (!sp.host) {   // join (or found) the rendezvous of this region table; it lives as long as a handle configured with it
+    static std::mutex mu;
+    static std::map<const void*, std::weak_ptr<HostRendezvous>> groups;
+    std::lock_guard<std::mutex> lock(mu);
+    for (auto it = groups.begin(); it != groups.end();) it = it->second.expired() ? groups.erase(it) : std::next(it);
+    std::shared_ptr<HostRendezvous> g = groups[sp.region[0]].lock();
+    if (!g) {
+      g = std::make_shared<HostRendezvous>();
+      g->world = sp.world;
+      groups[sp.region[0]] = g;
+    }
+    CE_REQUIRE(g->world == sp.world, "sequence-parallel host barrier: handles share region 0 with different rank counts");
+    sp.host = g;
+  }
+  return sp.host->arrive(sp.rank, sp.epoch, sp.host_barrier_ms);
+}
+
 int launch_sp_barrier(SeqPar& sp, const SpLayout& lay, cudaStream_t stream) {
   Ptrs8 f;
   for (int w = 0; w < 8; ++w) f.p[w] = w < sp.world ? sp.region[w] + lay.flags : nullptr;
   ++sp.epoch;
+  if (sp.host_barrier_ms > 0) return host_barrier(sp, stream);
   sp_barrier_kernel<<<1, 32, 0, stream>>>(f, sp.rank, sp.world, sp.epoch);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;

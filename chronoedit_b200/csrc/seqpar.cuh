@@ -4,17 +4,26 @@
 // the kernels that PRODUCE the data store it straight into the consuming rank's memory over NVLink (peer pointers obtained with
 // CUDA IPC) -- the RMSNorm+RoPE kernel scatters q | k by head, a copy kernel scatters v, the attention epilogue scatters the
 // output rows back to the ranks that own the tokens -- and a flag barrier in peer memory orders the phases.
+//
+// Test aid (ce_dit_sp_host_barrier): `world` handles of ONE process on ONE GPU can play the ranks, with ordinary device allocations
+// as regions.  The barrier is then a host rendezvous instead of the flag kernel, so no kernel ever waits for another rank's work.
 #pragma once
+#include <memory>
+
 #include "host_common.h"
 #include "ptx.cuh"
 
 namespace ce {
+
+struct HostRendezvous;
 
 struct SeqPar {
   int rank = 0, world = 1;
   uint8_t* region[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // same layout on every rank
   int64_t region_bytes = 0;
   uint32_t epoch = 0;
+  int host_barrier_ms = 0;                // > 0: launch_sp_barrier is a host rendezvous with this timeout (kept across configures)
+  std::shared_ptr<HostRendezvous> host;   // the rendezvous of this region table, joined at the first host barrier
 };
 
 struct SpLayout {   // byte offsets inside a rank's region
@@ -26,7 +35,10 @@ struct SpLayout {   // byte offsets inside a rank's region
 };
 SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world);
 
-// all ranks: everything this rank issued so far on `stream` (incl. its peer stores) is complete and visible before any rank continues
+// all ranks: everything this rank issued so far on `stream` (incl. its peer stores) is complete and visible before any rank continues.
+// With sp.host_barrier_ms > 0 no kernel is launched: the stream is synchronised and the calling thread waits for the other ranks'
+// threads (same process, same region[0]); a timeout is an error naming the rank and the barrier and poisons the group, so every
+// later barrier of it fails at once.  Refused while `stream` is capturing.
 int launch_sp_barrier(SeqPar& sp, const SpLayout& lay, cudaStream_t stream);
 // dst[r] + ((b * dst_rows_per_batch + dst_row0 + i) * cols_per_rank + c % cols_per_rank) = src[(b * rows_per_batch + i) * ld_src + c],
 // r = c / cols_per_rank   (v scatter: columns to the rank that owns the head)

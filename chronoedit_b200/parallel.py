@@ -112,14 +112,10 @@ def enable_sequence_parallel(model, batch: int, frames: int, height: int, width:
         raise CEError("enable_sequence_parallel needs an initialised torch.distributed process group (one process per GPU)")
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     L = _lib.lib()
-    if not model._packed:
-        model.pack_weights()
     disable_sequence_parallel(model)
     if world == 1:
         return 0
-    n = L.ce_dit_sp_region_bytes(model._handle, batch, frames, height, width, world)
-    if n < 0:
-        raise CEError(f"sequence parallel: tokens and heads must be divisible by the world size {world}")
+    n = sp_region_bytes(model, batch, frames, height, width, world)
     with torch.cuda.device(model.device):
         own = ctypes.c_void_p()
         check(L.ce_ipc_alloc(n, ctypes.byref(own)))
@@ -137,13 +133,43 @@ def enable_sequence_parallel(model, batch: int, frames: int, height: int, width:
             check(L.ce_ipc_open(hb, ctypes.byref(p)))
             ptrs.append(p.value)
             opened.append(p)
-        table = (ctypes.c_void_p * world)(*ptrs)
-        check(L.ce_dit_sp_configure(model._handle, rank, world, table, n))
-        torch.cuda.synchronize(model.device)
+        configure_sequence_parallel(model, rank, ptrs, n, {"own": own, "opened": opened})
     dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
-    model._sp_state = {"own": own, "opened": opened, "world": world, "bytes": n}
-    model._graphs = {}
     return int(n)
+
+
+def sp_region_bytes(model, batch: int, frames: int, height: int, width: int, world: int) -> int:
+    """Bytes of the peer region every rank needs for this geometry (ce_dit_sp_region_bytes); packs the weights first."""
+    from . import _lib
+    from ._lib import CEError
+
+    if not model._packed:
+        model.pack_weights()
+    n = _lib.lib().ce_dit_sp_region_bytes(model._handle, batch, frames, height, width, world)
+    if n < 0:
+        raise CEError(f"sequence parallel: tokens and heads must be divisible by the world size {world} (2 to 8)")
+    return int(n)
+
+
+def configure_sequence_parallel(model, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict) -> None:
+    """Hand rank `rank`'s table of peer-region addresses (one per rank, as seen from this process) to the model's C handle
+    (ce_dit_sp_configure) and switch the model into sequence-parallel mode.  `state` is kept as `model._sp_state` (with "world" and
+    "bytes" added) and holds whatever disable_sequence_parallel releases: the own region under "own" (freed with ce_ipc_free) and the
+    opened peer mappings under "opened" (closed with ce_ipc_close)."""
+    import ctypes
+
+    from . import _lib
+    from ._lib import check
+
+    if not model._packed:
+        model.pack_weights()
+    world = len(region_ptrs)
+    table = (ctypes.c_void_p * world)(*region_ptrs)
+    with torch.cuda.device(model.device):
+        check(_lib.lib().ce_dit_sp_configure(model._handle, rank, world, table, region_bytes))
+        torch.cuda.synchronize(model.device)
+    model._sp_state = dict(state, world=world, bytes=region_bytes)
+    model._graphs = {}
 
 
 def disable_sequence_parallel(model) -> None:
@@ -155,9 +181,10 @@ def disable_sequence_parallel(model) -> None:
     L = _lib.lib()
     torch.cuda.synchronize(model.device)
     L.ce_dit_sp_configure(model._handle, 0, 1, None, 0)
-    for p in st["opened"]:
+    for p in st.get("opened", ()):
         L.ce_ipc_close(p)
     if dist.is_initialized():
         dist.barrier()
-    L.ce_ipc_free(st["own"])
+    if st.get("own") is not None:
+        L.ce_ipc_free(st["own"])
     model._sp_state = None

@@ -543,9 +543,9 @@ class ChronoEditTransformer3DModel(nn.Module):
             ctx_buf, ctx_reuse = self._context_slot(txt_in, img_in, txt, img)
         try:
             with torch.cuda.device(self.device):
-                check(L.ce_dit_forward_ex(self._handle, ptr(x), ptr(t), ptr(txt), ptr(img), ptr(out), B, T, H, W, Lt, ptr(ws), ws.numel(),
-                                          ptr(b0), ptr(ctx_buf), ctx_buf.numel() if ctx_buf is not None else 0, ctx_reuse,
-                                          current_stream()))
+                self._check_forward(L.ce_dit_forward_ex(self._handle, ptr(x), ptr(t), ptr(txt), ptr(img), ptr(out), B, T, H, W, Lt, ptr(ws),
+                                                        ws.numel(), ptr(b0), ptr(ctx_buf), ctx_buf.numel() if ctx_buf is not None else 0,
+                                                        ctx_reuse, current_stream()), ctx_buf, ctx_reuse)
         finally:
             if caps:
                 check(L.ce_dit_set_capture(self._handle, None, None, 0))
@@ -569,8 +569,9 @@ class ChronoEditTransformer3DModel(nn.Module):
         def launch(xs, ts, txts, imgs, outs, reuse):
             ws = self._workspace(B, T, H, W, Lt)
             with torch.cuda.device(self.device):
-                check(L.ce_dit_forward_ex(self._handle, ptr(xs), ptr(ts), ptr(txts), ptr(imgs), ptr(outs), B, T, H, W, Lt, ptr(ws), ws.numel(),
-                                          None, ptr(ctx_buf), ctx_buf.numel() if ctx_buf is not None else 0, reuse, current_stream()))
+                self._check_forward(L.ce_dit_forward_ex(self._handle, ptr(xs), ptr(ts), ptr(txts), ptr(imgs), ptr(outs), B, T, H, W, Lt,
+                                                        ptr(ws), ws.numel(), None, ptr(ctx_buf),
+                                                        ctx_buf.numel() if ctx_buf is not None else 0, reuse, current_stream()), ctx_buf, reuse)
 
         g = self._graphs.get(key)
         if g is None or (self.cache_context and not ctx_reuse):
@@ -604,10 +605,10 @@ class ChronoEditTransformer3DModel(nn.Module):
         counter -- the unchanged pipeline passes the same `prompt_embeds` / `negative_prompt_embeds` / `image_embeds` objects at
         every step (pipeline_chronoedit.py:715-735)."""
         ver = lambda t: None if t is None else t._version
-        for e in self._ctx_cache:
+        for i, e in enumerate(self._ctx_cache):
             if e["txt"] is txt_in and e["img"] is img_in and e["txt_v"] == ver(txt_in) and e["img_v"] == ver(img_in):
-                self._ctx_cache.remove(e)
-                self._ctx_cache.append(e)   # most recently used last
+                # most recently used last; by position, since list.remove would compare the entries' tensors with ==
+                self._ctx_cache.append(self._ctx_cache.pop(i))
                 return e["buf"], 1
         B, Lt = txt.shape[0], txt.shape[1]
         n = _lib.lib().ce_dit_context_cache_bytes(self._handle, B, Lt)
@@ -622,6 +623,13 @@ class ChronoEditTransformer3DModel(nn.Module):
             buf = torch.empty(n, dtype=torch.uint8, device=self.device)
         self._ctx_cache.append(dict(txt=txt_in, img=img_in, txt_v=ver(txt_in), img_v=ver(img_in), buf=buf))
         return buf, 0
+
+    def _check_forward(self, rc, ctx_buf, ctx_reuse) -> None:
+        """check(rc) of a forward call.  A forward that was to fill a context-cache slot and failed may have stopped before writing all
+        of it (the K/V of later layers are projected inside the layer loop), so the slot is dropped rather than reused."""
+        if rc != 0 and ctx_buf is not None and not ctx_reuse:
+            self._ctx_cache = [e for e in self._ctx_cache if e["buf"] is not ctx_buf]
+        check(rc)
 
     def clear_context_cache(self) -> None:
         self._ctx_cache = []
@@ -655,10 +663,10 @@ class ChronoEditTransformer3DModel(nn.Module):
             ctx_buf, ctx_reuse = self._context_slot(encoder_hidden_states, encoder_hidden_states_image, encoder_hidden_states,
                                                     encoder_hidden_states_image)
         with torch.cuda.device(self.device):
-            check(L.ce_dit_forward_host_ex(self._handle, ptr(hidden_states), ptr(t), ptr(encoder_hidden_states),
-                                           ptr(encoder_hidden_states_image), ptr(out), B, T, H, W, Lt, ptr(st), st.numel(), ptr(ws),
-                                           ws.numel(), ptr(ctx_buf), ctx_buf.numel() if ctx_buf is not None else 0, ctx_reuse,
-                                           current_stream()))
+            self._check_forward(L.ce_dit_forward_host_ex(self._handle, ptr(hidden_states), ptr(t), ptr(encoder_hidden_states),
+                                                         ptr(encoder_hidden_states_image), ptr(out), B, T, H, W, Lt, ptr(st), st.numel(),
+                                                         ptr(ws), ws.numel(), ptr(ctx_buf), ctx_buf.numel() if ctx_buf is not None else 0,
+                                                         ctx_reuse, current_stream()), ctx_buf, ctx_reuse)
         if not return_device_sample:
             return out
         off = L.ce_dit_host_staging_sample_offset(self._handle, B, T, H, W, Lt)

@@ -302,6 +302,18 @@ int ce_rope_table_host(int head_dim, int frames, int height_patches, int width_p
                        int temporal_skip_len, float theta, float* cos_out_host, float* sin_out_host);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Test aid: the sequence-parallel forward on ONE GPU.  With timeout_ms > 0 the barriers between the phases of the exchange
+ * (ce_dit_sp_configure) launch no kernel: each one synchronises the rank's stream, then its thread waits until the threads of
+ * all `world` handles of this process configured with the same region table (same region_ptrs[0]) have arrived.  So `world`
+ * handles driven from `world` host threads, each on its own stream, with ordinary device allocations as regions, run the same
+ * kernels, address arithmetic and peer stores as `world` GPUs, and no kernel ever spins on another rank's progress.  A wait
+ * longer than timeout_ms fails with an error naming the rank and the barrier, and every later barrier of that group fails at
+ * once (configure again to start over).  The mode is refused while the stream is capturing a graph.  0 (the default) restores
+ * the device barrier.  The setting survives ce_dit_sp_configure.  The single-GPU forward is unaffected.
+ * ------------------------------------------------------------------------------------------------------------ */
+int ce_dit_sp_host_barrier(ce_dit* h, int timeout_ms);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Test aids: the DiT's fused-statistics path, one operator at a time.  When D % 256 == 0 the GEMM that writes a
  * row also writes per-(row, N tile) statistics of the values it stored, and the LayerNorm / RMSNorm that follows
  * merges those partials instead of reducing over the row.  Not needed to run the model.

@@ -221,3 +221,55 @@ def test_size_queries_reject_bad_geometry(handle):
     assert h.lib.ce_dit_workspace_bytes(h.h, 1, 2, 15, 24, 512) == -1    # odd latent height
     assert h.lib.ce_dit_workspace_bytes(h.h, 9, 2, 16, 24, 512) == -1    # batch 1..8
     assert h.lib.ce_dit_context_cache_bytes(h.h, 0, 512) == -1
+
+
+def test_context_cache_slots_follow_any_prompt_order():
+    """The context cache's two LRU slots (prompt and negative prompt) under any order of calls, not only strict alternation: a hit on
+    the older slot must move it to the back without comparing the entries' tensors, and a third prompt evicts the least recently used
+    slot and reuses its buffer."""
+    import chronoedit_b200 as ce
+
+    m = ce.ChronoEditTransformer3DModel(num_attention_heads=2, in_channels=36, ffn_dim=256, num_layers=1, image_dim=1280,
+                                        added_kv_proj_dim=256, text_dim=64, cache_context=True)
+    m._ensure_handle()
+    prompt, negative, other = (torch.randn(1, 8, 64) for _ in range(3))
+    img = torch.randn(1, 257, 1280)
+    slot = lambda txt: m._context_slot(txt, img, txt, img)
+    p_buf, reuse = slot(prompt)
+    assert reuse == 0
+    n_buf, reuse = slot(negative)
+    assert reuse == 0 and n_buf is not p_buf
+    for txt, buf in ((prompt, p_buf), (prompt, p_buf), (negative, n_buf), (negative, n_buf), (prompt, p_buf), (negative, n_buf)):
+        got, reuse = slot(txt)
+        assert reuse == 1 and got is buf
+    assert [e["txt"] is negative for e in m._ctx_cache] == [False, True]
+    got, reuse = slot(other)   # evicts the prompt, the least recently used
+    assert reuse == 0 and got is p_buf
+    assert slot(negative) == (n_buf, 1)
+    prompt.add_(1)   # an in-place update invalidates the entry
+    assert slot(other)[1] == 1 and slot(prompt)[1] == 0
+
+
+def test_failed_forward_does_not_leave_a_half_filled_context_slot():
+    """A forward that was to fill a context-cache slot and failed may have stopped before the K/V of later layers: its slot is dropped,
+    so the next call with the same prompt computes the context again.  A failed call that only read the slot keeps it."""
+    import chronoedit_b200 as ce
+
+    m = ce.ChronoEditTransformer3DModel(num_attention_heads=2, in_channels=36, ffn_dim=256, num_layers=1, image_dim=1280,
+                                        added_kv_proj_dim=256, text_dim=64, cache_context=True)
+    m._ensure_handle()
+    prompt, negative = torch.randn(1, 8, 64), torch.randn(1, 8, 64)
+    img = torch.randn(1, 257, 1280)
+    p_buf, _ = m._context_slot(prompt, img, prompt, img)
+    m._check_forward(0, p_buf, 0)
+    n_buf, reuse = m._context_slot(negative, img, negative, img)
+    assert reuse == 0
+    with pytest.raises(ce.CEError):
+        m._check_forward(-1, n_buf, 0)
+    assert [e["buf"] for e in m._ctx_cache] == [p_buf]
+    assert m._context_slot(negative, img, negative, img)[1] == 0
+    buf, reuse = m._context_slot(prompt, img, prompt, img)
+    assert (buf, reuse) == (p_buf, 1)
+    with pytest.raises(ce.CEError):
+        m._check_forward(-1, buf, 1)
+    assert m._context_slot(prompt, img, prompt, img) == (p_buf, 1)

@@ -1,6 +1,10 @@
 """Sequence-parallel DiT forward (tokens of one edit split over the GPUs of a node, q/k/v and attention output exchanged by peer
 stores inside the kernels, csrc/seqpar.cuh) against the single-GPU forward: bit-identical on every rank.  Needs >= 2 GPUs;
-skipped on a single-GPU machine."""
+skipped on a single-GPU machine.
+
+The kernels, their address arithmetic and the host wiring are covered on one GPU by tests/test_gpu_seqpar_one_gpu.py (host
+barrier, world 2 to 8).  What only this test covers is the real multi-GPU machinery: the device flag barrier (sp_barrier_kernel),
+the CUDA IPC handle exchange through torch.distributed, and peer stores over NVLink into another GPU's memory."""
 import os
 import subprocess
 import sys

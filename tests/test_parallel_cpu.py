@@ -80,3 +80,96 @@ def test_sequence_parallel_host_checks():
         parallel.enable_sequence_parallel(object(), 1, 2, 4, 4)
     assert _lib.lib().ce_dit_sp_region_bytes(None, 1, 2, 4, 4, 2) == -1
     parallel.disable_sequence_parallel(object())   # a model that never enabled it: no-op
+
+
+def _sp_handle(heads):
+    """A C handle of a 1-layer model with `heads` heads (no device needed: the sequence-parallel set-up calls are host-only)."""
+    import chronoedit_b200 as ce
+
+    m = ce.ChronoEditTransformer3DModel(num_attention_heads=heads, in_channels=36, ffn_dim=256, num_layers=1, image_dim=1280,
+                                        added_kv_proj_dim=heads * 128, text_dim=64)
+    return m, m._ensure_handle()
+
+
+def test_sp_region_bytes_matches_the_layout_restatement():
+    """ce_dit_sp_region_bytes against the Python sp_layout the one-GPU test derives its guard ranges from, for world 2 to 8, with
+    sub-buffer sizes that are and are not multiples of the 1024-byte alignment."""
+    from chronoedit_b200 import _lib
+    from tests.test_gpu_seqpar_one_gpu import sp_layout, sp_unwritten_ranges
+
+    L = _lib.lib()
+    padded = 0
+    for world in range(2, 9):
+        heads = world * (1 if world > 4 else 2)
+        m, h = _sp_handle(heads)
+        D = heads * 128
+        for B, (T, H, W) in ((1, (2, 16, 16)), (2, (2, 24, 20)), (1, (8, 18, 10)), (3, (2, 30, 42)), (2, (8, 90, 160))):
+            tokens = T * (H // 2) * (W // 2)
+            if tokens % world:
+                assert L.ce_dit_sp_region_bytes(h, B, T, H, W, world) == -1
+                continue
+            lay = sp_layout(B, tokens, D, 64, world)
+            assert L.ce_dit_sp_region_bytes(h, B, T, H, W, world) == lay["bytes"], (world, B, T, H, W)
+            offs = [lay[k] for k in ("q", "k", "v", "attn", "yout", "flags")]
+            assert all(o % 1024 == 0 for o in offs) and offs == sorted(offs)
+            assert lay["bytes"] - lay["flags"] == 1024 == 8 * 32 * 4   # the flags block: uint32 [8 * 32]
+            for name, nxt in (("q", "k"), ("k", "v"), ("v", "attn"), ("attn", "yout"), ("yout", "flags")):
+                assert 0 <= lay[nxt] - (lay[name] + lay["used"][name]) < 1024
+            gaps = sp_unwritten_ranges(lay)
+            assert gaps[-1] == ("flags", lay["flags"], lay["bytes"])
+            padded += len(gaps) - 1
+        del m
+    assert padded > 0, "no case exercised the alignment padding"
+
+
+def test_sp_region_bytes_refusals():
+    from chronoedit_b200 import _lib
+
+    L = _lib.lib()
+    m, h = _sp_handle(4)
+    assert L.ce_dit_sp_region_bytes(h, 1, 2, 32, 32, 2) > 0
+    assert L.ce_dit_sp_region_bytes(h, 1, 2, 32, 32, 1) == -1     # world 1 is not sequence parallel
+    assert L.ce_dit_sp_region_bytes(h, 1, 2, 32, 32, 9) == -1     # at most 8 ranks
+    assert L.ce_dit_sp_region_bytes(h, 0, 2, 32, 32, 2) == -1     # batch
+    assert L.ce_dit_sp_region_bytes(h, 1, 2, 18, 30, 4) == -1     # 270 tokens % 4
+    m3, h3 = _sp_handle(3)
+    assert L.ce_dit_sp_region_bytes(h3, 1, 2, 32, 32, 2) == -1    # 3 heads % 2
+    assert L.ce_dit_sp_region_bytes(h3, 1, 2, 24, 32, 3) > 0
+
+
+def test_sp_configure_refusals():
+    import ctypes
+
+    from chronoedit_b200 import _lib
+
+    L = _lib.lib()
+    m, h = _sp_handle(4)
+    regions = [ctypes.create_string_buffer(64) for _ in range(8)]
+    table = (ctypes.c_void_p * 8)(*[ctypes.addressof(r) for r in regions])
+
+    def refused(*args, msg):
+        assert L.ce_dit_sp_configure(*args) == -1
+        assert msg in L.ce_last_error().decode()
+
+    refused(None, 0, 2, table, 64, msg="null handle")
+    refused(h, 0, 9, table, 64, msg="arguments")
+    refused(h, -1, 2, table, 64, msg="arguments")
+    refused(h, 2, 2, table, 64, msg="arguments")
+    refused(h, 0, 2, None, 64, msg="arguments")
+    refused(h, 0, 2, table, 0, msg="arguments")
+    refused(h, 0, 8, table, 64, msg="head count must be divisible")
+    holes = (ctypes.c_void_p * 2)(ctypes.addressof(regions[0]), None)
+    refused(h, 0, 2, holes, 64, msg="null region pointer")
+    assert L.ce_dit_sp_configure(h, 1, 4, table, 64) == 0
+    assert L.ce_dit_sp_configure(h, 0, 1, None, 0) == 0            # world 1 switches it off
+
+
+def test_sp_host_barrier_arguments():
+    from chronoedit_b200 import _lib
+
+    L = _lib.lib()
+    m, h = _sp_handle(2)
+    assert L.ce_dit_sp_host_barrier(None, 1000) == -1 and b"ce_dit_sp_host_barrier: arguments" in L.ce_last_error()
+    assert L.ce_dit_sp_host_barrier(h, -1) == -1 and b"ce_dit_sp_host_barrier: arguments" in L.ce_last_error()
+    assert L.ce_dit_sp_host_barrier(h, 60000) == 0
+    assert L.ce_dit_sp_host_barrier(h, 0) == 0                     # back to the device barrier
