@@ -63,6 +63,25 @@ class LinearFp8ArgsC(ctypes.Structure):   # ce_linear_fp8_args
     _fields_ = [("base", LinearArgsC), ("a_scale", c_void_p), ("w_scale", c_void_p)]
 
 
+class Conv3dArgsC(ctypes.Structure):   # ce_conv3d_args
+    _fields_ = [
+        ("x", c_void_p), ("Tin", c_int32), ("Hin", c_int32), ("Win", c_int32), ("Cin", c_int32), ("w", c_void_p), ("bias", c_void_p),
+        ("Cout", c_int32), ("Cin_pad", c_int32), ("kt", c_int32), ("kh", c_int32), ("kw", c_int32), ("st", c_int32), ("sh", c_int32),
+        ("sw", c_int32), ("ph", c_int32), ("pw", c_int32), ("t_base", c_int32), ("y", c_void_p), ("Tout", c_int32), ("Hout", c_int32),
+        ("Wout", c_int32), ("resid", c_void_p), ("split_time", c_int32), ("planar_out", c_int32), ("clamp", c_int32),
+        ("planar_T", c_int32), ("planar_t0", c_int32),
+    ]
+
+
+class GemmAttentionArgsC(ctypes.Structure):   # ce_gemm_attention_args
+    _fields_ = [
+        ("x", c_void_p), ("D", c_int32), ("L", c_int32), ("H", c_int32), ("dk", c_int32), ("kpv", c_int32), ("wqk", c_void_p),
+        ("bqk", c_void_p), ("wv", c_void_p), ("bv", c_void_p), ("rule", c_int32), ("scale", c_float), ("bias", c_void_p),
+        ("bias_ld", c_int32), ("valid", c_int32), ("qk", c_void_p), ("vT", c_void_p), ("S", c_void_p), ("P", c_void_p),
+        ("out", c_void_p), ("ldo", c_int32),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/chronoedit_b200.h declares
 SIGNATURES = {
     "ce_abi_version": (c_int, []),
@@ -142,6 +161,12 @@ SIGNATURES = {
                                         c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     "ce_rmsnorm_rope_stats_bf16": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                            c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "ce_rms_silu_cl_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
+    "ce_upsample2x_cl_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "ce_im2row_bf16": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int,
+                               c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "ce_conv3d_cl_ex_bf16": (c_int, [POINTER(Conv3dArgsC), c_void_p]),
+    "ce_gemm_attention_bf16": (c_int, [POINTER(GemmAttentionArgsC), c_void_p]),
 }
 
 _lib = None

@@ -130,6 +130,8 @@ int launch_conv3d_cl(const ConvArgs& a, cudaStream_t stream) {
   CE_REQUIRE(a.sw >= 1 && a.sw <= 2 && a.sh >= 1 && a.sh <= 2, "conv: spatial stride 1 or 2");
   CE_REQUIRE(!a.split_time || a.Cout % 16 == 0, "conv: split_time needs Cout % 16 == 0");
   CE_REQUIRE(a.t_base + (a.Tout - 1) * a.st + a.kt <= a.Tin, "conv: temporal extent exceeds the input buffer");
+  CE_REQUIRE(!a.planar_out || (a.planar_t0 >= 0 && a.planar_t0 + a.Tout <= a.planar_T && !a.resid && !a.split_time),
+             "conv: planar output frames must lie inside the video, without resid or split_time");
   ConvGeom g;
   g.tiles_w = (a.Wout + TILE_W - 1) / TILE_W;
   g.tiles_h = (a.Hout + TILE_H - 1) / TILE_H;

@@ -314,4 +314,29 @@ int ce_clip_vision_encode(ce_encoder* h, const void* pixel_values, void* out, in
   return CE_OK;
 }
 
+// Test aid: one gemm_attention as the VAE mid-block, UMT5 or CLIP runs it, on caller-owned buffers.
+int ce_gemm_attention_bf16(const ce_gemm_attention_args* args, void* stream) {
+  CE_TRY(check_device());
+  CE_REQUIRE(args != nullptr, "ce_gemm_attention_bf16: null args");
+  const ce_gemm_attention_args& g = *args;
+  CE_REQUIRE(g.x && g.wqk && g.wv && g.qk && g.vT && g.S && g.P && g.out, "ce_gemm_attention_bf16: null buffer");
+  CE_REQUIRE(g.L > 0 && g.H > 0 && g.D > 0 && g.dk > 0 && g.D % 8 == 0 && g.dk % 8 == 0, "ce_gemm_attention_bf16: L, H > 0; D, dk % 8");
+  CE_REQUIRE(g.kpv >= g.L && g.kpv <= up8(g.L) && g.ldo >= g.H * g.dk, "ce_gemm_attention_bf16: kpv in [L, up8(L)], ldo >= H * dk");
+  CE_REQUIRE(g.rule >= SOFTMAX_SCALED && g.rule <= SOFTMAX_CLIP, "ce_gemm_attention_bf16: rule 0, 1 or 2");
+  if (g.rule == SOFTMAX_T5)
+    CE_REQUIRE(g.bias && g.bias_ld >= 2 * g.L - 1 && g.valid >= 1, "ce_gemm_attention_bf16: T5 needs bias, bias_ld >= 2L - 1, valid >= 1");
+  GemmAttention a;
+  a.x = reinterpret_cast<const bf16*>(g.x);
+  a.wqk = reinterpret_cast<const bf16*>(g.wqk); a.bqk = reinterpret_cast<const bf16*>(g.bqk);
+  a.wv = reinterpret_cast<const bf16*>(g.wv); a.bv = reinterpret_cast<const bf16*>(g.bv);
+  a.L = g.L; a.D = g.D; a.H = g.H; a.dk = g.dk; a.kpv = g.kpv;
+  a.sc.rule = static_cast<SoftmaxRule>(g.rule);
+  a.sc.scale = g.scale;
+  a.sc.bias = reinterpret_cast<const bf16*>(g.bias); a.sc.bias_ld = g.bias_ld; a.sc.Lq = g.L; a.sc.valid = g.valid;
+  a.qk = reinterpret_cast<bf16*>(g.qk); a.vT = reinterpret_cast<bf16*>(g.vT); a.S = g.S; a.P = reinterpret_cast<bf16*>(g.P);
+  a.out = reinterpret_cast<bf16*>(g.out); a.ldo = g.ldo;
+  Launcher run{reinterpret_cast<cudaStream_t>(stream), nullptr};
+  return gemm_attention(run, a);
+}
+
 }  // extern "C"

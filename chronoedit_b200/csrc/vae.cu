@@ -482,15 +482,55 @@ int64_t ce_vae_last_launch_count(const ce_vae* h) { return h ? h->launches : 0; 
 int ce_conv3d_cl_bf16(const void* x, int Tin, int Hin, int Win, int Cin, const void* w, const void* bias, int Cout, int kt, int kh, int kw, int st,
                       int sh, int sw, int ph, int pw, int t_base, void* y, int Tout, int Hout, int Wout, const void* resid, int split_time,
                       void* stream) {
+  ce_conv3d_args a = {};
+  a.x = x; a.Tin = Tin; a.Hin = Hin; a.Win = Win; a.Cin = Cin;
+  a.w = w; a.bias = bias; a.Cout = Cout; a.Cin_pad = round_up(Cin, 64);
+  a.kt = kt; a.kh = kh; a.kw = kw; a.st = st; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw; a.t_base = t_base;
+  a.y = y; a.Tout = Tout; a.Hout = Hout; a.Wout = Wout;
+  a.resid = resid; a.split_time = split_time;
+  return ce_conv3d_cl_ex_bf16(&a, stream);
+}
+
+// Test aids: the VAE's operators one at a time, through the launchers the handle uses (and their argument checks).
+int ce_conv3d_cl_ex_bf16(const ce_conv3d_args* args, void* stream) {
   int rc = check_device();
   if (rc) return rc;
+  CE_REQUIRE(args != nullptr, "ce_conv3d_cl_ex_bf16: null args");
   ConvArgs a;
-  a.x = reinterpret_cast<const bf16*>(x); a.Tin = Tin; a.Hin = Hin; a.Win = Win; a.Cin = Cin;
-  a.w = reinterpret_cast<const bf16*>(w); a.bias = reinterpret_cast<const bf16*>(bias); a.Cout = Cout; a.Cin_pad = round_up(Cin, 64);
-  a.kt = kt; a.kh = kh; a.kw = kw; a.st = st; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw; a.t_base = t_base;
-  a.y = reinterpret_cast<bf16*>(y); a.Tout = Tout; a.Hout = Hout; a.Wout = Wout;
-  a.resid = reinterpret_cast<const bf16*>(resid); a.split_time = split_time;
+  a.x = reinterpret_cast<const bf16*>(args->x); a.Tin = args->Tin; a.Hin = args->Hin; a.Win = args->Win; a.Cin = args->Cin;
+  a.w = reinterpret_cast<const bf16*>(args->w); a.bias = reinterpret_cast<const bf16*>(args->bias);
+  a.Cout = args->Cout; a.Cin_pad = args->Cin_pad;
+  a.kt = args->kt; a.kh = args->kh; a.kw = args->kw; a.st = args->st; a.sh = args->sh; a.sw = args->sw; a.ph = args->ph; a.pw = args->pw;
+  a.t_base = args->t_base;
+  a.y = reinterpret_cast<bf16*>(args->y); a.Tout = args->Tout; a.Hout = args->Hout; a.Wout = args->Wout;
+  a.resid = reinterpret_cast<const bf16*>(args->resid); a.split_time = args->split_time;
+  a.planar_out = args->planar_out; a.clamp = args->clamp; a.planar_T = args->planar_T; a.planar_t0 = args->planar_t0;
   return launch_conv3d_cl(a, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_rms_silu_cl_bf16(const void* x, const void* gamma, void* y, int64_t pixels, int C, int apply_silu, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(x && gamma && y && pixels >= 0, "ce_rms_silu_cl_bf16: null pointer / negative pixel count");
+  return launch_rms_silu_cl(reinterpret_cast<const bf16*>(x), reinterpret_cast<const bf16*>(gamma), reinterpret_cast<bf16*>(y), (size_t)pixels,
+                            C, apply_silu, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_upsample2x_cl_bf16(const void* x, void* y, int T, int H, int W, int C, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(x && y && T >= 0 && H >= 0 && W >= 0, "ce_upsample2x_cl_bf16: null pointer / negative size");
+  return launch_upsample2x_cl(reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(y), T, H, W, C, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_im2row_bf16(const void* x, int64_t sc, int64_t st, int64_t sh, int64_t sw, int Tin, int Hin, int Win, int Cin, void* A, int Kpad, int Tout,
+                   int Hout, int Wout, int kt, int kh, int kw, int ph, int pw, int t_base, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(x && A && sc >= 0 && st >= 0 && sh >= 0 && sw >= 0 && Tout >= 0 && Hout >= 0 && Wout >= 0,
+             "ce_im2row_bf16: null pointer / negative stride or size");
+  return launch_im2row(reinterpret_cast<const bf16*>(x), (size_t)sc, (size_t)st, (size_t)sh, (size_t)sw, Tin, Hin, Win, Cin,
+                       reinterpret_cast<bf16*>(A), Kpad, Tout, Hout, Wout, kt, kh, kw, ph, pw, t_base, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

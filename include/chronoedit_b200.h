@@ -388,6 +388,78 @@ int ce_rmsnorm_rope_stats_bf16(void* x, int ldx, int rows, int D, float eps, con
                                int stats_ld, int tiles, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Test aids: the VAE and encoder operators, one at a time, each with the argument checks of the model's own launches.
+ * Channels-last tensors are [T, H, W, C] bf16.  Not needed to run the model.
+ * ------------------------------------------------------------------------------------------------------------ */
+
+/* RMS_norm (+ SiLU) over the channels of x [pixels, C] -> y (C % 8 == 0, C <= 512), with the reference's bf16 rounding points:
+ * n = bf16(||x||), y = bf16(bf16(bf16(x / max(n, 1e-12)) * sqrt(C)) * gamma[c]), then y = bf16(silu(y)) when apply_silu != 0. */
+int ce_rms_silu_cl_bf16(const void* x, const void* gamma, void* y, int64_t pixels, int C, int apply_silu, void* stream);
+
+/* Nearest 2x spatial upsample: y [T, 2H, 2W, C] from x [T, H, W, C], C % 8 == 0. */
+int ce_upsample2x_cl_bf16(const void* x, void* y, int T, int H, int W, int C, void* stream);
+
+/* im2row of a stride-1 convolution: A [Tout*Hout*Wout, Kpad] (16-byte aligned) with
+ *   A[(to,oh,ow), ((dt*kh + dh)*kw + dw)*Cin + c] = x[c*sc + ti*st + hi*sh + wi*sw],  ti = t_base + to + dt, hi = oh + dh - ph,
+ *   wi = ow + dw - pw,
+ * zero where (ti, hi, wi) lies outside [0,Tin) x [0,Hin) x [0,Win) and in the columns K = kt*kh*kw*Cin .. Kpad-1
+ * (Kpad % 8 == 0, Kpad >= K).  Strides are in elements, so x may be planar [Cin, Tin, Hin, Win] or channels-last. */
+int ce_im2row_bf16(const void* x, int64_t sc, int64_t st, int64_t sh, int64_t sw, int Tin, int Hin, int Win, int Cin, void* A, int Kpad,
+                   int Tout, int Hout, int Wout, int kt, int kh, int kw, int ph, int pw, int t_base, void* stream);
+
+/* The convolution of ce_conv3d_cl_bf16 with every option of the VAE's launches. */
+typedef struct ce_conv3d_args {
+  const void* x;                 /* [Tin, Hin, Win, Cin] */
+  int32_t Tin, Hin, Win, Cin;    /* Cin % 8 == 0 */
+  const void* w;                 /* [Cout, kt*kh*kw, Cin_pad] */
+  const void* bias;              /* [Cout] or NULL */
+  int32_t Cout, Cin_pad;         /* Cin_pad % 64 == 0, Cin_pad >= Cin */
+  int32_t kt, kh, kw;
+  int32_t st, sh, sw;            /* sh, sw in {1, 2} */
+  int32_t ph, pw;
+  int32_t t_base;                /* first input frame of output frame 0 */
+  void* y;                       /* [Tout, Hout, Wout, Cout] (split_time: [2*Tout, Hout, Wout, Cout/2]; planar_out: see below) */
+  int32_t Tout, Hout, Wout;
+  const void* resid;             /* optional, same layout as y: y = bf16(bf16(conv) + resid) */
+  int32_t split_time;            /* 1: channel n goes to frame 2*to + n / (Cout/2), channel n % (Cout/2); Cout % 16 == 0 */
+  int32_t planar_out;            /* 1: y is planar [Cout, planar_T, Hout, Wout] and output frame to is stored at planar_t0 + to, */
+  int32_t clamp;                 /*    clamped to [-1, 1] when clamp != 0 (the decoder head); no resid or split_time with it */
+  int32_t planar_T, planar_t0;
+} ce_conv3d_args;
+int ce_conv3d_cl_ex_bf16(const ce_conv3d_args* args, void* stream);
+
+/* Multi-head self-attention composed of GEMMs over one sequence of L tokens, as the VAE mid-block (H = 1, dk = D) and both
+ * encoders run it; I = H * dk, L8 = L rounded up to 8.
+ *   q | k = x Wqk^T + bqk -> qk [L, 2I];  V^T = Wv x^T + bv -> vT [I, L8];  S_h = q_h k_h^T (fp32) -> S [H, L, L8];
+ *   P = bf16(softmax over keys j < L of the rule's score) -> P [H, L, L8], zero in columns L .. L8-1;
+ *   out[:, h*dk : (h+1)*dk] = bf16(P_h[:, 0:kpv] V_h) -> out [L, ldo].
+ * Score of key j in query row i of head h:
+ *   rule 0 (VAE):  S * scale;  rule 2 (CLIP):  bf16(bf16(S) * scale);
+ *   rule 1 (UMT5): bf16(bf16(S) + bias[h * bias_ld + (j - i) + L - 1]) over the keys j < valid only (1 <= valid; bias_ld >= 2L - 1).
+ * The caller owns every buffer: x with L8 readable rows of D (rows L .. L8-1 only reach columns of V^T that P.V does not sum
+ * over, or multiply zeros of P), qk [L8, 2I] (rows L .. L8-1 are read, never written), vT [I, L8], S [H, L, L8] fp32,
+ * P [H, L, L8], out [L, ldo].  kpv in [L, L8]: the keys P.V sums over (L8 only when V^T is finite there). */
+typedef struct ce_gemm_attention_args {
+  const void* x;                 /* [L8, D] */
+  int32_t D, L, H, dk, kpv;      /* D, dk % 8 == 0 */
+  const void* wqk;               /* [2I, D] = rows of Wq | Wk */
+  const void* bqk;               /* [2I] or NULL */
+  const void* wv;                /* [I, D] */
+  const void* bv;                /* [I] or NULL */
+  int32_t rule;                  /* 0 scaled (VAE), 1 T5 (UMT5), 2 CLIP */
+  float scale;
+  const void* bias;              /* rule 1: [H, bias_ld] bf16 */
+  int32_t bias_ld, valid;
+  void* qk;
+  void* vT;
+  float* S;
+  void* P;
+  void* out;
+  int32_t ldo;                   /* % 8 == 0, >= I */
+} ce_gemm_attention_args;
+int ce_gemm_attention_bf16(const ce_gemm_attention_args* args, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Sampling glue either side of the DiT call (SURVEY.md section 8(f) row 1): one launch per denoising step for
  *   noise = uncond + g*(cond - uncond)                                   chronoedit_diffusers/pipeline_chronoedit.py:736
  *   FlowUniPCMultistepScheduler.step: x0 conversion, UniC corrector, UniP predictor (solver_order 2, bh2, predict_x0,

@@ -59,6 +59,20 @@ def test_no_cpu_fallback():
                                        None) == -3 and b"no CPU fallback" in lib.ce_last_error()
     assert lib.ce_rmsnorm_rope_stats_bf16(L.ptr(a), 8, 8, 8, 1e-6, L.ptr(a), None, 1, None, None, 0, 8, L.ptr(st), 1, 1,
                                           None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    # the VAE and encoder operators: the device check comes first, valid arguments or not
+    assert lib.ce_rms_silu_cl_bf16(L.ptr(a), L.ptr(a), L.ptr(a), 8, 8, 1, None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    assert lib.ce_upsample2x_cl_bf16(L.ptr(a), L.ptr(a), 1, 1, 1, 8, None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    assert lib.ce_im2row_bf16(L.ptr(a), 1, 1, 1, 1, 1, 1, 1, 1, L.ptr(a), 8, 1, 1, 1, 1, 1, 1, 0, 0, 0,
+                              None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    ca = L.Conv3dArgsC(x=a.data_ptr(), Tin=1, Hin=1, Win=1, Cin=8, w=a.data_ptr(), Cout=8, Cin_pad=64, kt=1, kh=1, kw=1, st=1, sh=1, sw=1,
+                       y=a.data_ptr(), Tout=1, Hout=1, Wout=1, planar_out=1, clamp=1, planar_T=1)
+    assert lib.ce_conv3d_cl_ex_bf16(ctypes.byref(ca), None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    assert lib.ce_conv3d_cl_ex_bf16(None, None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    ga = L.GemmAttentionArgsC(x=a.data_ptr(), D=8, L=8, H=1, dk=8, kpv=8, wqk=a.data_ptr(), wv=a.data_ptr(), rule=1, scale=1.0,
+                              bias=a.data_ptr(), bias_ld=15, valid=0, qk=a.data_ptr(), vT=a.data_ptr(), S=st.data_ptr(), P=a.data_ptr(),
+                              out=a.data_ptr(), ldo=8)
+    assert lib.ce_gemm_attention_bf16(ctypes.byref(ga), None) == -3 and b"no CPU fallback" in lib.ce_last_error()
+    assert lib.ce_gemm_attention_bf16(None, None) == -3 and b"no CPU fallback" in lib.ce_last_error()
     # the sampler entry point: argument validation first, then the device check -- never a CPU evaluation
     args = L.UniPCStepArgsC()
     x = torch.zeros(64)
