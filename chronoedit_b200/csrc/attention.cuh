@@ -35,7 +35,7 @@ struct AttnArgs {
 
 int launch_attention(const AttnArgs& a, cudaStream_t stream);
 
-// The FP8 self-attention (attention_fp8.cu, DESIGN.md "FP8 attention"): Lq = Lk = L, head_dim 128, quantized operands.
+// The FP8 self-attention (attention.cu, DESIGN.md "FP8 attention"): Lq = Lk = L, head_dim 128, quantized operands.
 struct AttnFp8Args {
   int B = 0, H = 0, L = 0;
   const uint8_t* q = nullptr;   // e4m3 q[b, i, h*128 + d] at q + (b*L + i)*ldqk + h*128 + d
