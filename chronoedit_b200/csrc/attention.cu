@@ -10,8 +10,17 @@
 //   warpgroups 1,2  one 64-query half of the tile each, everything in registers:
 //                   S_j = Q K_j^T (wgmma, both operands from shared memory), online softmax (fp32: running max, exp2, row sum),
 //                   O += P_j V_j (wgmma, P_j straight from the S accumulator registers as the A operand)
-// The two warpgroups run independently, so the softmax of one overlaps the MMAs of the other on the tensor cores.
 // A tile row is 128 bytes (one swizzled box) in e4m3 and two in bf16; the rings hold 64 KB each, 2 bf16 or 4 e4m3 tiles deep.
+//
+// Two schedules of the consumer loop (attention_tiles<T, PIPE>), with bit-identical results:
+//   serial     (FP8, and bf16 as a reference: ce_debug_attention_kernel(1))  per key tile S_j, wait; softmax_j; P_j V_j, wait.
+//              Registers 40 / 232 per thread (producer / consumers).
+//   pipelined  (bf16, the default)  per key tile j >= 1: issue S_j, then P_{j-1} V_{j-1} (two commit groups, in that order),
+//              wait_group 1 for S_j, softmax_j while P_{j-1} V_{j-1} runs, wait_group 0, o *= alpha_j; a prologue (S_0 and
+//              its softmax) and a drain (the last P V) per key/value source.  o still sees ..., * alpha_j, + P_j V_j, and l and
+//              every P are computed as in the serial loop.  P alternates between two register fragments.  The two warpgroups
+//              take turns at issuing (named barriers 1 and 2), so that one's MMAs run while the other is in its softmax.
+//              Registers 24 / 240 (o, S_j and two P fragments: 160 of them).
 //
 // Where the two operand types differ:
 //   bf16  V_j is [keys, channels] (MN-major B).  o is rescaled by alpha before P V and accumulates in place; the row sum is
@@ -56,6 +65,15 @@ struct SmemLayout {
   static constexpr uint32_t total = bars + 256;
 };
 
+// mbar_wait with its timed loop out of line, for the pipelined consumers, which keep most of their setmaxnreg budget live
+// across the wait: ptxas caps the registers of code that can reach an inlined trap well below that budget (the loop spilled
+// 200 bytes and had its wgmmas serialised).  The call costs nothing on the fast path.  Not for waits between
+// wgmma.mma_async and its wait_group: a call there serialises the wgmmas (C7510).
+__device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity) { mbar_wait(bar, parity); }
+__device__ __forceinline__ void mbar_wait_outlined(uint64_t* bar, uint32_t parity) {
+  if (!mbar_try_wait(bar, parity)) mbar_wait_slow(bar, parity);
+}
+
 // 2^x on the FMA pipe, for the share of the exponentials that would otherwise queue on MUFU: x = n + f with n = rint(x) by the
 // 1.5 * 2^23 trick and |f| <= 1/2, 2^f by its degree-3 Taylor polynomial (relative error < 8e-4 in fp32, far below e4m3's 2^-4), n
 // added to the exponent field.  x is clamped to -126 so that the result stays a normal number (it rounds to e4m3 0 there); -inf
@@ -83,11 +101,14 @@ __device__ __forceinline__ void tma_load_tile(uint8_t* dst, const CUtensorMap* m
 }
 
 // The kernel body for operands of type T: bf16 (Args = AttnArgs) or e4m3 (Args = AttnFp8Args, one key/value source: k2 / v2
-// are not read).
-template <class T, class Args>
+// are not read).  PIPE selects the consumers' schedule: false, one serial chain per key tile (S_j, softmax_j, P_j V_j); true
+// (bf16 only), S_j and P_{j-1} V_{j-1} issued together and softmax_j run while P_{j-1} V_{j-1} executes.  Both apply the same
+// operations in the same order to o, l and every P, so their outputs are bit-identical.
+template <class T, bool PIPE, class Args>
 __device__ __forceinline__ void attention_tiles(const CUtensorMap* tma_q, const CUtensorMap* tma_k, const CUtensorMap* tma_v,
                                                 const CUtensorMap* tma_k2, const CUtensorMap* tma_v2, const Args& a) {
   constexpr bool FP8 = sizeof(T) == 1;
+  static_assert(!(FP8 && PIPE), "the FP8 kernel keeps the serial schedule: its ot / lt accumulators leave no room for a second S");
   using Smem = SmemLayout<T>;
   constexpr uint32_t TILE_BYTES = Smem::TILE_BYTES;
   constexpr int NS = Smem::NS;
@@ -141,7 +162,7 @@ __device__ __forceinline__ void attention_tiles(const CUtensorMap* tma_q, const 
 
   if (warp < 4) {
     // ---------------------------------------------------------------- producers
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<PIPE ? 24 : 40>();
     if (warp == 0 && elect_one_sync()) {
       mbar_arrive_expect_tx(&bars[Q_FULL], TILE_BYTES);
       tma_load_tile<T>(smem + Smem::q, tma_q, &bars[Q_FULL], h * HD, q0, b);
@@ -178,7 +199,7 @@ __device__ __forceinline__ void attention_tiles(const CUtensorMap* tma_q, const 
   }
 
   // ------------------------------------------------------------------ consumers: 64 query rows per warpgroup
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<PIPE ? 240 : 232>();
   const int wg = (warp >> 2) - 1;
   const bool signaller = (threadIdx.x & 127) == 0;
   const int quad = lane & 3;
@@ -193,10 +214,115 @@ __device__ __forceinline__ void attention_tiles(const CUtensorMap* tma_q, const 
       rf[hh] = (row < a.L ? a.q_scale[((size_t)b * a.L + row) * a.lds + h] : 1.f) * sl2;   // rows >= L are zeros, not stored
     }
   }
+  // ---- S = Q K^T of the key tile in stage s: KSTEPS 32-byte steps over head_dim (two 64-wide swizzled boxes in bf16, one in
+  // e4m3).  Issued and committed as one group; the caller fences and waits.
+  auto issue_s = [&](float (&sc)[64], int s) {
+    const uint32_t k_smem = smem_u32(smem + Smem::k) + s * TILE_BYTES;
+#pragma unroll
+    for (int kk = 0; kk < KSTEPS; ++kk) {
+      const uint32_t off = (kk >> 2) * BOX_BYTES + (kk & 3) * 32;
+      const uint64_t da = wgmma_desc_kmajor_sw128(q_smem + off), db = wgmma_desc_kmajor_sw128(k_smem + off);
+      if constexpr (FP8) wgmma_ss_e4m3<128>(sc, da, db, kk != 0);
+      else wgmma_ss<128, 0>(sc, da, db, kk != 0);
+    }
+    wgmma_commit();
+  };
+  // ---- P V of the value tile in stage s: KSTEPS steps over the keys; the A fragment of step kk is p[4kk .. 4kk + 3].
+  // bf16: acc = o, O += P V.  FP8: fresh accumulators acc = P^ V^ and lt = P^ 1 (lt[2hh] = lt[2hh + 1], every column of the
+  // ones tile, is the row sum of row r0 + 8hh).  One committed group.
+  auto issue_pv = [&](float (&acc)[64], float (&lt)[4], const uint32_t (&p)[4 * KSTEPS], int s) {
+    const uint32_t v_smem = smem_u32(smem + Smem::v) + s * TILE_BYTES;
+#pragma unroll
+    for (int kk = 0; kk < KSTEPS; ++kk) {
+      const uint32_t frag[4] = {p[4 * kk], p[4 * kk + 1], p[4 * kk + 2], p[4 * kk + 3]};
+      if constexpr (FP8) {
+        const uint32_t ones = smem_u32(smem + Smem::ones) + kk * 32;
+        if (kk == 0) {
+          wgmma_rs_e4m3_overwrite<128>(acc, frag, wgmma_desc_kmajor_sw128(v_smem));
+          wgmma_rs_e4m3_overwrite<8>(lt, frag, wgmma_desc_kmajor_sw128(ones));
+        } else {
+          wgmma_rs_e4m3<128>(acc, frag, wgmma_desc_kmajor_sw128(v_smem + kk * 32), 1);
+          wgmma_rs_e4m3<8>(lt, frag, wgmma_desc_kmajor_sw128(ones), 1);
+        }
+      } else {
+        wgmma_rs<128, 1>(acc, frag, wgmma_desc_mnmajor_sw128(v_smem + kk * 2048, BOX_BYTES), 1);
+      }
+    }
+    wgmma_commit();
+  };
+  auto release_k = [&](int s) {
+    if constexpr (FP8) {   // per warp: each has read its key scales from the stage
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars[K_EMPTY + s]);
+    } else if (signaller) {
+      mbar_arrive(&bars[K_EMPTY + s]);
+    }
+  };
+  auto release_v = [&](int s) {
+    if (signaller) mbar_arrive(&bars[V_EMPTY + s]);
+  };
+  // ---- online softmax on the accumulator registers of tile j (`valid` = keys left in the source, >= 1; >= 128: no masking):
+  // sc[4 * c + e + 2 * hh] is row r0 + 8 * hh, key 8 * c + 2 * quad + e.  Updates m (and l in bf16) and gives alpha, the
+  // factor of everything accumulated before this tile, and P as the A fragment of P V, for row r0 + 8hh:
+  //   bf16  p[2c + hh] = keys 8c + 2quad + {0, 1} (two bf16)
+  //   e4m3  p[2j + hh] = keys 8c + 2quad + {0, 1} for c = 2j, 2j + 1 (four e4m3)
+  auto softmax = [&](float (&sc)[64], int valid, float (&m)[2], float (&l)[2], uint32_t (&p)[4 * KSTEPS], float (&alpha)[2]) {
+    if (valid < BKV) {  // last key tile only (warp-uniform): masked scores -> -inf -> p = 0
+#pragma unroll
+      for (int i = 0; i < 64; ++i)
+        if (8 * (i >> 2) + 2 * quad + (i & 1) >= valid) sc[i] = -INFINITY;
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int c = 0; c < 16; ++c) mx = fmaxf(mx, fmaxf(sc[4 * c + 2 * hh], sc[4 * c + 2 * hh + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m[hh], mx * rf[hh]);   // finite: every tile has at least one valid key
+      alpha[hh] = fast_exp2(m[hh] - m_new);             // 0 on the first tile (m = -inf)
+      m[hh] = m_new;
+      if constexpr (FP8) {
+        const float mb = 8.f - m_new;   // 256 exp2(x - m) = exp2(x - m + 8)
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int c = 2 * jj;
+          // keys 8c + 2quad + e with c % 4 == 3 (a quarter) take exp2 on the FMA pipe, the rest on MUFU
+          const uint32_t lo = exp2_e4m3x2<false>(fmaf(sc[4 * c + 2 * hh], rf[hh], mb), fmaf(sc[4 * c + 2 * hh + 1], rf[hh], mb));
+          const float b0 = fmaf(sc[4 * c + 4 + 2 * hh], rf[hh], mb), b1 = fmaf(sc[4 * c + 4 + 2 * hh + 1], rf[hh], mb);
+          const uint32_t hi = (jj & 1) ? exp2_e4m3x2<true>(b0, b1) : exp2_e4m3x2<false>(b0, b1);
+          p[2 * jj + hh] = lo | (hi << 16);
+        }
+      } else {
+        float sum = 0.f;
+#pragma unroll
+        for (int c = 0; c < 16; ++c) {
+          const float p0 = fast_exp2(fmaf(sc[4 * c + 2 * hh], rf[hh], -m_new));
+          const float p1 = fast_exp2(fmaf(sc[4 * c + 2 * hh + 1], rf[hh], -m_new));
+          sum += p0 + p1;
+          p[2 * c + hh] = pack_bf16x2(p0, p1);
+        }
+        l[hh] = l[hh] * alpha[hh] + sum;
+      }
+    }
+  };
+  auto rescale = [&](float (&o)[64], const float (&alpha)[2]) {   // bf16: o *= alpha, before P_j V_j is added
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+      o[4 * c] *= alpha[0];
+      o[4 * c + 1] *= alpha[0];
+      o[4 * c + 2] *= alpha[1];
+      o[4 * c + 3] *= alpha[1];
+    }
+  };
+
   long long* timing = nullptr;   // phase hooks of the bf16 kernel (ce_debug_attention_timing); compiled out of FP8
   if constexpr (!FP8) timing = a.timing;
   const bool timed = timing != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 128;
-  long long tacc[3] = {0, 0, 0};   // cycles in S = Q K^T (incl. the wait for K), softmax, P V (incl. the wait for V)
+  // cycles of the three phases; serial schedule: S = Q K^T (incl. the wait for K), softmax, P V (incl. the wait for V);
+  // pipelined: up to S_j's result (waits for K_j / V_{j-1} and the turn, issue of S_j and P_{j-1} V_{j-1}, wait for S_j),
+  // softmax_j, wait for P_{j-1} V_{j-1} plus the rescale
+  long long tacc[3] = {0, 0, 0};
   long long tc0 = timed ? clock64() : 0;
 #define CE_TICK(slot)               \
   if (timed) {                      \
@@ -205,9 +331,33 @@ __device__ __forceinline__ void attention_tiles(const CUtensorMap* tma_q, const 
     tc0 = _t;                       \
   }
 
-  mbar_wait(&bars[Q_FULL], 0);
+  // Ping-pong (pipelined schedule): the two consumer warpgroups take turns at issuing their MMAs, so that the tensor cores run
+  // one warpgroup's S and P V while the other one is in its softmax.  Named barrier 1 + w is warpgroup w's turn: it syncs there
+  // before each issue point and hands the turn over (arrive at the other's barrier) after it.  Warpgroup 1 gives warpgroup 0
+  // the first turn and does not hand over after its last issue point, so every barrier sees as many arrivals as syncs: both
+  // walk T0 + T1 tiles and one drain per source, whatever Lq, Lk and Lk2 are.
+  const int n_src = T1 > 0 ? 2 : 1;
+  auto await_turn = [&]() {
+    if constexpr (PIPE) named_bar_sync(1 + wg, 256);
+  };
+  auto pass_turn = [&](bool last) {
+    if constexpr (PIPE) {
+      if (!(last && wg == 1)) named_bar_arrive(2 - wg, 256);
+    }
+  };
+  if constexpr (PIPE) {
+    if (wg == 1) named_bar_arrive(1, 256);
+  }
+
+  // The pipelined loop holds o, S_j and two P fragments across its waits: their timed slow path goes out of line
+  // (mbar_wait_outlined).
+  auto wait_full = [&](int bar, uint32_t parity) {
+    if constexpr (PIPE) mbar_wait_outlined(&bars[bar], parity);
+    else mbar_wait(&bars[bar], parity);
+  };
+  wait_full(Q_FULL, 0);
   uint32_t t = 0;   // position in the ring, over both sources
-  for (int src = 0; src < (T1 > 0 ? 2 : 1); ++src) {
+  for (int src = 0; src < n_src; ++src) {
     const int my_tiles = src ? T1 : T0;
     const int my_len = src ? Lk2 : Lk;
     float o[64];
@@ -216,24 +366,87 @@ __device__ __forceinline__ void attention_tiles(const CUtensorMap* tma_q, const 
     // per row: running max, row sum (bf16: this lane's share of it; FP8: the whole row's, from the tensor cores)
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 
-    for (int j = 0; j < my_tiles; ++j, ++t) {
-      const int s = t % NS;
-      const uint32_t parity = (t / NS) & 1;
-      const int valid = my_len - j * BKV;  // >= 1; >= 128 means no masking
-      // ---- S = Q K^T: KSTEPS 32-byte steps over head_dim (two 64-wide swizzled boxes in bf16, one in e4m3)
-      float sc[64];
-      mbar_wait(&bars[K_FULL + s], parity);
-      {
-        const uint32_t k_smem = smem_u32(smem + Smem::k) + s * TILE_BYTES;
+    if constexpr (PIPE) {
+      // ---- pipelined: prologue S_0 -> softmax_0; per tile j >= 1: issue S_j and P_{j-1} V_{j-1}, softmax_j while
+      // P_{j-1} V_{j-1} runs, then o *= alpha_j; drain P_{last} V_{last}.  o sees ..., * alpha_j, + P_j V_j as in the serial
+      // schedule.  P alternates between two fragments, so that softmax_j never writes the registers P V reads in flight.
+      float sc[64], alpha[2], lt_unused[4];
+      uint32_t pa[4 * KSTEPS], pb[4 * KSTEPS];
+      int s = t % NS;
+      wait_full(K_FULL + s, (t / NS) & 1);
+      await_turn();
+      wgmma_fence();
+      issue_s(sc, s);
+      pass_turn(false);
+      wgmma_wait<0>();
+      wgmma_fence_operand(sc);
+      release_k(s);
+      CE_TICK(0)
+      softmax(sc, my_len, m, l, pa, alpha);
+      rescale(o, alpha);
+      CE_TICK(1)
+      // tile j: P_{j-1} V_{j-1} from pv, softmax_j into pn
+      auto step = [&](uint32_t (&pv)[4 * KSTEPS], uint32_t (&pn)[4 * KSTEPS], int j) {
+        const int sn = (t + 1) % NS;
+        wait_full(K_FULL + sn, ((t + 1) / NS) & 1);
+        wait_full(V_FULL + s, (t / NS) & 1);
+        await_turn();
+        wgmma_fence_operand(o);   // o *= alpha and P_{j-1} complete before the issue, not sunk between the wgmmas
+        wgmma_fence_operand(pv);
         wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < KSTEPS; ++kk) {
-          const uint32_t off = (kk >> 2) * BOX_BYTES + (kk & 3) * 32;
-          const uint64_t da = wgmma_desc_kmajor_sw128(q_smem + off), db = wgmma_desc_kmajor_sw128(k_smem + off);
-          if constexpr (FP8) wgmma_ss_e4m3<128>(sc, da, db, kk != 0);
-          else wgmma_ss<128, 0>(sc, da, db, kk != 0);
-        }
-        wgmma_commit();
+        issue_s(sc, sn);   // committed first: wait_group 1 below retires it and leaves P V in flight
+        issue_pv(o, lt_unused, pv, s);
+        pass_turn(false);
+        wgmma_wait<1>();
+        wgmma_fence_operand(sc);
+        release_k(sn);
+        CE_TICK(0)
+        softmax(sc, my_len - j * BKV, m, l, pn, alpha);
+        CE_TICK(1)
+        wgmma_wait<0>();
+        wgmma_fence_operand(o);   // pv stays allocated up to here; rescale after the P V is done
+        wgmma_fence_operand(pv);
+        release_v(s);
+        rescale(o, alpha);
+        CE_TICK(2)
+        ++t;
+        s = sn;
+      };
+      auto drain = [&](uint32_t (&pv)[4 * KSTEPS]) {
+        wait_full(V_FULL + s, (t / NS) & 1);
+        await_turn();
+        wgmma_fence_operand(o);
+        wgmma_fence_operand(pv);
+        wgmma_fence();
+        issue_pv(o, lt_unused, pv, s);
+        pass_turn(src == n_src - 1);
+        wgmma_wait<0>();
+        wgmma_fence_operand(o);
+        wgmma_fence_operand(pv);
+        release_v(s);
+        CE_TICK(2)
+        ++t;
+      };
+      int j = 1;
+      for (; j + 1 < my_tiles; j += 2) {
+        step(pa, pb, j);
+        step(pb, pa, j + 1);
+      }
+      if (j < my_tiles) {
+        step(pa, pb, j);
+        drain(pb);
+      } else {
+        drain(pa);
+      }
+    } else {
+      for (int j = 0; j < my_tiles; ++j, ++t) {
+        const int s = t % NS;
+        const uint32_t parity = (t / NS) & 1;
+        const int valid = my_len - j * BKV;  // >= 1; >= 128 means no masking
+        float sc[64];
+        mbar_wait(&bars[K_FULL + s], parity);
+        wgmma_fence();
+        issue_s(sc, s);
         wgmma_wait<0>();
         if constexpr (FP8) {   // sc[4c + e + 2hh] is row r0 + 8hh, key 8c + 2quad + e: times the key's scale
           const float* kss = kscale + s * BKV;
@@ -246,104 +459,32 @@ __device__ __forceinline__ void attention_tiles(const CUtensorMap* tma_q, const 
             sc[4 * c + 3] *= ks.y;
           }
         }
-        if constexpr (FP8) {   // per warp: each has read its key scales from the stage
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bars[K_EMPTY + s]);
-        } else if (signaller) {
-          mbar_arrive(&bars[K_EMPTY + s]);
-        }
-      }
-      CE_TICK(0)
-      // ---- online softmax on the accumulator registers: sc[4 * c + e + 2 * hh] is row r0 + 8 * hh, key 8 * c + 2 * quad + e
-      if (valid < BKV) {  // last key tile only (warp-uniform): masked scores -> -inf -> p = 0
-#pragma unroll
-        for (int i = 0; i < 64; ++i)
-          if (8 * (i >> 2) + 2 * quad + (i & 1) >= valid) sc[i] = -INFINITY;
-      }
-      // P as the A fragment of P V, for row r0 + 8hh:
-      //   bf16  p[2c + hh] = keys 8c + 2quad + {0, 1} (two bf16)
-      //   e4m3  p[2j + hh] = keys 8c + 2quad + {0, 1} for c = 2j, 2j + 1 (four e4m3)
-      uint32_t p[4 * KSTEPS];
-      float alpha[2];
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        float mx = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < 16; ++c) mx = fmaxf(mx, fmaxf(sc[4 * c + 2 * hh], sc[4 * c + 2 * hh + 1]));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-        const float m_new = fmaxf(m[hh], mx * rf[hh]);   // finite: every tile has at least one valid key
-        alpha[hh] = fast_exp2(m[hh] - m_new);             // 0 on the first tile (m = -inf)
-        m[hh] = m_new;
-        if constexpr (FP8) {
-          const float mb = 8.f - m_new;   // 256 exp2(x - m) = exp2(x - m + 8)
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const int c = 2 * jj;
-            // keys 8c + 2quad + e with c % 4 == 3 (a quarter) take exp2 on the FMA pipe, the rest on MUFU
-            const uint32_t lo = exp2_e4m3x2<false>(fmaf(sc[4 * c + 2 * hh], rf[hh], mb), fmaf(sc[4 * c + 2 * hh + 1], rf[hh], mb));
-            const float b0 = fmaf(sc[4 * c + 4 + 2 * hh], rf[hh], mb), b1 = fmaf(sc[4 * c + 4 + 2 * hh + 1], rf[hh], mb);
-            const uint32_t hi = (jj & 1) ? exp2_e4m3x2<true>(b0, b1) : exp2_e4m3x2<false>(b0, b1);
-            p[2 * jj + hh] = lo | (hi << 16);
-          }
-        } else {
-          float sum = 0.f;
-#pragma unroll
-          for (int c = 0; c < 16; ++c) {
-            const float p0 = fast_exp2(fmaf(sc[4 * c + 2 * hh], rf[hh], -m_new));
-            const float p1 = fast_exp2(fmaf(sc[4 * c + 2 * hh + 1], rf[hh], -m_new));
-            sum += p0 + p1;
-            p[2 * c + hh] = pack_bf16x2(p0, p1);
-          }
-          l[hh] = l[hh] * alpha[hh] + sum;
-#pragma unroll
-          for (int c = 0; c < 16; ++c) {
-            o[4 * c + 2 * hh] *= alpha[hh];
-            o[4 * c + 2 * hh + 1] *= alpha[hh];
-          }
-        }
-      }
-      CE_TICK(1)
-      // ---- P V: KSTEPS steps over the keys; the A fragment of step kk is p[4kk .. 4kk + 3].
-      // bf16: O += P V.  FP8: fresh accumulators ot = P^ V^ and lt = P^ 1 (lt[2hh] = lt[2hh + 1], every column of the ones tile,
-      // is the row sum of row r0 + 8hh).
-      float ot[64], lt[4];
-      mbar_wait(&bars[V_FULL + s], parity);
-      {
-        const uint32_t v_smem = smem_u32(smem + Smem::v) + s * TILE_BYTES;
+        release_k(s);
+        CE_TICK(0)
+        uint32_t p[4 * KSTEPS];
+        float alpha[2];
+        softmax(sc, valid, m, l, p, alpha);
+        if constexpr (!FP8) rescale(o, alpha);
+        CE_TICK(1)
+        float ot[64], lt[4];
+        mbar_wait(&bars[V_FULL + s], parity);
         wgmma_fence();
+        issue_pv(FP8 ? ot : o, lt, p, s);
+        wgmma_wait<0>();
+        release_v(s);
+        if constexpr (FP8) {
+          l[0] = fmaf(l[0], alpha[0], lt[0]);
+          l[1] = fmaf(l[1], alpha[1], lt[2]);
 #pragma unroll
-        for (int kk = 0; kk < KSTEPS; ++kk) {
-          const uint32_t frag[4] = {p[4 * kk], p[4 * kk + 1], p[4 * kk + 2], p[4 * kk + 3]};
-          if constexpr (FP8) {
-            const uint32_t ones = smem_u32(smem + Smem::ones) + kk * 32;
-            if (kk == 0) {
-              wgmma_rs_e4m3_overwrite<128>(ot, frag, wgmma_desc_kmajor_sw128(v_smem));
-              wgmma_rs_e4m3_overwrite<8>(lt, frag, wgmma_desc_kmajor_sw128(ones));
-            } else {
-              wgmma_rs_e4m3<128>(ot, frag, wgmma_desc_kmajor_sw128(v_smem + kk * 32), 1);
-              wgmma_rs_e4m3<8>(lt, frag, wgmma_desc_kmajor_sw128(ones), 1);
-            }
-          } else {
-            wgmma_rs<128, 1>(o, frag, wgmma_desc_mnmajor_sw128(v_smem + kk * 2048, BOX_BYTES), 1);
+          for (int c = 0; c < 16; ++c) {
+            o[4 * c] = fmaf(o[4 * c], alpha[0], ot[4 * c]);
+            o[4 * c + 1] = fmaf(o[4 * c + 1], alpha[0], ot[4 * c + 1]);
+            o[4 * c + 2] = fmaf(o[4 * c + 2], alpha[1], ot[4 * c + 2]);
+            o[4 * c + 3] = fmaf(o[4 * c + 3], alpha[1], ot[4 * c + 3]);
           }
         }
-        wgmma_commit();
-        wgmma_wait<0>();
-        if (signaller) mbar_arrive(&bars[V_EMPTY + s]);
+        CE_TICK(2)
       }
-      if constexpr (FP8) {
-        l[0] = fmaf(l[0], alpha[0], lt[0]);
-        l[1] = fmaf(l[1], alpha[1], lt[2]);
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          o[4 * c] = fmaf(o[4 * c], alpha[0], ot[4 * c]);
-          o[4 * c + 1] = fmaf(o[4 * c + 1], alpha[0], ot[4 * c + 1]);
-          o[4 * c + 2] = fmaf(o[4 * c + 2], alpha[1], ot[4 * c + 2]);
-          o[4 * c + 3] = fmaf(o[4 * c + 3], alpha[1], ot[4 * c + 3]);
-        }
-      }
-      CE_TICK(2)
     }
 
     // ---- normalise and store this source's result: bf16(o / l), FP8 bf16(o s_v / l)
@@ -389,17 +530,20 @@ __device__ __forceinline__ void attention_tiles(const CUtensorMap* tma_q, const 
 #undef CE_TICK
 }
 
+// PIPE: the pipelined schedule (the default); !PIPE: the serial one, kept as the reference the pipelined one is tested against
+// (ce_debug_attention_kernel(1)).
+template <bool PIPE>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
                      const __grid_constant__ CUtensorMap tma_v, const __grid_constant__ CUtensorMap tma_k2,
                      const __grid_constant__ CUtensorMap tma_v2, AttnArgs a) {
-  attention_tiles<bf16>(&tma_q, &tma_k, &tma_v, &tma_k2, &tma_v2, a);
+  attention_tiles<bf16, PIPE>(&tma_q, &tma_k, &tma_v, &tma_k2, &tma_v2, a);
 }
 
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attention_fp8_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
                      const __grid_constant__ CUtensorMap tma_vt, AttnFp8Args a) {
-  attention_tiles<__nv_fp8_e4m3>(&tma_q, &tma_k, &tma_vt, &tma_k, &tma_vt, a);
+  attention_tiles<__nv_fp8_e4m3, false>(&tma_q, &tma_k, &tma_vt, &tma_k, &tma_vt, a);
 }
 
 // A token-major [B, L, H * 128] operand with row stride ld (elements), in 128-byte boxes of 128 rows (64 bf16 or 128 e4m3 wide).
@@ -423,7 +567,7 @@ int launch_tiles(void (*kernel)(Params...), int B, int H, int Lq, cudaStream_t s
 
 }  // namespace
 
-int launch_attention(const AttnArgs& a, cudaStream_t stream) {
+int launch_attention(const AttnArgs& a, cudaStream_t stream, bool pipelined) {
   CE_REQUIRE(a.B > 0 && a.H > 0 && a.Lq > 0 && a.Lk > 0, "attention: empty problem");
   CE_REQUIRE(a.peer_rows == 0 || (a.Lk2 == 0 && !a.accumulate && (a.Lq + a.peer_rows - 1) / a.peer_rows <= 8),
              "attention: the sequence-parallel output scatter serves the self-attention, with at most 8 peers");
@@ -442,7 +586,8 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
     tk2 = tk;
     tv2 = tv;
   }
-  return launch_tiles<bf16>(attention_fwd_kernel, a.B, a.H, a.Lq, stream, tq, tk, tv, tk2, tv2, a);
+  if (pipelined) return launch_tiles<bf16>(attention_fwd_kernel<true>, a.B, a.H, a.Lq, stream, tq, tk, tv, tk2, tv2, a);
+  return launch_tiles<bf16>(attention_fwd_kernel<false>, a.B, a.H, a.Lq, stream, tq, tk, tv, tk2, tv2, a);
 }
 
 int launch_attention_fp8(const AttnFp8Args& a, cudaStream_t stream) {

@@ -33,7 +33,8 @@ struct AttnArgs {
   int accumulate = 0;       // 1: out = bf16(float(bf16(attn)) + float(out))   (image + text cross-attention sum)
 };
 
-int launch_attention(const AttnArgs& a, cudaStream_t stream);
+// pipelined = false selects the serial schedule of the same kernel body (bit-identical output; a test and measurement aid).
+int launch_attention(const AttnArgs& a, cudaStream_t stream, bool pipelined = true);
 
 // The FP8 self-attention (attention.cu, DESIGN.md "FP8 attention"): Lq = Lk = L, head_dim 128, quantized operands.
 struct AttnFp8Args {

@@ -900,9 +900,13 @@ int ce_debug_attention_timing(long long* buf) {
   return CE_OK;
 }
 
-// Test aid: attention.cu is the only attention kernel of the sm_90a build (version 0, also the default -1).
+// Test and measurement aid: the schedule of the bf16 attention kernel for later ce_attention_bf16 / ce_attention_dual_bf16 calls
+// (process-wide, like the timing hook).  The DiT forward does not read it: it always runs the pipelined schedule.
+static std::atomic<bool> g_attn_serial{false};
 int ce_debug_attention_kernel(int version) {
-  if (version != -1 && version != 0) return ce::fail(ce::CE_ERR_INVALID, "attention kernel version must be -1 or 0");
+  if (version != -1 && version != 0 && version != 1)
+    return ce::fail(ce::CE_ERR_INVALID, "attention kernel version must be -1, 0 (pipelined) or 1 (serial)");
+  g_attn_serial.store(version == 1);
   return CE_OK;
 }
 
@@ -919,7 +923,7 @@ int ce_attention_bf16(const void* q, int ldq, const void* k, int ldk, const void
   a.scale = scale;
   a.accumulate = accumulate;
   a.timing = g_attn_timing.load();
-  return launch_attention(a, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attention(a, reinterpret_cast<cudaStream_t>(stream), !g_attn_serial.load());
 }
 
 int ce_attention_dual_bf16(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, const void* k2, int ldk2, const void* v2,
@@ -935,7 +939,7 @@ int ce_attention_dual_bf16(const void* q, int ldq, const void* k, int ldk, const
   a.v2 = reinterpret_cast<const bf16*>(v2); a.ldv2 = ldv2;
   a.out = reinterpret_cast<bf16*>(out); a.ldo = ldo;
   a.scale = scale;
-  return launch_attention(a, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attention(a, reinterpret_cast<cudaStream_t>(stream), !g_attn_serial.load());
 }
 
 int ce_layernorm_bf16(const void* x, int ldx, void* y, int ldy, int rows, int D, float eps, const float* scale, const float* shift,

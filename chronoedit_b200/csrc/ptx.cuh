@@ -77,6 +77,11 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Counts the calling warp's threads towards barrier `id` without waiting for it (the other half of a producer / consumer pair
+// of named_bar_sync).
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 // Register re-partition between the warpgroups of a CTA (executed by every thread of a warpgroup): the TMA producer warpgroup
 // gives registers up, the MMA warpgroups that hold the accumulators take them.
 template <int REGS>

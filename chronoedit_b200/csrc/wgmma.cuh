@@ -20,6 +20,20 @@ template <int PENDING>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory");
 }
+// Compiler-only fence on registers that an in-flight wgmma reads (A fragment) or writes (accumulator), in the CUTLASS style.
+// The compiler takes an asm statement's outputs as final when it returns, so it may reuse an A fragment's registers, or move
+// arithmetic on an accumulator across wgmma_wait.  An empty volatile asm that reads and writes each register, placed before the
+// issue and after the wait, pins them there: volatile asm statements keep their order.
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operand(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operand(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
+}
 
 // Shared-memory matrix descriptor, 128-byte swizzle: [0,14) address >> 4, [16,30) leading byte offset >> 4,
 // [32,46) stride byte offset >> 4, [62,64) swizzle mode (1 = 128 B).

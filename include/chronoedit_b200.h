@@ -274,11 +274,16 @@ int ce_attention_bf16(const void* q, int ldq, const void* k, int ldk, const void
                       int H, int Lq, int Lk, float scale, int accumulate, void* stream);
 
 /* Profiling aid: subsequent ce_attention_bf16 calls record, for the first consumer thread of block 0, into `buf` (device,
- * 16 x int64): [0] cycles in S = Q K^T, [1] in the softmax, [2] in P V, [3] key tiles walked; NULL stops. */
+ * 16 x int64) the cycles of three phases summed over the key tiles, and [3] the key tiles walked; NULL stops.
+ * Pipelined schedule (the default): [0] up to S_j's result (waits for K_j, V_{j-1} and the issue turn, issue of S_j and
+ * P_{j-1} V_{j-1}, wait for S_j), [1] the softmax of tile j, [2] the wait for P_{j-1} V_{j-1} plus the rescale of o.
+ * Serial schedule (version 1 below): [0] S = Q K^T incl. the wait for K, [1] the softmax, [2] P V incl. the wait for V. */
 int ce_debug_attention_timing(long long* buf);
 
-/* Kept for ABI stability only: earlier builds selected between several attention kernels here.  The sm_90a build has one, so
- * this call selects nothing: it accepts 0 and -1 (both mean that kernel) and rejects every other version. */
+/* Test and measurement aid: the schedule of the bf16 attention kernel for later ce_attention_bf16 / ce_attention_dual_bf16
+ * calls in this process.  0 and -1 (the default): the pipelined schedule, S of key tile j and P V of tile j-1 issued together
+ * and the softmax of tile j run under that P V.  1: the serial schedule (S, softmax, P V per tile) of the same kernel body,
+ * with bit-identical output.  Every other version is rejected.  The DiT forward always runs the pipelined schedule. */
 int ce_debug_attention_kernel(int version);
 
 /* Cross-attention with TWO key/value sources in one launch: out = bf16(SDPA(q,k,v)) + bf16(SDPA(q,k2,v2)) — the text and

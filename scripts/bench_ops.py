@@ -1,6 +1,8 @@
 #!/usr/bin/env python
 """Operator micro-benchmarks at the 14B / 720p shapes (CUDA events, warm-up, L2-busting operand rotation).
-    python scripts/bench_ops.py [attn] [attn8] [gemm [cublas]] [gemmk] [rows] [conv]
+    python scripts/bench_ops.py [attn] [attn8] [attnab] [gemm [cublas]] [gemmk] [rows] [conv]
+`attnab` times the bf16 attention's pipelined schedule (version 0) against its serial one (version 1, ce_debug_attention_kernel)
+in alternating rounds, and prints the median of each, the speed-up and the phase cycles of ce_debug_attention_timing.
 `attn8` times the self-attention in bf16 and as the FP8 attention runs it: the q | k and v quantizers and the e4m3 kernel.
 `gemm` times each block GEMM in bf16 and, in the fp8_* fields, as the FP8 mode runs it (quantization and e4m3 GEMM).
 `gemmk` times the bf16 o-proj GEMM over K and fits the time per wave of tiles to a + b K: `a` is the per-tile cost that does not
@@ -150,6 +152,68 @@ def bench_attn_dual(B=2, H=40, Lq=7200, Lk=512, Lk2=257):
     ms = timeit(fn)
     fl = 4.0 * B * H * Lq * (Lk + Lk2) * 128
     print(json.dumps({"op": "attention_dual", "B": B, "H": H, "Lq": Lq, "Lk": Lk, "Lk2": Lk2, "ms": round(ms, 4), "tflops": round(fl / ms / 1e9, 1)}), flush=True)
+
+
+def bench_attn_ab(B=2, H=40, Lq=7200, Lk=7200, Lk2=0, rounds=12, iters=5):
+    """Version 0 (pipelined) against version 1 (serial) of the bf16 attention on the same buffers: one timing of each per
+    round, alternated, median over the rounds.  Then one launch of each with the phase-timing hook on."""
+    import statistics
+
+    D = H * 128
+    self_attn = Lq == Lk and Lk2 == 0
+    nbuf = 2
+    if self_attn:
+        bufs = [torch.randn(B, Lq, 3 * D, device="cuda", dtype=torch.bfloat16) for _ in range(nbuf)]
+    else:
+        q = torch.randn(B, Lq, D, device="cuda", dtype=torch.bfloat16)
+        kv = torch.randn(B, Lk, 2 * D, device="cuda", dtype=torch.bfloat16)
+        kv2 = torch.randn(B, max(Lk2, 1), 2 * D, device="cuda", dtype=torch.bfloat16)
+    out = torch.empty(B, Lq, D, device="cuda", dtype=torch.bfloat16)
+    i = [0]
+    s = L.current_stream()
+
+    def fn():
+        if self_attn:
+            x = bufs[i[0] % nbuf]
+            i[0] += 1
+            L.check(lib.ce_attention_bf16(L.ptr(x), 3 * D, L.ptr(x[..., D:]), 3 * D, L.ptr(x[..., 2 * D:]), 3 * D, L.ptr(out), D, B, H, Lq, Lk,
+                                          1 / math.sqrt(128), 0, s))
+        elif Lk2:
+            L.check(lib.ce_attention_dual_bf16(L.ptr(q), D, L.ptr(kv), 2 * D, L.ptr(kv[..., D:]), 2 * D, L.ptr(kv2), 2 * D, L.ptr(kv2[..., D:]),
+                                               2 * D, L.ptr(out), D, B, H, Lq, Lk, Lk2, 1 / math.sqrt(128), s))
+        else:
+            L.check(lib.ce_attention_bf16(L.ptr(q), D, L.ptr(kv), 2 * D, L.ptr(kv[..., D:]), 2 * D, L.ptr(out), D, B, H, Lq, Lk,
+                                          1 / math.sqrt(128), 0, s))
+
+    ms = {0: [], 1: []}
+    try:
+        for v in (1, 0):   # warm-up of both
+            L.check(lib.ce_debug_attention_kernel(v))
+            timeit(fn, iters=2, warmup=2)
+        for _ in range(rounds):
+            for v in (1, 0):
+                L.check(lib.ce_debug_attention_kernel(v))
+                ms[v].append(timeit(fn, iters=iters, warmup=1))
+        phases = {}
+        buf = torch.zeros(16, dtype=torch.int64, device="cuda")
+        L.check(lib.ce_debug_attention_timing(L.ptr(buf)))
+        for v in (1, 0):
+            L.check(lib.ce_debug_attention_kernel(v))
+            buf.zero_()
+            fn()
+            torch.cuda.synchronize()
+            phases[v] = buf[:4].tolist()
+    finally:
+        L.check(lib.ce_debug_attention_timing(None))
+        L.check(lib.ce_debug_attention_kernel(-1))
+    fl = 4.0 * B * H * Lq * (Lk + Lk2) * 128
+    m0, m1 = statistics.median(ms[0]), statistics.median(ms[1])
+    print(json.dumps({"op": "attention_ab", "B": B, "H": H, "Lq": Lq, "Lk": Lk, "Lk2": Lk2, "rounds": rounds,
+                      "pipelined_ms": round(m0, 4), "serial_ms": round(m1, 4), "speedup": round(m1 / m0, 4),
+                      "pipelined_range_ms": [round(min(ms[0]), 4), round(max(ms[0]), 4)],
+                      "serial_range_ms": [round(min(ms[1]), 4), round(max(ms[1]), 4)],
+                      "pipelined_tflops": round(fl / m0 / 1e9, 1), "serial_tflops": round(fl / m1 / 1e9, 1),
+                      "phase_cycles_pipelined": phases[0], "phase_cycles_serial": phases[1]}), flush=True)
 
 
 # The six block GEMMs of the DiT at the 14B / 720p step (dit.cu), as dit.cu calls them: in-place residual (out == resid == x),
@@ -309,6 +373,10 @@ if __name__ == "__main__":
     if "attn8" in what:
         bench_attn8()
         bench_attn8(B=2, Lk=28800)
+    if "attnab" in what:
+        bench_attn_ab()
+        bench_attn_ab(B=1, Lq=28800, Lk=28800, rounds=10, iters=2)
+        bench_attn_ab(Lk=512, Lk2=257)
     if "attnself" in what:
         bench_attn()
         bench_attn(B=1, Lq=28800, Lk=28800, nbuf=2)
