@@ -134,6 +134,9 @@ SIGNATURES = {
     "ce_vae_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "ce_vae_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "ce_vae_last_launch_count": (c_int64, [c_void_p]),
+    "ce_vae_sp_region_bytes": (c_int64, [c_void_p, c_int, c_int, c_int]),
+    "ce_vae_sp_configure": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64]),
+    "ce_vae_sp_host_barrier": (c_int, [c_void_p, c_int]),
     "ce_conv3d_cl_bf16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                   c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "ce_linear_bf16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int,

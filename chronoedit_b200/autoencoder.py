@@ -190,6 +190,7 @@ class AutoencoderKLWan(nn.Module):
         self._packed: Dict[str, torch.Tensor] = {}
         self._is_packed = False
         self._ws: Optional[torch.Tensor] = None
+        self._sp_state: Optional[Dict] = None   # the split over ranks (parallel.enable_vae_sequence_parallel)
 
     def _register(self, dotted: str, p: nn.Parameter) -> None:
         mod = self
@@ -219,18 +220,23 @@ class AutoencoderKLWan(nn.Module):
         except Exception:
             pass
 
-    @torch.no_grad()
-    def pack_weights(self) -> None:
-        L = _lib.lib()
-        if self.device.type != "cuda":
-            raise CEError("AutoencoderKLWan must live on a CUDA (sm_90) device; there is no CPU path")
+    def _ensure_handle(self):
+        """The C handle (configuration only; pack_weights hands it the weights)."""
         if self._handle is None:
             c = self.config
             cfg = VAEConfigC(c.base_dim, c.z_dim, (_lib.c_int32 * 4)(*c.dim_mult), c.num_res_blocks,
                              (_lib.c_int32 * 3)(*[int(b) for b in c.temperal_downsample]))
             h = _lib.c_void_p()
-            check(L.ce_vae_create(_lib.ctypes.byref(cfg), _lib.ctypes.byref(h)))
+            check(_lib.lib().ce_vae_create(_lib.ctypes.byref(cfg), _lib.ctypes.byref(h)))
             self._handle = h
+        return self._handle
+
+    @torch.no_grad()
+    def pack_weights(self) -> None:
+        L = _lib.lib()
+        if self.device.type != "cuda":
+            raise CEError("AutoencoderKLWan must live on a CUDA (sm_90) device; there is no CPU path")
+        self._ensure_handle()
         packed = {}
         for name, p in self.named_parameters():
             t = pack_parameter(name, p.data)

@@ -659,7 +659,7 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
       LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, Lfull,
                                                  c.attention_head_dim, partials(ws.stats_qkv, 3 * tD), s, &sc));
       LAUNCH(CAT_OTHER, 0.0, launch_sp_scatter_cols(ws.qkv + 2 * D, 3 * D, B, L, D, vdst, sp.world, Dl, Lfull, tok0, s));
-      LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));
+      LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay.flags, s));
       AttnArgs a;
       a.B = B; a.H = Hl; a.Lq = Lfull; a.Lk = Lfull;
       a.q = reinterpret_cast<const bf16*>(sp.region[sp.rank] + lay.q); a.ldq = Dl;
@@ -671,7 +671,7 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
       a.out_col0 = sp.rank * Dl;
       a.scale = attn_scale;
       LAUNCH(CAT_ATTN, attention_flops(a), launch_attention(a, s));
-      LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));
+      LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay.flags, s));
       attn_in = reinterpret_cast<const bf16*>(sp.region[sp.rank] + lay.attn);
     } else {
       LAUNCH(CAT_ROWS, 8.0 * M * D, launch_rmsnorm_rope(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, L,
@@ -752,10 +752,10 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
     bf16* ydst[8];
     for (int w = 0; w < sp.world; ++w) ydst[w] = reinterpret_cast<bf16*>(sp.region[w] + lay.yout);
     LAUNCH(CAT_OTHER, 0.0, launch_sp_broadcast_rows(ws.yout, B, L, No, ydst, sp.world, Lfull, tok0, s));
-    LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));
+    LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay.flags, s));
     LAUNCH(CAT_OTHER, 0.0, launch_unpatchify(reinterpret_cast<const bf16*>(sp.region[sp.rank] + lay.yout), No, reinterpret_cast<bf16*>(sample), B,
                                              c.out_channels, frames, height, width, s));
-    LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay, s));   // nobody overwrites a peer's yout (next forward) before it has been read
+    LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay.flags, s));   // nobody overwrites a peer's yout (next forward) before it has been read
     return CE_OK;
   }
   LAUNCH(CAT_OTHER, 0.0, launch_unpatchify(ws.yout, No, reinterpret_cast<bf16*>(sample), B, c.out_channels, frames, height, width, s));

@@ -177,7 +177,7 @@ GemmAttention attention_of(const EncWs& ws, const ce_encoder_config& c, int b, i
   GemmAttention a;
   a.x = ws.xn + (size_t)b * L8 * D;
   a.wqk = wqk; a.bqk = bqk; a.wv = wv; a.bv = bv;
-  a.L = L; a.D = D; a.H = c.num_heads; a.dk = c.d_kv; a.kpv = L8;
+  a.L = L; a.D = D; a.H = c.num_heads; a.dk = c.d_kv; a.kpv = L8; a.q0 = 0; a.nq = L;
   a.qk = ws.qk + (size_t)b * L8 * 2 * I; a.vT = ws.vT; a.S = ws.S; a.P = ws.P;
   a.out = ws.attn + (size_t)b * L8 * I; a.ldo = I;
   return a;
@@ -329,7 +329,7 @@ int ce_gemm_attention_bf16(const ce_gemm_attention_args* args, void* stream) {
   a.x = reinterpret_cast<const bf16*>(g.x);
   a.wqk = reinterpret_cast<const bf16*>(g.wqk); a.bqk = reinterpret_cast<const bf16*>(g.bqk);
   a.wv = reinterpret_cast<const bf16*>(g.wv); a.bv = reinterpret_cast<const bf16*>(g.bv);
-  a.L = g.L; a.D = g.D; a.H = g.H; a.dk = g.dk; a.kpv = g.kpv;
+  a.L = g.L; a.D = g.D; a.H = g.H; a.dk = g.dk; a.kpv = g.kpv; a.q0 = 0; a.nq = g.L;
   a.sc.rule = static_cast<SoftmaxRule>(g.rule);
   a.sc.scale = g.scale;
   a.sc.bias = reinterpret_cast<const bf16*>(g.bias); a.sc.bias_ld = g.bias_ld; a.sc.Lq = g.L; a.sc.valid = g.valid;

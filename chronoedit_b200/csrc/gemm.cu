@@ -390,14 +390,16 @@ int gemm_attention(Launcher& run, const GemmAttention& a) {
   GemmArgs g;
   g.M = I; g.N = L8; g.K = a.D; g.out = a.vT; g.ldo = L8; g.bias_row = a.bv;
   CE_TRY(run([&] { return launch_gemm_bf16(a.wv, a.D, a.x, a.D, g, run.s); }));
+  CE_REQUIRE(a.q0 >= 0 && a.nq >= 1 && a.q0 + a.nq <= a.L, "gemm_attention: query rows outside [0, L)");
+  CE_REQUIRE(a.nq == a.L || a.sc.rule == SOFTMAX_SCALED, "gemm_attention: a query range needs the scaled softmax (no position bias)");
   for (int h = 0; h < a.H; ++h) {
     g = GemmArgs();
-    g.M = a.L; g.N = L8; g.K = a.dk; g.out_f32 = a.S + (size_t)h * a.L * L8; g.ld_f32 = L8;
-    CE_TRY(run([&] { return launch_gemm_bf16(a.qk + h * a.dk, 2 * I, a.qk + I + h * a.dk, 2 * I, g, run.s); }));
+    g.M = a.nq; g.N = L8; g.K = a.dk; g.out_f32 = a.S + (size_t)h * a.nq * L8; g.ld_f32 = L8;
+    CE_TRY(run([&] { return launch_gemm_bf16(a.qk + (size_t)a.q0 * 2 * I + h * a.dk, 2 * I, a.qk + I + h * a.dk, 2 * I, g, run.s); }));
   }
-  CE_TRY(run([&] { return launch_softmax_rows(a.S, L8, a.P, L8, a.H * a.L, a.L, a.sc, run.s); }));
+  CE_TRY(run([&] { return launch_softmax_rows(a.S, L8, a.P, L8, a.H * a.nq, a.L, a.sc, run.s); }));
   for (int h = 0; h < a.H; ++h)
-    CE_TRY(run_gemm(run, a.P + (size_t)h * a.L * L8, L8, a.vT + (size_t)h * a.dk * L8, L8, a.L, a.dk, a.kpv, a.out + h * a.dk, a.ldo));
+    CE_TRY(run_gemm(run, a.P + (size_t)h * a.nq * L8, L8, a.vT + (size_t)h * a.dk * L8, L8, a.nq, a.dk, a.kpv, a.out + h * a.dk, a.ldo));
   return CE_OK;
 }
 

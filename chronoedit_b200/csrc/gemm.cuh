@@ -69,11 +69,14 @@ int run_gemm(Launcher& run, const bf16* A, int lda, const bf16* W, int ldw, int 
 //                                                           does not read)
 //   P = one row-softmax launch (rule sc)   -> P [H, L, L8]
 //   per head: O_h = P_h[:, 0:kpv] V_h      -> out [L, I] (ld ldo)
+// Only the query rows [q0, q0 + nq) are computed past q|k and V^T: S and P are [H, nq, L8] and out is [nq, I]; every row is the same
+// sum over the same keys in the same order whatever range it is computed in (the VAE split over ranks computes its band of rows).
 // x [L8, D] (ld D), Wqk [2I, D], Wv [I, D]; bqk / bv may be null.  Every launch goes through `run`.
 struct GemmAttention {
   const bf16 *x, *wqk, *bqk, *wv, *bv;
   int L, D, H, dk;
   int kpv;   // keys P.V sums over: L, or L8 when P's padding columns are zero and V^T's are finite
+  int q0, nq;   // query rows: [0, L) for the whole sequence
   SoftmaxScores sc;
   bf16 *qk, *vT, *P, *out;
   float* S;

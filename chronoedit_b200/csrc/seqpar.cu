@@ -2,6 +2,7 @@
 
 #include <string.h>
 
+#include <algorithm>
 #include <chrono>
 #include <condition_variable>
 #include <map>
@@ -64,6 +65,25 @@ __global__ void sp_broadcast_rows_kernel(const bf16* __restrict__ src, int B, in
     const uint4 v = *reinterpret_cast<const uint4*>(src + r * ncols + c);
     for (int w = 0; w < world; ++w)
       *reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(dst.p[w]) + ((size_t)b * dst_rows_per_batch + dst_row0 + li) * ncols + c) = v;
+  }
+}
+
+struct SpCopies {
+  SpCopy c[8];
+};
+
+// blockIdx.y = job; V = uint4 when every address, pitch and size of the launch is 16-byte aligned, else one bf16 at a time
+template <typename V>
+__global__ void sp_copy_kernel(const __grid_constant__ SpCopies jobs) {
+  const SpCopy& j = jobs.c[blockIdx.y];
+  const int64_t nv = j.bytes / (int64_t)sizeof(V);
+  const int64_t total = nv * j.n0 * j.n1;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t v = i % nv, p = i / nv;
+    const int64_t i0 = p % j.n0, i1 = p / j.n0;
+    const V* s = reinterpret_cast<const V*>(reinterpret_cast<const uint8_t*>(j.src) + i1 * j.sp1 + i0 * j.sp0) + v;
+    V* d = reinterpret_cast<V*>(reinterpret_cast<uint8_t*>(j.dst) + i1 * j.dp1 + i0 * j.dp0) + v;
+    *d = *s;
   }
 }
 
@@ -165,9 +185,9 @@ static int host_barrier(SeqPar& sp, cudaStream_t stream) {
   return sp.host->arrive(sp.rank, sp.epoch, sp.host_barrier_ms);
 }
 
-int launch_sp_barrier(SeqPar& sp, const SpLayout& lay, cudaStream_t stream) {
+int launch_sp_barrier(SeqPar& sp, int64_t flags, cudaStream_t stream) {
   Ptrs8 f;
-  for (int w = 0; w < 8; ++w) f.p[w] = w < sp.world ? sp.region[w] + lay.flags : nullptr;
+  for (int w = 0; w < 8; ++w) f.p[w] = w < sp.world ? sp.region[w] + flags : nullptr;
   ++sp.epoch;
   if (sp.host_barrier_ms > 0) return host_barrier(sp, stream);
   sp_barrier_kernel<<<1, 32, 0, stream>>>(f, sp.rank, sp.world, sp.epoch);
@@ -193,6 +213,30 @@ int launch_sp_broadcast_rows(const bf16* src, int B, int rows_per_batch, int nco
   for (int w = 0; w < 8; ++w) d.p[w] = w < world ? dst[w] : nullptr;
   sp_broadcast_rows_kernel<<<grid_for((size_t)B * rows_per_batch * ncols / 8), 256, 0, stream>>>(src, B, rows_per_batch, ncols, d, world,
                                                                                                  dst_rows_per_batch, dst_row0);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
+
+int launch_sp_copy(const SpCopy* jobs, int n, cudaStream_t stream) {
+  CE_REQUIRE(n >= 1 && n <= 8, "sp copy: 1 to 8 jobs");
+  SpCopies c;
+  bool vec = true;
+  int64_t most = 0;
+  for (int i = 0; i < n; ++i) {
+    const SpCopy& j = jobs[i];
+    CE_REQUIRE(j.src && j.dst && j.bytes > 0 && j.bytes % 2 == 0 && j.n0 >= 1 && j.n1 >= 1, "sp copy: job");
+    const uint64_t bits = reinterpret_cast<uintptr_t>(j.src) | reinterpret_cast<uintptr_t>(j.dst) | (uint64_t)j.bytes | (uint64_t)j.sp0 |
+                          (uint64_t)j.sp1 | (uint64_t)j.dp0 | (uint64_t)j.dp1;
+    CE_REQUIRE((bits & 1) == 0, "sp copy: bf16 alignment");
+    vec = vec && (bits & 15) == 0;
+    most = std::max(most, j.bytes * j.n0 * j.n1);
+    c.c[i] = j;
+  }
+  const dim3 grid((unsigned)grid_for((size_t)(most / (vec ? 16 : 2))), (unsigned)n);
+  if (vec)
+    sp_copy_kernel<uint4><<<grid, 256, 0, stream>>>(c);
+  else
+    sp_copy_kernel<uint16_t><<<grid, 256, 0, stream>>>(c);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }

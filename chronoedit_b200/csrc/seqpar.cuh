@@ -36,10 +36,11 @@ struct SpLayout {   // byte offsets inside a rank's region
 SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world);
 
 // all ranks: everything this rank issued so far on `stream` (incl. its peer stores) is complete and visible before any rank continues.
+// The flags (uint32 [8 * 32]) lie at byte offset `flags` of every rank's region.
 // With sp.host_barrier_ms > 0 no kernel is launched: the stream is synchronised and the calling thread waits for the other ranks'
 // threads (same process, same region[0]); a timeout is an error naming the rank and the barrier and poisons the group, so every
 // later barrier of it fails at once.  Refused while `stream` is capturing.
-int launch_sp_barrier(SeqPar& sp, const SpLayout& lay, cudaStream_t stream);
+int launch_sp_barrier(SeqPar& sp, int64_t flags, cudaStream_t stream);
 // dst[r] + ((b * dst_rows_per_batch + dst_row0 + i) * cols_per_rank + c % cols_per_rank) = src[(b * rows_per_batch + i) * ld_src + c],
 // r = c / cols_per_rank   (v scatter: columns to the rank that owns the head)
 int launch_sp_scatter_cols(const bf16* src, int ld_src, int B, int rows_per_batch, int ncols, bf16* const* dst, int world, int cols_per_rank,
@@ -47,6 +48,16 @@ int launch_sp_scatter_cols(const bf16* src, int ld_src, int B, int rows_per_batc
 // every rank r: dst[r] + ((b * dst_rows_per_batch + dst_row0 + i) * ncols + c) = src[(b * rows_per_batch + i) * ncols + c]   (all-gather of rows)
 int launch_sp_broadcast_rows(const bf16* src, int B, int rows_per_batch, int ncols, bf16* const* dst, int world, int dst_rows_per_batch,
                              int dst_row0, cudaStream_t stream);
+// One launch of up to 8 strided copies, each to local or peer memory: for i1 < n1, i0 < n0, dst + i1 * dp1 + i0 * dp0 receives the `bytes`
+// bytes at src + i1 * sp1 + i0 * sp0 (byte offsets and sizes; bf16 data, so all of them even).  The VAE's band exchanges.
+struct SpCopy {
+  const void* src = nullptr;
+  void* dst = nullptr;
+  int64_t bytes = 0;
+  int n0 = 1, n1 = 1;
+  int64_t sp0 = 0, sp1 = 0, dp0 = 0, dp1 = 0;
+};
+int launch_sp_copy(const SpCopy* jobs, int n, cudaStream_t stream);
 // patchify of a token range: patches[(b, i), k] for global tokens tok0 .. tok0 + ntok - 1 of every sample
 int launch_patchify_range(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, int tok0, int ntok, cudaStream_t stream);
 

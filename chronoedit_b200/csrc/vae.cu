@@ -7,8 +7,16 @@
 // wgmma implicit GEMM of conv.cu reading its input (history frames + chunk) in place; the three small-Cin convolutions
 // (3->dim, z->top, 2z->2z) go through im2row + the wgmma GEMM; RMS_norm+SiLU / upsample are the row kernels of
 // vae_kernels.cu; the single-head mid attention is gemm_attention (gemm.cu) with H = 1.
+//
+// Split over the ranks of a node (ce_vae_sp_configure): rank r owns latent rows [r h / W, (r + 1) h / W) and the matching rows at
+// every resolution of the encoder and decoder.  Every buffer that feeds a convolution with three kernel rows holds the band plus one
+// halo row above and below; the neighbours store their edge rows into this rank's peer region, a barrier orders it, and a local copy
+// moves them into the halo rows (zero past the global top and bottom: the convolution's own zero padding).  The mid attention
+// gathers its normalised frame into every rank's region and computes the rank's query rows only; the outputs are gathered the same
+// way.  Every output element sums the same terms in the same order as on one GPU, so each rank returns the single-GPU bits.
 #include <math.h>
 
+#include <algorithm>
 #include <map>
 #include <string>
 #include <vector>
@@ -16,6 +24,7 @@
 #include "../../include/chronoedit_b200.h"
 #include "conv.cuh"
 #include "gemm.cuh"
+#include "seqpar.cuh"
 #include "vae_kernels.cuh"
 
 using namespace ce;
@@ -24,6 +33,7 @@ struct ce_vae {
   ce_vae_config cfg;
   WeightMap w;
   int64_t launches = 0;
+  SeqPar sp;   // the split over ranks (ce_vae_sp_configure): world == 1 means off
 };
 
 namespace {
@@ -39,10 +49,29 @@ struct Act {
 struct StreamBuf {  // input buffer of one streaming (causal) convolution: `hist` history frames, then the chunk
   bf16* p = nullptr;
   int hist = 0, tcap = 0, H = 0, W = 0, C = 0;
+  bool halo = false;    // split: every frame is a band with one halo row above and below (H counts them)
   bool primed = false;  // false until the first chunk went through (used for the "Rep" / pass-through first chunks)
 };
 
+// Byte offsets inside a rank's peer region for one pixel geometry H x W, the same for every frame count.
+struct VaeSpLayout {
+  int64_t flags = 0;        // uint32 [8 * 32] barrier flags; first, so that every geometry finds them in the same place
+  int64_t halo = 0;         // [2 sets][from above, from below][halo_slot]: the neighbours' edge rows of one chunk
+  int64_t halo_slot = 0;
+  int64_t frame = 0;        // [2 sets][frame_bytes]: the mid attention's normalised frame [up8(h w), top] bf16
+  int64_t frame_bytes = 0;
+  int64_t video = 0;        // [3, video_frames, H, W] bf16: the pixels of one decode chunk
+  int video_frames = 0;
+  int64_t moments = 0;      // [2 sets][moments_bytes]: one latent frame of encode moments [2 z_dim, h, w] bf16
+  int64_t moments_bytes = 0;
+  int64_t bytes = 0;
+};
+
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
+template <class T>
+T* at(T* p, size_t off) {   // planning passes carry null pointers
+  return p ? p + off : nullptr;
+}
 
 // One encode or decode call.  `dry` = planning pass: the same walk without launches, in which the two bump allocators measure the
 // workspace and every weight is looked up with its packed element count before anything is launched.
@@ -57,9 +86,21 @@ struct Run {
   WeightLookup weights{h->w};
   Launcher run{s, &h->launches};
   int rc = 0;
+  // the split: this rank's band is latent rows [band0, band1) of `rows`; world == 1: the whole frame
+  int rank, world;
+  int rows = 0, band0 = 0, band1 = 0;
+  const VaeSpLayout* lay = nullptr;   // null when planning
+  int64_t halo_row_max = 0;           // the largest halo row of a chunk (T W C bf16), in bytes
 
-  Run(ce_vae* h_, cudaStream_t s_, uint8_t* persist_base, uint8_t* scratch_base)
-      : h(h_), s(s_), dry(persist_base == nullptr), persist(persist_base), scratch(scratch_base) {}
+  Run(ce_vae* h_, cudaStream_t s_, uint8_t* persist_base, uint8_t* scratch_base, int rank_ = 0, int world_ = 1)
+      : h(h_), s(s_), dry(persist_base == nullptr), persist(persist_base), scratch(scratch_base), rank(rank_), world(world_) {}
+
+  bool split() const { return world > 1; }
+  void set_band(int latent_rows) {
+    rows = latent_rows;
+    band0 = (int)((int64_t)rank * latent_rows / world);
+    band1 = (int)((int64_t)(rank + 1) * latent_rows / world);
+  }
 
   void* take_scratch_bytes(size_t bytes) {
     void* p = scratch.take<uint8_t>((int64_t)bytes);
@@ -79,19 +120,22 @@ struct Run {
   void launch(Launch&& l) {
     if (!dry && !rc) rc = run(l);
   }
+  void cuda(cudaError_t e) {
+    if (e != cudaSuccess && !rc) rc = fail(CE_ERR_CUDA, cudaGetErrorString(e));
+  }
 
   // ---- streaming conv input buffers
-  StreamBuf& stream(const std::string& name, int hist, int tcap, int H, int W_, int C) {
+  StreamBuf& stream(const std::string& name, int hist, int tcap, int H, int W_, int C, bool halo = false) {
     auto it = streams.find(name);
     if (it != streams.end()) return it->second;
     StreamBuf b;
-    b.hist = hist; b.tcap = tcap; b.H = H; b.W = W_; b.C = C;
-    const size_t elems = (size_t)(hist + tcap) * H * W_ * C;
+    b.halo = halo && split();
+    b.hist = hist; b.tcap = tcap; b.H = b.halo ? H + 2 : H; b.W = W_; b.C = C;
+    const size_t elems = (size_t)(hist + tcap) * b.H * W_ * C;
     b.p = persist.take<bf16>((int64_t)elems);
-    if (!dry && hist > 0) {
-      cudaError_t e = cudaMemsetAsync(b.p, 0, (size_t)hist * H * W_ * C * 2, s);  // zero history = causal zero padding
-      if (e != cudaSuccess && !rc) rc = fail(CE_ERR_CUDA, cudaGetErrorString(e));
-    }
+    // zero history = causal zero padding; split: also the halo rows past the global edge, which nothing writes
+    const size_t zero = split() ? elems : (size_t)hist * b.H * W_ * C;
+    if (!dry && zero > 0) cuda(cudaMemsetAsync(b.p, 0, zero * 2, s));
     return streams.emplace(name, b).first->second;
   }
   Act chunk_of(StreamBuf& b, int T) {
@@ -107,15 +151,60 @@ struct Run {
     const size_t fb = (size_t)b.H * b.W * b.C * 2;
     for (int i = 0; i < b.hist; ++i) {  // ascending order: sources are always at or after the destination
       const int src = T + i;            // frame index inside [hist ; chunk]
-      cudaError_t e = cudaMemcpyAsync(reinterpret_cast<uint8_t*>(b.p) + (size_t)i * fb, reinterpret_cast<uint8_t*>(b.p) + (size_t)src * fb, fb,
-                                      cudaMemcpyDeviceToDevice, s);
-      if (e != cudaSuccess && !rc) rc = fail(CE_ERR_CUDA, cudaGetErrorString(e));
+      cuda(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(b.p) + (size_t)i * fb, reinterpret_cast<uint8_t*>(b.p) + (size_t)src * fb, fb,
+                           cudaMemcpyDeviceToDevice, s));
     }
   }
   void copy(const Act& src, bf16* dst) {
     if (dry) return;
-    cudaError_t e = cudaMemcpyAsync(dst, src.p, src.numel() * 2, cudaMemcpyDeviceToDevice, s);
-    if (e != cudaSuccess && !rc) rc = fail(CE_ERR_CUDA, cudaGetErrorString(e));
+    cuda(cudaMemcpyAsync(dst, src.p, src.numel() * 2, cudaMemcpyDeviceToDevice, s));
+  }
+
+  // ---- the exchange between ranks
+  uint8_t* region(int w) const { return h->sp.region[w]; }
+  void barrier() { launch([&] { return launch_sp_barrier(h->sp, lay->flags, s); }); }
+  void peer_copies(const SpCopy* jobs, int n) {
+    if (n > 0) launch([&] { return launch_sp_copy(jobs, n, s); });
+  }
+  void copy_2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height) {
+    if (!dry && !rc) cuda(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, height, cudaMemcpyDeviceToDevice, s));
+  }
+  // A halo'd buffer holds T frames of band + 2 rows of W * C; rows 0 and band + 1 are the neighbours' edge rows.  The ones past the
+  // global top and bottom are zero.
+  void zero_edges(bf16* buf, int T, int band, int W, int C) {
+    if (dry || rc) return;
+    const size_t row = (size_t)W * C * 2, fr = (band + 2) * row;
+    if (rank == 0) cuda(cudaMemset2DAsync(buf, fr, 0, row, T, s));
+    if (rank == world - 1) cuda(cudaMemset2DAsync(reinterpret_cast<uint8_t*>(buf) + (band + 1) * row, fr, 0, row, T, s));
+  }
+  // The band rows of the halo'd buffer are written: store the first one into the rank above's "from below" slot and the last one into
+  // the rank below's "from above" slot, barrier, then copy what the neighbours stored into rows 0 and band + 1.  Exchange i uses slot
+  // set i mod 2, so a slot is rewritten only after every rank has passed the barrier that follows its unpacking.
+  void halo_exchange(bf16* buf, int T, int band, int W, int C) {
+    const int64_t row = (int64_t)W * C * 2, fr = (band + 2) * row;
+    halo_row_max = std::max(halo_row_max, T * row);
+    if (dry || rc) return;
+    if (T * row > lay->halo_slot) {
+      rc = fail(CE_ERR_INVALID, "vae sequence parallel: a halo row is larger than the region's slot");
+      return;
+    }
+    const int set = (int)(h->sp.epoch & 1);
+    auto slot = [&](int w, int below) { return region(w) + lay->halo + (2 * set + below) * lay->halo_slot; };
+    uint8_t* b = reinterpret_cast<uint8_t*>(buf);
+    SpCopy j[2];
+    int n = 0;
+    if (rank > 0) {
+      j[n].src = b + row; j[n].dst = slot(rank - 1, 1); j[n].bytes = row; j[n].n0 = T; j[n].sp0 = fr; j[n].dp0 = row;
+      ++n;
+    }
+    if (rank < world - 1) {
+      j[n].src = b + band * row; j[n].dst = slot(rank + 1, 0); j[n].bytes = row; j[n].n0 = T; j[n].sp0 = fr; j[n].dp0 = row;
+      ++n;
+    }
+    peer_copies(j, n);
+    barrier();
+    if (rank > 0) copy_2d(b, fr, slot(rank, 0), row, row, T);
+    if (rank < world - 1) copy_2d(b + (band + 1) * row, fr, slot(rank, 1), row, row, T);
   }
 
   // ---- primitive ops
@@ -123,23 +212,32 @@ struct Run {
     const bf16* g = weights.any<bf16>(gamma_name, x.C);
     launch([&] { return launch_rms_silu_cl(x.p, g, y, x.pixels(), x.C, silu ? 1 : 0, s); });
   }
+  // rms into the chunk of a stream buffer; with halo rows one launch per frame (a frame's band rows are not next to the next frame's)
+  void rms_into(const Act& x, const std::string& gamma_name, const StreamBuf& b, bf16* y, bool silu) {
+    if (!b.halo) return rms(x, gamma_name, y, silu);
+    for (int f = 0; f < x.T; ++f) {
+      Act xf = x;
+      xf.T = 1; xf.p = at(x.p, f * x.frame());
+      rms(xf, gamma_name, at(y, f * (x.frame() + 2 * (size_t)x.W * x.C) + (size_t)x.W * x.C), silu);
+    }
+  }
   // implicit-GEMM conv reading `in` = [Tin frames] (history included) -> out
   void conv(const std::string& name, const bf16* in, int Tin, int Hin, int Win, int Cin, Act& out, int kt, int kh, int kw, int st, int sh,
-            int sw, int ph, int pw, const bf16* resid = nullptr, int split_time = 0) {
+            int sw, int ph, int pw, const bf16* resid = nullptr, int split_time = 0, int t_base = 0) {
     ConvArgs a;
     a.Cout = split_time ? out.C * 2 : out.C; a.Cin_pad = round_up(Cin, 64);
     a.w = weights.any<bf16>(name + ".weight", (int64_t)a.Cout * kt * kh * kw * a.Cin_pad);
     a.bias = weights.any<bf16>(name + ".bias", a.Cout);
     a.x = in; a.Tin = Tin; a.Hin = Hin; a.Win = Win; a.Cin = Cin;
     a.kt = kt; a.kh = kh; a.kw = kw; a.st = st; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw;
-    a.t_base = 0;
+    a.t_base = t_base;
     a.y = out.p; a.Tout = split_time ? out.T / 2 : out.T; a.Hout = out.H; a.Wout = out.W;
     a.resid = resid; a.split_time = split_time;
     launch([&] { return launch_conv3d_cl(a, s); });
   }
-  // streaming causal conv (kt = 3): x is already in the stream buffer's chunk region
+  // streaming causal conv (kt = 3): x is already in the stream buffer's chunk region; halo rows replace the rows' zero padding
   void causal_conv(const std::string& name, StreamBuf& b, int T, Act& out, int kh, const bf16* resid = nullptr, int split_time = 0) {
-    conv(name, b.p, b.hist + T, b.H, b.W, b.C, out, 3, kh, kh, 1, 1, 1, kh / 2, kh / 2, resid, split_time);
+    conv(name, b.p, b.hist + T, b.H, b.W, b.C, out, 3, kh, kh, 1, 1, 1, b.halo ? 0 : kh / 2, kh / 2, resid, split_time);
     push_history(b, T);
     b.primed = true;
   }
@@ -149,30 +247,50 @@ struct Run {
   }
 
   // ---- blocks
-  // ResidualBlock.forward (wan2pt1.py:201-220)
-  Act res_block(const std::string& n, const Act& x, int Cout, int tcap) {
-    StreamBuf& sa = stream(n + ".residual.2", 2, tcap, x.H, x.W, x.C);
+  // ResidualBlock.forward (wan2pt1.py:201-220).  halo_out (split only): the output feeds a stride-2 downsample, so it is written
+  // with halo rows (one launch per frame) and its edge rows are exchanged.
+  Act res_block(const std::string& n, const Act& x, int Cout, int tcap, bool halo_out = false) {
+    StreamBuf& sa = stream(n + ".residual.2", 2, tcap, x.H, x.W, x.C, true);
     Act a_in = chunk_of(sa, x.T);
-    rms(x, n + ".residual.0.gamma", a_in.p, true);
+    rms_into(x, n + ".residual.0.gamma", sa, a_in.p, true);
+    if (sa.halo) halo_exchange(a_in.p, x.T, x.H, x.W, x.C);
     Act t1 = scratch_act(x.T, x.H, x.W, Cout);
     causal_conv(n + ".residual.2", sa, x.T, t1, 3);
-    StreamBuf& sb = stream(n + ".residual.6", 2, tcap, x.H, x.W, Cout);
+    StreamBuf& sb = stream(n + ".residual.6", 2, tcap, x.H, x.W, Cout, true);
     Act b_in = chunk_of(sb, x.T);
-    rms(t1, n + ".residual.3.gamma", b_in.p, true);
+    rms_into(t1, n + ".residual.3.gamma", sb, b_in.p, true);
+    if (sb.halo) halo_exchange(b_in.p, x.T, x.H, x.W, Cout);
     const bf16* hres = x.p;
     if (x.C != Cout) {
       Act sc = scratch_act(x.T, x.H, x.W, Cout);
       conv(n + ".shortcut", x.p, x.T, x.H, x.W, x.C, sc, 1, 1, 1, 1, 1, 1, 0, 0);
       hres = sc.p;
     }
-    Act out = scratch_act(x.T, x.H, x.W, Cout);
-    causal_conv(n + ".residual.6", sb, x.T, out, 3, hres);
+    if (!(halo_out && split())) {
+      Act out = scratch_act(x.T, x.H, x.W, Cout);
+      causal_conv(n + ".residual.6", sb, x.T, out, 3, hres);
+      return out;
+    }
+    Act out = scratch_act(x.T, x.H + 2, x.W, Cout);
+    const size_t row = (size_t)x.W * Cout;
+    for (int f = 0; f < x.T; ++f) {
+      Act of = out;
+      of.T = 1; of.H = x.H; of.p = at(out.p, f * out.frame() + row);
+      conv(n + ".residual.6", sb.p, sb.hist + x.T, sb.H, sb.W, sb.C, of, 3, 3, 3, 1, 1, 1, 0, 1, at(hres, f * x.H * row), 0, f);
+    }
+    push_history(sb, x.T);
+    sb.primed = true;
+    zero_edges(out.p, x.T, x.H, x.W, Cout);
+    halo_exchange(out.p, x.T, x.H, x.W, Cout);
     return out;
   }
 
-  // AttentionBlock.forward (wan2pt1.py:240-259): per frame, single head of width C over H*W tokens
+  // AttentionBlock.forward (wan2pt1.py:240-259): per frame, single head of width C over H*W tokens.  Split: every rank stores its band
+  // of the normalised frame into every rank's region, computes q|k and V^T of the whole frame and S, softmax, P.V, the projection
+  // and the residual for its own rows.
   Act attn_block(const std::string& n, const Act& x) {
-    const int C = x.C, P = x.H * x.W, Ppad = round_up(P, 8);
+    const int C = x.C, P = rows * x.W, Ppad = round_up(P, 8);
+    const int q0 = band0 * x.W, nq = x.H * x.W;
     Act xn = scratch_act(x.T, x.H, x.W, C);
     rms(x, n + ".norm.gamma", xn.p, false);
     Act out = scratch_act(x.T, x.H, x.W, C);
@@ -183,19 +301,29 @@ struct Run {
     a.bv = a.bqk ? a.bqk + 2 * C : nullptr;
     const bf16* wproj = weights.any<bf16>(n + ".proj.weight", (int64_t)C * C);
     const bf16* bproj = weights.any<bf16>(n + ".proj.bias", C);
-    a.L = P; a.D = C; a.H = 1; a.dk = C; a.kpv = P;
+    a.L = P; a.D = C; a.H = 1; a.dk = C; a.kpv = P; a.q0 = q0; a.nq = nq;
     a.sc.rule = SOFTMAX_SCALED;
     a.sc.scale = 1.0f / sqrtf((float)C);
     a.qk = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * 2 * C * 2));
     a.vT = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)C * Ppad * 2));
-    a.S = reinterpret_cast<float*>(take_scratch_bytes((size_t)P * Ppad * 4));
-    a.P = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * Ppad * 2));
-    a.out = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * C * 2));
+    a.S = reinterpret_cast<float*>(take_scratch_bytes((size_t)nq * Ppad * 4));
+    a.P = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)nq * Ppad * 2));
+    a.out = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)nq * C * 2));
     a.ldo = C;
     for (int f = 0; f < x.T && !dry && !rc; ++f) {
-      a.x = xn.p + (size_t)f * P * C;
-      rc = gemm_attention(run, a);
-      gemm(a.out, C, wproj, C, P, C, C, out.p + (size_t)f * P * C, C, bproj, EPI_BIAS_RESID, x.p + (size_t)f * P * C, C);   // proj + identity
+      a.x = xn.p + (size_t)f * nq * C;
+      if (split()) {
+        const int set = (int)(h->sp.epoch & 1);
+        SpCopy j[8];
+        for (int w = 0; w < world; ++w) {
+          j[w].src = a.x; j[w].dst = region(w) + lay->frame + set * lay->frame_bytes + (int64_t)q0 * C * 2; j[w].bytes = (int64_t)nq * C * 2;
+        }
+        peer_copies(j, world);
+        barrier();
+        a.x = reinterpret_cast<const bf16*>(region(rank) + lay->frame + set * lay->frame_bytes);
+      }
+      if (!rc) rc = gemm_attention(run, a);
+      gemm(a.out, C, wproj, C, nq, C, C, out.p + (size_t)f * nq * C, C, bproj, EPI_BIAS_RESID, x.p + (size_t)f * nq * C, C);   // proj + identity
     }
     return out;
   }
@@ -215,25 +343,39 @@ struct Run {
         x = y;
       }
     }
-    Act up = scratch_act(x.T, 2 * x.H, 2 * x.W, C);
-    launch([&] { return launch_upsample2x_cl(x.p, up.p, x.T, x.H, x.W, C, s); });
+    if (!split()) {
+      Act up = scratch_act(x.T, 2 * x.H, 2 * x.W, C);
+      launch([&] { return launch_upsample2x_cl(x.p, up.p, x.T, x.H, x.W, C, s); });
+      Act out = scratch_act(x.T, 2 * x.H, 2 * x.W, C / 2);
+      conv(n + ".resample.1", up.p, up.T, up.H, up.W, C, out, 1, 3, 3, 1, 1, 1, 1, 1);
+      return out;
+    }
+    Act up = scratch_act(x.T, 2 * x.H + 2, 2 * x.W, C);   // halo'd: one launch per frame into the band rows
+    for (int f = 0; f < x.T; ++f) {
+      const bf16* xf = at(x.p, f * x.frame());
+      bf16* uf = at(up.p, f * up.frame() + (size_t)2 * x.W * C);
+      launch([&] { return launch_upsample2x_cl(xf, uf, 1, x.H, x.W, C, s); });
+    }
+    zero_edges(up.p, x.T, 2 * x.H, 2 * x.W, C);
+    halo_exchange(up.p, x.T, 2 * x.H, 2 * x.W, C);
     Act out = scratch_act(x.T, 2 * x.H, 2 * x.W, C / 2);
-    conv(n + ".resample.1", up.p, up.T, up.H, up.W, C, out, 1, 3, 3, 1, 1, 1, 1, 1);
+    conv(n + ".resample.1", up.p, up.T, up.H, up.W, C, out, 1, 3, 3, 1, 1, 1, 0, 1);
     return out;
   }
 
-  // Resample downsample2d / downsample3d (wan2pt1.py:145-159)
+  // Resample downsample2d / downsample3d (wan2pt1.py:145-159).  Split: x is halo'd; ph = -1 skips its row above, and the row below
+  // the band (zero at the global bottom) is what ZeroPad2d(0,1,0,1) and the stride-2 window read there.
   Act downsample(const std::string& n, const Act& x, bool temporal, int tcap_out_spatial) {
-    const int C = x.C;
-    const int Ho = (x.H + 1 - 3) / 2 + 1, Wo = (x.W + 1 - 3) / 2 + 1;
+    const int C = x.C, band = split() ? x.H - 2 : x.H, ph = split() ? -1 : 0;
+    const int Ho = (band + 1 - 3) / 2 + 1, Wo = (x.W + 1 - 3) / 2 + 1;
     if (!temporal) {
       Act out = scratch_act(x.T, Ho, Wo, C);
-      conv(n + ".resample.1", x.p, x.T, x.H, x.W, C, out, 1, 3, 3, 1, 2, 2, 0, 0);  // ZeroPad2d(0,1,0,1) = OOB zero fill
+      conv(n + ".resample.1", x.p, x.T, x.H, x.W, C, out, 1, 3, 3, 1, 2, 2, ph, 0);  // ZeroPad2d(0,1,0,1) = OOB zero fill
       return out;
     }
     StreamBuf& st = stream(n + ".time_conv", 1, tcap_out_spatial, Ho, Wo, C);
     Act sp = chunk_of(st, x.T);
-    conv(n + ".resample.1", x.p, x.T, x.H, x.W, C, sp, 1, 3, 3, 1, 2, 2, 0, 0);
+    conv(n + ".resample.1", x.p, x.T, x.H, x.W, C, sp, 1, 3, 3, 1, 2, 2, ph, 0);
     if (!st.primed) {  // first chunk passes through and becomes the history (:147-150)
       st.primed = true;
       Act out = scratch_act(x.T, Ho, Wo, C);
@@ -248,15 +390,52 @@ struct Run {
     return out;
   }
 
-  // small-Cin conv: im2row + GEMM.  x addressed by strides (planar or channels-last)
+  // small-Cin conv: im2row + GEMM.  x addressed by strides (planar or channels-last); output row oh reads rows oh + dh - ph of x
   void small_conv(const std::string& name, const bf16* x, size_t sc, size_t st_, size_t sh, size_t sw, int Tin, int Hin, int Win, int Cin,
-                  int t_base, int kt, int kh, bf16* out, int ldo, int Tout, int Cout) {
+                  int t_base, int kt, int kh, bf16* out, int ldo, int Tout, int Hout, int ph, int Cout) {
     const int K = kt * kh * kh * Cin, Kpad = round_up(K, 8);
-    bf16* A = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)Tout * Hin * Win * Kpad * 2));
+    bf16* A = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)Tout * Hout * Win * Kpad * 2));
     const bf16* w = weights.any<bf16>(name + ".weight", (int64_t)Cout * Kpad);
     const bf16* b = weights.any<bf16>(name + ".bias", Cout);
-    launch([&] { return launch_im2row(x, sc, st_, sh, sw, Tin, Hin, Win, Cin, A, Kpad, Tout, Hin, Win, kt, kh, kh, kh / 2, kh / 2, t_base, s); });
-    gemm(A, Kpad, w, Kpad, Tout * Hin * Win, Cout, Kpad, out, ldo, b);
+    launch([&] {
+      return launch_im2row(x, sc, st_, sh, sw, Tin, Hin, Win, Cin, A, Kpad, Tout, Hout, Win, kt, kh, kh, ph, kh / 2, t_base, s);
+    });
+    gemm(A, Kpad, w, Kpad, Tout * Hout * Win, Cout, Kpad, out, ldo, b);
+  }
+
+  // ---- gathering the outputs (split)
+  // band = the decoder head's planar output [3, T, band rows, W] of this rank; store it into every rank's region video buffer
+  // [3, video_frames, H, W], barrier, then copy the whole chunk into frames t0 .. t0 + T - 1 of the caller's video [3, T_px, H, W].
+  void gather_video(const bf16* band, bf16* video, int T_px, int t0, int T, int H, int W) {
+    if (dry || rc) return;
+    const int64_t plane = (int64_t)H * W * 2, chan = lay->video_frames * plane;
+    const int64_t r0 = (int64_t)band0 * 8 * W * 2, bytes = (int64_t)(band1 - band0) * 8 * W * 2;
+    SpCopy j[8];
+    for (int w = 0; w < world; ++w) {
+      j[w].src = band; j[w].dst = region(w) + lay->video + r0; j[w].bytes = bytes;
+      j[w].n0 = T; j[w].sp0 = bytes; j[w].dp0 = plane; j[w].n1 = 3; j[w].sp1 = T * bytes; j[w].dp1 = chan;
+    }
+    peer_copies(j, world);
+    barrier();
+    copy_2d(reinterpret_cast<uint8_t*>(video) + t0 * plane, (size_t)T_px * plane, region(rank) + lay->video, chan, T * plane, 3);
+  }
+  // band = this rank's moments [2 z_dim, Tl, band rows, w] (planar); latent frame t of every rank's band into every rank's region,
+  // barrier, then the whole frame into moments [2 z_dim, Tl, h, w].
+  void gather_moments(const bf16* band, bf16* moments, int t, int Tl, int Cm, int w) {
+    if (dry || rc) return;
+    const int set = (int)(h->sp.epoch & 1);
+    const int nb = band1 - band0;
+    const int64_t plane = (int64_t)rows * w * 2, bplane = (int64_t)nb * w * 2;
+    SpCopy j[8];
+    for (int r = 0; r < world; ++r) {
+      j[r].src = reinterpret_cast<const uint8_t*>(band) + t * bplane;
+      j[r].dst = region(r) + lay->moments + set * lay->moments_bytes + (int64_t)band0 * w * 2;
+      j[r].bytes = bplane; j[r].n0 = Cm; j[r].sp0 = Tl * bplane; j[r].dp0 = plane;
+    }
+    peer_copies(j, world);
+    barrier();
+    copy_2d(reinterpret_cast<uint8_t*>(moments) + t * plane, (size_t)Tl * plane, region(rank) + lay->moments + set * lay->moments_bytes, plane,
+            plane, Cm);
   }
 };
 
@@ -305,18 +484,28 @@ int run_decode(Run& R, const bf16* z, bf16* video, int Tl, int h, int w, int cla
   const int top = top_dim(c), zc = c.z_dim;
   const int T_px = 1 + 4 * (Tl - 1);
   const size_t zplane = (size_t)Tl * h * w;
+  R.set_band(h);
+  const int a = R.band0, nb = R.band1 - R.band0;   // the band's latent rows
   std::vector<LayerSpec> layers = decoder_layers(c);
   int t_out = 0;
   for (int i = 0; i < Tl && !R.rc; ++i) {
     R.reset_scratch();
     int cap = 1;  // frames a non-first chunk carries at the current depth (x2 after every upsample3d): stream capacity
-    // conv2 (1x1x1 on the planar z) -> straight into the stream buffer of decoder.conv1
-    StreamBuf& s1 = R.stream("decoder.conv1", 2, 1, h, w, zc);
+    // conv2 (1x1x1 on the planar z) -> straight into the stream buffer of decoder.conv1; split: the band's rows and the halo rows
+    // that exist, read from the whole z
+    StreamBuf& s1 = R.stream("decoder.conv1", 2, 1, nb, w, zc, true);
     Act x0 = R.chunk_of(s1, 1);
-    R.small_conv("conv2", z, zplane, (size_t)h * w, (size_t)w, 1, Tl, h, w, zc, /*t_base=*/i, 1, 1, x0.p, zc, 1, zc);
+    if (!s1.halo) {
+      R.small_conv("conv2", z, zplane, (size_t)h * w, (size_t)w, 1, Tl, h, w, zc, /*t_base=*/i, 1, 1, x0.p, zc, 1, h, 0, zc);
+    } else {
+      const int lo = std::max(a - 1, 0), hi = std::min(a + nb + 1, h);
+      R.small_conv("conv2", at(z, (size_t)lo * w), zplane, (size_t)h * w, (size_t)w, 1, Tl, hi - lo, w, zc, /*t_base=*/i, 1, 1,
+                   at(x0.p, (size_t)(lo - a + 1) * w * zc), zc, 1, hi - lo, 0, zc);
+    }
     // decoder.conv1: 3x3x3 causal with Cin = z_dim: im2row over [history ; chunk] (channels-last) + GEMM
-    Act x = R.scratch_act(1, h, w, top);
-    R.small_conv("decoder.conv1", s1.p, 1, (size_t)h * w * zc, (size_t)w * zc, (size_t)zc, s1.hist + 1, h, w, zc, 0, 3, 3, x.p, top, 1, top);
+    Act x = R.scratch_act(1, nb, w, top);
+    R.small_conv("decoder.conv1", s1.p, 1, (size_t)s1.H * w * zc, (size_t)w * zc, (size_t)zc, s1.hist + 1, s1.H, w, zc, 0, 3, 3, x.p, top, 1, nb,
+                 s1.halo ? 0 : 1, top);
     R.push_history(s1, 1);
     x = R.res_block("decoder.middle.0", x, top, cap);
     x = R.attn_block("decoder.middle.1", x);
@@ -331,21 +520,28 @@ int run_decode(Run& R, const bf16* z, bf16* video, int Tl, int h, int w, int cla
         if (l.mode == 1) cap *= 2;
       }
     }
-    // head: RMS + SiLU + conv dim->3, planar clamped store straight into the output video
-    StreamBuf& sh = R.stream("decoder.head.2", 2, cap, x.H, x.W, x.C);
+    // head: RMS + SiLU + conv dim->3, planar clamped store straight into the output video (split: into a planar band [3, T, rows, W],
+    // then gathered)
+    StreamBuf& sh = R.stream("decoder.head.2", 2, cap, x.H, x.W, x.C, true);
     Act hin = R.chunk_of(sh, x.T);
-    R.rms(x, "decoder.head.0.gamma", hin.p, true);
+    R.rms_into(x, "decoder.head.0.gamma", sh, hin.p, true);
+    if (sh.halo) R.halo_exchange(hin.p, x.T, x.H, x.W, x.C);
     {
       ConvArgs a;
-      a.x = sh.p; a.Tin = sh.hist + x.T; a.Hin = x.H; a.Win = x.W; a.Cin = x.C;
+      a.x = sh.p; a.Tin = sh.hist + x.T; a.Hin = sh.H; a.Win = x.W; a.Cin = x.C;
       a.Cout = 3; a.Cin_pad = round_up(x.C, 64);
       a.w = R.weights.any<bf16>("decoder.head.2.weight", (int64_t)3 * 27 * a.Cin_pad);
       a.bias = R.weights.any<bf16>("decoder.head.2.bias", 3);
-      a.kt = 3; a.kh = 3; a.kw = 3; a.ph = 1; a.pw = 1;
+      a.kt = 3; a.kh = 3; a.kw = 3; a.ph = sh.halo ? 0 : 1; a.pw = 1;
       a.y = video; a.Tout = x.T; a.Hout = x.H; a.Wout = x.W;
       a.planar_out = 1; a.clamp = clamp; a.planar_T = T_px; a.planar_t0 = t_out;
+      if (R.split()) {
+        a.y = reinterpret_cast<bf16*>(R.take_scratch_bytes((size_t)3 * x.T * x.H * x.W * 2));
+        a.planar_T = x.T; a.planar_t0 = 0;
+      }
       R.launch([&] { return launch_conv3d_cl(a, R.s); });
       R.push_history(sh, x.T);
+      if (R.split()) R.gather_video(a.y, video, T_px, t_out, x.T, 8 * h, x.W);
     }
     t_out += x.T;
   }
@@ -359,22 +555,27 @@ int run_encode(Run& R, const bf16* video, bf16* mu, int T, int H, int Wd) {
   const ce_vae_config& c = R.h->cfg;
   const int top = top_dim(c), zc = c.z_dim;
   const int Tl = 1 + (T - 1) / 4, h = H / 8, w = Wd / 8;
+  R.set_band(h);
+  const int nb = R.band1 - R.band0;   // the band's latent rows
   std::vector<LayerSpec> layers = encoder_layers(c);
-  bf16* enc_out = R.persist.take<bf16>((int64_t)Tl * h * w * 2 * zc);  // head outputs of every chunk, channels-last
+  bf16* enc_out = R.persist.take<bf16>((int64_t)Tl * nb * w * 2 * zc);  // head outputs of every chunk, channels-last
   int t_lat = 0;
   for (int f0 = 0; f0 < T && !R.rc;) {
     const int Tc = f0 == 0 ? 1 : 4;
     R.reset_scratch();
     int cap = 4;
-    Act x = R.scratch_act(Tc, H, Wd, c.dim);
-    // encoder.conv1: 3x3x3 causal with Cin = 3 straight from the planar video (its own past frames are the history)
-    R.small_conv("encoder.conv1", video, (size_t)T * H * Wd, (size_t)H * Wd, (size_t)Wd, 1, T, H, Wd, 3, /*t_base=*/f0 - 2, 3, 3, x.p, c.dim, Tc,
-                 c.dim);
-    int idx = 0;
-    for (const LayerSpec& l : layers) {
-      const std::string n = "encoder.downsamples." + std::to_string(idx++);
+    Act x = R.scratch_act(Tc, 8 * nb, Wd, c.dim);
+    // encoder.conv1: 3x3x3 causal with Cin = 3 straight from the planar video (its own past frames are the history).  Split: the
+    // band's pixel rows and the rows around it, read from the whole video from the row above the band on (zero padding only at the
+    // global top and bottom)
+    const int skip = R.band0 > 0 ? 8 * R.band0 - 1 : 0;
+    R.small_conv("encoder.conv1", at(video, (size_t)skip * Wd), (size_t)T * H * Wd, (size_t)H * Wd, (size_t)Wd, 1, T, H - skip, Wd, 3,
+                 /*t_base=*/f0 - 2, 3, 3, x.p, c.dim, Tc, 8 * nb, R.band0 > 0 ? 0 : 1, c.dim);
+    for (size_t li = 0; li < layers.size(); ++li) {
+      const LayerSpec& l = layers[li];
+      const std::string n = "encoder.downsamples." + std::to_string(li);
       if (l.res) {
-        x = R.res_block(n, x, l.cout, cap);
+        x = R.res_block(n, x, l.cout, cap, li + 1 < layers.size() && !layers[li + 1].res);
       } else {
         x = R.downsample(n, x, l.mode == 1, cap);
         if (l.mode == 1) cap = cap > 1 ? cap / 2 : 1;
@@ -383,13 +584,14 @@ int run_encode(Run& R, const bf16* video, bf16* mu, int T, int H, int Wd) {
     x = R.res_block("encoder.middle.0", x, top, cap);
     x = R.attn_block("encoder.middle.1", x);
     x = R.res_block("encoder.middle.2", x, top, cap);
-    StreamBuf& sh = R.stream("encoder.head.2", 2, cap, x.H, x.W, x.C);
+    StreamBuf& sh = R.stream("encoder.head.2", 2, cap, x.H, x.W, x.C, true);
     Act hin = R.chunk_of(sh, x.T);
-    R.rms(x, "encoder.head.0.gamma", hin.p, true);
+    R.rms_into(x, "encoder.head.0.gamma", sh, hin.p, true);
+    if (sh.halo) R.halo_exchange(hin.p, x.T, x.H, x.W, x.C);
     Act o;
     o.T = x.T; o.H = x.H; o.W = x.W; o.C = 2 * zc;
-    o.p = R.dry ? nullptr : enc_out + (size_t)t_lat * h * w * 2 * zc;
-    if (x.H != h || x.W != w) return fail(CE_ERR_INVALID, "vae encode: spatial size mismatch (H, W must be multiples of 8)");
+    o.p = R.dry ? nullptr : enc_out + (size_t)t_lat * nb * w * 2 * zc;
+    if (x.H != nb || x.W != w) return fail(CE_ERR_INVALID, "vae encode: spatial size mismatch (H, W must be multiples of 8)");
     R.causal_conv("encoder.head.2", sh, x.T, o, 3);
     t_lat += x.T;
     f0 += Tc;
@@ -397,11 +599,17 @@ int run_encode(Run& R, const bf16* video, bf16* mu, int T, int H, int Wd) {
   if (!R.rc && t_lat != Tl) return fail(CE_ERR_INVALID, "vae encode: produced frame count mismatch");
   // conv1 (1x1x1, 2z -> 2z) then keep the first z channels (posterior mean)
   R.reset_scratch();
-  const size_t P = (size_t)Tl * h * w;
+  const size_t P = (size_t)Tl * nb * w;
   bf16* q = reinterpret_cast<bf16*>(R.take_scratch_bytes(P * 2 * zc * 2));
   const bf16* w1 = R.weights.any<bf16>("conv1.weight", (int64_t)4 * zc * zc);
   R.gemm(enc_out, 2 * zc, w1, 2 * zc, (int)P, 2 * zc, 2 * zc, q, 2 * zc, R.weights.any<bf16>("conv1.bias", 2 * zc));
-  R.launch([&] { return launch_cl_to_planar(q, 2 * zc, mu, P, 2 * zc, R.s); });  // moments = mean | logvar
+  if (!R.split()) {
+    R.launch([&] { return launch_cl_to_planar(q, 2 * zc, mu, P, 2 * zc, R.s); });  // moments = mean | logvar
+    return R.rc;
+  }
+  bf16* band = reinterpret_cast<bf16*>(R.take_scratch_bytes(P * 2 * zc * 2));   // the band's moments, planar
+  R.launch([&] { return launch_cl_to_planar(q, 2 * zc, band, P, 2 * zc, R.s); });
+  for (int t = 0; t < Tl; ++t) R.gather_moments(band, mu, t, Tl, 2 * zc, w);
   return R.rc;
 }
 
@@ -413,6 +621,37 @@ int check_geometry(const ce_vae* h, int T, int H, int W, bool decode) {
     CE_REQUIRE(T >= 1 && (T - 1) % 4 == 0, "vae encode: frame count must be 1 + 4k (the reference fails otherwise)");
     CE_REQUIRE(H % 8 == 0 && W % 8 == 0 && H >= 8 && W >= 8, "vae encode: H, W must be multiples of 8");
   }
+  if (h->sp.world > 1) {
+    const int rows = decode ? H : H / 8;
+    if (rows < h->sp.world)
+      return fail(CE_ERR_INVALID, "vae sequence parallel: " + std::to_string(rows) + " latent rows cannot be split over " +
+                                      std::to_string(h->sp.world) + " ranks (at least one row per rank)");
+  }
+  return CE_OK;
+}
+
+int count_temporal(const ce_vae_config& c) { return (c.temporal_downsample[0] != 0) + (c.temporal_downsample[1] != 0) + (c.temporal_downsample[2] != 0); }
+
+// The peer region's layout for pixel geometry H x W.  The halo slot holds the largest halo row of any chunk: a planning pass of one
+// 4-frame encode chunk and of one decode chunk past the first (later chunks have the same shapes) measures it.
+int vae_sp_layout(ce_vae* h, int H, int W, int world, VaeSpLayout& L) {
+  const ce_vae_config& c = h->cfg;
+  const int lh = H / 8, lw = W / 8;
+  Run enc(h, nullptr, nullptr, nullptr, 0, world), dec(h, nullptr, nullptr, nullptr, 0, world);
+  CE_TRY(run_encode(enc, nullptr, nullptr, 5, H, W));
+  CE_TRY(run_decode(dec, nullptr, nullptr, 2, lh, lw, 0));
+  auto al = [](int64_t v) { return (v + 1023) & ~int64_t(1023); };
+  L = VaeSpLayout();
+  L.flags = 0;
+  L.halo = 1024;
+  L.halo_slot = al(std::max(enc.halo_row_max, dec.halo_row_max));
+  L.frame = L.halo + 4 * L.halo_slot;
+  L.frame_bytes = al((int64_t)up8(lh * lw) * top_dim(c) * 2);
+  L.video = L.frame + 2 * L.frame_bytes;
+  L.video_frames = 1 << count_temporal(c);
+  L.moments = L.video + al((int64_t)3 * L.video_frames * H * W * 2);
+  L.moments_bytes = al((int64_t)2 * c.z_dim * lh * lw * 2);
+  L.bytes = L.moments + 2 * L.moments_bytes;
   return CE_OK;
 }
 
@@ -440,7 +679,7 @@ int ce_vae_set_weight(ce_vae* h, const char* name, const void* ptr, int64_t nume
 
 int64_t ce_vae_workspace_bytes(ce_vae* h, int decode, int frames, int height, int width) {
   if (check_geometry(h, frames, height, width, decode != 0)) return -1;
-  Run plan(h, nullptr, nullptr, nullptr);
+  Run plan(h, nullptr, nullptr, nullptr, h->sp.rank, h->sp.world);
   int rc = decode ? run_decode(plan, nullptr, nullptr, frames, height, width, 0) : run_encode(plan, nullptr, nullptr, frames, height, width);
   return rc || plan.weights.rc ? -1 : plan.workspace_bytes();
 }
@@ -452,18 +691,37 @@ static int run(ce_vae* h, bool decode, const void* in, void* out, int frames, in
   if ((rc = check_geometry(h, frames, height, width, decode))) return rc;
   CE_REQUIRE(in && out && workspace, "vae: null argument");
   CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "vae: workspace must be 256-byte aligned");
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  VaeSpLayout lay;
+  if (h->sp.world > 1) {   // every refusal of the split comes before its first barrier
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CE_CHECK_CUDA(cudaStreamIsCapturing(s, &cs));
+    CE_REQUIRE(cs == cudaStreamCaptureStatusNone, "vae sequence parallel: the stream is capturing (the split VAE cannot be captured)");
+    const int H = decode ? 8 * height : height, W = decode ? 8 * width : width;
+    CE_TRY(vae_sp_layout(h, H, W, h->sp.world, lay));
+    if (lay.bytes > h->sp.region_bytes)
+      return fail(CE_ERR_WORKSPACE, "vae sequence parallel: a " + std::to_string(H) + " x " + std::to_string(W) + " call needs a peer region of " +
+                                        std::to_string(lay.bytes) + " bytes, the handle was configured with " +
+                                        std::to_string(h->sp.region_bytes) + " (ce_vae_sp_region_bytes)");
+  }
   // plan first: sizes of the persistent region (stream buffers) and of the per-chunk scratch
-  Run plan(h, nullptr, nullptr, nullptr);
+  Run plan(h, nullptr, nullptr, nullptr, h->sp.rank, h->sp.world);
   rc = decode ? run_decode(plan, nullptr, nullptr, frames, height, width, 0) : run_encode(plan, nullptr, nullptr, frames, height, width);
   if (rc || (rc = plan.weights.rc)) return rc;
   const int64_t need = plan.workspace_bytes();
   if (need > workspace_bytes)
     return fail(CE_ERR_WORKSPACE, "vae: workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(workspace_bytes));
   uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
-  Run R(h, reinterpret_cast<cudaStream_t>(stream), base, base + plan.persist.bytes());
+  Run R(h, s, base, base + plan.persist.bytes(), h->sp.rank, h->sp.world);
+  R.lay = &lay;
   h->launches = 0;
-  return decode ? run_decode(R, reinterpret_cast<const bf16*>(in), reinterpret_cast<bf16*>(out), frames, height, width, clamp)
-                : run_encode(R, reinterpret_cast<const bf16*>(in), reinterpret_cast<bf16*>(out), frames, height, width);
+  rc = decode ? run_decode(R, reinterpret_cast<const bf16*>(in), reinterpret_cast<bf16*>(out), frames, height, width, clamp)
+              : run_encode(R, reinterpret_cast<const bf16*>(in), reinterpret_cast<bf16*>(out), frames, height, width);
+  if (!rc && R.split()) {   // nobody stores into a peer's region (next call) before the peer has read it
+    R.barrier();
+    rc = R.rc;
+  }
+  return rc;
 }
 
 int ce_vae_encode(ce_vae* h, const void* video, void* mean, int frames, int height, int width, void* workspace, int64_t workspace_bytes,
@@ -477,6 +735,46 @@ int ce_vae_decode(ce_vae* h, const void* z, void* video, int latent_frames, int 
 }
 
 int64_t ce_vae_last_launch_count(const ce_vae* h) { return h ? h->launches : 0; }
+
+int64_t ce_vae_sp_region_bytes(ce_vae* h, int height, int width, int world) {
+  CE_REQUIRE(h, "ce_vae_sp_region_bytes: null handle");
+  CE_REQUIRE(world >= 2 && world <= 8, "ce_vae_sp_region_bytes: world must be 2 to 8");
+  CE_REQUIRE(height % 8 == 0 && width % 8 == 0 && height >= 8 && width >= 8, "ce_vae_sp_region_bytes: height, width must be multiples of 8");
+  if (height / 8 < world)
+    return fail(CE_ERR_INVALID, "ce_vae_sp_region_bytes: " + std::to_string(height / 8) + " latent rows cannot be split over " +
+                                    std::to_string(world) + " ranks (at least one row per rank)");
+  VaeSpLayout L;
+  CE_TRY(vae_sp_layout(h, height, width, world, L));
+  return L.bytes;
+}
+
+int ce_vae_sp_configure(ce_vae* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes) {
+  CE_REQUIRE(h, "ce_vae_sp_configure: null handle");
+  const int host_barrier_ms = h->sp.host_barrier_ms;
+  if (world == 1) {
+    h->sp = SeqPar();
+    h->sp.host_barrier_ms = host_barrier_ms;
+    return CE_OK;
+  }
+  CE_REQUIRE(world >= 2 && world <= 8 && rank >= 0 && rank < world && region_ptrs && region_bytes > 0, "ce_vae_sp_configure: arguments");
+  for (int w = 0; w < world; ++w)
+    CE_REQUIRE(region_ptrs[w] != nullptr && (reinterpret_cast<uintptr_t>(region_ptrs[w]) & 255) == 0,
+               "ce_vae_sp_configure: region pointers must be non-null and 256-byte aligned");
+  h->sp = SeqPar();
+  h->sp.host_barrier_ms = host_barrier_ms;
+  h->sp.rank = rank;
+  h->sp.world = world;
+  h->sp.region_bytes = region_bytes;
+  for (int w = 0; w < world; ++w) h->sp.region[w] = reinterpret_cast<uint8_t*>(region_ptrs[w]);
+  return CE_OK;
+}
+
+int ce_vae_sp_host_barrier(ce_vae* h, int timeout_ms) {
+  CE_REQUIRE(h && timeout_ms >= 0, "ce_vae_sp_host_barrier: arguments");
+  h->sp.host_barrier_ms = timeout_ms;
+  h->sp.host.reset();   // the next barrier joins the rendezvous afresh
+  return CE_OK;
+}
 
 // One implicit-GEMM convolution (parity tests / profiling).  Layouts as in conv.cuh.
 int ce_conv3d_cl_bf16(const void* x, int Tin, int Hin, int Win, int Cin, const void* w, const void* bias, int Cout, int kt, int kh, int kw, int st,

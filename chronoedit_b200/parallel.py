@@ -188,3 +188,97 @@ def disable_sequence_parallel(model) -> None:
     if st.get("own") is not None:
         L.ce_ipc_free(st["own"])
     model._sp_state = None
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# The VAE of one edit split over the ranks of a node (row bands, see include/chronoedit_b200.h, ce_vae_sp_*)
+# ----------------------------------------------------------------------------------------------------------------------
+def enable_vae_sequence_parallel(vae, height: int, width: int, group=None) -> int:
+    """Split `vae.encode` / `vae.decode` of ONE edit over the ranks of `group` (one process per GPU of a node) by horizontal bands of
+    rows: rank r owns latent rows [r h / world, (r + 1) h / world) and only the rows that cross the band edges (and the mid attention's
+    input) travel, by peer stores over NVLink into the other ranks' regions.  Called with the SAME full inputs on every rank, encode and
+    decode return the full result on every rank, bit-identical to the single-GPU call.
+
+    `height` x `width` is the edit's pixel geometry: one configuration serves the encode of any 1 + 4k frames at that size and the
+    decode of any latent frame count at height / 8 x width / 8.  Allocates this rank's peer region (ce_ipc_alloc), exchanges the CUDA
+    IPC handles through torch.distributed and configures the handle (ce_vae_sp_configure).  Returns the region size in bytes."""
+    import ctypes
+
+    from . import _lib
+    from ._lib import CEError, check
+
+    if not dist.is_initialized():
+        raise CEError("enable_vae_sequence_parallel needs an initialised torch.distributed process group (one process per GPU)")
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    L = _lib.lib()
+    disable_vae_sequence_parallel(vae)
+    if world == 1:
+        return 0
+    n = vae_sp_region_bytes(vae, height, width, world)
+    with torch.cuda.device(vae.device):
+        own = ctypes.c_void_p()
+        check(L.ce_ipc_alloc(n, ctypes.byref(own)))
+        hbuf = (ctypes.c_uint8 * 64)()
+        check(L.ce_ipc_get_handle(own, hbuf))
+        handles = [None] * world
+        dist.all_gather_object(handles, bytes(hbuf), group=group)
+        ptrs, opened = [], []
+        for w in range(world):
+            if w == rank:
+                ptrs.append(own.value)
+                continue
+            p = ctypes.c_void_p()
+            hb = (ctypes.c_uint8 * 64).from_buffer_copy(handles[w])
+            check(L.ce_ipc_open(hb, ctypes.byref(p)))
+            ptrs.append(p.value)
+            opened.append(p)
+        configure_vae_sequence_parallel(vae, rank, ptrs, n, {"own": own, "opened": opened, "group": group})
+    dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
+    return int(n)
+
+
+def vae_sp_region_bytes(vae, height: int, width: int, world: int) -> int:
+    """Bytes of the peer region every rank needs for pixel geometry height x width (ce_vae_sp_region_bytes)."""
+    from . import _lib
+    from ._lib import check
+
+    n = _lib.lib().ce_vae_sp_region_bytes(vae._ensure_handle(), height, width, world)
+    if n < 0:
+        check(int(n))
+    return int(n)
+
+
+def configure_vae_sequence_parallel(vae, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict) -> None:
+    """Hand rank `rank`'s table of peer-region addresses (one per rank, as seen from this process) to the VAE's C handle
+    (ce_vae_sp_configure).  `state` is kept as `vae._sp_state` and holds what disable_vae_sequence_parallel releases: the own region
+    under "own" (ce_ipc_free) and the opened peer mappings under "opened" (ce_ipc_close)."""
+    import ctypes
+
+    from . import _lib
+    from ._lib import check
+
+    world = len(region_ptrs)
+    table = (ctypes.c_void_p * world)(*region_ptrs)
+    with torch.cuda.device(vae.device):
+        check(_lib.lib().ce_vae_sp_configure(vae._ensure_handle(), rank, world, table, region_bytes))
+        torch.cuda.synchronize(vae.device)
+    vae._sp_state = dict(state, world=world, bytes=region_bytes)
+
+
+def disable_vae_sequence_parallel(vae) -> None:
+    """Back to the single-GPU VAE; releases what enable_vae_sequence_parallel allocated and opened."""
+    from . import _lib
+
+    st = getattr(vae, "_sp_state", None)
+    if not st:
+        return
+    L = _lib.lib()
+    torch.cuda.synchronize(vae.device)
+    L.ce_vae_sp_configure(vae._handle, 0, 1, None, 0)
+    for p in st.get("opened", ()):
+        L.ce_ipc_close(p)
+    if st.get("own") is not None:
+        if dist.is_initialized():
+            dist.barrier(group=st.get("group"))   # no peer still maps the region when it is freed
+        L.ce_ipc_free(st["own"])
+    vae._sp_state = None

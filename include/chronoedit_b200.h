@@ -212,6 +212,26 @@ int ce_vae_decode(ce_vae* h, const void* z, void* video, int latent_frames, int 
 int64_t ce_vae_last_launch_count(const ce_vae* h);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * The VAE split over the `world` ranks of a node (one process per GPU), for the latency of one edit: rank r encodes and
+ * decodes latent rows [r h / world, (r + 1) h / world) (and the matching rows at every resolution), exchanges only the rows
+ * that cross the band edges and the mid attention's input by peer stores into the other ranks' regions, and every rank
+ * returns the full result, bit-identical to the single-GPU call.  Call ce_vae_encode / ce_vae_decode with the same full
+ * inputs on every rank; ce_vae_workspace_bytes reports the band's need while the split is configured.
+ *   ce_vae_sp_region_bytes: bytes of the peer region every rank needs for pixel geometry height x width (multiples of 8, at
+ *     least `world` latent rows, world 2 to 8).  One region serves an encode of any 1 + 4k frames at height x width and a
+ *     decode of any latent frame count at height / 8 x width / 8, and any smaller geometry whose need fits; -1 on refusal.
+ *   ce_vae_sp_configure: region_ptrs[w] = rank w's region as seen from this process (ce_ipc_alloc / ce_ipc_open, 256-byte
+ *     aligned).  world = 1 switches the split off.
+ *   ce_vae_sp_host_barrier: as ce_dit_sp_host_barrier, for the VAE's barriers (a test aid: `world` handles of one process on
+ *     one GPU play the ranks).
+ * A call refuses, before any launch, fewer latent rows than ranks, a geometry whose need exceeds region_bytes and a capturing
+ * stream.
+ * ------------------------------------------------------------------------------------------------------------ */
+int64_t ce_vae_sp_region_bytes(ce_vae* h, int height, int width, int world);
+int ce_vae_sp_configure(ce_vae* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes);
+int ce_vae_sp_host_barrier(ce_vae* h, int timeout_ms);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Encoders in front of the loop (SURVEY.md section 8(f) row 3), once per edit:
  *   transformers.UMT5EncoderModel   -- pipeline_chronoedit.py:205-244  self.text_encoder(ids, mask).last_hidden_state
  *   transformers.CLIPVisionModel    -- pipeline_chronoedit.py:246-254  self.image_encoder(**image, output_hidden_states=True).hidden_states[-2]
