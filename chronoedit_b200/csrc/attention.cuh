@@ -24,7 +24,7 @@ struct AttnArgs {
   int ldo = 0;
   float scale = 0.f;        // 1/sqrt(head_dim)
   long long* timing = nullptr;  // optional [16] device counters: phase cycles of thread 128 of block (0,0,0) (profiling aid)
-  // sequence-parallel output scatter (csrc/seqpar.cu): when peer_rows > 0, query row i of sample b is stored at
+  // sequence-parallel output scatter (csrc/dit.cu): when peer_rows > 0, query row i of sample b is stored at
   //   out_peer[i / peer_rows] + ((b * peer_rows + i % peer_rows) * ldo + h * head_dim + out_col0)
   // i.e. straight into the attention-output buffer of the rank that owns that token (its own pointer or a peer's, NVLink).
   bf16* out_peer[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};

@@ -76,6 +76,32 @@ struct Workspace {
   int64_t bytes;
 };
 
+// Sequence parallelism (ce_dit_sp_configure): the tokens of one edit are split over the ranks, and the only exchange is around the
+// self-attention (heads <-> tokens, "Ulysses" layout, reference: chronoedit_diffsynth/wan_video_new_chronoedit.py:330-355,
+// 1448-1498).  The RMSNorm+RoPE kernel scatters q | k by head, a copy scatters v, the attention epilogue scatters the output rows back
+// to the ranks that own the tokens, and a copy all-gathers the head output.  Byte offsets inside a rank's peer region:
+struct SpLayout {
+  int64_t q, k, v;      // gathered q / k / v of the heads this rank owns: [B, L, D / world] bf16 each
+  int64_t attn;         // attention output of the tokens this rank owns: [B * L / world, D] bf16
+  int64_t yout;         // full head output [B * L, out_channels * 4] bf16 (every rank gets all of it)
+  int64_t flags;        // uint32 [8 * 32]
+  int64_t bytes;
+};
+
+SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world) {
+  auto al = [](int64_t v) { return (v + 1023) & ~int64_t(1023); };
+  SpLayout l;
+  const int64_t g = al(B * L * (D / world) * 2);
+  l.q = 0;
+  l.k = g;
+  l.v = 2 * g;
+  l.attn = 3 * g;
+  l.yout = l.attn + al(B * (L / world) * D * 2);
+  l.flags = l.yout + al(B * L * No * 2);
+  l.bytes = l.flags + 1024;
+  return l;
+}
+
 // Keys of the FP8 attention's V^T rows: L rounded up to the 32-key groups of its layout.
 int vt_keys(int L) { return (L + 31) / 32 * 32; }
 
@@ -447,32 +473,14 @@ int64_t ce_dit_sp_region_bytes(const ce_dit* h, int batch, int frames, int heigh
 
 int ce_dit_sp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes) {
   CE_REQUIRE(h, "ce_dit_sp_configure: null handle");
-  const int host_barrier_ms = h->sp.host_barrier_ms;
-  if (world <= 1) {
-    h->sp = SeqPar();
-    h->sp.host_barrier_ms = host_barrier_ms;
-    return CE_OK;
-  }
-  CE_REQUIRE(world <= 8 && rank >= 0 && rank < world && region_ptrs && region_bytes > 0, "ce_dit_sp_configure: arguments");
-  CE_REQUIRE(h->cfg.num_attention_heads % world == 0, "ce_dit_sp_configure: the head count must be divisible by the number of ranks");
-  h->sp = SeqPar();
-  h->sp.host_barrier_ms = host_barrier_ms;
-  h->sp.rank = rank;
-  h->sp.world = world;
-  h->sp.region_bytes = region_bytes;
-  for (int w = 0; w < world; ++w) {
-    CE_REQUIRE(region_ptrs[w] != nullptr, "ce_dit_sp_configure: null region pointer");
-    h->sp.region[w] = reinterpret_cast<uint8_t*>(region_ptrs[w]);
-  }
+  SeqPar sp = h->sp;
+  CE_TRY(sp_configure(sp, "ce_dit_sp_configure", rank, world, region_ptrs, region_bytes));
+  CE_REQUIRE(h->cfg.num_attention_heads % sp.world == 0, "ce_dit_sp_configure: the head count must be divisible by the number of ranks");
+  h->sp = sp;
   return CE_OK;
 }
 
-int ce_dit_sp_host_barrier(ce_dit* h, int timeout_ms) {
-  CE_REQUIRE(h && timeout_ms >= 0, "ce_dit_sp_host_barrier: arguments");
-  h->sp.host_barrier_ms = timeout_ms;
-  h->sp.host.reset();   // the next barrier joins the rendezvous afresh
-  return CE_OK;
-}
+int ce_dit_sp_host_barrier(ce_dit* h, int timeout_ms) { return sp_set_host_barrier(h ? &h->sp : nullptr, "ce_dit_sp_host_barrier", timeout_ms); }
 
 int ce_dit_set_capture(ce_dit* h, const int32_t* layers, void* const* dst, int n) {
   CE_REQUIRE(h && n >= 0 && (n == 0 || (layers && dst)), "ce_dit_set_capture: arguments");
@@ -609,8 +617,7 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   const float attn_scale = 1.0f / sqrtf((float)c.attention_head_dim);
 
   // ---- patch embedding (Conv3d k=s=(1,2,2) as im2row + GEMM, :429-430)
-  if (spx) LAUNCH(CAT_OTHER, 0.0, launch_patchify_range(reinterpret_cast<const bf16*>(hidden_states), ws.patches, B, c.in_channels, frames, height, width, tok0, L, s));
-  else LAUNCH(CAT_OTHER, 0.0, launch_patchify(reinterpret_cast<const bf16*>(hidden_states), ws.patches, B, c.in_channels, frames, height, width, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_patchify(reinterpret_cast<const bf16*>(hidden_states), ws.patches, B, c.in_channels, frames, height, width, tok0, L, s));
   if ((rc = linear(h, s, W.patch, ws.patches, M, D, Kp, ws.x, epi(EPI_BIAS, ws.stats_x, 1)))) return rc;
 
   // ---- condition embedder (:147-165)
@@ -650,15 +657,19 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
       const int Hl = H / sp.world, Dl = D / sp.world;
       SpScatter sc;
       sc.world = sp.world; sc.heads_per_rank = Hl; sc.L_total = Lfull; sc.rows_per_batch = L; sc.tok0 = tok0;
-      bf16* vdst[8];
+      SpCopy vj[8];   // v columns of rank w's heads into rows [tok0, tok0 + L) of every sample of its v buffer
       for (int w = 0; w < sp.world; ++w) {
         sc.dst[0][w] = reinterpret_cast<bf16*>(sp.region[w] + lay.q);
         sc.dst[1][w] = reinterpret_cast<bf16*>(sp.region[w] + lay.k);
-        vdst[w] = reinterpret_cast<bf16*>(sp.region[w] + lay.v);
+        vj[w].src = ws.qkv + 2 * D + w * Dl;
+        vj[w].dst = sp.region[w] + lay.v + (int64_t)tok0 * Dl * 2;
+        vj[w].bytes = Dl * 2;
+        vj[w].n0 = L; vj[w].sp0 = 3 * D * 2; vj[w].dp0 = Dl * 2;
+        vj[w].n1 = B; vj[w].sp1 = (int64_t)L * 3 * D * 2; vj[w].dp1 = (int64_t)Lfull * Dl * 2;
       }
       LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(ws.qkv, 3 * D, M, D, c.eps, lw.norm_q1, lw.norm_k1, 2, h->rope_cos, h->rope_sin, Lfull,
                                                  c.attention_head_dim, partials(ws.stats_qkv, 3 * tD), s, &sc));
-      LAUNCH(CAT_OTHER, 0.0, launch_sp_scatter_cols(ws.qkv + 2 * D, 3 * D, B, L, D, vdst, sp.world, Dl, Lfull, tok0, s));
+      LAUNCH(CAT_OTHER, 0.0, launch_sp_copy(vj, sp.world, s));
       LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay.flags, s));
       AttnArgs a;
       a.B = B; a.H = Hl; a.Lq = Lfull; a.Lk = Lfull;
@@ -749,9 +760,14 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, ws.modf + D, ws.modf, 2 * D, L, nullptr, nullptr, 1));
   if ((rc = linear(h, s, W.proj_out, ws.xn, M, No, D, ws.yout, epi(EPI_BIAS)))) return rc;
   if (spx) {   // every rank gets the whole head output (rows all-gathered by peer stores), then un-patchifies the full sample
-    bf16* ydst[8];
-    for (int w = 0; w < sp.world; ++w) ydst[w] = reinterpret_cast<bf16*>(sp.region[w] + lay.yout);
-    LAUNCH(CAT_OTHER, 0.0, launch_sp_broadcast_rows(ws.yout, B, L, No, ydst, sp.world, Lfull, tok0, s));
+    SpCopy yj[8];   // this rank's rows into rows [tok0, tok0 + L) of every sample of every rank's yout
+    for (int w = 0; w < sp.world; ++w) {
+      yj[w].src = ws.yout;
+      yj[w].dst = sp.region[w] + lay.yout + (int64_t)tok0 * No * 2;
+      yj[w].bytes = (int64_t)L * No * 2;
+      yj[w].n0 = B; yj[w].sp0 = (int64_t)L * No * 2; yj[w].dp0 = (int64_t)Lfull * No * 2;
+    }
+    LAUNCH(CAT_OTHER, 0.0, launch_sp_copy(yj, sp.world, s));
     LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay.flags, s));
     LAUNCH(CAT_OTHER, 0.0, launch_unpatchify(reinterpret_cast<const bf16*>(sp.region[sp.rank] + lay.yout), No, reinterpret_cast<bf16*>(sample), B,
                                              c.out_channels, frames, height, width, s));

@@ -277,17 +277,16 @@ void dispatch_row_kernel(int D, bool from_partials, Launch&& launch) {
 }
 
 // ---------------------------------------------------------------------------------------------
-__global__ void patchify_kernel(const bf16* __restrict__ x, bf16* __restrict__ patches, int B, int C, int T, int H, int W) {
+__global__ void patchify_kernel(const bf16* __restrict__ x, bf16* __restrict__ patches, int B, int C, int T, int H, int W, int tok0, int ntok) {
   const int hp = H >> 1, wp = W >> 1;
   const int K = C * 4;
-  const size_t total = (size_t)B * T * hp * wp * K;
+  const size_t total = (size_t)B * ntok * K;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int k = (int)(i % K);
-    size_t r = i / K;
-    const int j = (int)(r % wp); r /= wp;
-    const int ii = (int)(r % hp); r /= hp;
-    const int f = (int)(r % T);
-    const int b = (int)(r / T);
+    const size_t r = i / K;
+    const int tok = tok0 + (int)(r % ntok);
+    const int b = (int)(r / ntok);
+    const int j = tok % wp, ii = (tok / wp) % hp, f = tok / (wp * hp);
     const int c = k >> 2, dh = (k >> 1) & 1, dw = k & 1;
     patches[i] = x[((((size_t)b * C + c) * T + f) * H + (2 * ii + dh)) * W + (2 * j + dw)];
   }
@@ -659,11 +658,12 @@ int launch_rmsnorm_rope(bf16* x, int ldx, int rows, int D, float eps, const bf16
   return CE_OK;
 }
 
-int launch_patchify(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, cudaStream_t stream) {
+int launch_patchify(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, int tok0, int ntok, cudaStream_t stream) {
   CE_REQUIRE(H % 2 == 0 && W % 2 == 0, "patchify: H, W must be even");
-  const size_t total = (size_t)B * T * (H / 2) * (W / 2) * C * 4;
+  CE_REQUIRE(tok0 >= 0 && ntok > 0 && tok0 + ntok <= T * (H / 2) * (W / 2), "patchify: token range");
+  const size_t total = (size_t)B * ntok * C * 4;
   const int grid = (int)((total + 255) / 256 < device_sm_count() * 16 ? (total + 255) / 256 : device_sm_count() * 16);
-  patchify_kernel<<<grid, 256, 0, stream>>>(x, patches, B, C, T, H, W);
+  patchify_kernel<<<grid, 256, 0, stream>>>(x, patches, B, C, T, H, W, tok0, ntok);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }

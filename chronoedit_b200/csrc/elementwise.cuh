@@ -22,7 +22,7 @@ int launch_layernorm(const bf16* x, int ldx, bf16* y, int ldy, int rows, int D, 
                      int mod_stride, int rows_per_batch, const float* weight, const float* bias, int scale_is_1p, const RowPartials& ps,
                      cudaStream_t stream);
 
-// Sequence-parallel scatter of the normalised q | k (csrc/seqpar.cu): rows are the LOCAL tokens of this rank (rows_per_batch each,
+// Sequence-parallel scatter of the normalised q | k (csrc/dit.cu): rows are the LOCAL tokens of this rank (rows_per_batch each,
 // global token = tok0 + local index), RoPE uses the global token, and instead of being written back in place the vector of head h
 // goes to the rank that owns head h:  dst[mat][h / heads_per_rank] + ((b * L_total + token) * (heads_per_rank * head_dim)
 // + (h % heads_per_rank) * head_dim + offset inside the head).
@@ -74,8 +74,9 @@ int launch_softmax_rows(const float* S, int lds, bf16* P, int ldp, int rows, int
 // The fp32 validation forward's: P fp32 = softmax(s * scale) with expf.
 int launch_softmax_rows_f32(const float* S, int lds, float* P, int ldp, int rows, int cols, float scale, cudaStream_t stream);
 
-// patches[(b,f,i,j), c*4 + dh*2 + dw] = x[b, c, f, 2i+dh, 2j+dw]   (im2row for the k=s=(1,2,2) patch-embedding conv, :368,429-430)
-int launch_patchify(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, cudaStream_t stream);
+// patches[(b, tok - tok0), c*4 + dh*2 + dw] = x[b, c, f, 2i+dh, 2j+dw] for the tokens tok = (f, i, j) in [tok0, tok0 + ntok) of every
+// sample   (im2row for the k=s=(1,2,2) patch-embedding conv, :368,429-430; a token range for sequence parallelism)
+int launch_patchify(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, int tok0, int ntok, cudaStream_t stream);
 // out[b, c, f, 2i+dh, 2j+dw] = y[(b,f,i,j), (dh*2+dw)*C + c]       (unpatchify permute of :463-467)
 int launch_unpatchify(const bf16* y, int ldy, bf16* out, int B, int C, int T, int H, int W, cudaStream_t stream);
 

@@ -38,36 +38,6 @@ __global__ void sp_barrier_kernel(Ptrs8 flags, int rank, int world, uint32_t epo
   __threadfence_system();
 }
 
-__global__ void sp_scatter_cols_kernel(const bf16* __restrict__ src, int ld_src, int B, int rows_per_batch, int ncols, Ptrs8 dst, int cols_per_rank,
-                                       int dst_rows_per_batch, int dst_row0) {
-  const int nv = ncols / 8;
-  const size_t total = (size_t)B * rows_per_batch * nv;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i % nv) * 8;
-    const size_t r = i / nv;
-    const int li = (int)(r % rows_per_batch);
-    const int b = (int)(r / rows_per_batch);
-    const uint4 v = *reinterpret_cast<const uint4*>(src + r * ld_src + c);
-    bf16* d = reinterpret_cast<bf16*>(dst.p[c / cols_per_rank]) + ((size_t)b * dst_rows_per_batch + dst_row0 + li) * cols_per_rank + c % cols_per_rank;
-    *reinterpret_cast<uint4*>(d) = v;
-  }
-}
-
-__global__ void sp_broadcast_rows_kernel(const bf16* __restrict__ src, int B, int rows_per_batch, int ncols, Ptrs8 dst, int world, int dst_rows_per_batch,
-                                         int dst_row0) {
-  const int nv = ncols / 8;
-  const size_t total = (size_t)B * rows_per_batch * nv;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i % nv) * 8;
-    const size_t r = i / nv;
-    const int li = (int)(r % rows_per_batch);
-    const int b = (int)(r / rows_per_batch);
-    const uint4 v = *reinterpret_cast<const uint4*>(src + r * ncols + c);
-    for (int w = 0; w < world; ++w)
-      *reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(dst.p[w]) + ((size_t)b * dst_rows_per_batch + dst_row0 + li) * ncols + c) = v;
-  }
-}
-
 struct SpCopies {
   SpCopy c[8];
 };
@@ -87,36 +57,7 @@ __global__ void sp_copy_kernel(const __grid_constant__ SpCopies jobs) {
   }
 }
 
-__global__ void patchify_range_kernel(const bf16* __restrict__ x, bf16* __restrict__ patches, int B, int C, int T, int H, int W, int tok0, int ntok) {
-  const int hp = H >> 1, wp = W >> 1;
-  const int K = C * 4;
-  const size_t total = (size_t)B * ntok * K;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int k = (int)(i % K);
-    size_t r = i / K;
-    const int tok = tok0 + (int)(r % ntok);
-    const int b = (int)(r / ntok);
-    const int j = tok % wp, ii = (tok / wp) % hp, f = tok / (wp * hp);
-    const int c = k >> 2, dh = (k >> 1) & 1, dw = k & 1;
-    patches[i] = x[((((size_t)b * C + c) * T + f) * H + (2 * ii + dh)) * W + (2 * j + dw)];
-  }
-}
-
 }  // namespace
-
-SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world) {
-  auto al = [](int64_t v) { return (v + 1023) & ~int64_t(1023); };
-  SpLayout l;
-  const int64_t g = al(B * L * (D / world) * 2);
-  l.q = 0;
-  l.k = g;
-  l.v = 2 * g;
-  l.attn = 3 * g;
-  l.yout = l.attn + al(B * (L / world) * D * 2);
-  l.flags = l.yout + al(B * L * No * 2);
-  l.bytes = l.flags + 1024;
-  return l;
-}
 
 // The host barrier's rendezvous: one per region table (keyed on region[0]) among the handles of this process.
 struct HostRendezvous {
@@ -163,6 +104,31 @@ struct HostRendezvous {
   }
 };
 
+int sp_configure(SeqPar& sp, const char* who, int rank, int world, void* const* regions, int64_t bytes) {
+  SeqPar c;
+  c.host_barrier_ms = sp.host_barrier_ms;
+  if (world != 1) {
+    CE_REQUIRE(world >= 2 && world <= 8 && rank >= 0 && rank < world && regions && bytes > 0, std::string(who) + ": arguments");
+    for (int w = 0; w < world; ++w) {
+      CE_REQUIRE(regions[w] != nullptr && (reinterpret_cast<uintptr_t>(regions[w]) & 255) == 0,
+                 std::string(who) + ": null region pointer or one not 256-byte aligned");
+      c.region[w] = reinterpret_cast<uint8_t*>(regions[w]);
+    }
+    c.rank = rank;
+    c.world = world;
+    c.region_bytes = bytes;
+  }
+  sp = c;
+  return CE_OK;
+}
+
+int sp_set_host_barrier(SeqPar* sp, const char* who, int timeout_ms) {
+  CE_REQUIRE(sp && timeout_ms >= 0, std::string(who) + ": arguments");
+  sp->host_barrier_ms = timeout_ms;
+  sp->host.reset();   // the next barrier joins the rendezvous afresh
+  return CE_OK;
+}
+
 static int host_barrier(SeqPar& sp, cudaStream_t stream) {
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   CE_CHECK_CUDA(cudaStreamIsCapturing(stream, &cs));
@@ -195,28 +161,6 @@ int launch_sp_barrier(SeqPar& sp, int64_t flags, cudaStream_t stream) {
   return CE_OK;
 }
 
-int launch_sp_scatter_cols(const bf16* src, int ld_src, int B, int rows_per_batch, int ncols, bf16* const* dst, int world, int cols_per_rank,
-                           int dst_rows_per_batch, int dst_row0, cudaStream_t stream) {
-  CE_REQUIRE(ncols % 8 == 0 && cols_per_rank % 8 == 0 && ld_src % 8 == 0 && world <= 8 && cols_per_rank * world == ncols, "sp scatter: shapes");
-  Ptrs8 d;
-  for (int w = 0; w < 8; ++w) d.p[w] = w < world ? dst[w] : nullptr;
-  sp_scatter_cols_kernel<<<grid_for((size_t)B * rows_per_batch * ncols / 8), 256, 0, stream>>>(src, ld_src, B, rows_per_batch, ncols, d, cols_per_rank,
-                                                                                               dst_rows_per_batch, dst_row0);
-  CE_CHECK_CUDA(cudaGetLastError());
-  return CE_OK;
-}
-
-int launch_sp_broadcast_rows(const bf16* src, int B, int rows_per_batch, int ncols, bf16* const* dst, int world, int dst_rows_per_batch,
-                             int dst_row0, cudaStream_t stream) {
-  CE_REQUIRE(ncols % 8 == 0 && world <= 8, "sp broadcast: shapes");
-  Ptrs8 d;
-  for (int w = 0; w < 8; ++w) d.p[w] = w < world ? dst[w] : nullptr;
-  sp_broadcast_rows_kernel<<<grid_for((size_t)B * rows_per_batch * ncols / 8), 256, 0, stream>>>(src, B, rows_per_batch, ncols, d, world,
-                                                                                                 dst_rows_per_batch, dst_row0);
-  CE_CHECK_CUDA(cudaGetLastError());
-  return CE_OK;
-}
-
 int launch_sp_copy(const SpCopy* jobs, int n, cudaStream_t stream) {
   CE_REQUIRE(n >= 1 && n <= 8, "sp copy: 1 to 8 jobs");
   SpCopies c;
@@ -237,13 +181,6 @@ int launch_sp_copy(const SpCopy* jobs, int n, cudaStream_t stream) {
     sp_copy_kernel<uint4><<<grid, 256, 0, stream>>>(c);
   else
     sp_copy_kernel<uint16_t><<<grid, 256, 0, stream>>>(c);
-  CE_CHECK_CUDA(cudaGetLastError());
-  return CE_OK;
-}
-
-int launch_patchify_range(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, int tok0, int ntok, cudaStream_t stream) {
-  CE_REQUIRE(H % 2 == 0 && W % 2 == 0 && ntok > 0, "patchify(range): shapes");
-  patchify_range_kernel<<<grid_for((size_t)B * ntok * C * 4), 256, 0, stream>>>(x, patches, B, C, T, H, W, tok0, ntok);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }

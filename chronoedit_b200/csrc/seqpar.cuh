@@ -1,12 +1,12 @@
-// Sequence parallelism for single-edit latency (SURVEY.md section 8(f) row 2): the tokens of ONE edit are split over the ranks of
-// a node, every rank holds all weights, and the only exchange is around the self-attention (heads <-> tokens, "Ulysses" layout,
-// reference: chronoedit_diffsynth/wan_video_new_chronoedit.py:330-355, 1448-1498).  Here the exchange is not a collective call:
-// the kernels that PRODUCE the data store it straight into the consuming rank's memory over NVLink (peer pointers obtained with
-// CUDA IPC) -- the RMSNorm+RoPE kernel scatters q | k by head, a copy kernel scatters v, the attention epilogue scatters the
-// output rows back to the ranks that own the tokens -- and a flag barrier in peer memory orders the phases.
+// The peer group of a model split over the ranks of a node (SURVEY.md section 8(f) row 2): every rank holds all weights and a peer
+// region of the same layout, the kernels that produce exchanged data store it straight into the consuming rank's region over NVLink
+// (peer pointers obtained with CUDA IPC), and a flag barrier in peer memory orders the phases.  What is here serves every split
+// model: the handle's configuration, the barrier and a batched copy to local or peer memory.  The region layouts and the exchanges
+// that use them live with their model (sp_layout in dit.cu, vae_sp_layout in vae.cu).
 //
-// Test aid (ce_dit_sp_host_barrier): `world` handles of ONE process on ONE GPU can play the ranks, with ordinary device allocations
-// as regions.  The barrier is then a host rendezvous instead of the flag kernel, so no kernel ever waits for another rank's work.
+// Test aid (ce_dit_sp_host_barrier, ce_vae_sp_host_barrier): `world` handles of ONE process on ONE GPU can play the ranks, with
+// ordinary device allocations as regions.  The barrier is then a host rendezvous instead of the flag kernel, so no kernel ever waits
+// for another rank's work.
 #pragma once
 #include <memory>
 
@@ -26,14 +26,12 @@ struct SeqPar {
   std::shared_ptr<HostRendezvous> host;   // the rendezvous of this region table, joined at the first host barrier
 };
 
-struct SpLayout {   // byte offsets inside a rank's region
-  int64_t q, k, v;      // gathered q / k / v of the heads this rank owns: [B, L, D / world] bf16 each
-  int64_t attn;         // attention output of the tokens this rank owns: [B * L / world, D] bf16
-  int64_t yout;         // full head output [B * L, out_channels * 4] bf16 (every rank gets all of it)
-  int64_t flags;        // uint32 [8 * 32]
-  int64_t bytes;
-};
-SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world);
+// Configures `sp` for rank `rank` of `world` with one region pointer per rank.  world == 1 switches the split off; any other world
+// outside 2..8 is refused, and so is a null or not 256-byte aligned region pointer.  host_barrier_ms is kept.  A refusal names `who`
+// and leaves `sp` unchanged.
+int sp_configure(SeqPar& sp, const char* who, int rank, int world, void* const* regions, int64_t bytes);
+// timeout_ms > 0: launch_sp_barrier becomes the host rendezvous with that timeout; 0: the device barrier.  `sp` may be null (refused).
+int sp_set_host_barrier(SeqPar* sp, const char* who, int timeout_ms);
 
 // all ranks: everything this rank issued so far on `stream` (incl. its peer stores) is complete and visible before any rank continues.
 // The flags (uint32 [8 * 32]) lie at byte offset `flags` of every rank's region.
@@ -41,15 +39,9 @@ SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world);
 // threads (same process, same region[0]); a timeout is an error naming the rank and the barrier and poisons the group, so every
 // later barrier of it fails at once.  Refused while `stream` is capturing.
 int launch_sp_barrier(SeqPar& sp, int64_t flags, cudaStream_t stream);
-// dst[r] + ((b * dst_rows_per_batch + dst_row0 + i) * cols_per_rank + c % cols_per_rank) = src[(b * rows_per_batch + i) * ld_src + c],
-// r = c / cols_per_rank   (v scatter: columns to the rank that owns the head)
-int launch_sp_scatter_cols(const bf16* src, int ld_src, int B, int rows_per_batch, int ncols, bf16* const* dst, int world, int cols_per_rank,
-                           int dst_rows_per_batch, int dst_row0, cudaStream_t stream);
-// every rank r: dst[r] + ((b * dst_rows_per_batch + dst_row0 + i) * ncols + c) = src[(b * rows_per_batch + i) * ncols + c]   (all-gather of rows)
-int launch_sp_broadcast_rows(const bf16* src, int B, int rows_per_batch, int ncols, bf16* const* dst, int world, int dst_rows_per_batch,
-                             int dst_row0, cudaStream_t stream);
 // One launch of up to 8 strided copies, each to local or peer memory: for i1 < n1, i0 < n0, dst + i1 * dp1 + i0 * dp0 receives the `bytes`
-// bytes at src + i1 * sp1 + i0 * sp0 (byte offsets and sizes; bf16 data, so all of them even).  The VAE's band exchanges.
+// bytes at src + i1 * sp1 + i0 * sp0 (byte offsets and sizes; bf16 data, so all of them even).  16-byte copies when every address,
+// pitch and size of the launch is a multiple of 16.
 struct SpCopy {
   const void* src = nullptr;
   void* dst = nullptr;
@@ -58,7 +50,5 @@ struct SpCopy {
   int64_t sp0 = 0, sp1 = 0, dp0 = 0, dp1 = 0;
 };
 int launch_sp_copy(const SpCopy* jobs, int n, cudaStream_t stream);
-// patchify of a token range: patches[(b, i), k] for global tokens tok0 .. tok0 + ntok - 1 of every sample
-int launch_patchify_range(const bf16* x, bf16* patches, int B, int C, int T, int H, int W, int tok0, int ntok, cudaStream_t stream);
 
 }  // namespace ce

@@ -750,31 +750,10 @@ int64_t ce_vae_sp_region_bytes(ce_vae* h, int height, int width, int world) {
 
 int ce_vae_sp_configure(ce_vae* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes) {
   CE_REQUIRE(h, "ce_vae_sp_configure: null handle");
-  const int host_barrier_ms = h->sp.host_barrier_ms;
-  if (world == 1) {
-    h->sp = SeqPar();
-    h->sp.host_barrier_ms = host_barrier_ms;
-    return CE_OK;
-  }
-  CE_REQUIRE(world >= 2 && world <= 8 && rank >= 0 && rank < world && region_ptrs && region_bytes > 0, "ce_vae_sp_configure: arguments");
-  for (int w = 0; w < world; ++w)
-    CE_REQUIRE(region_ptrs[w] != nullptr && (reinterpret_cast<uintptr_t>(region_ptrs[w]) & 255) == 0,
-               "ce_vae_sp_configure: region pointers must be non-null and 256-byte aligned");
-  h->sp = SeqPar();
-  h->sp.host_barrier_ms = host_barrier_ms;
-  h->sp.rank = rank;
-  h->sp.world = world;
-  h->sp.region_bytes = region_bytes;
-  for (int w = 0; w < world; ++w) h->sp.region[w] = reinterpret_cast<uint8_t*>(region_ptrs[w]);
-  return CE_OK;
+  return sp_configure(h->sp, "ce_vae_sp_configure", rank, world, region_ptrs, region_bytes);
 }
 
-int ce_vae_sp_host_barrier(ce_vae* h, int timeout_ms) {
-  CE_REQUIRE(h && timeout_ms >= 0, "ce_vae_sp_host_barrier: arguments");
-  h->sp.host_barrier_ms = timeout_ms;
-  h->sp.host.reset();   // the next barrier joins the rendezvous afresh
-  return CE_OK;
-}
+int ce_vae_sp_host_barrier(ce_vae* h, int timeout_ms) { return sp_set_host_barrier(h ? &h->sp : nullptr, "ce_vae_sp_host_barrier", timeout_ms); }
 
 // One implicit-GEMM convolution (parity tests / profiling).  Layouts as in conv.cuh.
 int ce_conv3d_cl_bf16(const void* x, int Tin, int Hin, int Win, int Cin, const void* w, const void* bias, int Cout, int kt, int kh, int kw, int st,

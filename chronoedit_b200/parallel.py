@@ -91,6 +91,75 @@ def gather_objects(local: Sequence, dst: int = 0):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# The peer group of a split model: one region per rank, opened by every other rank through CUDA IPC (csrc/seqpar.cuh)
+# ----------------------------------------------------------------------------------------------------------------------
+def _open_peer_regions(n: int, group) -> tuple:
+    """Allocates this rank's peer region of `n` bytes (ce_ipc_alloc), all-gathers the 64-byte CUDA IPC handles over `group` (plumbing
+    only) and opens the other ranks' regions.  Returns the pointer table (one address per rank, as seen from this process) and the
+    state _release_peer_regions frees."""
+    import ctypes
+
+    from . import _lib
+    from ._lib import check
+
+    L = _lib.lib()
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    own = ctypes.c_void_p()
+    check(L.ce_ipc_alloc(n, ctypes.byref(own)))
+    hbuf = (ctypes.c_uint8 * 64)()
+    check(L.ce_ipc_get_handle(own, hbuf))
+    handles = [None] * world
+    dist.all_gather_object(handles, bytes(hbuf), group=group)
+    ptrs, opened = [], []
+    for w in range(world):
+        if w == rank:
+            ptrs.append(own.value)
+            continue
+        p = ctypes.c_void_p()
+        hb = (ctypes.c_uint8 * 64).from_buffer_copy(handles[w])
+        check(L.ce_ipc_open(hb, ctypes.byref(p)))
+        ptrs.append(p.value)
+        opened.append(p)
+    return ptrs, {"own": own, "opened": opened, "group": group}
+
+
+def _configure_peer_regions(obj, entry: str, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict) -> None:
+    """Hands the pointer table to the C configure `entry` of obj's handle and keeps `state` as obj._sp_state, with "world" and "bytes"
+    added."""
+    import ctypes
+
+    from . import _lib
+    from ._lib import check
+
+    world = len(region_ptrs)
+    table = (ctypes.c_void_p * world)(*region_ptrs)
+    with torch.cuda.device(obj.device):
+        check(getattr(_lib.lib(), entry)(obj._ensure_handle(), rank, world, table, region_bytes))
+        torch.cuda.synchronize(obj.device)
+    obj._sp_state = dict(state, world=world, bytes=region_bytes)
+
+
+def _release_peer_regions(obj, entry: str) -> None:
+    """Switches obj's handle back to one GPU (C configure `entry`, world 1), closes the opened peer mappings and frees the own region
+    once no rank of the state's group still maps it."""
+    from . import _lib
+
+    st = getattr(obj, "_sp_state", None)
+    if not st:
+        return
+    L = _lib.lib()
+    torch.cuda.synchronize(obj.device)
+    getattr(L, entry)(obj._handle, 0, 1, None, 0)
+    for p in st.get("opened", ()):
+        L.ce_ipc_close(p)
+    if st.get("own") is not None:
+        if dist.is_initialized():
+            dist.barrier(group=st.get("group"))
+        L.ce_ipc_free(st["own"])
+    obj._sp_state = None
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # Sequence parallelism for single-edit latency (SURVEY.md section 8(f) row 2)
 # ----------------------------------------------------------------------------------------------------------------------
 def enable_sequence_parallel(model, batch: int, frames: int, height: int, width: int, group=None) -> int:
@@ -103,37 +172,18 @@ def enable_sequence_parallel(model, batch: int, frames: int, height: int, width:
     rank -- computes 1/world of the tokens per rank, exchanges q/k/v and the attention output by peer stores over NVLink inside the
     kernels (no collective call on the data path), and returns the same full sample on every rank, bit-identical to the single-GPU
     forward.  Geometry-specific: call again for another latent shape.  Returns the region size in bytes."""
-    import ctypes
-
-    from . import _lib
-    from ._lib import CEError, check
+    from ._lib import CEError
 
     if not dist.is_initialized():
         raise CEError("enable_sequence_parallel needs an initialised torch.distributed process group (one process per GPU)")
-    rank, world = dist.get_rank(group), dist.get_world_size(group)
-    L = _lib.lib()
     disable_sequence_parallel(model)
+    world = dist.get_world_size(group)
     if world == 1:
         return 0
     n = sp_region_bytes(model, batch, frames, height, width, world)
     with torch.cuda.device(model.device):
-        own = ctypes.c_void_p()
-        check(L.ce_ipc_alloc(n, ctypes.byref(own)))
-        hbuf = (ctypes.c_uint8 * 64)()
-        check(L.ce_ipc_get_handle(own, hbuf))
-        handles = [None] * world
-        dist.all_gather_object(handles, bytes(hbuf), group=group)
-        ptrs, opened = [], []
-        for w in range(world):
-            if w == rank:
-                ptrs.append(own.value)
-                continue
-            p = ctypes.c_void_p()
-            hb = (ctypes.c_uint8 * 64).from_buffer_copy(handles[w])
-            check(L.ce_ipc_open(hb, ctypes.byref(p)))
-            ptrs.append(p.value)
-            opened.append(p)
-        configure_sequence_parallel(model, rank, ptrs, n, {"own": own, "opened": opened})
+        ptrs, state = _open_peer_regions(n, group)
+        configure_sequence_parallel(model, dist.get_rank(group), ptrs, n, state)
     dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
     return int(n)
 
@@ -154,40 +204,17 @@ def sp_region_bytes(model, batch: int, frames: int, height: int, width: int, wor
 def configure_sequence_parallel(model, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict) -> None:
     """Hand rank `rank`'s table of peer-region addresses (one per rank, as seen from this process) to the model's C handle
     (ce_dit_sp_configure) and switch the model into sequence-parallel mode.  `state` is kept as `model._sp_state` (with "world" and
-    "bytes" added) and holds whatever disable_sequence_parallel releases: the own region under "own" (freed with ce_ipc_free) and the
-    opened peer mappings under "opened" (closed with ce_ipc_close)."""
-    import ctypes
-
-    from . import _lib
-    from ._lib import check
-
+    "bytes" added) and holds whatever disable_sequence_parallel releases: the own region under "own" (freed with ce_ipc_free, after a
+    barrier on the process group under "group") and the opened peer mappings under "opened" (closed with ce_ipc_close)."""
     if not model._packed:
         model.pack_weights()
-    world = len(region_ptrs)
-    table = (ctypes.c_void_p * world)(*region_ptrs)
-    with torch.cuda.device(model.device):
-        check(_lib.lib().ce_dit_sp_configure(model._handle, rank, world, table, region_bytes))
-        torch.cuda.synchronize(model.device)
-    model._sp_state = dict(state, world=world, bytes=region_bytes)
+    _configure_peer_regions(model, "ce_dit_sp_configure", rank, region_ptrs, region_bytes, state)
     model._graphs = {}
 
 
 def disable_sequence_parallel(model) -> None:
-    from . import _lib
-
-    st = getattr(model, "_sp_state", None)
-    if not st:
-        return
-    L = _lib.lib()
-    torch.cuda.synchronize(model.device)
-    L.ce_dit_sp_configure(model._handle, 0, 1, None, 0)
-    for p in st.get("opened", ()):
-        L.ce_ipc_close(p)
-    if dist.is_initialized():
-        dist.barrier()
-    if st.get("own") is not None:
-        L.ce_ipc_free(st["own"])
-    model._sp_state = None
+    """Back to the single-GPU forward; releases what enable_sequence_parallel allocated and opened."""
+    _release_peer_regions(model, "ce_dit_sp_configure")
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -202,37 +229,18 @@ def enable_vae_sequence_parallel(vae, height: int, width: int, group=None) -> in
     `height` x `width` is the edit's pixel geometry: one configuration serves the encode of any 1 + 4k frames at that size and the
     decode of any latent frame count at height / 8 x width / 8.  Allocates this rank's peer region (ce_ipc_alloc), exchanges the CUDA
     IPC handles through torch.distributed and configures the handle (ce_vae_sp_configure).  Returns the region size in bytes."""
-    import ctypes
-
-    from . import _lib
-    from ._lib import CEError, check
+    from ._lib import CEError
 
     if not dist.is_initialized():
         raise CEError("enable_vae_sequence_parallel needs an initialised torch.distributed process group (one process per GPU)")
-    rank, world = dist.get_rank(group), dist.get_world_size(group)
-    L = _lib.lib()
     disable_vae_sequence_parallel(vae)
+    world = dist.get_world_size(group)
     if world == 1:
         return 0
     n = vae_sp_region_bytes(vae, height, width, world)
     with torch.cuda.device(vae.device):
-        own = ctypes.c_void_p()
-        check(L.ce_ipc_alloc(n, ctypes.byref(own)))
-        hbuf = (ctypes.c_uint8 * 64)()
-        check(L.ce_ipc_get_handle(own, hbuf))
-        handles = [None] * world
-        dist.all_gather_object(handles, bytes(hbuf), group=group)
-        ptrs, opened = [], []
-        for w in range(world):
-            if w == rank:
-                ptrs.append(own.value)
-                continue
-            p = ctypes.c_void_p()
-            hb = (ctypes.c_uint8 * 64).from_buffer_copy(handles[w])
-            check(L.ce_ipc_open(hb, ctypes.byref(p)))
-            ptrs.append(p.value)
-            opened.append(p)
-        configure_vae_sequence_parallel(vae, rank, ptrs, n, {"own": own, "opened": opened, "group": group})
+        ptrs, state = _open_peer_regions(n, group)
+        configure_vae_sequence_parallel(vae, dist.get_rank(group), ptrs, n, state)
     dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
     return int(n)
 
@@ -251,34 +259,11 @@ def vae_sp_region_bytes(vae, height: int, width: int, world: int) -> int:
 def configure_vae_sequence_parallel(vae, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict) -> None:
     """Hand rank `rank`'s table of peer-region addresses (one per rank, as seen from this process) to the VAE's C handle
     (ce_vae_sp_configure).  `state` is kept as `vae._sp_state` and holds what disable_vae_sequence_parallel releases: the own region
-    under "own" (ce_ipc_free) and the opened peer mappings under "opened" (ce_ipc_close)."""
-    import ctypes
-
-    from . import _lib
-    from ._lib import check
-
-    world = len(region_ptrs)
-    table = (ctypes.c_void_p * world)(*region_ptrs)
-    with torch.cuda.device(vae.device):
-        check(_lib.lib().ce_vae_sp_configure(vae._ensure_handle(), rank, world, table, region_bytes))
-        torch.cuda.synchronize(vae.device)
-    vae._sp_state = dict(state, world=world, bytes=region_bytes)
+    under "own" (ce_ipc_free, after a barrier on the process group under "group") and the opened peer mappings under "opened"
+    (ce_ipc_close)."""
+    _configure_peer_regions(vae, "ce_vae_sp_configure", rank, region_ptrs, region_bytes, state)
 
 
 def disable_vae_sequence_parallel(vae) -> None:
     """Back to the single-GPU VAE; releases what enable_vae_sequence_parallel allocated and opened."""
-    from . import _lib
-
-    st = getattr(vae, "_sp_state", None)
-    if not st:
-        return
-    L = _lib.lib()
-    torch.cuda.synchronize(vae.device)
-    L.ce_vae_sp_configure(vae._handle, 0, 1, None, 0)
-    for p in st.get("opened", ()):
-        L.ce_ipc_close(p)
-    if st.get("own") is not None:
-        if dist.is_initialized():
-            dist.barrier(group=st.get("group"))   # no peer still maps the region when it is freed
-        L.ce_ipc_free(st["own"])
-    vae._sp_state = None
+    _release_peer_regions(vae, "ce_vae_sp_configure")

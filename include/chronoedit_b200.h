@@ -121,7 +121,8 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
  * memory.  Every rank passes the SAME full inputs and receives the same full sample, bit-identical to the single-GPU forward.
  *   region: one device buffer of ce_dit_sp_region_bytes(...) per rank, allocated with ce_ipc_alloc (zeroed), shared with the peers
  *   through ce_ipc_get_handle / ce_ipc_open (CUDA IPC; the 64-byte handles travel by any host channel, e.g. torch.distributed);
- *   region_ptrs[w] = address of rank w's region in THIS process.  world = 1 switches it off.
+ *   region_ptrs[w] = address of rank w's region in THIS process (non-null, 256-byte aligned).  world = 1 switches it off; any
+ *   other world outside 2..8 is refused, and so is a head count that world does not divide.
  * ------------------------------------------------------------------------------------------------------------ */
 int64_t ce_dit_sp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width, int world);
 int ce_dit_sp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes);
@@ -221,7 +222,7 @@ int64_t ce_vae_last_launch_count(const ce_vae* h);
  *     least `world` latent rows, world 2 to 8).  One region serves an encode of any 1 + 4k frames at height x width and a
  *     decode of any latent frame count at height / 8 x width / 8, and any smaller geometry whose need fits; -1 on refusal.
  *   ce_vae_sp_configure: region_ptrs[w] = rank w's region as seen from this process (ce_ipc_alloc / ce_ipc_open, 256-byte
- *     aligned).  world = 1 switches the split off.
+ *     aligned).  world = 1 switches the split off; any other world outside 2..8 is refused.
  *   ce_vae_sp_host_barrier: as ce_dit_sp_host_barrier, for the VAE's barriers (a test aid: `world` handles of one process on
  *     one GPU play the ranks).
  * A call refuses, before any launch, fewer latent rows than ranks, a geometry whose need exceeds region_bytes and a capturing

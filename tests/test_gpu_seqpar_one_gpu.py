@@ -11,23 +11,18 @@ q / k / v / attention / head-output buffers keep a byte pattern); the inputs are
 launch are checked under the host barrier too, so a regression fails with a timeout message instead of reaching a device barrier.
 
 tests/test_gpu_seqpar.py keeps what only several GPUs can show: the device flag barrier, CUDA IPC and NVLink peer stores."""
-import gc
-import threading
 import time
 
 import pytest
 import torch
 
-gpu = pytest.mark.gpu
+from tests.sp_one_gpu import BARRIER_MS, SHORT_MS, _clean_device, assert_pattern_kept, guarded_regions, run_ranks  # noqa: F401
 
-GUARD = 64 << 10        # bytes of pattern after every region
-PATTERN = 0xA5
-BARRIER_MS = 60000      # host barrier timeout of the bit-equality runs
-SHORT_MS = 2000         # of the refusal tests: a refusal that regressed times out at the first barrier
+gpu = pytest.mark.gpu
 
 
 def sp_layout(B, L, D, No, world):
-    """Python restatement of sp_layout (csrc/seqpar.cu): byte offsets of a rank's peer region for B samples of L tokens, width D and
+    """Python restatement of sp_layout (csrc/dit.cu): byte offsets of a rank's peer region for B samples of L tokens, width D and
     No = out_channels * 4 head outputs.  Sub-buffers start at multiples of 1024 bytes; the flags block (uint32 [8 * 32]) ends it."""
     al = lambda v: (v + 1023) & ~1023
     qkv = B * L * (D // world) * 2          # q, k, v: [B, L, D / world] bf16 each
@@ -88,34 +83,6 @@ def _mirrors(first, world):
     return out
 
 
-def _run_ranks(models, args, timeout=600):
-    """model(*args) on every model at once, each from its own thread on its own stream; returns the samples.  A thread's exception is
-    raised here."""
-    torch.cuda.synchronize()
-    outs, errs = [None] * len(models), [None] * len(models)
-
-    def work(r):
-        try:
-            s = torch.cuda.Stream()
-            with torch.cuda.stream(s):
-                outs[r] = models[r](*args, return_dict=False)[0]
-            s.synchronize()
-        except BaseException as e:   # noqa: BLE001 -- re-raised in the test's thread
-            errs[r] = e
-
-    threads = [threading.Thread(target=work, args=(r,), daemon=True, name=f"sp-rank-{r}") for r in range(len(models))]
-    for t in threads:
-        t.start()
-    for t in threads:
-        t.join(timeout)
-    stuck = [t.name for t in threads if t.is_alive()]
-    assert not stuck, f"rank threads still running after {timeout} s: {stuck}"
-    for r, e in enumerate(errs):
-        if e is not None:
-            raise AssertionError(f"rank {r} failed: {e!r}") from e
-    return outs
-
-
 def _rank_diffs(out, ref, world):
     """Largest |out - ref| over the sample positions of each rank's tokens (rank r owns tokens [r L / world, (r + 1) L / world))."""
     _, _, T, H, W = ref.shape
@@ -144,7 +111,7 @@ def _sequence_parallel_matches_single(models, steps, latent, world, oracle_check
     n = parallel.sp_region_bytes(m0, B, T, H, W, world)
     lay = sp_layout(B, T * (H // 2) * (W // 2), m0.config.num_attention_heads * 128, m0.config.out_channels * 4, world)
     assert lay["bytes"] == n
-    regions = [torch.full((n + GUARD,), PATTERN, dtype=torch.uint8, device=m0.device) for _ in range(world)]
+    regions = guarded_regions(n, world, m0.device)
     ptrs = [r.data_ptr() for r in regions]
     from chronoedit_b200 import _lib
 
@@ -154,7 +121,7 @@ def _sequence_parallel_matches_single(models, steps, latent, world, oracle_check
             parallel.configure_sequence_parallel(m, r, ptrs, n, {})
         bad = []
         for it, st in enumerate(steps):
-            outs = _run_ranks(models, st)
+            outs = run_ranks(lambda r: models[r](*st, return_dict=False)[0], world, timeout=600)
             torch.cuda.synchronize()
             for r, o in enumerate(outs):
                 if not torch.equal(o, refs[it]):
@@ -164,10 +131,7 @@ def _sequence_parallel_matches_single(models, steps, latent, world, oracle_check
         for m in models:
             parallel.disable_sequence_parallel(m)
     torch.cuda.synchronize()
-    for r, region in enumerate(regions):
-        for what, a, b in sp_unwritten_ranges(lay) + [("guard band", n, n + GUARD)]:
-            hit = (region[a:b] != PATTERN).nonzero()
-            assert hit.numel() == 0, f"rank {r}'s region: {hit.numel()} bytes of its {what} [{a}, {b}) were written (first at {a + int(hit[0])})"
+    assert_pattern_kept(regions, n, sp_unwritten_ranges(lay))
     for m in models:   # every handle is back on the single-GPU forward
         assert torch.equal(m(*steps[0], return_dict=False)[0], refs[0])
     for st, before in zip(steps, inputs):
@@ -199,20 +163,6 @@ CASES = [
     ("14b_width", 40, 1, 13824, (2, 32, 40), 2, (2, 4, 8)),  # 20 / 10 / 5 heads per rank, 80 rows per rank at world 8
     ("flagship_tokens", 40, 1, 13824, (8, 90, 160), 2, (2,)),  # 28 800 tokens: the geometry of scripts/bench_seqpar.py
 ]
-
-
-@pytest.fixture
-def _clean_device():
-    torch.cuda.synchronize()
-    gc.collect()
-    torch.cuda.empty_cache()
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    yield
-    torch.cuda.synchronize()
-    print(f"  [{time.perf_counter() - t0:.1f} s, peak {torch.cuda.max_memory_reserved() / 2**30:.2f} GiB reserved]", flush=True)
-    gc.collect()
-    torch.cuda.empty_cache()
 
 
 @gpu

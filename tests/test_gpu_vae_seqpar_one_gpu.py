@@ -7,24 +7,18 @@ Asserted per case: every rank's encode moments and decode video are bit-identica
 under one configuration; the guard band after each region and its barrier flags (only the device barrier writes them) keep their byte
 pattern; the inputs are unchanged; after disabling the split each handle gives the single-GPU bits again.
 
-tests/test_gpu_vae_seqpar.py keeps what only several GPUs can show: the device flag barrier, CUDA IPC and NVLink peer stores."""
-import gc
+tests/test_gpu_seqpar.py keeps what only several GPUs can show: the device flag barrier, CUDA IPC and NVLink peer stores."""
 import os
-import threading
 import time
 
 import pytest
 import torch
 
 from oracle.vae_oracle import VAEConfig
+from tests.sp_one_gpu import BARRIER_MS, SHORT_MS, _clean_device, assert_pattern_kept, guarded_regions, run_ranks  # noqa: F401
 from tests.test_vae_seqpar_cpu import vae_sp_layout
 
 gpu = pytest.mark.gpu
-
-GUARD = 64 << 10
-PATTERN = 0xA5
-BARRIER_MS = 60000
-SHORT_MS = 2000
 
 
 def _vae(cfg, seed, dev, sd=None):
@@ -67,32 +61,6 @@ def _call(vae, call):
     return vae.decode(x, return_dict=False)[0]
 
 
-def _run_ranks(vaes, call, timeout=900):
-    torch.cuda.synchronize()
-    outs, errs = [None] * len(vaes), [None] * len(vaes)
-
-    def work(r):
-        try:
-            s = torch.cuda.Stream()
-            with torch.cuda.stream(s):
-                outs[r] = _call(vaes[r], call)
-            s.synchronize()
-        except BaseException as e:   # noqa: BLE001 -- re-raised in the test's thread
-            errs[r] = e
-
-    threads = [threading.Thread(target=work, args=(r,), daemon=True, name=f"vae-rank-{r}") for r in range(len(vaes))]
-    for t in threads:
-        t.start()
-    for t in threads:
-        t.join(timeout)
-    stuck = [t.name for t in threads if t.is_alive()]
-    assert not stuck, f"rank threads still running after {timeout} s: {stuck}"
-    for r, e in enumerate(errs):
-        if e is not None:
-            raise AssertionError(f"rank {r} failed: {e!r}") from e
-    return outs
-
-
 def _row_diffs(out, ref):
     d = (out.float() - ref.float()).abs()
     rows = d.amax(dim=tuple(i for i in range(d.dim()) if i != d.dim() - 2))
@@ -115,14 +83,14 @@ def _split_matches_single(vaes, H, W, calls, world, refs=None):
     cfg = VAEConfig(dim=c.base_dim, z_dim=c.z_dim, dim_mult=tuple(c.dim_mult), num_res_blocks=c.num_res_blocks,
                     temperal_downsample=tuple(c.temperal_downsample))
     assert vae_sp_layout(cfg, H, W)["bytes"] == n
-    regions = [torch.full((n + GUARD,), PATTERN, dtype=torch.uint8, device=v0.device) for _ in range(world)]
+    regions = guarded_regions(n, world, v0.device)
     try:
         for r, v in enumerate(vaes):
             _lib.check(_lib.lib().ce_vae_sp_host_barrier(v._ensure_handle(), BARRIER_MS))
             parallel.configure_vae_sequence_parallel(v, r, [g.data_ptr() for g in regions], n, {})
         bad = []
         for i, call in enumerate(calls):
-            outs = _run_ranks(vaes, call)
+            outs = run_ranks(lambda r: _call(vaes[r], call), world, timeout=900)
             torch.cuda.synchronize()
             for r, o in enumerate(outs):
                 if not torch.equal(o, refs[i]):
@@ -133,10 +101,7 @@ def _split_matches_single(vaes, H, W, calls, world, refs=None):
             parallel.disable_vae_sequence_parallel(v)
             _lib.lib().ce_vae_sp_host_barrier(v._handle, 0)
     torch.cuda.synchronize()
-    for r, region in enumerate(regions):
-        for what, a, b in (("barrier flags", 0, 1024), ("guard band", n, n + GUARD)):
-            hit = (region[a:b] != PATTERN).nonzero()
-            assert hit.numel() == 0, f"rank {r}'s region: {hit.numel()} bytes of its {what} [{a}, {b}) were written"
+    assert_pattern_kept(regions, n, [("barrier flags", 0, 1024)])
     for v in vaes:   # every handle is back on the single-GPU call
         assert torch.equal(_call(v, calls[0]), refs[0])
     for c, before in zip(calls, inputs):
@@ -159,20 +124,6 @@ def _calls(cfg, H, W, dev, seed, enc_frames=(5, 9), dec_frames=(2, 3)):
     h, w = H // 8, W // 8
     return [("enc", _video(enc_frames[0], H, W, dev, seed), False), ("dec", _latent(cfg.z_dim, dec_frames[0], h, w, dev, seed + 1), False),
             ("dec", 2.5 * _latent(cfg.z_dim, dec_frames[1], h, w, dev, seed + 2), True), ("enc", _video(enc_frames[1], H, W, dev, seed + 3), False)]
-
-
-@pytest.fixture
-def _clean_device():
-    torch.cuda.synchronize()
-    gc.collect()
-    torch.cuda.empty_cache()
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    yield
-    torch.cuda.synchronize()
-    print(f"  [{time.perf_counter() - t0:.1f} s, peak {torch.cuda.max_memory_reserved() / 2**30:.2f} GiB reserved]", flush=True)
-    gc.collect()
-    torch.cuda.empty_cache()
 
 
 # (name, config, H, W, worlds): latent rows h = H / 8 split over the ranks

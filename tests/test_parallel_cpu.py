@@ -1,6 +1,7 @@
 """world_size-2 gloo test (CPU) of the N>1 path: edit sharding and the one-time weight broadcast."""
 import os
 import socket
+import types
 
 import pytest
 import torch
@@ -137,15 +138,16 @@ def test_sp_region_bytes_refusals():
     assert L.ce_dit_sp_region_bytes(h3, 1, 2, 24, 32, 3) > 0
 
 
-def test_sp_configure_refusals():
+def test_sp_configure_refusals_with_aligned_regions():
+    """The DiT's configure refuses what the VAE's does (world outside 1..8, rank, table, size, null or not 256-byte aligned region)
+    and a head count the world does not divide; it accepts 256-byte aligned regions and world 1 switches it off."""
     import ctypes
 
     from chronoedit_b200 import _lib
 
     L = _lib.lib()
     m, h = _sp_handle(4)
-    regions = [ctypes.create_string_buffer(64) for _ in range(8)]
-    table = (ctypes.c_void_p * 8)(*[ctypes.addressof(r) for r in regions])
+    table = (ctypes.c_void_p * 8)(*[4096 * (w + 1) for w in range(8)])   # configure never dereferences the addresses
 
     def refused(*args, msg):
         assert L.ce_dit_sp_configure(*args) == -1
@@ -153,15 +155,41 @@ def test_sp_configure_refusals():
 
     refused(None, 0, 2, table, 64, msg="null handle")
     refused(h, 0, 9, table, 64, msg="arguments")
+    refused(h, 0, 0, table, 64, msg="arguments")
     refused(h, -1, 2, table, 64, msg="arguments")
     refused(h, 2, 2, table, 64, msg="arguments")
     refused(h, 0, 2, None, 64, msg="arguments")
     refused(h, 0, 2, table, 0, msg="arguments")
     refused(h, 0, 8, table, 64, msg="head count must be divisible")
-    holes = (ctypes.c_void_p * 2)(ctypes.addressof(regions[0]), None)
+    holes = (ctypes.c_void_p * 2)(4096, None)
     refused(h, 0, 2, holes, 64, msg="null region pointer")
+    misaligned = (ctypes.c_void_p * 2)(4096, 8192 + 16)
+    refused(h, 0, 2, misaligned, 64, msg="256-byte aligned")
     assert L.ce_dit_sp_configure(h, 1, 4, table, 64) == 0
     assert L.ce_dit_sp_configure(h, 0, 1, None, 0) == 0            # world 1 switches it off
+
+
+@pytest.mark.parametrize("disable,entry", [("disable_sequence_parallel", "ce_dit_sp_configure"),
+                                           ("disable_vae_sequence_parallel", "ce_vae_sp_configure")])
+def test_disable_barriers_on_the_group_of_the_regions(monkeypatch, disable, entry):
+    """Before the own region is freed, disable waits for the ranks of the group the regions were opened with, not the default group."""
+    from chronoedit_b200 import _lib
+
+    calls = []
+
+    class Lib:
+        def __getattr__(self, name):
+            return lambda *a: calls.append((name,) + a) or 0
+
+    monkeypatch.setattr(_lib, "lib", lambda: Lib())
+    monkeypatch.setattr(dist, "is_initialized", lambda: True)
+    monkeypatch.setattr(dist, "barrier", lambda group=None: calls.append(("barrier", group)))
+    monkeypatch.setattr(torch.cuda, "synchronize", lambda device=None: None)
+    group = object()
+    obj = types.SimpleNamespace(device="cuda:0", _handle="handle", _sp_state={"own": "own", "opened": ["peer"], "group": group})
+    getattr(parallel, disable)(obj)
+    assert calls == [(entry, "handle", 0, 1, None, 0), ("ce_ipc_close", "peer"), ("barrier", group), ("ce_ipc_free", "own")]
+    assert obj._sp_state is None
 
 
 def test_sp_host_barrier_arguments():
