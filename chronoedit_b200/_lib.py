@@ -107,6 +107,11 @@ SIGNATURES = {
     "ce_ipc_open": (c_int, [c_void_p, POINTER(c_void_p)]),
     "ce_ipc_close": (c_int, [c_void_p]),
     "ce_dit_set_capture": (c_int, [c_void_p, c_void_p, c_void_p, c_int]),
+    "ce_dit_teacache_probe_bytes": (c_int64, [c_void_p, c_int]),
+    "ce_dit_teacache_probe": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "ce_dit_set_residual_record": (c_int, [c_void_p, c_void_p, c_int64]),
+    "ce_dit_forward_cached": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                      c_void_p, c_int64, c_void_p]),
     "ce_dit_host_staging_bytes": (c_int64, [c_void_p, c_int, c_int, c_int, c_int, c_int]),
     "ce_dit_forward_host": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                     c_int, c_int, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),

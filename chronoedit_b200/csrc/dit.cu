@@ -53,6 +53,9 @@ struct ce_dit {
   float* fp8_scale = nullptr;
   // FP8 self-attention (ce_dit_set_attention_fp8): independent of the weights' dtype
   bool attn_fp8 = false;
+  // TeaCache record mode (ce_dit_set_residual_record): every forward leaves x_after_blocks - x_before_blocks here
+  void* resid_rec = nullptr;
+  int64_t resid_rec_bytes = 0;
 };
 
 enum { CAT_GEMM = 0, CAT_ATTN = 1, CAT_ROWS = 2, CAT_OTHER = 3, NUM_CATS = 4 };
@@ -390,6 +393,20 @@ static int linear(ce_dit* h, cudaStream_t s, const Linear& w, const bf16* A, int
   return CE_OK;
 }
 
+// The time path of the condition embedder (:147-159): sinusoid, time embedder (fp32, temb rounded to bf16) and, when `tproj` is
+// given, time_proj into tproj [B, 6D] bf16 (the reference's timestep_proj).
+static int time_path(ce_dit* h, cudaStream_t s, const Weights& W, const float* timestep, int B, float* sin_emb, float* h1,
+                     float* temb_f32, bf16* temb_bf16, bf16* tproj) {
+  const ce_dit_config& c = h->cfg;
+  const int D = D_of(c);
+  LAUNCH(CAT_OTHER, 0.0, launch_timestep_sinusoid(timestep, sin_emb, B, c.freq_dim, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_small_linear(sin_emb, c.freq_dim, W.time1_w, W.time1_b, 0, D, B, /*act=*/1, 0, h1, nullptr, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_small_linear(h1, D, W.time2_w, W.time2_b, 0, D, B, 0, 0, temb_f32, temb_bf16, s));  // temb = (...).type_as(bf16)
+  if (tproj)
+    LAUNCH(CAT_OTHER, 0.0, launch_small_linear(temb_f32, D, W.time_proj_w, W.time_proj_b, 1, 6 * D, B, 0, /*in_silu_bf16=*/1, nullptr, tproj, s));
+  return CE_OK;
+}
+
 // ---- internals shared with dit_fp32.cu
 const WeightMap& ce_dit_internal_weights_f32(const ce_dit* h) { return h->w32; }
 int ce_dit_internal_rope(ce_dit* h, int frames, int hp, int wp, cudaStream_t s, const float** cos_out, const float** sin_out) {
@@ -571,6 +588,12 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   if (ws.bytes > workspace_bytes)
     return fail(CE_ERR_WORKSPACE, "workspace too small: need " + std::to_string(ws.bytes) + " bytes, got " + std::to_string(workspace_bytes));
   CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
+  bf16* const rec = reinterpret_cast<bf16*>(h->resid_rec);
+  if (rec) {
+    CE_REQUIRE(!spx, "TeaCache residual record: sequence parallelism is not built for it");
+    CE_REQUIRE(h->resid_rec_bytes >= (int64_t)M * D * (int64_t)sizeof(bf16),
+               "TeaCache residual record: buffer too small for this forward (needs batch * tokens * inner dim bf16)");
+  }
   if ((rc = ensure_rope(h, frames, hp, wp, s))) return rc;   // always the full table [Lfull, 64]
   h->fp8_q = ws.fp8_q;
   h->fp8_scale = ws.fp8_scale;
@@ -619,12 +642,10 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   // ---- patch embedding (Conv3d k=s=(1,2,2) as im2row + GEMM, :429-430)
   LAUNCH(CAT_OTHER, 0.0, launch_patchify(reinterpret_cast<const bf16*>(hidden_states), ws.patches, B, c.in_channels, frames, height, width, tok0, L, s));
   if ((rc = linear(h, s, W.patch, ws.patches, M, D, Kp, ws.x, epi(EPI_BIAS, ws.stats_x, 1)))) return rc;
+  if (rec) CE_CHECK_CUDA(cudaMemcpyAsync(rec, ws.x, (size_t)M * D * sizeof(bf16), cudaMemcpyDeviceToDevice, s));   // x_before_blocks
 
   // ---- condition embedder (:147-165)
-  LAUNCH(CAT_OTHER, 0.0, launch_timestep_sinusoid(timestep, ws.sin_emb, B, c.freq_dim, s));
-  LAUNCH(CAT_OTHER, 0.0, launch_small_linear(ws.sin_emb, c.freq_dim, W.time1_w, W.time1_b, 0, D, B, /*act=*/1, 0, ws.h1, nullptr, s));
-  LAUNCH(CAT_OTHER, 0.0, launch_small_linear(ws.h1, D, W.time2_w, W.time2_b, 0, D, B, 0, 0, ws.temb_f32, ws.temb_bf16, s));  // temb = (...).type_as(bf16)
-  LAUNCH(CAT_OTHER, 0.0, launch_small_linear(ws.temb_f32, D, W.time_proj_w, W.time_proj_b, 1, 6 * D, B, 0, /*in_silu_bf16=*/1, nullptr, ws.tproj, s));
+  if ((rc = time_path(h, s, W, timestep, B, ws.sin_emb, ws.h1, ws.temb_f32, ws.temb_bf16, ws.tproj))) return rc;
   LAUNCH(CAT_OTHER, 0.0, launch_add_table(W.block_table, c.num_layers, ws.tproj, 6 * D, ws.mod, B, D, 6, s, /*scale chunks 1,4 -> 1+scale*/ 0x12u));
   LAUNCH(CAT_OTHER, 0.0, launch_add_table(W.head_table, 1, ws.temb_bf16, D, ws.modf, B, D, 2, s, /*chunk 1 = scale*/ 0x2u));
   // text: Linear -> GELU(tanh) -> Linear
@@ -755,6 +776,7 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
     for (const auto& cap : h->capture)
       if (cap.first == i) CE_CHECK_CUDA(cudaMemcpyAsync(cap.second, ws.x, (size_t)M * D * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
   }
+  if (rec) LAUNCH(CAT_ROWS, 6.0 * M * D, launch_sub_from(ws.x, rec, (int64_t)M * D, s));   // residual = bf16(x_after - x_before)
 
   // ---- output head (:451-467): modf = [B, 2, D] with shift = chunk 0, scale = chunk 1
   LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, ws.modf + D, ws.modf, 2 * D, L, nullptr, nullptr, 1));
@@ -774,6 +796,108 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
     LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(sp, lay.flags, s));   // nobody overwrites a peer's yout (next forward) before it has been read
     return CE_OK;
   }
+  LAUNCH(CAT_OTHER, 0.0, launch_unpatchify(ws.yout, No, reinterpret_cast<bf16*>(sample), B, c.out_channels, frames, height, width, s));
+  return CE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- TeaCache
+static bool aligned256(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) == 0; }
+
+// The probe's scratch: sinusoid [B, freq_dim] f32, h1 and temb [B, D] f32, temb [B, D] bf16.
+static int64_t probe_bytes(const ce_dit_config& c, int B, float** sin_emb, float** h1, float** temb_f32, bf16** temb_bf16, void* base) {
+  Bump b(base);
+  float* p0 = b.take<float>((int64_t)B * c.freq_dim);
+  float* p1 = b.take<float>((int64_t)B * D_of(c));
+  float* p2 = b.take<float>((int64_t)B * D_of(c));
+  bf16* p3 = b.take<bf16>((int64_t)B * D_of(c));
+  if (sin_emb) { *sin_emb = p0; *h1 = p1; *temb_f32 = p2; *temb_bf16 = p3; }
+  return b.bytes();
+}
+
+int64_t ce_dit_teacache_probe_bytes(const ce_dit* h, int batch) {
+  if (!h || batch < 1 || batch > 8) return -1;
+  return probe_bytes(h->cfg, batch, nullptr, nullptr, nullptr, nullptr, nullptr);
+}
+
+int ce_dit_teacache_probe(ce_dit* h, const float* timestep, int batch, const void* prev_tproj, void* tproj_out, float* sums_out,
+                          void* workspace, int64_t workspace_bytes, void* stream_v) {
+  CE_REQUIRE(h && timestep && tproj_out && workspace, "ce_dit_teacache_probe: null argument");
+  CE_REQUIRE(h->sp.world <= 1, "ce_dit_teacache_probe: TeaCache is not built for sequence parallelism");
+  CE_REQUIRE(batch >= 1 && batch <= 8, "ce_dit_teacache_probe: batch must be 1..8");
+  CE_REQUIRE(prev_tproj == nullptr || sums_out != nullptr, "ce_dit_teacache_probe: prev_tproj needs sums_out");
+  CE_REQUIRE(aligned256(tproj_out) && aligned256(workspace) && aligned256(prev_tproj) && aligned256(sums_out),
+             "ce_dit_teacache_probe: tproj_out, prev_tproj, sums_out and workspace must be 256-byte aligned");
+  const int64_t need = probe_bytes(h->cfg, batch, nullptr, nullptr, nullptr, nullptr, nullptr);
+  if (workspace_bytes < need)
+    return fail(CE_ERR_WORKSPACE, "ce_dit_teacache_probe: workspace too small: need " + std::to_string(need) + " bytes, got " +
+                                      std::to_string(workspace_bytes));
+  int rc = check_device();
+  if (rc) return rc;
+  Weights W;
+  if ((rc = resolve_weights(h, W))) return rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
+  float *sin_emb, *h1, *temb_f32;
+  bf16* temb_bf16;
+  probe_bytes(h->cfg, batch, &sin_emb, &h1, &temb_f32, &temb_bf16, workspace);
+  bf16* tproj = reinterpret_cast<bf16*>(tproj_out);
+  if ((rc = time_path(h, s, W, timestep, batch, sin_emb, h1, temb_f32, temb_bf16, tproj))) return rc;
+  if (prev_tproj)
+    LAUNCH(CAT_OTHER, 0.0, launch_l1_pair_sums(tproj, reinterpret_cast<const bf16*>(prev_tproj), (int64_t)batch * 6 * D_of(h->cfg), sums_out, s));
+  return CE_OK;
+}
+
+int ce_dit_set_residual_record(ce_dit* h, void* buf, int64_t bytes) {
+  CE_REQUIRE(h, "ce_dit_set_residual_record: null handle");
+  CE_REQUIRE(buf == nullptr || (aligned256(buf) && bytes > 0), "ce_dit_set_residual_record: the buffer must be 256-byte aligned and non-empty");
+  CE_REQUIRE(buf == nullptr || h->sp.world <= 1, "ce_dit_set_residual_record: TeaCache is not built for sequence parallelism");
+  h->resid_rec = buf;
+  h->resid_rec_bytes = buf ? bytes : 0;
+  return CE_OK;
+}
+
+int ce_dit_forward_cached(ce_dit* h, const void* hidden_states, const float* timestep, const void* residual, int64_t residual_bytes,
+                          void* sample, int batch, int frames, int height, int width, int text_len, void* workspace,
+                          int64_t workspace_bytes, void* stream_v) {
+  CE_REQUIRE(h && hidden_states && timestep && residual && sample && workspace, "ce_dit_forward_cached: null argument");
+  CE_REQUIRE(h->sp.world <= 1, "ce_dit_forward_cached: TeaCache is not built for sequence parallelism");
+  CE_REQUIRE(aligned256(residual) && aligned256(workspace), "ce_dit_forward_cached: residual and workspace must be 256-byte aligned");
+  int rc = validate_geometry(h, batch, frames, height, width, text_len);
+  if (rc) return rc;
+  const ce_dit_config& c = h->cfg;
+  const int B = batch, hp = height / c.patch_h, wp = width / c.patch_w;
+  const int L = frames * hp * wp, M = B * L, D = D_of(c), Kp = c.in_channels * 4, No = c.out_channels * 4;
+  CE_REQUIRE(residual_bytes >= (int64_t)M * D * (int64_t)sizeof(bf16),
+             "ce_dit_forward_cached: residual too small for this geometry (batch * tokens * inner dim bf16)");
+  Weights W;
+  if ((rc = resolve_weights(h, W))) return rc;
+  Workspace ws = carve(c, workspace, B, L, text_len, 257, W.fp8, h->attn_fp8);
+  if (ws.bytes > workspace_bytes)
+    return fail(CE_ERR_WORKSPACE, "ce_dit_forward_cached: workspace too small: need " + std::to_string(ws.bytes) + " bytes, got " +
+                                      std::to_string(workspace_bytes));
+  if ((rc = check_device())) return rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
+  h->fp8_q = ws.fp8_q;
+  h->fp8_scale = ws.fp8_scale;
+  const bool st = D % 256 == 0;
+  const RowPartials px = st ? RowPartials{ws.stats_x, D / 256, D / 256, 256} : RowPartials{};
+  h->launches = 0;
+  // x = bf16(x0 + residual): the patch-embedding GEMM's residual epilogue, which also leaves the head LayerNorm's row statistics
+  LAUNCH(CAT_OTHER, 0.0, launch_patchify(reinterpret_cast<const bf16*>(hidden_states), ws.patches, B, c.in_channels, frames, height, width, 0, L, s));
+  GemmArgs g;
+  g.epi = EPI_BIAS_RESID;
+  g.resid = reinterpret_cast<const bf16*>(residual);
+  g.ldr = D;
+  if (st) {
+    g.stats_out = ws.stats_x;
+    g.stats_mode = 1;
+  }
+  if ((rc = linear(h, s, W.patch, ws.patches, M, D, Kp, ws.x, g))) return rc;
+  if ((rc = time_path(h, s, W, timestep, B, ws.sin_emb, ws.h1, ws.temb_f32, ws.temb_bf16, nullptr))) return rc;
+  LAUNCH(CAT_OTHER, 0.0, launch_add_table(W.head_table, 1, ws.temb_bf16, D, ws.modf, B, D, 2, s, /*chunk 1 = scale*/ 0x2u));
+  LAUNCH(CAT_ROWS, 4.0 * M * D, launch_layernorm(ws.x, D, ws.xn, D, M, D, c.eps, ws.modf + D, ws.modf, 2 * D, L, nullptr, nullptr, 1, px, s));
+  GemmArgs gh;
+  gh.epi = EPI_BIAS;
+  if ((rc = linear(h, s, W.proj_out, ws.xn, M, No, D, ws.yout, gh))) return rc;
   LAUNCH(CAT_OTHER, 0.0, launch_unpatchify(ws.yout, No, reinterpret_cast<bf16*>(sample), B, c.out_channels, frames, height, width, s));
   return CE_OK;
 }

@@ -385,6 +385,50 @@ __global__ void add_table_kernel(const float* __restrict__ table, int table_rows
   }
 }
 
+// TeaCache probe: one CTA of L1_THREADS threads, so the summation order depends on n only.  Thread i accumulates elements i,
+// i + L1_THREADS, ... in index order; the warps then reduce by xor shuffles and warp 0 adds the 32 warp sums the same way.
+constexpr int L1_THREADS = 1024;
+__global__ void __launch_bounds__(L1_THREADS)
+l1_pair_sums_kernel(const bf16* __restrict__ a, const bf16* __restrict__ b, int64_t n, float* __restrict__ out) {
+  __shared__ float2 part[L1_THREADS / 32];
+  float d = 0.f, m = 0.f;
+  for (int64_t i = threadIdx.x; i < n; i += L1_THREADS) {
+    const float bv = __bfloat162float(b[i]);
+    d += fabsf(bf16_round(__bfloat162float(a[i]) - bv));   // (a - b) is a bf16 tensor in the reference
+    m += fabsf(bv);
+  }
+  d = warp_sum(d);
+  m = warp_sum(m);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) part[warp] = make_float2(d, m);
+  __syncthreads();
+  if (warp == 0) {
+    d = warp_sum(part[lane].x);
+    m = warp_sum(part[lane].y);
+    if (lane == 0) {
+      out[0] = d;
+      out[1] = m;
+    }
+  }
+}
+
+// r = bf16(x - r), 8 bf16 per thread and step
+__global__ void sub_from_kernel(const uint4* __restrict__ x, uint4* __restrict__ r, int64_t n8) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint4 xv = x[i];
+    uint4 rv = r[i];
+    const uint32_t* xs = reinterpret_cast<const uint32_t*>(&xv);
+    uint32_t* rs = reinterpret_cast<uint32_t*>(&rv);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 a = unpack_bf16x2(xs[k]), c = unpack_bf16x2(rs[k]);
+      const __nv_bfloat162 y = __floats2bfloat162_rn(a.x - c.x, a.y - c.y);
+      rs[k] = *reinterpret_cast<const uint32_t*>(&y);
+    }
+    r[i] = rv;
+  }
+}
+
 // One CTA per row: the row's absolute maximum (exact in fp32), then q = e4m3_satfinite(x / s) with s = amax / 448 (1 for a zero
 // row) as IEEE divisions, the same operations as the torch expression of the rule (DESIGN.md, "FP8 mode").  The second read of
 // the row comes from L1 / L2.
@@ -702,6 +746,23 @@ int launch_add_table(const float* table, int table_rows, const bf16* src, int sr
   const int grid = (int)((total + 255) / 256 < device_sm_count() * 8 ? (total + 255) / 256 : device_sm_count() * 8);
   const int src_per_chunk = src_ld >= chunks * n ? 1 : 0;
   add_table_kernel<<<grid, 256, 0, stream>>>(table, table_rows, src, src_ld, src_per_chunk, dst, B, n, chunks, plus_one_mask);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
+
+int launch_l1_pair_sums(const bf16* a, const bf16* b, int64_t n, float* out, cudaStream_t stream) {
+  CE_REQUIRE(n > 0, "l1_pair_sums: empty vectors");
+  l1_pair_sums_kernel<<<1, L1_THREADS, 0, stream>>>(a, b, n, out);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
+
+int launch_sub_from(const bf16* x, bf16* r, int64_t n, cudaStream_t stream) {
+  CE_REQUIRE(n % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(r) & 15) == 0,
+             "sub_from: n % 8 and 16-byte aligned operands");
+  const int64_t n8 = n / 8;
+  const int grid = (int)((n8 + 255) / 256 < device_sm_count() * 8 ? (n8 + 255) / 256 : device_sm_count() * 8);
+  sub_from_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(r), n8);
   CE_CHECK_CUDA(cudaGetLastError());
   return CE_OK;
 }

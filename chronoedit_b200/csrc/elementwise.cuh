@@ -96,4 +96,9 @@ int launch_timestep_sinusoid(const float* t, float* emb, int B, int dim, cudaStr
 int launch_add_table(const float* table, int table_rows, const bf16* src, int src_ld, float* dst, int B, int n,
                      int chunks, cudaStream_t stream, unsigned plus_one_mask = 0);
 
+// TeaCache probe: out[0] = sum_i |bf16(a[i] - b[i])|, out[1] = sum_i |b[i]| in fp32, one launch with a summation order fixed by n.
+int launch_l1_pair_sums(const bf16* a, const bf16* b, int64_t n, float* out, cudaStream_t stream);
+// TeaCache residual: r[i] = bf16(x[i] - r[i]) in place on r (n % 8 == 0, both 16-byte aligned).
+int launch_sub_from(const bf16* x, bf16* r, int64_t n, cudaStream_t stream);
+
 }  // namespace ce

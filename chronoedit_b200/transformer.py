@@ -19,6 +19,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from . import teacache as _tc
 from ._lib import CEError, DiTConfigC, check, current_stream, ptr
 
 # reference `_keep_in_fp32_modules` (transformer_chronoedit.py:338)
@@ -234,6 +235,13 @@ class ChronoEditTransformer3DModel(nn.Module):
         self.last_captures: Dict[int, torch.Tensor] = {}
         self._fp8 = False
         self._fp8_attention = False
+        # opt-in TeaCache (enable_teacache): settings, per-conditioning states, the probe's buffers and the per-call records
+        self._teacache: Optional[Dict[str, Any]] = None
+        self._tc_slots = 2
+        self._tc_states: list = []   # entries: dict(txt=, img=, txt_v=, img_v=, slot=, policy=, prev=, spare=, resid=, geom=)
+        self._tc_next_slot = 0
+        self._tc_probe: Dict[str, Any] = {}
+        self._tc_records: list = []
 
     # ------------------------------------------------------------------------------------------ plumbing
     @property
@@ -250,6 +258,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._graphs = {}
         self._ctx_cache = []
         self._workspaces = {}
+        self._drop_teacache_states()
         return super()._apply(fn, *a, **k)
 
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
@@ -260,6 +269,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         # assign=True the parameters are new tensors, so the fused device buffers must be rebuilt as well
         self._ctx_cache = []
         self._graphs = {}
+        self._drop_teacache_states()   # the stored residuals came from the old weights
         if assign:
             self._packed = False
         return super().load_state_dict(state_dict, strict=strict, assign=assign)
@@ -314,6 +324,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._graphs = {}
         self._ctx_cache = []
         self._workspaces = {}
+        self._drop_teacache_states()
 
     @property
     def fp8_attention_enabled(self) -> bool:
@@ -495,6 +506,12 @@ class ChronoEditTransformer3DModel(nn.Module):
             raise CEError(f"hidden_states has {C} channels, model expects {self.config.in_channels}")
         if (encoder_hidden_states_image is None) != (self.config.image_dim is None):
             raise CEError("encoder_hidden_states_image must be passed iff the model was built with image_dim")
+        if self._teacache is not None:
+            if return_block0 or capture_layers:
+                raise CEError("return_block0 / capture_layers are not available while TeaCache is on (a skipped step runs no "
+                              "blocks): call disable_teacache() first")
+            if getattr(self, "_sp_state", None):
+                raise CEError("TeaCache is not built for sequence parallelism: disable one of the two")
         x = hidden_states.to(device=dev, dtype=torch.bfloat16).contiguous()
         t = timestep.to(device=dev, dtype=torch.float32).reshape(-1)
         if t.numel() == 1 and B > 1:
@@ -515,7 +532,10 @@ class ChronoEditTransformer3DModel(nn.Module):
         if capture_layers:
             caps = {int(l): torch.empty(B * L_tok, Dm, dtype=torch.bfloat16, device=dev) for l in capture_layers}
         # (no graph replay in sequence-parallel mode: the peer barrier's epoch is a launch argument and must advance every forward)
-        if self.use_cuda_graph and not caps and b0 is None and not getattr(self, "_sp_state", None):
+        # (no graph replay with TeaCache either: each call chooses between two launch sequences after a device-to-host read)
+        if self._teacache is not None:
+            self._teacache_forward(x, t, txt, img, out, encoder_hidden_states, encoder_hidden_states_image)
+        elif self.use_cuda_graph and not caps and b0 is None and not getattr(self, "_sp_state", None):
             out = self._graphed_forward(x, t, txt, img, encoder_hidden_states, encoder_hidden_states_image)
         else:
             self._native_forward(x, t, txt, img, out, b0, caps, encoder_hidden_states, encoder_hidden_states_image)
@@ -633,6 +653,138 @@ class ChronoEditTransformer3DModel(nn.Module):
 
     def clear_context_cache(self) -> None:
         self._ctx_cache = []
+
+    # ------------------------------------------------------------------------------------------ TeaCache
+    def enable_teacache(self, tea_cache_l1_thresh: float, num_inference_steps: int,
+                        tea_cache_model_id: str = _tc.DEFAULT_MODEL_ID) -> None:
+        """Opt-in TeaCache (DESIGN.md, "TeaCache"), the reference DiffSynth pipeline's `tea_cache_l1_thresh` /
+        `tea_cache_model_id`: on a step whose timestep modulation moved little since the last computed step, skip every block
+        and add the residual the blocks produced then.  One state per conditioning (the same encoder_hidden_states /
+        encoder_hidden_states_image objects at the same version), so the pipeline's cond and uncond calls are kept apart.
+        `num_inference_steps` must be the schedule's length: the first and last step of it always compute.  Drops earlier
+        states.  Not available with sequence parallelism, return_block0 or capture_layers; CUDA-graph replay is not used."""
+        _tc.coefficients(tea_cache_model_id)   # raises on an unknown id, listing the supported ones
+        if int(num_inference_steps) < 1:
+            raise ValueError("num_inference_steps must be >= 1")
+        if getattr(self, "_sp_state", None):
+            raise CEError("TeaCache is not built for sequence parallelism: disable it first")
+        self._teacache = dict(thresh=float(tea_cache_l1_thresh), steps=int(num_inference_steps), model_id=tea_cache_model_id)
+        self.reset_teacache()
+
+    def disable_teacache(self) -> None:
+        """Back to the plain forward.  The call records stay readable until the next enable_teacache / reset_teacache."""
+        self._teacache = None
+        self._drop_teacache_states()
+
+    def reset_teacache(self) -> None:
+        """Forget every conditioning's state and the call records: the next call of each conditioning is step 0."""
+        self._drop_teacache_states()
+        self._tc_records = []
+        self._tc_next_slot = 0
+
+    @property
+    def teacache_enabled(self) -> bool:
+        return self._teacache is not None
+
+    @property
+    def teacache_records(self) -> Tuple["_tc.Record", ...]:
+        """One record per forward since enable_teacache / reset_teacache: (slot, step, rel, acc, computed)."""
+        return tuple(self._tc_records)
+
+    def _drop_teacache_states(self) -> None:
+        self._tc_states = []
+        self._tc_probe = {}
+
+    def _teacache_state(self, txt_in, img_in) -> Dict[str, Any]:
+        """The state of this conditioning, keyed like `_context_slot`: the same tensor objects at the same version.  Up to
+        `_tc_slots` states, least recently used dropped first; a new state starts at step 0."""
+        ver = lambda t: None if t is None else t._version
+        for i, e in enumerate(self._tc_states):
+            if e["txt"] is txt_in and e["img"] is img_in and e["txt_v"] == ver(txt_in) and e["img_v"] == ver(img_in):
+                self._tc_states.append(self._tc_states.pop(i))
+                return e
+        if len(self._tc_states) >= self._tc_slots:
+            self._tc_states.pop(0)
+        c = self._teacache
+        e = dict(txt=txt_in, img=img_in, txt_v=ver(txt_in), img_v=ver(img_in), slot=self._tc_next_slot,
+                 policy=_tc.TeaCacheState(c["steps"], c["thresh"], c["model_id"]), prev=None, spare=None, resid=None, geom=None)
+        self._tc_next_slot += 1
+        self._tc_states.append(e)
+        return e
+
+    def _teacache_forward(self, x, t, txt, img, out, txt_in, img_in) -> None:
+        """One TeaCache call: the probe (time path, and the two sums against the previous call's modulation when the rule
+        evaluates rel), one 8-byte device-to-host read, the rule, then either the forward with the residual recorded or the
+        forward without blocks.  A call whose geometry differs from the stored residual's computes (see DESIGN.md)."""
+        B, _, T, H, W = x.shape
+        D = self.config.num_attention_heads * self.config.attention_head_dim
+        st = self._teacache_state(txt_in, img_in)
+        pol: _tc.TeaCacheState = st["policy"]
+        if st["spare"] is None or st["spare"].numel() != B * 6 * D:
+            st["spare"] = torch.empty(B * 6 * D, dtype=torch.bfloat16, device=self.device)
+        cur = st["spare"]
+        prev = st["prev"] if st["prev"] is not None and st["prev"].numel() == cur.numel() else None
+        sums = self._native_probe(t, prev if pol.needs_rel() else None, cur)
+        rel = None if sums is None else _tc.rel_from_sums(sums[0], sums[1], B * 6 * D)
+        st["prev"], st["spare"] = cur, st["prev"]   # prev = t_mod on every call, skipped or not
+        geom = (B, T, H, W)
+        step, computed = pol.decide(rel, force_compute=st["geom"] != geom)
+        if computed:
+            if st["geom"] != geom:
+                st["resid"] = torch.empty(B * (T * (H // 2) * (W // 2)) * D, dtype=torch.bfloat16, device=self.device)
+                st["geom"] = None
+            self._native_teacache_forward(x, t, txt, img, out, txt_in, img_in, st["resid"], True)
+            st["geom"] = geom
+        else:
+            self._native_teacache_forward(x, t, txt, img, out, txt_in, img_in, st["resid"], False)
+        self._tc_records.append(_tc.Record(st["slot"], step, rel, pol.acc, computed))
+
+    def _native_probe(self, t, prev, cur):
+        """ce_dit_teacache_probe: the timestep modulation of t into `cur` ([B * 6D] bf16); with `prev` also the two sums, read
+        back through pinned memory (the only device-to-host read of a TeaCache call).  Returns (sum |cur - prev|, sum |prev|)
+        or None."""
+        if not self._packed:
+            self.pack_weights()
+        L = _lib.lib()
+        B = t.numel()
+        pr = self._tc_probe
+        if pr.get("batch") != B:
+            n = L.ce_dit_teacache_probe_bytes(self._handle, B)
+            if n < 0:
+                check(-1)
+            pr.update(batch=B, ws=torch.empty(n, dtype=torch.uint8, device=self.device),
+                      sums=torch.empty(64, dtype=torch.float32, device=self.device))
+            if "host" not in pr:
+                pr["host"] = torch.empty(2, dtype=torch.float32).pin_memory()
+                pr["event"] = torch.cuda.Event()
+        with torch.cuda.device(self.device):
+            check(L.ce_dit_teacache_probe(self._handle, ptr(t), B, ptr(prev), ptr(cur), ptr(pr["sums"] if prev is not None else None),
+                                          ptr(pr["ws"]), pr["ws"].numel(), current_stream()))
+            if prev is None:
+                return None
+            pr["host"].copy_(pr["sums"][:2], non_blocking=True)
+            pr["event"].record()
+        pr["event"].synchronize()
+        s0, s1 = pr["host"].tolist()
+        return s0, s1
+
+    def _native_teacache_forward(self, x, t, txt, img, out, txt_in, img_in, resid, record: bool) -> None:
+        """record: the full forward (ce_dit_forward_ex, context cache as configured) leaving bf16(x_after_blocks -
+        x_before_blocks) in `resid`.  Otherwise ce_dit_forward_cached: x_before_blocks + resid, then the output head."""
+        L = _lib.lib()
+        if record:
+            check(L.ce_dit_set_residual_record(self._handle, ptr(resid), resid.numel() * 2))
+            try:
+                self._native_forward(x, t, txt, img, out, None, {}, txt_in, img_in)
+            finally:
+                check(L.ce_dit_set_residual_record(self._handle, None, 0))
+            return
+        B, _, T, H, W = x.shape
+        Lt = txt.shape[1]
+        ws = self._workspace(B, T, H, W, Lt)
+        with torch.cuda.device(self.device):
+            check(L.ce_dit_forward_cached(self._handle, ptr(x), ptr(t), ptr(resid), resid.numel() * 2, ptr(out), B, T, H, W, Lt,
+                                          ptr(ws), ws.numel(), current_stream()))
 
     @torch.no_grad()
     def forward_host(self, hidden_states: torch.Tensor, timestep: torch.Tensor, encoder_hidden_states: torch.Tensor,
@@ -809,6 +961,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         if lora_state_dict is None:
             self._lora_adapters.clear()   # merged: a second fuse_lora must not add them again
         self._ctx_cache = []              # cross-attention K/V cached from the old weights are stale
+        self._drop_teacache_states()      # and so are the TeaCache residuals
         return n
 
     # ------------------------------------------------------------------------------------------ loading

@@ -135,6 +135,30 @@ int ce_ipc_close(void* ptr);
 /* Parity aid: from now on every forward copies the output of block layers[i] ([B*L, D] bf16) to dst[i] (n = 0 clears). */
 int ce_dit_set_capture(ce_dit* h, const int32_t* layers, void* const* dst, int n);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * TeaCache (DESIGN.md, "TeaCache"; reference: chronoedit_diffsynth/wan_video_new_chronoedit.py:1190-1239, 1434-1492): skip every
+ * block on a step whose timestep modulation moved little since the last computed step and add the residual the blocks produced
+ * then.  The policy lives with the caller; these calls give it the three device pieces.  All three refuse sequence parallelism.
+ *
+ * ce_dit_teacache_probe: the time path alone (sinusoid, time embedder, time_proj) for `timestep` [B] fp32 into tproj_out [B, 6D] bf16,
+ *   bit-identical to the forward's timestep_proj.  With prev_tproj (the [B, 6D] of an earlier call) non-NULL it also writes
+ *   sums_out[0] = sum |bf16(tproj - prev)| and sums_out[1] = sum |prev| (fp32, a summation order fixed by B * 6D).  workspace:
+ *   ce_dit_teacache_probe_bytes(h, batch) bytes.  Every buffer is a device buffer, 256-byte aligned.
+ * ce_dit_set_residual_record: from now on every forward leaves residual = bf16(x_after_blocks - x_before_blocks) [B*L, D] bf16 in
+ *   buf (x_before_blocks: the token stream right after the patch embedding).  The sample is unchanged.  A forward whose residual
+ *   does not fit in `bytes` is refused.  buf = NULL switches it off.
+ * ce_dit_forward_cached: the forward with the blocks replaced by x = bf16(x_before_blocks + residual), then the output head and
+ *   unpatchify.  The geometry arguments and the workspace are those of ce_dit_forward_ex; the text and image embedders, the
+ *   context cache and the blocks are not touched.
+ * ------------------------------------------------------------------------------------------------------------ */
+int64_t ce_dit_teacache_probe_bytes(const ce_dit* h, int batch);
+int ce_dit_teacache_probe(ce_dit* h, const float* timestep, int batch, const void* prev_tproj, void* tproj_out, float* sums_out,
+                          void* workspace, int64_t workspace_bytes, void* stream);
+int ce_dit_set_residual_record(ce_dit* h, void* buf, int64_t bytes);
+int ce_dit_forward_cached(ce_dit* h, const void* hidden_states, const float* timestep, const void* residual, int64_t residual_bytes,
+                          void* sample, int batch, int frames, int height, int width, int text_len, void* workspace,
+                          int64_t workspace_bytes, void* stream);
+
 /* Same call with every tensor in (pinned) HOST memory: H2D copies of the inputs, forward, D2H of the sample, all on
  * `stream`, which is synchronised before returning.  `staging` is a device buffer of at least
  * ce_dit_host_staging_bytes(...) bytes.  This is the end-to-end ("e2e") path bench.py times. */
