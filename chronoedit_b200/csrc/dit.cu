@@ -12,6 +12,7 @@
 // With FP8 attention on (ce_dit_set_attention_fp8) the self-attention becomes quantize(q|k) -> quantize(v) -> attention_fp8.
 #include <math.h>
 
+#include <algorithm>
 #include <atomic>
 #include <map>
 #include <string>
@@ -42,6 +43,8 @@ struct ce_dit {
   std::vector<std::pair<int, void*>> capture;
   // sequence parallelism (ce_dit_sp_configure): world == 1 means off
   ce::SeqPar sp;
+  // batch split (ce_dit_bp_configure): rank r computes samples [r B / world, (r + 1) B / world) of each call; world == 1 means off
+  ce::SeqPar bp;
   // optional per-category device timing (CUDA events on the launch stream around every kernel)
   bool profiling = false;
   std::vector<cudaEvent_t> ev;       // pairs (begin, end)
@@ -104,6 +107,12 @@ SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world) {
   l.bytes = l.flags + 1024;
   return l;
 }
+
+// Batch split (ce_dit_bp_configure): a rank's peer region is the flags block (uint32 [8 * 32], first), then two sample slots, each
+// [batch, out_channels, frames, height, width] bf16 rounded up to 1024 bytes.  The slot size follows from the region size, so a region
+// sized for one geometry serves every call whose full sample fits.
+constexpr int64_t kBpFlagsBytes = 1024;
+int64_t bp_slot_bytes(int64_t region_bytes) { return std::max<int64_t>(0, (region_bytes - kBpFlagsBytes) / 2) & ~int64_t(1023); }
 
 // Keys of the FP8 attention's V^T rows: L rounded up to the 32-key groups of its layout.
 int vt_keys(int L) { return (L + 31) / 32 * 32; }
@@ -407,6 +416,55 @@ static int time_path(ce_dit* h, cudaStream_t s, const Weights& W, const float* t
   return CE_OK;
 }
 
+// Batch split: the refusals of a split call, all before its first launch.  `sample_elems`: elements of one output sample.
+static int bp_check(const ce_dit* h, const char* who, int batch, int64_t sample_elems, bool block_capture, cudaStream_t s) {
+  const SeqPar& bp = h->bp;
+  if (batch % bp.world != 0)
+    return fail(CE_ERR_INVALID, std::string(who) + ": batch split: a batch of " + std::to_string(batch) + " does not divide over " +
+                                    std::to_string(bp.world) + " ranks.  Only a call that carries the whole CFG pair is split: the unchanged "
+                                    "diffusers pipeline's batch-1 calls are not split (it calls with the prompt and the negative prompt "
+                                    "one at a time).  Run the pair as one batch-2 call, or switch the split off (ce_dit_bp_configure with "
+                                    "world 1)");
+  const int64_t need = (int64_t)batch * sample_elems * (int64_t)sizeof(bf16), slot = bp_slot_bytes(bp.region_bytes);
+  if (need > slot)
+    return fail(CE_ERR_WORKSPACE, std::string(who) + ": batch split: the call's sample needs a slot of " + std::to_string(need) +
+                                      " bytes, the peer region holds slots of " + std::to_string(slot) + " (ce_dit_bp_region_bytes)");
+  CE_REQUIRE(!block_capture, std::string(who) + ": batch split: no block capture / block0_out (each rank runs only its own samples)");
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CE_CHECK_CUDA(cudaStreamIsCapturing(s, &cs));
+  CE_REQUIRE(cs == cudaStreamCaptureStatusNone,
+             std::string(who) + ": batch split: the stream is capturing (the exchange's barrier epoch advances every call, so it cannot be "
+                                "replayed from a graph)");
+  return CE_OK;
+}
+
+// Batch split: the exchange that ends every split call.  This rank's samples, already at their offset in the caller's buffer, go into
+// every peer's slot of the current set; one barrier; then the other ranks' samples come from the own slot into the caller's buffer.
+// The set alternates with the barrier epoch's parity, so one barrier per call suffices: a rank reads set p of call n before it reaches
+// the barrier of call n + 1, and no peer writes set p again before it has passed that barrier.
+static int bp_exchange(ce_dit* h, void* sample, int batch, int64_t sample_elems, cudaStream_t s) {
+  SeqPar& bp = h->bp;
+  const int64_t part = (int64_t)(batch / bp.world) * sample_elems * (int64_t)sizeof(bf16);
+  const int64_t set = kBpFlagsBytes + (int64_t)(bp.epoch & 1) * bp_slot_bytes(bp.region_bytes);
+  uint8_t* out = reinterpret_cast<uint8_t*>(sample);
+  SpCopy put[8], get[8];
+  int n = 0;
+  for (int w = 0; w < bp.world; ++w) {
+    if (w == bp.rank) continue;
+    put[n].src = out + bp.rank * part;
+    put[n].dst = bp.region[w] + set + bp.rank * part;
+    put[n].bytes = part;
+    get[n].src = bp.region[bp.rank] + set + w * part;
+    get[n].dst = out + w * part;
+    get[n].bytes = part;
+    ++n;
+  }
+  LAUNCH(CAT_OTHER, 0.0, launch_sp_copy(put, n, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(bp, 0, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_sp_copy(get, n, s));
+  return CE_OK;
+}
+
 // ---- internals shared with dit_fp32.cu
 const WeightMap& ce_dit_internal_weights_f32(const ce_dit* h) { return h->w32; }
 int ce_dit_internal_rope(ce_dit* h, int frames, int hp, int wp, cudaStream_t s, const float** cos_out, const float** sin_out) {
@@ -417,6 +475,7 @@ int ce_dit_internal_rope(ce_dit* h, int frames, int hp, int wp, cudaStream_t s, 
   return CE_OK;
 }
 const ce_dit_config* ce_dit_internal_config(const ce_dit* h) { return &h->cfg; }
+int ce_dit_internal_bp_world(const ce_dit* h) { return h->bp.world; }
 
 extern "C" {
 
@@ -499,6 +558,19 @@ int ce_dit_sp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs
 
 int ce_dit_sp_host_barrier(ce_dit* h, int timeout_ms) { return sp_set_host_barrier(h ? &h->sp : nullptr, "ce_dit_sp_host_barrier", timeout_ms); }
 
+int64_t ce_dit_bp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width, int world) {
+  if (!h || world < 2 || world > 8 || batch < 1 || batch > 8 || batch % world != 0 || frames < 1 || height < 1 || width < 1) return -1;
+  const int64_t sample = (int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16);
+  return kBpFlagsBytes + 2 * ((sample + 1023) & ~int64_t(1023));
+}
+
+int ce_dit_bp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes) {
+  CE_REQUIRE(h, "ce_dit_bp_configure: null handle");
+  return sp_configure(h->bp, "ce_dit_bp_configure", rank, world, region_ptrs, region_bytes);
+}
+
+int ce_dit_bp_host_barrier(ce_dit* h, int timeout_ms) { return sp_set_host_barrier(h ? &h->bp : nullptr, "ce_dit_bp_host_barrier", timeout_ms); }
+
 int ce_dit_set_capture(ce_dit* h, const int32_t* layers, void* const* dst, int n) {
   CE_REQUIRE(h && n >= 0 && (n == 0 || (layers && dst)), "ce_dit_set_capture: arguments");
   h->capture.clear();
@@ -552,10 +624,11 @@ int ce_dit_forward(ce_dit* h, const void* hidden_states, const float* timestep, 
                            width, text_len, workspace, workspace_bytes, block0_out, nullptr, 0, 0, stream_v);
 }
 
-int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timestep, const void* encoder_hidden_states,
-                      const void* encoder_hidden_states_image, void* sample, int batch, int frames, int height, int width,
-                      int text_len, void* workspace, int64_t workspace_bytes, void* block0_out, void* ctx_cache,
-                      int64_t ctx_cache_bytes, int ctx_reuse, void* stream_v) {
+// The forward of the samples this rank computes (all of them without the batch split).
+static int forward_samples(ce_dit* h, const void* hidden_states, const float* timestep, const void* encoder_hidden_states,
+                           const void* encoder_hidden_states_image, void* sample, int batch, int frames, int height, int width,
+                           int text_len, void* workspace, int64_t workspace_bytes, void* block0_out, void* ctx_cache,
+                           int64_t ctx_cache_bytes, int ctx_reuse, void* stream_v) {
   CE_REQUIRE(h && hidden_states && timestep && encoder_hidden_states && sample && workspace, "ce_dit_forward: null argument");
   CE_REQUIRE(ctx_reuse == 0 || ctx_cache != nullptr, "ce_dit_forward_ex: ctx_reuse needs a context cache");
   int rc = check_device();
@@ -800,6 +873,35 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   return CE_OK;
 }
 
+// Byte address of sample `first` of a [batch, ...] tensor with `per_sample` bytes per sample (NULL stays NULL).
+static const void* sample_at(const void* p, int first, int64_t per_sample) {
+  return p ? static_cast<const uint8_t*>(p) + first * per_sample : nullptr;
+}
+
+int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timestep, const void* encoder_hidden_states,
+                      const void* encoder_hidden_states_image, void* sample, int batch, int frames, int height, int width,
+                      int text_len, void* workspace, int64_t workspace_bytes, void* block0_out, void* ctx_cache,
+                      int64_t ctx_cache_bytes, int ctx_reuse, void* stream_v) {
+  if (!h || h->bp.world <= 1)
+    return forward_samples(h, hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image, sample, batch, frames, height,
+                           width, text_len, workspace, workspace_bytes, block0_out, ctx_cache, ctx_cache_bytes, ctx_reuse, stream_v);
+  // batch split: this rank's samples through the forward above (the token split, when configured too, runs on them unchanged), then
+  // the exchange
+  CE_REQUIRE(hidden_states && timestep && encoder_hidden_states && sample && workspace, "ce_dit_forward: null argument");
+  CE_TRY(validate_geometry(h, batch, frames, height, width, text_len));
+  const ce_dit_config& c = h->cfg;
+  const int64_t pixels = (int64_t)frames * height * width, out_elems = c.out_channels * pixels;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
+  CE_TRY(bp_check(h, "ce_dit_forward_ex", batch, out_elems, block0_out != nullptr || !h->capture.empty(), s));
+  const int Bl = batch / h->bp.world, s0 = h->bp.rank * Bl;
+  CE_TRY(forward_samples(h, sample_at(hidden_states, s0, c.in_channels * pixels * 2), timestep + s0,
+                         sample_at(encoder_hidden_states, s0, (int64_t)text_len * c.text_dim * 2),
+                         sample_at(encoder_hidden_states_image, s0, (int64_t)257 * c.image_dim * 2),
+                         const_cast<void*>(sample_at(sample, s0, out_elems * 2)), Bl, frames, height, width, text_len, workspace,
+                         workspace_bytes, nullptr, ctx_cache, ctx_cache_bytes, ctx_reuse, stream_v));
+  return bp_exchange(h, sample, batch, out_elems, s);
+}
+
 // ---------------------------------------------------------------------------------------------- TeaCache
 static bool aligned256(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) == 0; }
 
@@ -855,9 +957,9 @@ int ce_dit_set_residual_record(ce_dit* h, void* buf, int64_t bytes) {
   return CE_OK;
 }
 
-int ce_dit_forward_cached(ce_dit* h, const void* hidden_states, const float* timestep, const void* residual, int64_t residual_bytes,
-                          void* sample, int batch, int frames, int height, int width, int text_len, void* workspace,
-                          int64_t workspace_bytes, void* stream_v) {
+static int forward_cached_samples(ce_dit* h, const void* hidden_states, const float* timestep, const void* residual,
+                                  int64_t residual_bytes, void* sample, int batch, int frames, int height, int width, int text_len,
+                                  void* workspace, int64_t workspace_bytes, void* stream_v) {
   CE_REQUIRE(h && hidden_states && timestep && residual && sample && workspace, "ce_dit_forward_cached: null argument");
   CE_REQUIRE(h->sp.world <= 1, "ce_dit_forward_cached: TeaCache is not built for sequence parallelism");
   CE_REQUIRE(aligned256(residual) && aligned256(workspace), "ce_dit_forward_cached: residual and workspace must be 256-byte aligned");
@@ -900,6 +1002,26 @@ int ce_dit_forward_cached(ce_dit* h, const void* hidden_states, const float* tim
   if ((rc = linear(h, s, W.proj_out, ws.xn, M, No, D, ws.yout, gh))) return rc;
   LAUNCH(CAT_OTHER, 0.0, launch_unpatchify(ws.yout, No, reinterpret_cast<bf16*>(sample), B, c.out_channels, frames, height, width, s));
   return CE_OK;
+}
+
+int ce_dit_forward_cached(ce_dit* h, const void* hidden_states, const float* timestep, const void* residual, int64_t residual_bytes,
+                          void* sample, int batch, int frames, int height, int width, int text_len, void* workspace,
+                          int64_t workspace_bytes, void* stream_v) {
+  if (!h || h->bp.world <= 1)
+    return forward_cached_samples(h, hidden_states, timestep, residual, residual_bytes, sample, batch, frames, height, width, text_len,
+                                  workspace, workspace_bytes, stream_v);
+  // batch split: the residual is this rank's, [batch / world * tokens, D]; a skipped call ends in the same exchange as a computed one
+  CE_REQUIRE(hidden_states && timestep && residual && sample && workspace, "ce_dit_forward_cached: null argument");
+  CE_TRY(validate_geometry(h, batch, frames, height, width, text_len));
+  const ce_dit_config& c = h->cfg;
+  const int64_t pixels = (int64_t)frames * height * width, out_elems = c.out_channels * pixels;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
+  CE_TRY(bp_check(h, "ce_dit_forward_cached", batch, out_elems, false, s));
+  const int Bl = batch / h->bp.world, s0 = h->bp.rank * Bl;
+  CE_TRY(forward_cached_samples(h, sample_at(hidden_states, s0, c.in_channels * pixels * 2), timestep + s0, residual, residual_bytes,
+                                const_cast<void*>(sample_at(sample, s0, out_elems * 2)), Bl, frames, height, width, text_len, workspace,
+                                workspace_bytes, stream_v));
+  return bp_exchange(h, sample, batch, out_elems, s);
 }
 
 int64_t ce_dit_host_staging_bytes(const ce_dit* h, int batch, int frames, int height, int width, int text_len) {

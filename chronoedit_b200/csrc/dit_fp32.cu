@@ -336,6 +336,7 @@ struct Ctx32 {
 const WeightMap& ce_dit_internal_weights_f32(const ce_dit* h);
 int ce_dit_internal_rope(ce_dit* h, int frames, int hp, int wp, cudaStream_t s, const float** cos_out, const float** sin_out);
 const ce_dit_config* ce_dit_internal_config(const ce_dit* h);
+int ce_dit_internal_bp_world(const ce_dit* h);
 
 extern "C" {
 
@@ -350,6 +351,8 @@ int ce_dit_forward_fp32(ce_dit* h, const float* hidden_states, const float* time
                         const float* encoder_hidden_states_image, float* sample, int batch, int frames, int height, int width, int text_len,
                         void* workspace, int64_t workspace_bytes, float* block_out, void* stream_v) {
   CE_REQUIRE(h && hidden_states && timestep && encoder_hidden_states && sample && workspace, "ce_dit_forward_fp32: null argument");
+  CE_REQUIRE(ce_dit_internal_bp_world(h) <= 1,
+             "ce_dit_forward_fp32: the validation forward is not built for the batch split: switch it off (ce_dit_bp_configure with world 1)");
   const ce_dit_config& c = *ce_dit_internal_config(h);
   CE_REQUIRE(batch >= 1 && batch <= 8 && (frames == 2 || frames == c.rope_temporal_skip_len) && height % c.patch_h == 0 && width % c.patch_w == 0,
              "ce_dit_forward_fp32: geometry (same rules as ce_dit_forward)");

@@ -123,9 +123,10 @@ def _open_peer_regions(n: int, group) -> tuple:
     return ptrs, {"own": own, "opened": opened, "group": group}
 
 
-def _configure_peer_regions(obj, entry: str, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict) -> None:
-    """Hands the pointer table to the C configure `entry` of obj's handle and keeps `state` as obj._sp_state, with "world" and "bytes"
-    added."""
+def _configure_peer_regions(obj, entry: str, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict,
+                            attr: str = "_sp_state") -> None:
+    """Hands the pointer table to the C configure `entry` of obj's handle and keeps `state` as obj.<attr> (the token split's
+    "_sp_state" or the batch split's "_bp_state"), with "rank", "world" and "bytes" added."""
     import ctypes
 
     from . import _lib
@@ -136,15 +137,15 @@ def _configure_peer_regions(obj, entry: str, rank: int, region_ptrs: Sequence[in
     with torch.cuda.device(obj.device):
         check(getattr(_lib.lib(), entry)(obj._ensure_handle(), rank, world, table, region_bytes))
         torch.cuda.synchronize(obj.device)
-    obj._sp_state = dict(state, world=world, bytes=region_bytes)
+    setattr(obj, attr, dict(state, rank=rank, world=world, bytes=region_bytes))
 
 
-def _release_peer_regions(obj, entry: str) -> None:
-    """Switches obj's handle back to one GPU (C configure `entry`, world 1), closes the opened peer mappings and frees the own region
-    once no rank of the state's group still maps it."""
+def _release_peer_regions(obj, entry: str, attr: str = "_sp_state") -> None:
+    """Switches obj's handle back to one GPU (C configure `entry`, world 1), closes the opened peer mappings of the state obj.<attr>
+    and frees the own region once no rank of the state's group still maps it."""
     from . import _lib
 
-    st = getattr(obj, "_sp_state", None)
+    st = getattr(obj, attr, None)
     if not st:
         return
     L = _lib.lib()
@@ -156,7 +157,7 @@ def _release_peer_regions(obj, entry: str) -> None:
         if dist.is_initialized():
             dist.barrier(group=st.get("group"))
         L.ce_ipc_free(st["own"])
-    obj._sp_state = None
+    setattr(obj, attr, None)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -215,6 +216,79 @@ def configure_sequence_parallel(model, rank: int, region_ptrs: Sequence[int], re
 def disable_sequence_parallel(model) -> None:
     """Back to the single-GPU forward; releases what enable_sequence_parallel allocated and opened."""
     _release_peer_regions(model, "ce_dit_sp_configure")
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# The batch of a DiT forward split over the ranks of a node: the CFG pair of one edit on two GPUs (include/chronoedit_b200.h, ce_dit_bp_*)
+# ----------------------------------------------------------------------------------------------------------------------
+def enable_cfg_parallel(model, batch: int, frames: int, height: int, width: int, group=None) -> int:
+    """Split the batch of every forward over the ranks of `group` (one process per GPU of a node): rank r computes samples
+    [r B / world, (r + 1) B / world) of a call's batch B with the unchanged forward, and one exchange of the finished samples by peer
+    stores over NVLink gives every rank the full batch, bit-identical to the single-GPU forward.  For the CFG pair (prompt and negative
+    prompt as one batch-2 call, as `scheduler.step_cfg` and bench.py run it) that puts each half of the pair on its own GPU.
+    Called with the SAME full inputs on every rank.  FP8 weights (`enable_fp8`), FP8 attention (`enable_fp8_attention`) and TeaCache
+    (`enable_teacache`, one state per conditioning, decided on the rank's own samples) work unchanged with it on.  A call whose batch
+    the ranks do not divide is refused: the unchanged diffusers pipeline's two batch-1 calls per step are not split.  CUDA graphs are
+    not replayed while it is on.
+
+    `batch` x (frames, height, width) sizes the region: any later call whose full sample is no larger is accepted (a region for 8
+    latent frames also serves the cut to 2).  Returns the region size in bytes.
+
+    On 4 or 8 GPUs it composes with the token split as a grid: the batch over 2 ranks, the tokens of each half over W / 2 ranks.
+    With dist.new_group, token groups {0 .. W/2 - 1} and {W/2 .. W - 1}, pair groups {r, r + W/2}; every rank calls:
+
+        parallel.enable_sequence_parallel(model, B // 2, T, H, W, group=token_group)   # the token split sees the local batch
+        parallel.enable_cfg_parallel(model, B, T, H, W, group=pair_group)
+    """
+    from ._lib import CEError
+
+    if not dist.is_initialized():
+        raise CEError("enable_cfg_parallel needs an initialised torch.distributed process group (one process per GPU)")
+    disable_cfg_parallel(model)
+    world = dist.get_world_size(group)
+    if world == 1:
+        return 0
+    n = cfg_region_bytes(model, batch, frames, height, width, world)
+    with torch.cuda.device(model.device):
+        ptrs, state = _open_peer_regions(n, group)
+        configure_cfg_parallel(model, dist.get_rank(group), ptrs, n, state)
+    dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
+    return int(n)
+
+
+def cfg_region_bytes(model, batch: int, frames: int, height: int, width: int, world: int) -> int:
+    """Bytes of the peer region every rank of the batch split needs for this geometry (ce_dit_bp_region_bytes)."""
+    from . import _lib
+    from ._lib import CEError
+
+    n = _lib.lib().ce_dit_bp_region_bytes(model._ensure_handle(), batch, frames, height, width, world)
+    if n < 0:
+        raise CEError(f"batch split: the batch ({batch}) must divide by the world size ({world}, 2 to 8) and the geometry must be valid")
+    return int(n)
+
+
+def configure_cfg_parallel(model, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict) -> None:
+    """Hand rank `rank`'s table of peer-region addresses (one per rank, as seen from this process) to the model's C handle
+    (ce_dit_bp_configure) and switch the model's batch split on.  `state` is kept as `model._bp_state` (with "rank", "world" and
+    "bytes" added) and holds what disable_cfg_parallel releases, as for configure_sequence_parallel.  The token split's state
+    (`model._sp_state`) is not touched."""
+    _configure_peer_regions(model, "ce_dit_bp_configure", rank, region_ptrs, region_bytes, state, "_bp_state")
+    _drop_sample_caches(model)
+
+
+def disable_cfg_parallel(model) -> None:
+    """Back to computing every sample of a call on this GPU; releases what enable_cfg_parallel allocated and opened."""
+    if getattr(model, "_bp_state", None):
+        _release_peer_regions(model, "ce_dit_bp_configure", "_bp_state")
+        _drop_sample_caches(model)
+
+
+def _drop_sample_caches(model) -> None:
+    """What a model keeps per sample of a call (the context cache's K/V, the TeaCache states) holds the samples of the old share, and
+    a captured graph has the old launches."""
+    model._graphs = {}
+    model.clear_context_cache()
+    model._drop_teacache_states()
 
 
 # ----------------------------------------------------------------------------------------------------------------------

@@ -531,11 +531,13 @@ class ChronoEditTransformer3DModel(nn.Module):
         caps: Dict[int, torch.Tensor] = {}
         if capture_layers:
             caps = {int(l): torch.empty(B * L_tok, Dm, dtype=torch.bfloat16, device=dev) for l in capture_layers}
-        # (no graph replay in sequence-parallel mode: the peer barrier's epoch is a launch argument and must advance every forward)
+        # (no graph replay in sequence-parallel or batch-split mode: the peer barrier's epoch is a launch argument and must advance
+        # every forward)
         # (no graph replay with TeaCache either: each call chooses between two launch sequences after a device-to-host read)
         if self._teacache is not None:
             self._teacache_forward(x, t, txt, img, out, encoder_hidden_states, encoder_hidden_states_image)
-        elif self.use_cuda_graph and not caps and b0 is None and not getattr(self, "_sp_state", None):
+        elif (self.use_cuda_graph and not caps and b0 is None and not getattr(self, "_sp_state", None)
+              and not getattr(self, "_bp_state", None)):
             out = self._graphed_forward(x, t, txt, img, encoder_hidden_states, encoder_hidden_states_image)
         else:
             self._native_forward(x, t, txt, img, out, b0, caps, encoder_hidden_states, encoder_hidden_states_image)
@@ -545,6 +547,16 @@ class ChronoEditTransformer3DModel(nn.Module):
             return (out,)
         return Transformer2DModelOutput(sample=out)
 
+    def _local_samples(self, B: int) -> Tuple[int, int]:
+        """(first, count) of the samples of a B-sample call this handle computes: its share under the batch split
+        (parallel.enable_cfg_parallel), else all of them.  The workspace, the context cache and the TeaCache buffers are sized by
+        `count`.  A batch the ranks do not divide is left whole here, for the forward to refuse."""
+        st = getattr(self, "_bp_state", None)
+        if not st or B % st["world"]:
+            return 0, B
+        n = B // st["world"]
+        return st["rank"] * n, n
+
     def _native_forward(self, x, t, txt, img, out, b0, caps, txt_in, img_in) -> None:
         """The one place the DiT forward reaches the C ABI (ce_dit_forward_ex).  x [B,C,T,H,W] bf16, t [B] fp32, txt / img bf16,
         all contiguous on the module's device; `out` (and the optional block captures) are written in place."""
@@ -553,7 +565,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         B, _, T, H, W = x.shape
         Lt = txt.shape[1]
         L = _lib.lib()
-        ws = self._workspace(B, T, H, W, Lt)
+        ws = self._workspace(self._local_samples(B)[1], T, H, W, Lt)
         if caps:
             lay = (_lib.c_int32 * len(caps))(*caps.keys())
             dst = (_lib.c_void_p * len(caps))(*[v.data_ptr() for v in caps.values()])
@@ -630,7 +642,7 @@ class ChronoEditTransformer3DModel(nn.Module):
                 # most recently used last; by position, since list.remove would compare the entries' tensors with ==
                 self._ctx_cache.append(self._ctx_cache.pop(i))
                 return e["buf"], 1
-        B, Lt = txt.shape[0], txt.shape[1]
+        B, Lt = self._local_samples(txt.shape[0])[1], txt.shape[1]
         n = _lib.lib().ce_dit_context_cache_bytes(self._handle, B, Lt)
         if n < 0:
             check(-1)
@@ -715,19 +727,25 @@ class ChronoEditTransformer3DModel(nn.Module):
     def _teacache_forward(self, x, t, txt, img, out, txt_in, img_in) -> None:
         """One TeaCache call: the probe (time path, and the two sums against the previous call's modulation when the rule
         evaluates rel), one 8-byte device-to-host read, the rule, then either the forward with the residual recorded or the
-        forward without blocks.  A call whose geometry differs from the stored residual's computes (see DESIGN.md)."""
+        forward without blocks.  A call whose geometry differs from the stored residual's computes (see DESIGN.md).  Under the batch
+        split the rule sees only this rank's samples: the probe takes their timesteps, and the modulation and the residual are theirs."""
         B, _, T, H, W = x.shape
         D = self.config.num_attention_heads * self.config.attention_head_dim
+        bp = getattr(self, "_bp_state", None)
+        if bp and B % bp["world"]:   # before the probe's launches; the forward itself would refuse it too
+            raise CEError(f"batch split: a batch of {B} does not divide over {bp['world']} ranks.  Only a call that carries the whole CFG "
+                          "pair is split: the unchanged diffusers pipeline's batch-1 calls are not split.  Run the pair as one batch-2 call")
+        s0, B = self._local_samples(B)
         st = self._teacache_state(txt_in, img_in)
         pol: _tc.TeaCacheState = st["policy"]
         if st["spare"] is None or st["spare"].numel() != B * 6 * D:
             st["spare"] = torch.empty(B * 6 * D, dtype=torch.bfloat16, device=self.device)
         cur = st["spare"]
         prev = st["prev"] if st["prev"] is not None and st["prev"].numel() == cur.numel() else None
-        sums = self._native_probe(t, prev if pol.needs_rel() else None, cur)
+        sums = self._native_probe(t[s0: s0 + B], prev if pol.needs_rel() else None, cur)
         rel = None if sums is None else _tc.rel_from_sums(sums[0], sums[1], B * 6 * D)
         st["prev"], st["spare"] = cur, st["prev"]   # prev = t_mod on every call, skipped or not
-        geom = (B, T, H, W)
+        geom = (x.shape[0], s0, B, T, H, W)   # the rank's share too: a residual of other samples is not reused
         step, computed = pol.decide(rel, force_compute=st["geom"] != geom)
         if computed:
             if st["geom"] != geom:
@@ -781,7 +799,7 @@ class ChronoEditTransformer3DModel(nn.Module):
             return
         B, _, T, H, W = x.shape
         Lt = txt.shape[1]
-        ws = self._workspace(B, T, H, W, Lt)
+        ws = self._workspace(self._local_samples(B)[1], T, H, W, Lt)
         with torch.cuda.device(self.device):
             check(L.ce_dit_forward_cached(self._handle, ptr(x), ptr(t), ptr(resid), resid.numel() * 2, ptr(out), B, T, H, W, Lt,
                                           ptr(ws), ws.numel(), current_stream()))
@@ -802,7 +820,7 @@ class ChronoEditTransformer3DModel(nn.Module):
                 raise CEError("forward_host expects contiguous CPU bf16 tensors")
         t = timestep.to(torch.float32).contiguous()
         L = _lib.lib()
-        ws = self._workspace(B, T, H, W, Lt)
+        ws = self._workspace(self._local_samples(B)[1], T, H, W, Lt)
         n = L.ce_dit_host_staging_bytes(self._handle, B, T, H, W, Lt)
         st = self._workspaces.get("staging")
         if st is None or st.numel() < n:

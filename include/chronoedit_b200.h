@@ -126,6 +126,26 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
  * ------------------------------------------------------------------------------------------------------------ */
 int64_t ce_dit_sp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width, int world);
 int ce_dit_sp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Batch split ("CFG parallelism") over the GPUs of one node: rank r of `world` computes samples [r B / world, (r + 1) B / world) of
+ * each call's batch B through the unchanged forward, and every rank returns the full batch.  The samples never interact inside the
+ * forward, so the only exchange is at its end: each rank stores its samples into every peer's region, one barrier, and copies the
+ * other ranks' samples from its own region into the caller's buffer.  Every rank passes the SAME full inputs.  It composes with FP8
+ * weights, FP8 attention and TeaCache (ce_dit_forward_cached ends in the same exchange), and with the token split (ce_dit_sp_*,
+ * configured for the local batch B / world) as a grid: the token split runs on the rank's samples, the batch exchange follows.
+ *   region: the flags block (1 KB, first), then two sample slots of [batch, out_channels, frames, height, width] bf16 (each rounded
+ *   up to 1 KB) that alternate from call to call, so each call needs one barrier.  Any later call whose full sample fits a slot is
+ *   accepted.  ce_dit_bp_region_bytes returns -1 for a world outside 2..8 or a batch it does not divide.
+ *   ce_dit_bp_configure: as ce_dit_sp_configure (same refusals); world = 1 switches the split off.
+ *   ce_dit_bp_host_barrier: the test aid of ce_dit_sp_host_barrier, for this group's barrier.
+ * A split call refuses, before any launch: a batch the ranks do not divide (so the unchanged diffusers pipeline's batch-1 calls are
+ * not split), a sample larger than a slot, block capture or block0_out, and a capturing stream.  ce_dit_forward_fp32 is refused.
+ * ------------------------------------------------------------------------------------------------------------ */
+int64_t ce_dit_bp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width, int world);
+int ce_dit_bp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes);
+int ce_dit_bp_host_barrier(ce_dit* h, int timeout_ms);
+
 int ce_ipc_alloc(int64_t bytes, void** ptr);
 int ce_ipc_free(void* ptr);
 int ce_ipc_get_handle(void* ptr, void* handle_out_64_bytes);
