@@ -104,6 +104,10 @@ SIGNATURES = {
     "ce_dit_bp_region_bytes": (c_int64, [c_void_p, c_int, c_int, c_int, c_int, c_int]),
     "ce_dit_bp_configure": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64]),
     "ce_dit_bp_host_barrier": (c_int, [c_void_p, c_int]),
+    "ce_dit_cp_region_bytes": (c_int64, [c_void_p, c_int, c_int, c_int, c_int]),
+    "ce_dit_cp_configure": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64]),
+    "ce_dit_cp_exchange": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "ce_dit_cp_host_barrier": (c_int, [c_void_p, c_int]),
     "ce_ipc_alloc": (c_int, [c_int64, POINTER(c_void_p)]),
     "ce_ipc_free": (c_int, [c_void_p]),
     "ce_ipc_get_handle": (c_int, [c_void_p, c_void_p]),

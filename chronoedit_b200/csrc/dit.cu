@@ -45,6 +45,9 @@ struct ce_dit {
   ce::SeqPar sp;
   // batch split (ce_dit_bp_configure): rank r computes samples [r B / world, (r + 1) B / world) of each call; world == 1 means off
   ce::SeqPar bp;
+  // call-pair group (ce_dit_cp_configure): rank 0 computes the prompt call of a CFG pair, rank 1 the negative-prompt call, and
+  // ce_dit_cp_exchange swaps the two samples; world == 1 means off.  Exclusive with `bp`.
+  ce::SeqPar cp;
   // optional per-category device timing (CUDA events on the launch stream around every kernel)
   bool profiling = false;
   std::vector<cudaEvent_t> ev;       // pairs (begin, end)
@@ -108,11 +111,12 @@ SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world) {
   return l;
 }
 
-// Batch split (ce_dit_bp_configure): a rank's peer region is the flags block (uint32 [8 * 32], first), then two sample slots, each
-// [batch, out_channels, frames, height, width] bf16 rounded up to 1024 bytes.  The slot size follows from the region size, so a region
-// sized for one geometry serves every call whose full sample fits.
-constexpr int64_t kBpFlagsBytes = 1024;
-int64_t bp_slot_bytes(int64_t region_bytes) { return std::max<int64_t>(0, (region_bytes - kBpFlagsBytes) / 2) & ~int64_t(1023); }
+// Batch split (ce_dit_bp_configure) and call pair (ce_dit_cp_configure): a rank's peer region is the flags block (uint32 [8 * 32],
+// first), then two sample slots, each [batch, out_channels, frames, height, width] bf16 rounded up to 1024 bytes (the full batch of a
+// split call, or one whole call of a pair).  The slot size follows from the region size, so a region sized for one geometry serves
+// every call whose full sample fits.
+constexpr int64_t kSlotFlagsBytes = 1024;
+int64_t slot_bytes(int64_t region_bytes) { return std::max<int64_t>(0, (region_bytes - kSlotFlagsBytes) / 2) & ~int64_t(1023); }
 
 // Keys of the FP8 attention's V^T rows: L rounded up to the 32-key groups of its layout.
 int vt_keys(int L) { return (L + 31) / 32 * 32; }
@@ -425,7 +429,7 @@ static int bp_check(const ce_dit* h, const char* who, int batch, int64_t sample_
                                     "diffusers pipeline's batch-1 calls are not split (it calls with the prompt and the negative prompt "
                                     "one at a time).  Run the pair as one batch-2 call, or switch the split off (ce_dit_bp_configure with "
                                     "world 1)");
-  const int64_t need = (int64_t)batch * sample_elems * (int64_t)sizeof(bf16), slot = bp_slot_bytes(bp.region_bytes);
+  const int64_t need = (int64_t)batch * sample_elems * (int64_t)sizeof(bf16), slot = slot_bytes(bp.region_bytes);
   if (need > slot)
     return fail(CE_ERR_WORKSPACE, std::string(who) + ": batch split: the call's sample needs a slot of " + std::to_string(need) +
                                       " bytes, the peer region holds slots of " + std::to_string(slot) + " (ce_dit_bp_region_bytes)");
@@ -438,31 +442,38 @@ static int bp_check(const ce_dit* h, const char* who, int batch, int64_t sample_
   return CE_OK;
 }
 
-// Batch split: the exchange that ends every split call.  This rank's samples, already at their offset in the caller's buffer, go into
-// every peer's slot of the current set; one barrier; then the other ranks' samples come from the own slot into the caller's buffer.
-// The set alternates with the barrier epoch's parity, so one barrier per call suffices: a rank reads set p of call n before it reaches
-// the barrier of call n + 1, and no peer writes set p again before it has passed that barrier.
-static int bp_exchange(ce_dit* h, void* sample, int batch, int64_t sample_elems, cudaStream_t s) {
-  SeqPar& bp = h->bp;
-  const int64_t part = (int64_t)(batch / bp.world) * sample_elems * (int64_t)sizeof(bf16);
-  const int64_t set = kBpFlagsBytes + (int64_t)(bp.epoch & 1) * bp_slot_bytes(bp.region_bytes);
-  uint8_t* out = reinterpret_cast<uint8_t*>(sample);
+// The exchange of a slot group (the batch split's `bp`, the call pair's `cp`).  `part` bytes at `own` go to offset rank * stride of
+// every peer's slot of the current set; one barrier; then for every peer w the `part` bytes at offset w * stride of the own slot go to
+// dst + w * stride.  The batch split passes its samples' place in the caller's buffer (stride = part); the call pair passes the two
+// samples of the pair (stride 0: a slot holds the one sample of the other call).
+// The set alternates with the barrier epoch's parity, so one barrier per exchange suffices: a rank reads set p of exchange n before it
+// reaches the barrier of exchange n + 1, and no peer writes set p again before it has passed that barrier.
+static int slot_exchange(ce_dit* h, SeqPar& g, const void* own, void* dst, int64_t part, int64_t stride, cudaStream_t s) {
+  const int64_t set = kSlotFlagsBytes + (int64_t)(g.epoch & 1) * slot_bytes(g.region_bytes);
   SpCopy put[8], get[8];
   int n = 0;
-  for (int w = 0; w < bp.world; ++w) {
-    if (w == bp.rank) continue;
-    put[n].src = out + bp.rank * part;
-    put[n].dst = bp.region[w] + set + bp.rank * part;
+  for (int w = 0; w < g.world; ++w) {
+    if (w == g.rank) continue;
+    put[n].src = own;
+    put[n].dst = g.region[w] + set + g.rank * stride;
     put[n].bytes = part;
-    get[n].src = bp.region[bp.rank] + set + w * part;
-    get[n].dst = out + w * part;
+    get[n].src = g.region[g.rank] + set + w * stride;
+    get[n].dst = reinterpret_cast<uint8_t*>(dst) + w * stride;
     get[n].bytes = part;
     ++n;
   }
   LAUNCH(CAT_OTHER, 0.0, launch_sp_copy(put, n, s));
-  LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(bp, 0, s));
+  LAUNCH(CAT_OTHER, 0.0, launch_sp_barrier(g, 0, s));
   LAUNCH(CAT_OTHER, 0.0, launch_sp_copy(get, n, s));
   return CE_OK;
+}
+
+// Batch split: the exchange that ends every split call.  This rank's samples, already at their offset in the caller's buffer, go into
+// every peer's slot; the other ranks' samples come from the own slot into the caller's buffer.
+static int bp_exchange(ce_dit* h, void* sample, int batch, int64_t sample_elems, cudaStream_t s) {
+  SeqPar& bp = h->bp;
+  const int64_t part = (int64_t)(batch / bp.world) * sample_elems * (int64_t)sizeof(bf16);
+  return slot_exchange(h, bp, reinterpret_cast<uint8_t*>(sample) + bp.rank * part, sample, part, part, s);
 }
 
 // ---- internals shared with dit_fp32.cu
@@ -561,15 +572,56 @@ int ce_dit_sp_host_barrier(ce_dit* h, int timeout_ms) { return sp_set_host_barri
 int64_t ce_dit_bp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width, int world) {
   if (!h || world < 2 || world > 8 || batch < 1 || batch > 8 || batch % world != 0 || frames < 1 || height < 1 || width < 1) return -1;
   const int64_t sample = (int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16);
-  return kBpFlagsBytes + 2 * ((sample + 1023) & ~int64_t(1023));
+  return kSlotFlagsBytes + 2 * ((sample + 1023) & ~int64_t(1023));
 }
 
 int ce_dit_bp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes) {
   CE_REQUIRE(h, "ce_dit_bp_configure: null handle");
+  CE_REQUIRE(world == 1 || h->cp.world <= 1,
+             "ce_dit_bp_configure: the call-pair split is configured (ce_dit_cp_configure): the two CFG splits are exclusive, switch it off first");
   return sp_configure(h->bp, "ce_dit_bp_configure", rank, world, region_ptrs, region_bytes);
 }
 
 int ce_dit_bp_host_barrier(ce_dit* h, int timeout_ms) { return sp_set_host_barrier(h ? &h->bp : nullptr, "ce_dit_bp_host_barrier", timeout_ms); }
+
+int64_t ce_dit_cp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width) {
+  if (!h || batch < 1 || batch > 8 || frames < 1 || height < 1 || width < 1) return -1;
+  const int64_t sample = (int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16);
+  return kSlotFlagsBytes + 2 * ((sample + 1023) & ~int64_t(1023));
+}
+
+int ce_dit_cp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes) {
+  CE_REQUIRE(h, "ce_dit_cp_configure: null handle");
+  CE_REQUIRE(world == 1 || h->bp.world <= 1,
+             "ce_dit_cp_configure: the batch split is configured (ce_dit_bp_configure): the two CFG splits are exclusive, switch it off first");
+  SeqPar cp = h->cp;
+  CE_TRY(sp_configure(cp, "ce_dit_cp_configure", rank, world, region_ptrs, region_bytes));
+  CE_REQUIRE(cp.world <= 2, "ce_dit_cp_configure: a CFG pair has two calls: world must be 1 (off) or 2");
+  h->cp = cp;
+  return CE_OK;
+}
+
+int ce_dit_cp_exchange(ce_dit* h, const void* own_sample, void* other_sample, int batch, int frames, int height, int width, void* stream_v) {
+  CE_REQUIRE(h && own_sample && other_sample, "ce_dit_cp_exchange: null argument");
+  CE_REQUIRE(h->cp.world == 2, "ce_dit_cp_exchange: the call-pair split is not configured (ce_dit_cp_configure with world 2)");
+  CE_REQUIRE(batch >= 1 && batch <= 8 && frames >= 1 && height >= 1 && width >= 1, "ce_dit_cp_exchange: geometry");
+  CE_REQUIRE(((reinterpret_cast<uintptr_t>(own_sample) | reinterpret_cast<uintptr_t>(other_sample)) & 1) == 0,
+             "ce_dit_cp_exchange: the samples must be bf16-aligned");
+  const int64_t need = (int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16);
+  const int64_t slot = slot_bytes(h->cp.region_bytes);
+  if (need > slot)
+    return fail(CE_ERR_WORKSPACE, "ce_dit_cp_exchange: the call's sample needs a slot of " + std::to_string(need) +
+                                      " bytes, the peer region holds slots of " + std::to_string(slot) + " (ce_dit_cp_region_bytes)");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CE_CHECK_CUDA(cudaStreamIsCapturing(s, &cs));
+  CE_REQUIRE(cs == cudaStreamCaptureStatusNone,
+             "ce_dit_cp_exchange: the stream is capturing (the exchange's barrier epoch advances every pair, so it cannot be replayed from "
+             "a graph)");
+  return slot_exchange(h, h->cp, own_sample, other_sample, need, 0, s);
+}
+
+int ce_dit_cp_host_barrier(ce_dit* h, int timeout_ms) { return sp_set_host_barrier(h ? &h->cp : nullptr, "ce_dit_cp_host_barrier", timeout_ms); }
 
 int ce_dit_set_capture(ce_dit* h, const int32_t* layers, void* const* dst, int n) {
   CE_REQUIRE(h && n >= 0 && (n == 0 || (layers && dst)), "ce_dit_set_capture: arguments");

@@ -2,7 +2,7 @@
 // region of the same layout, the kernels that produce exchanged data store it straight into the consuming rank's region over NVLink
 // (peer pointers obtained with CUDA IPC), and a flag barrier in peer memory orders the phases.  What is here serves every split
 // model: the handle's configuration, the barrier and a batched copy to local or peer memory.  The region layouts and the exchanges
-// that use them live with their model (sp_layout and the batch split's slots in dit.cu, vae_sp_layout in vae.cu).
+// that use them live with their model (sp_layout and the slots of the batch split and the call pair in dit.cu, vae_sp_layout in vae.cu).
 //
 // Test aid (ce_dit_sp_host_barrier, ce_vae_sp_host_barrier): `world` handles of ONE process on ONE GPU can play the ranks, with
 // ordinary device allocations as regions.  The barrier is then a host rendezvous instead of the flag kernel, so no kernel ever waits

@@ -126,7 +126,7 @@ def _open_peer_regions(n: int, group) -> tuple:
 def _configure_peer_regions(obj, entry: str, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict,
                             attr: str = "_sp_state") -> None:
     """Hands the pointer table to the C configure `entry` of obj's handle and keeps `state` as obj.<attr> (the token split's
-    "_sp_state" or the batch split's "_bp_state"), with "rank", "world" and "bytes" added."""
+    "_sp_state", the batch split's "_bp_state" or the call pair's "_cp_state"), with "rank", "world" and "bytes" added."""
     import ctypes
 
     from . import _lib
@@ -244,6 +244,9 @@ def enable_cfg_parallel(model, batch: int, frames: int, height: int, width: int,
 
     if not dist.is_initialized():
         raise CEError("enable_cfg_parallel needs an initialised torch.distributed process group (one process per GPU)")
+    if getattr(model, "_cp_state", None):   # before any region is allocated; ce_dit_bp_configure refuses it too
+        raise CEError("enable_cfg_parallel: the call-pair split (enable_cfg_parallel_calls) is on: the two CFG splits are exclusive, "
+                      "disable it first")
     disable_cfg_parallel(model)
     world = dist.get_world_size(group)
     if world == 1:
@@ -280,6 +283,94 @@ def disable_cfg_parallel(model) -> None:
     """Back to computing every sample of a call on this GPU; releases what enable_cfg_parallel allocated and opened."""
     if getattr(model, "_bp_state", None):
         _release_peer_regions(model, "ce_dit_bp_configure", "_bp_state")
+        _drop_sample_caches(model)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# The two calls of the unchanged pipeline's CFG pair on two ranks (include/chronoedit_b200.h, ce_dit_cp_*)
+# ----------------------------------------------------------------------------------------------------------------------
+def enable_cfg_parallel_calls(model, batch: int, frames: int, height: int, width: int, group=None) -> int:
+    """Compute the two calls of each CFG step of the unchanged diffusers pipeline on two ranks (one process per GPU): the pipeline
+    calls the transformer once with `prompt_embeds` and once with `negative_prompt_embeds`, with the same latents and timestep.  From
+    then on the model takes its calls in pairs: rank 0 of `group` computes the first call (the prompt), rank 1 the second (the negative
+    prompt), each with the ordinary single-GPU forward, and at the second call one exchange by peer stores over NVLink gives each rank
+    the other's sample.  Every rank runs the same pipeline with the SAME inputs and gets both samples, bit-identical to one GPU.
+
+    Rank 1 returns a sample filled with NaN from the first call of a pair; the exchange of the second call overwrites it in place,
+    stream-ordered before the pipeline's guidance combine reads it.  So the mode needs classifier-free guidance
+    (`guidance_scale > 1`, the pipeline's `do_classifier_free_guidance`): the second call of a pair must pass the same
+    `hidden_states` and `timestep` objects (unchanged in place) and the same `encoder_hidden_states_image` as the first, or it raises
+    CEError on every rank before any launch.  A guidance-free run therefore raises at its second step.
+
+    FP8 weights (`enable_fp8`), FP8 attention (`enable_fp8_attention`), TeaCache and the context cache work unchanged: a rank keeps
+    the state of the one conditioning it computes, so every TeaCache decision equals the single-GPU run's.  Refused while on:
+    `return_block0`, `capture_layers`, `forward_host`, `forward_fp32`, a capturing stream and `enable_cfg_parallel`.  CUDA graphs are
+    not replayed.
+
+    `batch` x (frames, height, width) sizes the region for one call: any later call whose sample is no larger is accepted (a region for
+    8 latent frames also serves temporal reasoning's cut to 2).  Returns the region size in bytes.
+
+    On 4 or 8 GPUs it composes with the token split as a grid: each call's tokens over W / 2 ranks, the pair over 2.  With
+    dist.new_group, token groups {0 .. W/2 - 1} and {W/2 .. W - 1}, pair groups {j, j + W/2}; every rank calls:
+
+        parallel.enable_sequence_parallel(model, B, T, H, W, group=token_group)   # the call's own batch (1 in the pipeline)
+        parallel.enable_cfg_parallel_calls(model, B, T, H, W, group=pair_group)
+
+    and every rank of token group 0 computes the prompt calls, every rank of token group 1 the negative-prompt calls.
+    """
+    from ._lib import CEError
+
+    if not dist.is_initialized():
+        raise CEError("enable_cfg_parallel_calls needs an initialised torch.distributed process group (one process per GPU)")
+    if getattr(model, "_bp_state", None):   # before any region is allocated; ce_dit_cp_configure refuses it too
+        raise CEError("enable_cfg_parallel_calls: the batch split (enable_cfg_parallel) is on: the two CFG splits are exclusive, "
+                      "disable it first")
+    disable_cfg_parallel_calls(model)
+    world = dist.get_world_size(group)
+    if world == 1:
+        return 0
+    if world != 2:
+        raise CEError(f"enable_cfg_parallel_calls: a CFG pair has two calls: the group must have 2 ranks, not {world}")
+    n = cfg_calls_region_bytes(model, batch, frames, height, width)
+    with torch.cuda.device(model.device):
+        ptrs, state = _open_peer_regions(n, group)
+        configure_cfg_parallel_calls(model, dist.get_rank(group), ptrs, n, state)
+    dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
+    return int(n)
+
+
+def cfg_calls_region_bytes(model, batch: int, frames: int, height: int, width: int) -> int:
+    """Bytes of the peer region each of the two ranks needs for calls of this geometry (ce_dit_cp_region_bytes)."""
+    from . import _lib
+    from ._lib import CEError
+
+    n = _lib.lib().ce_dit_cp_region_bytes(model._ensure_handle(), batch, frames, height, width)
+    if n < 0:
+        raise CEError(f"call-pair split: invalid geometry (batch {batch}, 1 to 8; frames {frames}, height {height}, width {width})")
+    return int(n)
+
+
+def configure_cfg_parallel_calls(model, rank: int, region_ptrs: Sequence[int], region_bytes: int, state: Dict) -> None:
+    """Hand rank `rank`'s table of the two peer-region addresses (as seen from this process) to the model's C handle
+    (ce_dit_cp_configure) and switch the call-pair split on.  `state` is kept as `model._cp_state` (with "rank", "world" and "bytes"
+    added) and holds what disable_cfg_parallel_calls releases, as for configure_sequence_parallel.  The next call is the first of a
+    pair."""
+    _configure_peer_regions(model, "ce_dit_cp_configure", rank, region_ptrs, region_bytes, state, "_cp_state")
+    model._cp_pair = None
+    _drop_sample_caches(model)
+
+
+def disable_cfg_parallel_calls(model) -> None:
+    """Back to computing every call on this GPU; releases what enable_cfg_parallel_calls allocated and opened.  A pair whose second
+    call never came is dropped with a warning."""
+    if getattr(model, "_cp_state", None):
+        if getattr(model, "_cp_pair", None) is not None:
+            import warnings
+
+            warnings.warn("disable_cfg_parallel_calls: the first call of a CFG pair is still open (its second call never came); "
+                          "dropping it")
+        model._cp_pair = None
+        _release_peer_regions(model, "ce_dit_cp_configure", "_cp_state")
         _drop_sample_caches(model)
 
 

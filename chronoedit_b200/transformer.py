@@ -373,6 +373,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         (tests/test_gpu_fp32_mode.py); far slower than forward() and not part of any benchmark."""
         if not getattr(self, "_fp32_keepalive", None):
             raise CEError("call enable_fp32_validation(fp32_state_dict) first")
+        self._refuse_cp("forward_fp32")
         dev = self.device
         B, C, T, H, W = hidden_states.shape
         x = hidden_states.to(device=dev, dtype=torch.float32).contiguous()
@@ -512,6 +513,9 @@ class ChronoEditTransformer3DModel(nn.Module):
                               "blocks): call disable_teacache() first")
             if getattr(self, "_sp_state", None):
                 raise CEError("TeaCache is not built for sequence parallelism: disable one of the two")
+        cp = getattr(self, "_cp_state", None)
+        role, pair = self._cp_role(hidden_states, timestep, encoder_hidden_states_image, return_block0, capture_layers) if cp else (0, None)
+        computes = not cp or role == cp["rank"]
         x = hidden_states.to(device=dev, dtype=torch.bfloat16).contiguous()
         t = timestep.to(device=dev, dtype=torch.float32).reshape(-1)
         if t.numel() == 1 and B > 1:
@@ -534,13 +538,18 @@ class ChronoEditTransformer3DModel(nn.Module):
         # (no graph replay in sequence-parallel or batch-split mode: the peer barrier's epoch is a launch argument and must advance
         # every forward)
         # (no graph replay with TeaCache either: each call chooses between two launch sequences after a device-to-host read)
-        if self._teacache is not None:
+        # (a call of a CFG pair that the other rank computes runs no forward and touches no per-conditioning state)
+        if not computes:
+            pass
+        elif self._teacache is not None:
             self._teacache_forward(x, t, txt, img, out, encoder_hidden_states, encoder_hidden_states_image)
         elif (self.use_cuda_graph and not caps and b0 is None and not getattr(self, "_sp_state", None)
-              and not getattr(self, "_bp_state", None)):
+              and not getattr(self, "_bp_state", None) and not cp):
             out = self._graphed_forward(x, t, txt, img, encoder_hidden_states, encoder_hidden_states_image)
         else:
             self._native_forward(x, t, txt, img, out, b0, caps, encoder_hidden_states, encoder_hidden_states_image)
+        if cp:
+            out = self._cp_finish(role, pair, computes, out, hidden_states, timestep, encoder_hidden_states_image)
         self.last_block0 = b0
         self.last_captures = caps
         if not return_dict:
@@ -556,6 +565,58 @@ class ChronoEditTransformer3DModel(nn.Module):
             return 0, B
         n = B // st["world"]
         return st["rank"] * n, n
+
+    def _refuse_cp(self, who: str) -> None:
+        if getattr(self, "_cp_state", None):
+            raise CEError(f"{who} is not available with the call-pair split (parallel.enable_cfg_parallel_calls pairs the calls of "
+                          "forward()): call parallel.disable_cfg_parallel_calls first")
+
+    def _cp_role(self, hidden_states, timestep, img_in, return_block0, capture_layers) -> Tuple[int, Optional[Dict[str, Any]]]:
+        """Call-pair split (parallel.enable_cfg_parallel_calls): (role of this call, the open pair's record for role 1).  Role 0 is
+        the first call of a pair (the prompt, computed by rank 0), role 1 the second (the negative prompt, computed by rank 1).  Every
+        refusal comes before any launch.  A second call that does not pair with the first (by object identity and in-place version,
+        so no host sync) drops the pair and raises: every rank sees the same calls, so every rank raises at the same call and no rank
+        waits at the exchange's barrier."""
+        if return_block0 or capture_layers:
+            raise CEError("return_block0 / capture_layers are not available with the call-pair split (each rank computes one call "
+                          "of a pair): call parallel.disable_cfg_parallel_calls first")
+        if self.device.type == "cuda" and torch.cuda.is_current_stream_capturing():
+            raise CEError("call-pair split: the stream is capturing (the exchange's barrier epoch advances every pair, so it cannot "
+                          "be replayed from a graph)")
+        pair = getattr(self, "_cp_pair", None)
+        if pair is None:
+            return 0, None
+        self._cp_pair = None
+        same = (hidden_states is pair["x"] and hidden_states._version == pair["x_v"] and tuple(hidden_states.shape) == pair["x_shape"]
+                and timestep is pair["t"] and timestep._version == pair["t_v"] and tuple(timestep.shape) == pair["t_shape"]
+                and img_in is pair["img"])
+        if not same:
+            raise CEError("call-pair split: this call does not pair with the previous one.  The second call of a CFG pair must pass "
+                          "the same hidden_states and timestep tensors, unchanged, and the same encoder_hidden_states_image as the "
+                          "first: the mode needs classifier-free guidance (guidance_scale > 1, two transformer calls per step).  The "
+                          "open pair is dropped; the next call starts a new one")
+        return 1, pair
+
+    def _cp_finish(self, role, pair, computes, out, hidden_states, timestep, img_in) -> torch.Tensor:
+        """Call-pair split, after this rank's forward (when it computes this call).  Role 0: rank 1 fills its sample with bf16 NaN
+        (0xFFFF) on the stream, and the pair is opened holding the sample.  Role 1: ce_dit_cp_exchange swaps the two samples, so
+        rank 1's role-0 sample, still held by the caller, receives the prompt call's result in place, and rank 0 returns the
+        negative-prompt call's.  Everything is stream-ordered: the guidance combine that follows on the current stream sees both."""
+        if role == 0:
+            if not computes:
+                out.view(torch.int16).fill_(-1)
+            self._cp_pair = dict(x=hidden_states, x_v=hidden_states._version, x_shape=tuple(hidden_states.shape), t=timestep,
+                                 t_v=timestep._version, t_shape=tuple(timestep.shape), img=img_in, out0=out)
+            return out
+        out0 = pair["out0"]
+        self._native_cp_exchange(*((out, out0) if computes else (out0, out)))
+        return out
+
+    def _native_cp_exchange(self, own, other) -> None:
+        """ce_dit_cp_exchange on the current stream: `own` into the peer's slot, one barrier, the peer's sample into `other`."""
+        B, _, T, H, W = own.shape
+        with torch.cuda.device(self.device):
+            check(_lib.lib().ce_dit_cp_exchange(self._ensure_handle(), ptr(own), ptr(other), B, T, H, W, current_stream()))
 
     def _native_forward(self, x, t, txt, img, out, b0, caps, txt_in, img_in) -> None:
         """The one place the DiT forward reaches the C ABI (ce_dit_forward_ex).  x [B,C,T,H,W] bf16, t [B] fp32, txt / img bf16,
@@ -811,6 +872,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         """End-to-end variant: all tensors are (pinned) HOST bf16/fp32 tensors; H2D, forward and D2H happen inside the
         C-ABI call (ce_dit_forward_host_ex).  Returns the host sample tensor (and, with `return_device_sample`, a view of the same
         sample still on the device -- valid until the next forward_host call -- for the scheduler step)."""
+        self._refuse_cp("forward_host")
         if not self._packed:
             self.pack_weights()
         B, C, T, H, W = hidden_states.shape

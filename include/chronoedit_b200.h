@@ -137,7 +137,8 @@ int ce_dit_sp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs
  *   region: the flags block (1 KB, first), then two sample slots of [batch, out_channels, frames, height, width] bf16 (each rounded
  *   up to 1 KB) that alternate from call to call, so each call needs one barrier.  Any later call whose full sample fits a slot is
  *   accepted.  ce_dit_bp_region_bytes returns -1 for a world outside 2..8 or a batch it does not divide.
- *   ce_dit_bp_configure: as ce_dit_sp_configure (same refusals); world = 1 switches the split off.
+ *   ce_dit_bp_configure: as ce_dit_sp_configure (same refusals); world = 1 switches the split off.  Refused while the call-pair
+ *   split below is configured.
  *   ce_dit_bp_host_barrier: the test aid of ce_dit_sp_host_barrier, for this group's barrier.
  * A split call refuses, before any launch: a batch the ranks do not divide (so the unchanged diffusers pipeline's batch-1 calls are
  * not split), a sample larger than a slot, block capture or block0_out, and a capturing stream.  ce_dit_forward_fp32 is refused.
@@ -145,6 +146,26 @@ int ce_dit_sp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs
 int64_t ce_dit_bp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width, int world);
 int ce_dit_bp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes);
 int ce_dit_bp_host_barrier(ce_dit* h, int timeout_ms);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Call-pair split over two GPUs: the unchanged diffusers pipeline computes a CFG step as two batch-1 calls with the same latents and
+ * timestep, one with the prompt and one with the negative prompt.  Rank 0 computes the first call, rank 1 the second, each with the
+ * ordinary ce_dit_forward_ex (the token split underneath when configured); ce_dit_forward_ex itself does not look at this group.
+ * After both, ce_dit_cp_exchange gives each rank the other's sample.
+ *   region: the batch split's layout for one whole call: the flags block (1 KB, first), then two slots of [batch, out_channels,
+ *   frames, height, width] bf16 (each rounded up to 1 KB) that alternate from pair to pair, so each pair needs one barrier.  A region
+ *   sized for 8 latent frames serves temporal reasoning's cut to 2.  ce_dit_cp_region_bytes returns -1 for an invalid geometry.
+ *   ce_dit_cp_configure: as ce_dit_bp_configure (same refusals), and a world other than 1 or 2 is refused; world = 1 switches it
+ *   off.  Refused while the batch split is configured: the two CFG splits are exclusive.  The token split composes with either.
+ *   ce_dit_cp_exchange: `own_sample` into the peer's slot of the current set; one barrier; the peer's sample from this rank's own slot
+ *   into `other_sample`.  Three launches on `stream`, stream-ordered with the forward before and whatever reads the samples after.
+ *   Refused before any launch: the group not configured, a sample larger than a slot, and a capturing stream.
+ *   ce_dit_cp_host_barrier: the test aid of ce_dit_sp_host_barrier, for this group's barrier.
+ * ------------------------------------------------------------------------------------------------------------ */
+int64_t ce_dit_cp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width);
+int ce_dit_cp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes);
+int ce_dit_cp_exchange(ce_dit* h, const void* own_sample, void* other_sample, int batch, int frames, int height, int width, void* stream);
+int ce_dit_cp_host_barrier(ce_dit* h, int timeout_ms);
 
 int ce_ipc_alloc(int64_t bytes, void** ptr);
 int ce_ipc_free(void* ptr);
