@@ -166,6 +166,9 @@ SIGNATURES = {
     "ce_rope_table_host": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "ce_linear_ex_bf16": (c_int, [POINTER(LinearArgsC), c_void_p]),
     "ce_linear_fp8_ex": (c_int, [POINTER(LinearFp8ArgsC), c_void_p]),
+    "ce_linear_lora_bf16": (c_int, [POINTER(LinearArgsC), c_void_p, c_int, c_void_p]),
+    "ce_linear_lora_fp8": (c_int, [POINTER(LinearFp8ArgsC), c_void_p, c_int, c_void_p]),
+    "ce_dit_set_lora": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int32), c_int]),
     "ce_quantize_rows_fp8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "ce_dit_set_attention_fp8": (c_int, [c_void_p, c_int]),
     "ce_quantize_heads_fp8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),

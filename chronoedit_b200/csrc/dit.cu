@@ -26,6 +26,12 @@
 
 namespace ce {
 const std::string& last_error();
+// One block GEMM's run-time LoRA entry (ce_dit_set_lora): a_cat [rank, K] and the pre-scaled b_cat [N, rank], bf16 device memory
+struct LoraGemm {
+  const void* a_cat = nullptr;
+  const void* b_cat = nullptr;
+  int rank = 0;
+};
 }
 
 using namespace ce;
@@ -62,9 +68,18 @@ struct ce_dit {
   // TeaCache record mode (ce_dit_set_residual_record): every forward leaves x_after_blocks - x_before_blocks here
   void* resid_rec = nullptr;
   int64_t resid_rec_bytes = 0;
+  // run-time LoRA (ce_dit_set_lora): [num_layers * CE_LORA_TARGETS] entries, empty when off; lora_rmax = their largest rank
+  std::vector<ce::LoraGemm> lora;
+  int lora_rmax = 0;
+  // the current forward's workspace slices for one GEMM's down-projection [Mx, lora_rmax] and low-rank term [Mx, max(3D, F)]
+  bf16* lora_mid = nullptr;
+  bf16* lora_term = nullptr;
 };
 
 enum { CAT_GEMM = 0, CAT_ATTN = 1, CAT_ROWS = 2, CAT_OTHER = 3, NUM_CATS = 4 };
+// ce_dit_set_lora's targets (include/chronoedit_b200.h): the GEMMs of LayerWeights in its order
+enum { LORA_QKV = 0, LORA_OUT1, LORA_Q2, LORA_KV, LORA_ADD_KV, LORA_OUT2, LORA_FFN1, LORA_FFN2 };
+static_assert(LORA_FFN2 + 1 == CE_LORA_TARGETS, "one LoRA target per block GEMM");
 
 namespace {
 
@@ -82,6 +97,8 @@ struct Workspace {
   float* qk_scale;    //                     [M, 2H] their (token, head) scales
   uint8_t* vt8;       //                     [B, H, 128, Lpad] e4m3 V^T
   float* v_scale;     //                     [B, D] its (sample, channel) scales
+  bf16* lora_mid;     // run-time LoRA only: [Mx, R_max] x A_cat^T of one GEMM (Mx = max(M, B Lt, B Li))
+  bf16* lora_term;    //                     [Mx, max(3D, F)] its low-rank term
   int64_t bytes;
 };
 
@@ -121,7 +138,7 @@ int64_t slot_bytes(int64_t region_bytes) { return std::max<int64_t>(0, (region_b
 // Keys of the FP8 attention's V^T rows: L rounded up to the 32-key groups of its layout.
 int vt_keys(int L) { return (L + 31) / 32 * 32; }
 
-Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li, bool fp8, bool attn_fp8) {
+Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li, bool fp8, bool attn_fp8, int lora_rmax = 0) {
   const int64_t D = D_of(c), F = c.ffn_dim, M = (int64_t)B * L;
   const int64_t Kp = (int64_t)c.in_channels * c.patch_t * c.patch_h * c.patch_w;
   const int64_t No = (int64_t)c.out_channels * c.patch_t * c.patch_h * c.patch_w;
@@ -161,6 +178,9 @@ Workspace carve(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li
   w.qk_scale = attn_fp8 ? b.take<float>(M * 2 * H) : nullptr;
   w.vt8 = attn_fp8 ? b.take<uint8_t>((int64_t)B * D * vt_keys(L)) : nullptr;
   w.v_scale = attn_fp8 ? b.take<float>((int64_t)B * D) : nullptr;
+  const int64_t Mx = std::max<int64_t>(M, (int64_t)B * std::max(Lt, Li));
+  w.lora_mid = lora_rmax ? b.take<bf16>(Mx * lora_rmax) : nullptr;
+  w.lora_term = lora_rmax ? b.take<bf16>(Mx * std::max<int64_t>(3 * D, F)) : nullptr;
   w.bytes = b.bytes();
   return w;
 }
@@ -389,19 +409,36 @@ static double attention_flops(const AttnArgs& a) { return 4.0 * a.B * a.H * (dou
 // out[M, N] = epilogue(A[M, K] x W^T + bias) with A and out dense.  `e` brings the epilogue fields (epi, resid, gate,
 // stats_out / stats_mode); the statistics come one per N tile of gemm_tile_n(N).  An e4m3 weight takes two launches: the
 // per-row quantization of A into the workspace, then the FP8 GEMM.
-static int linear(ce_dit* h, cudaStream_t s, const Linear& w, const bf16* A, int M, int N, int K, bf16* out, GemmArgs e) {
+// With a LoRA entry `lo` of rank R > 0 (ce_dit_set_lora), two bf16 GEMMs come first: mid = bf16(A a_cat^T) [M, R], from the bf16 A
+// (before any quantization), and term = bf16(mid b_cat^T) [M, N]; the main GEMM's epilogue adds the term (LoraAddend).
+static int linear(ce_dit* h, cudaStream_t s, const Linear& w, const bf16* A, int M, int N, int K, bf16* out, GemmArgs e,
+                  const LoraGemm* lo = nullptr) {
   GemmArgs g = e;
   g.M = M; g.N = N; g.K = K;
   g.out = out; g.ldo = N;
   g.bias = w.bias;
   if (g.stats_out) g.stats_ld = (N + gemm_tile_n(N) - 1) / gemm_tile_n(N);
+  LoraAddend la;
+  const LoraAddend* lp = nullptr;
+  if (lo && lo->rank > 0) {
+    const int R = lo->rank;
+    GemmArgs d;
+    d.M = M; d.N = R; d.K = K; d.out = h->lora_mid; d.ldo = R;
+    LAUNCH(CAT_GEMM, 2.0 * M * (double)R * K, launch_gemm_bf16(A, K, static_cast<const bf16*>(lo->a_cat), K, d, s));
+    GemmArgs u;
+    u.M = M; u.N = N; u.K = R; u.out = h->lora_term; u.ldo = N;
+    LAUNCH(CAT_GEMM, 2.0 * M * (double)N * R, launch_gemm_bf16(h->lora_mid, R, static_cast<const bf16*>(lo->b_cat), R, u, s));
+    la.t = h->lora_term;
+    la.ld = N;
+    lp = &la;
+  }
   if (w.dtype == 2) {
     LAUNCH(CAT_ROWS, 3.0 * M * (double)K + 4.0 * M, launch_quantize_rows_fp8(A, K, M, K, h->fp8_q, K, h->fp8_scale, s));
     LAUNCH(CAT_GEMM, 2.0 * M * (double)N * K,
            launch_gemm_fp8(reinterpret_cast<const e4m3*>(h->fp8_q), K, h->fp8_scale, static_cast<const e4m3*>(w.weight), K,
-                           w.weight_scale, g, s));
+                           w.weight_scale, g, s, lp));
   } else {
-    LAUNCH(CAT_GEMM, 2.0 * M * (double)N * K, launch_gemm_bf16(A, K, static_cast<const bf16*>(w.weight), K, g, s));
+    LAUNCH(CAT_GEMM, 2.0 * M * (double)N * K, launch_gemm_bf16(A, K, static_cast<const bf16*>(w.weight), K, g, s, lp));
   }
   return CE_OK;
 }
@@ -487,6 +524,7 @@ int ce_dit_internal_rope(ce_dit* h, int frames, int hp, int wp, cudaStream_t s, 
 }
 const ce_dit_config* ce_dit_internal_config(const ce_dit* h) { return &h->cfg; }
 int ce_dit_internal_bp_world(const ce_dit* h) { return h->bp.world; }
+bool ce_dit_internal_lora_set(const ce_dit* h) { return !h->lora.empty(); }
 
 extern "C" {
 
@@ -538,7 +576,7 @@ int64_t ce_dit_workspace_bytes(const ce_dit* h, int batch, int frames, int heigh
   Weights w;
   resolve_weights(h, w);   // only w.fp8 is read here, and it is set even before every weight has been registered
   const int L = frames * (height / h->cfg.patch_h) * (width / h->cfg.patch_w);
-  return carve(h->cfg, nullptr, batch, L, text_len, 257, w.fp8, h->attn_fp8).bytes;
+  return carve(h->cfg, nullptr, batch, L, text_len, 257, w.fp8, h->attn_fp8, h->lora_rmax).bytes;
 }
 
 int64_t ce_dit_last_launch_count(const ce_dit* h) { return h ? h->launches : 0; }
@@ -709,7 +747,8 @@ static int forward_samples(ce_dit* h, const void* hidden_states, const float* ti
   const SpLayout lay = spx ? sp_layout(B, Lfull, D, No, sp.world) : SpLayout();
   if (spx && lay.bytes > sp.region_bytes) return fail(CE_ERR_WORKSPACE, "sequence parallel: peer region too small (ce_dit_sp_region_bytes)");
   CE_REQUIRE(!(spx && W.fp8), "sequence parallelism is not built for FP8 weights: run the FP8 mode on one GPU");
-  Workspace ws = carve(c, workspace, B, L, Lt, Li, W.fp8, h->attn_fp8);
+  CE_REQUIRE(!(spx && !h->lora.empty()), "sequence parallelism is not built for run-time LoRA: clear it first (ce_dit_set_lora with n = 0)");
+  Workspace ws = carve(c, workspace, B, L, Lt, Li, W.fp8, h->attn_fp8, h->lora_rmax);
   if (ws.bytes > workspace_bytes)
     return fail(CE_ERR_WORKSPACE, "workspace too small: need " + std::to_string(ws.bytes) + " bytes, got " + std::to_string(workspace_bytes));
   CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
@@ -722,6 +761,10 @@ static int forward_samples(ce_dit* h, const void* hidden_states, const float* ti
   if ((rc = ensure_rope(h, frames, hp, wp, s))) return rc;   // always the full table [Lfull, 64]
   h->fp8_q = ws.fp8_q;
   h->fp8_scale = ws.fp8_scale;
+  h->lora_mid = ws.lora_mid;
+  h->lora_term = ws.lora_term;
+  // run-time LoRA entry of layer i's GEMM `target`, or null
+  auto lora_of = [&](int i, int target) { return h->lora.empty() ? nullptr : &h->lora[(size_t)i * CE_LORA_TARGETS + target]; };
   // step-invariant context (text / image embedders and every block's cross-attention K/V, :52-60, :147-165): kept in the
   // caller's cache across the steps of one edit when one is given; recomputed into the workspace otherwise
   const int64_t kv_t_elems = (int64_t)B * Lt * 2 * D, kv_i_elems = c.image_dim > 0 ? (int64_t)B * Li * 2 * D : 0;
@@ -795,7 +838,7 @@ static int forward_samples(ce_dit* h, const void* hidden_states, const float* ti
     const float* mod = ws.mod + (size_t)i * B * 6 * D;  // [B, 6, D]: shift, scale, gate, c_shift, c_scale, c_gate
     // 1. self-attention
     LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, mod + 1 * D, mod + 0 * D, 6 * D, L, nullptr, nullptr, 1));
-    if ((rc = linear(h, s, lw.qkv, ws.xn, M, 3 * D, D, ws.qkv, epi(EPI_BIAS, ws.stats_qkv, 2)))) return rc;
+    if ((rc = linear(h, s, lw.qkv, ws.xn, M, 3 * D, D, ws.qkv, epi(EPI_BIAS, ws.stats_qkv, 2), lora_of(i, LORA_QKV)))) return rc;
     const bf16* attn_in = ws.attn;
     if (spx) {
       // heads <-> tokens exchange by peer stores: q | k normalised + rotated and scattered by head, v scattered by head, barrier,
@@ -857,21 +900,21 @@ static int forward_samples(ce_dit* h, const void* hidden_states, const float* ti
         LAUNCH(CAT_ATTN, attention_flops(a), launch_attention(a, s));
       }
     }
-    if ((rc = linear(h, s, lw.out1, attn_in, M, D, D, ws.x, resid_epi(mod + 2 * D)))) return rc;
+    if ((rc = linear(h, s, lw.out1, attn_in, M, D, D, ws.x, resid_epi(mod + 2 * D), lora_of(i, LORA_OUT1)))) return rc;
     // 2. cross-attention
     LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, nullptr, nullptr, 0, 0, lw.norm2_w, lw.norm2_b, 0));
     bf16* q2 = ws.qkv;  // [M, D]
-    if ((rc = linear(h, s, lw.q2, ws.xn, M, D, D, q2, epi(EPI_BIAS, ws.stats_q2, 2)))) return rc;
+    if ((rc = linear(h, s, lw.q2, ws.xn, M, D, D, q2, epi(EPI_BIAS, ws.stats_q2, 2), lora_of(i, LORA_Q2)))) return rc;
     LAUNCH(CAT_ROWS, 4.0 * M * D, launch_rmsnorm_rope(q2, D, M, D, c.eps, lw.norm_q2, nullptr, 1, nullptr, nullptr, 0, c.attention_head_dim,
                                                       partials(ws.stats_q2, tD), s));
     bf16* kv_text = kv_text_of(i);
     bf16* kv_img = kv_img_of(i);
     if (ctx_compute) {
-      if ((rc = linear(h, s, lw.kv, ws.ctx_text, B * Lt, 2 * D, D, kv_text, epi(EPI_BIAS)))) return rc;
+      if ((rc = linear(h, s, lw.kv, ws.ctx_text, B * Lt, 2 * D, D, kv_text, epi(EPI_BIAS), lora_of(i, LORA_KV)))) return rc;
       LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(kv_text, 2 * D, B * Lt, D, c.eps, lw.norm_k2, nullptr, 1, nullptr, nullptr, 0, c.attention_head_dim,
                                                      RowPartials{}, s));
       if (c.image_dim > 0) {
-        if ((rc = linear(h, s, lw.add_kv, ws.ctx_img, B * Li, 2 * D, D, kv_img, epi(EPI_BIAS)))) return rc;
+        if ((rc = linear(h, s, lw.add_kv, ws.ctx_img, B * Li, 2 * D, D, kv_img, epi(EPI_BIAS), lora_of(i, LORA_ADD_KV)))) return rc;
         LAUNCH(CAT_OTHER, 0.0, launch_rmsnorm_rope(kv_img, 2 * D, B * Li, D, c.eps, lw.norm_added_k, nullptr, 1, nullptr, nullptr, 0, c.attention_head_dim,
                                                        RowPartials{}, s));
       }
@@ -891,11 +934,11 @@ static int forward_samples(ce_dit* h, const void* hidden_states, const float* ti
       a.scale = attn_scale;
       LAUNCH(CAT_ATTN, attention_flops(a), launch_attention(a, s));
     }
-    if ((rc = linear(h, s, lw.out2, ws.attn, M, D, D, ws.x, resid_epi(nullptr)))) return rc;
+    if ((rc = linear(h, s, lw.out2, ws.attn, M, D, D, ws.x, resid_epi(nullptr), lora_of(i, LORA_OUT2)))) return rc;
     // 3. feed-forward
     LAUNCH(CAT_ROWS, 4.0 * M * D, ln(ws.x, ws.xn, mod + 4 * D, mod + 3 * D, 6 * D, L, nullptr, nullptr, 1));
-    if ((rc = linear(h, s, lw.ffn1, ws.xn, M, F, D, ws.hbuf, epi(EPI_BIAS_GELU_TANH)))) return rc;
-    if ((rc = linear(h, s, lw.ffn2, ws.hbuf, M, D, F, ws.x, resid_epi(mod + 5 * D)))) return rc;
+    if ((rc = linear(h, s, lw.ffn1, ws.xn, M, F, D, ws.hbuf, epi(EPI_BIAS_GELU_TANH), lora_of(i, LORA_FFN1)))) return rc;
+    if ((rc = linear(h, s, lw.ffn2, ws.hbuf, M, D, F, ws.x, resid_epi(mod + 5 * D), lora_of(i, LORA_FFN2)))) return rc;
     if (i == 0 && block0_out)
       CE_CHECK_CUDA(cudaMemcpyAsync(block0_out, ws.x, (size_t)M * D * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
     for (const auto& cap : h->capture)
@@ -1162,6 +1205,61 @@ int ce_linear_fp8_ex(const ce_linear_fp8_args* a, void* stream) {
   CE_REQUIRE(a != nullptr, "ce_linear_fp8_ex: null args");
   return launch_gemm_fp8(reinterpret_cast<const e4m3*>(a->base.A), a->base.lda, a->a_scale, reinterpret_cast<const e4m3*>(a->base.W),
                          a->base.ldw, a->w_scale, gemm_args_of(&a->base), reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_linear_lora_bf16(const ce_linear_args* a, const void* term, int ldt, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(a != nullptr, "ce_linear_lora_bf16: null args");
+  LoraAddend lo;
+  lo.t = reinterpret_cast<const bf16*>(term);
+  lo.ld = ldt;
+  return launch_gemm_bf16(reinterpret_cast<const bf16*>(a->A), a->lda, reinterpret_cast<const bf16*>(a->W), a->ldw, gemm_args_of(a),
+                          reinterpret_cast<cudaStream_t>(stream), &lo);
+}
+
+int ce_linear_lora_fp8(const ce_linear_fp8_args* a, const void* term, int ldt, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(a != nullptr, "ce_linear_lora_fp8: null args");
+  LoraAddend lo;
+  lo.t = reinterpret_cast<const bf16*>(term);
+  lo.ld = ldt;
+  return launch_gemm_fp8(reinterpret_cast<const e4m3*>(a->base.A), a->base.lda, a->a_scale, reinterpret_cast<const e4m3*>(a->base.W),
+                         a->base.ldw, a->w_scale, gemm_args_of(&a->base), reinterpret_cast<cudaStream_t>(stream), &lo);
+}
+
+int ce_dit_set_lora(ce_dit* h, const void* const* a_cat, const void* const* b_cat, const int32_t* rank, int n) {
+  CE_REQUIRE(h, "ce_dit_set_lora: null handle");
+  const ce_dit_config& c = h->cfg;
+  if (n == 0) {
+    h->lora.clear();
+    h->lora_rmax = 0;
+    return CE_OK;
+  }
+  CE_REQUIRE(n == c.num_layers * CE_LORA_TARGETS && a_cat && b_cat && rank,
+             "ce_dit_set_lora: the tables need num_layers * CE_LORA_TARGETS entries (or n = 0 to clear)");
+  auto aligned16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  std::vector<LoraGemm> t(n);
+  int rmax = 0;
+  for (int i = 0; i < n; ++i) {
+    const int target = i % CE_LORA_TARGETS;
+    const std::string at = "ce_dit_set_lora: entry " + std::to_string(i) + " (layer " + std::to_string(i / CE_LORA_TARGETS) +
+                           ", target " + std::to_string(target) + "): ";
+    if (rank[i] < 0 || rank[i] % 8 != 0) return fail(CE_ERR_INVALID, at + "rank must be a multiple of 8 (zero-padded), 0 for none");
+    if (rank[i] == 0) continue;
+    if (!a_cat[i] || !b_cat[i] || !aligned16(a_cat[i]) || !aligned16(b_cat[i]))
+      return fail(CE_ERR_INVALID, at + "a_cat / b_cat must be non-null, 16-byte aligned device pointers");
+    if (target == LORA_ADD_KV && c.image_dim <= 0) return fail(CE_ERR_INVALID, at + "the model has no image projection (add_kv_proj)");
+    t[i].a_cat = a_cat[i];
+    t[i].b_cat = b_cat[i];
+    t[i].rank = rank[i];
+    rmax = std::max(rmax, (int)rank[i]);
+  }
+  if (rmax == 0) t.clear();
+  h->lora = std::move(t);
+  h->lora_rmax = rmax;
+  return CE_OK;
 }
 
 int ce_dit_set_attention_fp8(ce_dit* h, int enabled) {

@@ -96,11 +96,14 @@ __device__ __forceinline__ void stage_operands(const Staging<BN>& st, const Gemm
 // their stores, since out and resid may alias), the stored values written back to the staging tile, then the
 // statistics with the consumers' lane layout (4 lanes per row, lane q summing columns 8j + 2q, 8j + 2q + 1 for ascending j, then
 // the xor-1 and xor-2 shuffles), so they are the same bits as when the consumers computed them from their registers.
-template <int BN>
-__device__ __forceinline__ void drain_tile(const Staging<BN>& st, const GemmArgs& g, int mb, int nb) {
+// LORA: the low-rank term (LoraAddend) is loaded beside the residual and added first, y = bf16(y + t), so GELU, the gate and
+// the statistics see the post-LoRA output.
+template <int BN, bool LORA>
+__device__ __forceinline__ void drain_tile(const Staging<BN>& st, const GemmArgs& g, const LoraAddend& lo, int mb, int nb) {
   constexpr int CPR = Staging<BN>::CPR;
   constexpr int ITERS = BN / 32;              // chunks per lane per group
-  constexpr int U = ITERS < 4 ? ITERS : 4;    // residual loads in flight per lane (8 spill under the epilogue warps' 88 registers)
+  // residual loads in flight per lane (8 spill under the epilogue warps' 88 registers; with the LoRA term beside them, 4 spill)
+  constexpr int U = LORA ? (ITERS < 2 ? ITERS : 2) : (ITERS < 4 ? ITERS : 4);
   const int lane = threadIdx.x & 31;
   const bool resid_epi = g.epi == EPI_BIAS_GATE_RESID || g.epi == EPI_BIAS_RESID;
   const bool gate_epi = g.epi == EPI_BIAS_GATE_RESID;
@@ -113,6 +116,14 @@ __device__ __forceinline__ void drain_tile(const Staging<BN>& st, const GemmArgs
       for (int u = 0; u < U; ++u) {
         const int idx = lane + 32 * (i0 + u), m = mb * BM + grp * 8 + idx / CPR, n = nb * BN + (idx % CPR) * 8;
         rw[u] = resid_epi && m < g.M && n < g.N ? *reinterpret_cast<const uint4*>(g.resid + (size_t)m * g.ldr + n) : make_uint4(0, 0, 0, 0);
+      }
+      uint4 lw[LORA ? U : 1];
+      if constexpr (LORA) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const int idx = lane + 32 * (i0 + u), m = mb * BM + grp * 8 + idx / CPR, n = nb * BN + (idx % CPR) * 8;
+          lw[u] = m < g.M && n < g.N ? *reinterpret_cast<const uint4*>(lo.t + (size_t)m * lo.ld + n) : make_uint4(0, 0, 0, 0);
+        }
       }
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -131,6 +142,12 @@ __device__ __forceinline__ void drain_tile(const Staging<BN>& st, const GemmArgs
         for (int e = 0; e < 4; ++e) {
           const float2 yv = unpack_bf16x2(v[e]);
           float y0 = yv.x, y1 = yv.y;
+          if constexpr (LORA) {
+            const uint32_t lu = e == 0 ? lw[u].x : e == 1 ? lw[u].y : e == 2 ? lw[u].z : lw[u].w;
+            const float2 tv = unpack_bf16x2(lu);
+            y0 = bf16_round(y0 + tv.x);
+            y1 = bf16_round(y1 + tv.y);
+          }
           if (gelu) {
             if (g.epi == EPI_BIAS_GELU_TANH) {
               y0 = bf16_round(gelu_tanh_f(y0));
@@ -199,9 +216,9 @@ __device__ __forceinline__ void drain_tile(const Staging<BN>& st, const GemmArgs
 //   epilogue warps  (warps 1-3 of warpgroup 0) GELU, residual / gate, the stores and the row statistics (drain_tile), while the
 //                   consumers run the next tile
 // The arithmetic and its rounding points are those of a single pass from the accumulators; the output is the same bits.
-template <int BN, int STAGES, class T>
+template <int BN, int STAGES, class T, bool LORA>
 __device__ __forceinline__ void gemm_tiles(const CUtensorMap* tma_a, const CUtensorMap* tma_b, const GemmArgs& g, const float* s_a,
-                                           const float* s_w) {
+                                           const float* s_w, const LoraAddend& lo) {
   constexpr int KB = BK_OF<T>;
   constexpr bool FP8 = sizeof(T) == 1;
   const int tiles_m = (g.M + BM - 1) / BM;
@@ -237,7 +254,7 @@ __device__ __forceinline__ void gemm_tiles(const CUtensorMap* tma_a, const CUten
               if (g.out) {
                 int mb, nb;
                 tile_coords(t, tiles_m, tiles_n, g.group_m, mb, nb);
-                drain_tile<BN>(st, g, mb, nb);
+                drain_tile<BN, LORA>(st, g, lo, mb, nb);
               }
               mbar_arrive(st.drained);
             }
@@ -310,18 +327,33 @@ __device__ __forceinline__ void gemm_tiles(const CUtensorMap* tma_a, const CUten
 template <int BN, int STAGES>
 __global__ void __launch_bounds__(RING_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g) {
-  gemm_tiles<BN, STAGES, bf16>(&tma_a, &tma_b, g, nullptr, nullptr);
+  gemm_tiles<BN, STAGES, bf16, false>(&tma_a, &tma_b, g, nullptr, nullptr, LoraAddend());
 }
 
 template <int BN, int STAGES>
 __global__ void __launch_bounds__(RING_THREADS, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g, const float* s_a,
                 const float* s_w) {
-  gemm_tiles<BN, STAGES, e4m3>(&tma_a, &tma_b, g, s_a, s_w);
+  gemm_tiles<BN, STAGES, e4m3, false>(&tma_a, &tma_b, g, s_a, s_w, LoraAddend());
+}
+
+// The same kernels with the LoRA addend in the epilogue (separate kernels, so that the ones above keep their parameters and code).
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(RING_THREADS, 1)
+gemm_bf16_lora_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g, LoraAddend lo) {
+  gemm_tiles<BN, STAGES, bf16, true>(&tma_a, &tma_b, g, nullptr, nullptr, lo);
+}
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(RING_THREADS, 1)
+gemm_fp8_lora_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, GemmArgs g, const float* s_a,
+                     const float* s_w, LoraAddend lo) {
+  gemm_tiles<BN, STAGES, e4m3, true>(&tma_a, &tma_b, g, s_a, s_w, lo);
 }
 
 template <class T>
-int launch_gemm(const T* A, int lda, const float* s_a, const T* W, int ldw, const float* s_w, const GemmArgs& g, cudaStream_t stream) {
+int launch_gemm(const T* A, int lda, const float* s_a, const T* W, int ldw, const float* s_w, const GemmArgs& g, cudaStream_t stream,
+                const LoraAddend* lo) {
   constexpr bool fp8 = sizeof(T) == 1;
   CE_REQUIRE(g.M > 0 && g.N > 0 && g.K > 0, "gemm: empty problem");
   CE_REQUIRE(g.N % 8 == 0, "gemm: N must be a multiple of 8");
@@ -337,6 +369,10 @@ int launch_gemm(const T* A, int lda, const float* s_a, const T* W, int ldw, cons
   if (g.epi == EPI_BIAS_GATE_RESID)
     CE_REQUIRE(g.gate != nullptr && g.gate_stride % 4 == 0 && g.rows_per_batch > 0 && (reinterpret_cast<uintptr_t>(g.gate) & 15) == 0,
                "gemm: gate epilogue needs gate, 16-byte aligned");
+  if (lo)
+    CE_REQUIRE(lo->t != nullptr && g.out != nullptr && g.out_f32 == nullptr && lo->ld % 8 == 0 && lo->ld >= g.N &&
+                   (reinterpret_cast<uintptr_t>(lo->t) & 15) == 0,
+               "gemm: the LoRA addend needs out (no out_f32), a 16-byte aligned term, ld % 8 == 0 and ld >= N");
   if (g.stats_mode) CE_REQUIRE(g.stats_out != nullptr && g.out != nullptr && g.stats_ld >= (g.N + gemm_tile_n(g.N) - 1) / gemm_tile_n(g.N) &&
                                (g.stats_mode == 1 || g.stats_mode == 2), "gemm: stats_out / stats_ld / stats_mode");
   GemmArgs a = g;
@@ -353,10 +389,20 @@ int launch_gemm(const T* A, int lda, const float* s_a, const T* W, int ldw, cons
   const int tiles = ((a.M + BM - 1) / BM) * ((a.N + bn - 1) / bn);
   // Ring depth: what is left of the 227 KB beside the staging tile (64 KB at BN = 256, where one stage of 48 KB has to go).
   if constexpr (fp8) {
+    if (lo) {
+      if (bn == 256) return launch_ring_gemm<256, 3, Staging<256>::BYTES>(gemm_fp8_lora_kernel<256, 3>, tiles, stream, ta, tb, a, s_a, s_w, *lo);
+      if (bn == 128) return launch_ring_gemm<128, 6, Staging<128>::BYTES>(gemm_fp8_lora_kernel<128, 6>, tiles, stream, ta, tb, a, s_a, s_w, *lo);
+      return launch_ring_gemm<64, 8, Staging<64>::BYTES>(gemm_fp8_lora_kernel<64, 8>, tiles, stream, ta, tb, a, s_a, s_w, *lo);
+    }
     if (bn == 256) return launch_ring_gemm<256, 3, Staging<256>::BYTES>(gemm_fp8_kernel<256, 3>, tiles, stream, ta, tb, a, s_a, s_w);
     if (bn == 128) return launch_ring_gemm<128, 6, Staging<128>::BYTES>(gemm_fp8_kernel<128, 6>, tiles, stream, ta, tb, a, s_a, s_w);
     return launch_ring_gemm<64, 8, Staging<64>::BYTES>(gemm_fp8_kernel<64, 8>, tiles, stream, ta, tb, a, s_a, s_w);
   } else {
+    if (lo) {
+      if (bn == 256) return launch_ring_gemm<256, 3, Staging<256>::BYTES>(gemm_bf16_lora_kernel<256, 3>, tiles, stream, ta, tb, a, *lo);
+      if (bn == 128) return launch_ring_gemm<128, 6, Staging<128>::BYTES>(gemm_bf16_lora_kernel<128, 6>, tiles, stream, ta, tb, a, *lo);
+      return launch_ring_gemm<64, 8, Staging<64>::BYTES>(gemm_bf16_lora_kernel<64, 8>, tiles, stream, ta, tb, a, *lo);
+    }
     if (bn == 256) return launch_ring_gemm<256, 3, Staging<256>::BYTES>(gemm_bf16_kernel<256, 3>, tiles, stream, ta, tb, a);
     if (bn == 128) return launch_ring_gemm<128, 6, Staging<128>::BYTES>(gemm_bf16_kernel<128, 6>, tiles, stream, ta, tb, a);
     return launch_ring_gemm<64, 8, Staging<64>::BYTES>(gemm_bf16_kernel<64, 8>, tiles, stream, ta, tb, a);
@@ -365,15 +411,15 @@ int launch_gemm(const T* A, int lda, const float* s_a, const T* W, int ldw, cons
 
 }  // namespace
 
-int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmArgs& g, cudaStream_t stream) {
-  return launch_gemm<bf16>(A, lda, nullptr, W, ldw, nullptr, g, stream);
+int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmArgs& g, cudaStream_t stream, const LoraAddend* lora) {
+  return launch_gemm<bf16>(A, lda, nullptr, W, ldw, nullptr, g, stream, lora);
 }
 
 int launch_gemm_fp8(const e4m3* Aq, int lda, const float* s_a, const e4m3* Wq, int ldw, const float* s_w, const GemmArgs& g,
-                    cudaStream_t stream) {
+                    cudaStream_t stream, const LoraAddend* lora) {
   CE_REQUIRE(s_a != nullptr && s_w != nullptr && (reinterpret_cast<uintptr_t>(s_w) & 7) == 0,
              "gemm_fp8: a_scale and w_scale are required, w_scale 8-byte aligned");
-  return launch_gemm<e4m3>(Aq, lda, s_a, Wq, ldw, s_w, g, stream);
+  return launch_gemm<e4m3>(Aq, lda, s_a, Wq, ldw, s_w, g, stream, lora);
 }
 
 int run_gemm(Launcher& run, const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K, bf16* out, int ldo, const bf16* bias, int epi,

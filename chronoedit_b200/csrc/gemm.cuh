@@ -45,16 +45,25 @@ struct GemmArgs {
   int group_m = 0;              // tile rasterisation: M-tiles per group (L2 reuse); 0 = chosen by launch_gemm_bf16
 };
 
+// Run-time LoRA (dit.cu linear()): the low-rank term t [M, ld] bf16 (ld % 8 == 0, ld >= N, 16-byte aligned), added as
+// y = bf16(y + t) right after y = bf16(acc + bias), before GELU, residual / gate and the row statistics.  Given to the launch, it
+// selects the kernels built with this addend; without it the launch runs the kernels that have none.  Not with out_f32.
+struct LoraAddend {
+  const bf16* t = nullptr;
+  int ld = 0;
+};
+
 // N tile width launch_gemm_bf16 uses for a given N (the granularity of GemmArgs::stats_out)
 inline int gemm_tile_n(int N) { return N >= 256 ? 256 : (N >= 128 ? 128 : 64); }
 
 // out[M,N] = epilogue(A[M,K] (row-major, lda) x W[N,K]^T (row-major = nn.Linear weight, ldw)).
-int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmArgs& g, cudaStream_t stream);
+int launch_gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, const GemmArgs& g, cudaStream_t stream,
+                     const LoraAddend* lora = nullptr);
 
 // The FP8 mode's GEMM: y[m,n] = (sum_k Aq[m,k] Wq[n,k] * s_a[m]) * s_w[n] with e4m3 operands (Aq row-major, lda; Wq row-major, ldw;
 // lda, ldw multiples of 16) and fp32 scales s_a[M], s_w[N]; out[M,N] = epilogue(y) exactly as launch_gemm_bf16 applies it to acc.
 int launch_gemm_fp8(const e4m3* Aq, int lda, const float* s_a, const e4m3* Wq, int ldw, const float* s_w, const GemmArgs& g,
-                    cudaStream_t stream);
+                    cudaStream_t stream, const LoraAddend* lora = nullptr);
 
 // One launch_gemm_bf16 through `run`, with only the epilogue fields bias / epi / resid.
 int run_gemm(Launcher& run, const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K, bf16* out, int ldo, const bf16* bias = nullptr,

@@ -24,6 +24,12 @@ from ._lib import CEError, DiTConfigC, check, current_stream, ptr
 
 # reference `_keep_in_fp32_modules` (transformer_chronoedit.py:338)
 KEEP_FP32 = ("time_embedder", "scale_shift_table", "norm1", "norm2", "norm3")
+# Run-time LoRA (set_adapters): block linear layer -> (ce_dit_set_lora target, part of the fused GEMM's N, parts).  The fused QKV
+# and context K | V GEMMs stack their layers' rows, so an adapter's lora_B lands at rows [part * N, (part + 1) * N) of the target.
+LORA_TARGETS = {"attn1.to_q": (0, 0, 3), "attn1.to_k": (0, 1, 3), "attn1.to_v": (0, 2, 3), "attn1.to_out.0": (1, 0, 1),
+                "attn2.to_q": (2, 0, 1), "attn2.to_k": (3, 0, 2), "attn2.to_v": (3, 1, 2), "attn2.add_k_proj": (4, 0, 2),
+                "attn2.add_v_proj": (4, 1, 2), "attn2.to_out.0": (5, 0, 1), "ffn.net.0.proj": (6, 0, 1), "ffn.net.2": (7, 0, 1)}
+LORA_NUM_TARGETS = 8
 
 # The FP8 mode's weights: the six per-token GEMMs of every block (attn1.to_qkv is the fused to_q | to_k | to_v).  The patch
 # embedding, the condition embedders, proj_out and the step-invariant cross-attention K/V projections stay bf16.
@@ -232,6 +238,14 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._ctx_slots = 2
         self._ctx_cache: list = []   # entries: dict(txt=, img=, txt_v=, img_v=, shape=, buf=)
         self._lora_adapters: Dict[str, Dict[str, torch.Tensor]] = {}
+        # run-time LoRA (set_adapters): the active set [(name, weight)] in activation order, the on / off switch, and what the
+        # handle holds: key (set, scale, device) of the packed tables, the tables {(layer, target): (A_cat, B_raw, col_scale, B_cat)}
+        self._lora_set: list = []
+        self._lora_on = True
+        self._lora_gen = 0      # bumped whenever a loaded adapter's content may have changed: part of the tables' key
+        self._lora_scale = 1.0  # the last attention_kwargs["scale"]: forward_host, which takes none, keeps it
+        self._lora_key = None
+        self._lora_tables: Dict[Tuple[int, int], Tuple[torch.Tensor, ...]] = {}
         self.last_captures: Dict[int, torch.Tensor] = {}
         self._fp8 = False
         self._fp8_attention = False
@@ -259,6 +273,9 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._ctx_cache = []
         self._workspaces = {}
         self._drop_teacache_states()
+        if self._lora_key is not None:   # the packed LoRA tables are rebuilt on the new device (or cleared from the handle)
+            self._lora_key = ("moved",)
+        self._lora_tables = {}
         return super()._apply(fn, *a, **k)
 
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
@@ -374,6 +391,8 @@ class ChronoEditTransformer3DModel(nn.Module):
         if not getattr(self, "_fp32_keepalive", None):
             raise CEError("call enable_fp32_validation(fp32_state_dict) first")
         self._refuse_cp("forward_fp32")
+        if self._lora_active():
+            raise CEError("forward_fp32 is not built for run-time LoRA (set_adapters): call disable_lora() first")
         dev = self.device
         B, C, T, H, W = hidden_states.shape
         x = hidden_states.to(device=dev, dtype=torch.float32).contiguous()
@@ -492,13 +511,18 @@ class ChronoEditTransformer3DModel(nn.Module):
         return_block0: bool = False,
         capture_layers: Optional[Tuple[int, ...]] = None,
     ) -> Union[Transformer2DModelOutput, Tuple[torch.Tensor]]:
-        # attention_kwargs["scale"] only matters for un-fused PEFT LoRA layers (transformer_chronoedit.py:406-419): without the
-        # PEFT backend the reference warns and ignores it (:416-419); this mirror holds fused weights only, so it does the same.
-        if attention_kwargs is not None and float(attention_kwargs.get("scale", 1.0)) != 1.0:
+        # attention_kwargs["scale"] only matters for un-fused PEFT LoRA layers (transformer_chronoedit.py:406-419): it multiplies
+        # every active adapter's scaling (PEFT's scale_lora_layers).  With no adapter active at run time the reference warns and
+        # ignores it (:416-419), and so does this mirror.
+        lora_scale = 1.0 if attention_kwargs is None else float(attention_kwargs.get("scale", 1.0))
+        if lora_scale != 1.0 and not self._lora_active():
             import warnings
 
             warnings.warn("Passing `scale` via `attention_kwargs` when not using the PEFT backend is ineffective "
                           "(LoRA must be fused with fuse_lora(lora_scale=...) before inference).")
+        if self._lora_active() and getattr(self, "_sp_state", None):
+            raise CEError("run-time LoRA (set_adapters) is not built for sequence parallelism: call disable_lora() or disable the "
+                          "sequence-parallel mode first")
         dev = self.device
         if hidden_states.dim() != 5:
             raise CEError("hidden_states must be [B, C, T, H, W]")
@@ -516,6 +540,8 @@ class ChronoEditTransformer3DModel(nn.Module):
         cp = getattr(self, "_cp_state", None)
         role, pair = self._cp_role(hidden_states, timestep, encoder_hidden_states_image, return_block0, capture_layers) if cp else (0, None)
         computes = not cp or role == cp["rank"]
+        self._lora_scale = lora_scale
+        self._lora_sync(lora_scale)
         x = hidden_states.to(device=dev, dtype=torch.bfloat16).contiguous()
         t = timestep.to(device=dev, dtype=torch.float32).reshape(-1)
         if t.numel() == 1 and B > 1:
@@ -538,13 +564,14 @@ class ChronoEditTransformer3DModel(nn.Module):
         # (no graph replay in sequence-parallel or batch-split mode: the peer barrier's epoch is a launch argument and must advance
         # every forward)
         # (no graph replay with TeaCache either: each call chooses between two launch sequences after a device-to-host read)
+        # (nor with run-time LoRA: a set change moves the tables the captured launches would read)
         # (a call of a CFG pair that the other rank computes runs no forward and touches no per-conditioning state)
         if not computes:
             pass
         elif self._teacache is not None:
             self._teacache_forward(x, t, txt, img, out, encoder_hidden_states, encoder_hidden_states_image)
         elif (self.use_cuda_graph and not caps and b0 is None and not getattr(self, "_sp_state", None)
-              and not getattr(self, "_bp_state", None) and not cp):
+              and not getattr(self, "_bp_state", None) and not cp and not self._lora_active()):
             out = self._graphed_forward(x, t, txt, img, encoder_hidden_states, encoder_hidden_states_image)
         else:
             self._native_forward(x, t, txt, img, out, b0, caps, encoder_hidden_states, encoder_hidden_states_image)
@@ -873,6 +900,10 @@ class ChronoEditTransformer3DModel(nn.Module):
         C-ABI call (ce_dit_forward_host_ex).  Returns the host sample tensor (and, with `return_device_sample`, a view of the same
         sample still on the device -- valid until the next forward_host call -- for the scheduler step)."""
         self._refuse_cp("forward_host")
+        if self._lora_active() and getattr(self, "_sp_state", None):
+            raise CEError("run-time LoRA (set_adapters) is not built for sequence parallelism: call disable_lora() or disable the "
+                          "sequence-parallel mode first")
+        self._lora_sync(self._lora_scale)   # no attention_kwargs here: the scale of the last forward() call
         if not self._packed:
             self.pack_weights()
         B, C, T, H, W = hidden_states.shape
@@ -925,8 +956,10 @@ class ChronoEditTransformer3DModel(nn.Module):
 
     def _parse_lora(self, lora_state_dict: Dict[str, torch.Tensor], adapter_name: Optional[str]):
         """Pass 1 of fuse_lora: key grammar, name mapping, presence of both factors, shapes.  Nothing is modified here, so a bad
-        file leaves the model untouched.  Returns [(parameter, A, B, alpha or None)]."""
+        file leaves the model untouched.  Returns [(parameter, A, B, alpha or None, module name)]; for a block weight that
+        enable_fp8() replaced, the parameter is its `weight_fp8` buffer (run-time LoRA reads its shape only)."""
         params = dict(self.named_parameters())
+        params.update({n[: -len("_fp8")]: b for n, b in self.named_buffers() if n.endswith(".weight_fp8")})
         pairs: Dict[str, Dict[str, torch.Tensor]] = {}
         for key, val in lora_state_dict.items():
             k = key
@@ -975,7 +1008,7 @@ class ChronoEditTransformer3DModel(nn.Module):
             r = A.shape[0]
             if A.dim() != 2 or B.dim() != 2 or A.shape != (r, w.shape[1]) or B.shape != (w.shape[0], r):
                 raise CEError(f"fuse_lora: shapes of '{mod}' do not match: A {tuple(A.shape)} B {tuple(B.shape)} W {tuple(w.shape)}")
-            plan.append((w, A, B, float(d["alpha"]) if "alpha" in d else None))
+            plan.append((w, A, B, float(d["alpha"]) if "alpha" in d else None, mod))
         return plan
 
     def load_lora_adapter(self, state_dict: Dict[str, torch.Tensor], prefix: Optional[str] = "transformer", network_alphas=None,
@@ -988,9 +1021,14 @@ class ChronoEditTransformer3DModel(nn.Module):
         name = adapter_name or f"default_{len(self._lora_adapters)}"
         self._parse_lora(state_dict, None)   # fail now, not at fuse time
         self._lora_adapters[name] = dict(state_dict)
+        self._lora_gen += 1   # the name may be in the active set with other content: the packed tables are stale
 
     def unload_lora(self) -> None:
         self._lora_adapters.clear()
+        self._lora_gen += 1
+        if self._lora_set:
+            self._lora_set = []
+            self._lora_changed()
 
     @torch.no_grad()
     def fuse_lora(self, *args, **kwargs) -> int:
@@ -1008,6 +1046,9 @@ class ChronoEditTransformer3DModel(nn.Module):
         touched.  One-time weight preparation with torch matmuls; not on the per-step path.  Returns the number of weights updated."""
         if self._fp8:
             raise CEError("fuse_lora after enable_fp8(): fuse the LoRA into the bf16 weights first, then call enable_fp8()")
+        if self._lora_active():
+            raise CEError("fuse_lora while adapters are active at run time (set_adapters): merging a run-time set into the weights "
+                          "is not built; call disable_lora() or delete_adapters(...) first")
         lora_state_dict = kwargs.pop("lora_state_dict", None)
         if args and isinstance(args[0], dict):        # fuse_lora(state_dict[, lora_scale])
             lora_state_dict, args = args[0], args[1:]
@@ -1028,7 +1069,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         n = 0
         deltas = []
         for plan in plans:
-            for w, A, B, alpha in plan:
+            for w, A, B, alpha, _ in plan:
                 A, B = A.to(w.device, w.dtype), B.to(w.device, w.dtype)
                 r = A.shape[0]
                 delta = (B @ A) * (float(lora_scale) * (alpha if alpha is not None else float(r)) / r)   # peft get_delta_weight
@@ -1040,9 +1081,159 @@ class ChronoEditTransformer3DModel(nn.Module):
             n += 1
         if lora_state_dict is None:
             self._lora_adapters.clear()   # merged: a second fuse_lora must not add them again
+            self._lora_set = []           # and a (switched-off) run-time set of them is gone with them
+            self._lora_gen += 1
         self._ctx_cache = []              # cross-attention K/V cached from the old weights are stale
         self._drop_teacache_states()      # and so are the TeaCache residuals
         return n
+
+    # ------------------------------------------------------------------------------------------ run-time LoRA
+    # diffusers' PEFT names (PeftAdapterMixin), so pipe.set_adapters(...) reaches this module unchanged.  DESIGN.md, "Run-time LoRA".
+    def set_adapters(self, adapter_names, weights=None) -> None:
+        """Run the adapters `adapter_names` (loaded with load_lora_adapter) beside the block GEMMs, without touching the weights:
+        each linear layer an adapter covers computes base + bf16(bf16(x A^T) B^T) * weight * alpha / r, summed over the set.
+        `weights` is one number for all or one per adapter (default 1; None in a list means 1, as in diffusers).  Everything is validated before anything changes: an
+        unknown name, and an adapter on a module other than a block linear layer (LORA_TARGETS; merge those with fuse_lora), are
+        refused.  The factors are packed once, on the module's device, in bf16.  Works with FP8 weights and FP8 attention, the
+        context cache, TeaCache, the batch and call-pair splits and forward_host; not with sequence parallelism or forward_fp32.
+        A new set drops the context cache, the TeaCache states and captured CUDA graphs; graphs are not replayed while a set is
+        active.  An empty list clears the set."""
+        names = [adapter_names] if isinstance(adapter_names, str) else list(adapter_names)
+        if weights is None:
+            ws = [1.0] * len(names)
+        elif isinstance(weights, (int, float)):
+            ws = [float(weights)] * len(names)
+        else:
+            ws = list(weights)
+            if len(ws) != len(names):
+                raise ValueError(f"set_adapters: {len(names)} adapters but {len(ws)} weights")
+            if not all(w is None or isinstance(w, (int, float)) for w in ws):
+                raise CEError("set_adapters: per-block weight dicts are not built; pass one number (or None for 1) per adapter")
+            ws = [1.0 if w is None else float(w) for w in ws]
+        missing = [n for n in names if n not in self._lora_adapters]
+        if missing:
+            raise CEError(f"set_adapters: no loaded adapter named {missing}; loaded: {sorted(self._lora_adapters)}")
+        if len(set(names)) != len(names):
+            raise CEError(f"set_adapters: an adapter is named twice in {names}")
+        for n in names:
+            self._lora_entries(n)
+        if names and getattr(self, "_sp_state", None):
+            raise CEError("run-time LoRA (set_adapters) is not built for sequence parallelism: disable the sequence-parallel mode first")
+        self._lora_set = list(zip(names, ws))
+        self._lora_on = True
+        self._lora_changed()
+        if self.device.type == "cuda":
+            self._lora_sync(self._lora_scale)
+
+    def disable_lora(self) -> None:
+        """Switch the active set off (the forward is the plain one again); enable_lora() switches it back on."""
+        self._lora_on = False
+        self._lora_changed()
+
+    def enable_lora(self) -> None:
+        self._lora_on = True
+        self._lora_changed()
+
+    def delete_adapters(self, adapter_names) -> None:
+        """Drop loaded adapters, and take them out of the active set."""
+        names = [adapter_names] if isinstance(adapter_names, str) else list(adapter_names)
+        missing = [n for n in names if n not in self._lora_adapters]
+        if missing:
+            raise CEError(f"delete_adapters: no loaded adapter named {missing}")
+        for n in names:
+            del self._lora_adapters[n]
+        self._lora_gen += 1
+        kept = [(n, w) for n, w in self._lora_set if n not in names]
+        if kept != self._lora_set:
+            self._lora_set = kept
+            self._lora_changed()
+
+    def active_adapters(self) -> list:
+        """The names of the set chosen with set_adapters, in activation order (also while disable_lora() has it off)."""
+        return [n for n, _ in self._lora_set]
+
+    def _lora_active(self) -> bool:
+        return self._lora_on and bool(self._lora_set)
+
+    def _lora_changed(self) -> None:
+        """A set, weight or on / off change: what was computed with the old set is stale."""
+        self._ctx_cache = []
+        self._graphs = {}
+        self._drop_teacache_states()
+
+    def _lora_entries(self, name):
+        """[(layer, target, part, A, B, alpha or None)] of a loaded adapter; refuses a module that is not a block linear layer."""
+        out = []
+        for _, A, B, alpha, mod in self._parse_lora(self._lora_adapters[name], None):
+            head, _, sub = mod.partition(".")
+            layer, _, sub = sub.partition(".")
+            if head != "blocks" or not layer.isdigit() or sub not in LORA_TARGETS:
+                raise CEError(f"set_adapters: adapter '{name}' has a LoRA on '{mod}', which is not a block linear layer.  Run-time "
+                              f"LoRA covers {', '.join(LORA_TARGETS)} of every block; merge an adapter on other modules into the "
+                              "weights with fuse_lora instead")
+            target, part, _ = LORA_TARGETS[sub]
+            out.append((int(layer), target, part, A, B, alpha))
+        return out
+
+    @torch.no_grad()
+    def _lora_pack(self) -> Dict[Tuple[int, int], Tuple[torch.Tensor, ...]]:
+        """The active set as ce_dit_set_lora tables, on the module's device: per (layer, target) A_cat [R, K] (every adapter's
+        lora_A stacked in activation order, R padded to 8 with zero rows), B_raw [N, R] (lora_B at its part's rows, zeros
+        elsewhere) and col_scale [R] fp32 (weight * alpha / r of the column's adapter)."""
+        groups: Dict[Tuple[int, int], list] = {}
+        for name, weight in self._lora_set:
+            for layer, target, part, A, B, alpha in self._lora_entries(name):
+                r = A.shape[0]
+                groups.setdefault((layer, target), []).append((part, A, B, weight * (alpha / r if alpha is not None else 1.0)))
+        parts_of = {t: p for t, _, p in LORA_TARGETS.values()}
+        dev = self.device
+        tables = {}
+        for (layer, target), ents in groups.items():
+            R = sum(A.shape[0] for _, A, _, _ in ents)
+            Rp = (R + 7) // 8 * 8
+            K, Np = ents[0][1].shape[1], ents[0][2].shape[0]
+            a_cat = torch.zeros(Rp, K, dtype=torch.bfloat16, device=dev)
+            b_raw = torch.zeros(Np * parts_of[target], Rp, dtype=torch.bfloat16, device=dev)
+            col_scale = torch.zeros(Rp, dtype=torch.float32, device=dev)
+            c = 0
+            for part, A, B, scaling in ents:
+                r = A.shape[0]
+                a_cat[c: c + r] = A.to(device=dev, dtype=torch.bfloat16)
+                b_raw[part * Np: (part + 1) * Np, c: c + r] = B.to(device=dev, dtype=torch.bfloat16)
+                col_scale[c: c + r] = scaling
+                c += r
+            tables[(layer, target)] = (a_cat, b_raw, col_scale)
+        return tables
+
+    @torch.no_grad()
+    def _lora_sync(self, scale: float) -> None:
+        """Bring the handle's LoRA tables to the active set at `scale` (attention_kwargs["scale"]).  Nothing happens while they are
+        current, so the per-step path does no work for them; a new set packs the factors, a new scale only rescales B_cat
+        = bf16(B_raw * col_scale * scale) on the device.  Any change drops the workspaces and everything _lora_changed drops."""
+        want = self._lora_active()
+        key = (self._lora_gen, tuple(self._lora_set), str(self.device), float(scale)) if want else None
+        if key == self._lora_key:
+            return
+        L = _lib.lib()
+        h = self._ensure_handle()
+        if want:
+            old = self._lora_key
+            if not (self._lora_tables and old and old[:3] == key[:3]):
+                self._lora_tables = {k: v[:3] for k, v in self._lora_pack().items()}
+            self._lora_tables = {k: (a, b, cs, (b.float() * (cs * key[3])).to(torch.bfloat16).contiguous())
+                                 for k, (a, b, cs, *_) in self._lora_tables.items()}
+            n = self.config.num_layers * LORA_NUM_TARGETS
+            a_p, b_p, r_p = (_lib.c_void_p * n)(), (_lib.c_void_p * n)(), (_lib.c_int32 * n)()
+            for (layer, target), (a, _, _, b) in self._lora_tables.items():
+                i = layer * LORA_NUM_TARGETS + target
+                a_p[i], b_p[i], r_p[i] = a.data_ptr(), b.data_ptr(), a.shape[0]
+            check(L.ce_dit_set_lora(h, a_p, b_p, r_p, n))
+        else:
+            check(L.ce_dit_set_lora(h, None, None, None, 0))
+            self._lora_tables = {}
+        self._lora_key = key
+        self._workspaces = {}
+        self._lora_changed()
 
     # ------------------------------------------------------------------------------------------ loading
     @classmethod

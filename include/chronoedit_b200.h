@@ -83,10 +83,27 @@ int ce_dit_weights_complete(const ce_dit* h);
  * flag, so query it after setting it.  Sequence parallelism is refused while it is on. */
 int ce_dit_set_attention_fp8(ce_dit* h, int enabled);
 
+/* Run-time LoRA (DESIGN.md, "Run-time LoRA"): low-rank terms beside the block GEMMs, without touching the weights.  The tables
+ * hold num_layers * CE_LORA_TARGETS entries, entry layer * CE_LORA_TARGETS + target, targets in this order:
+ *   0 attn1.to_qkv   1 attn1.to_out.0   2 attn2.to_q   3 attn2.to_kv   4 attn2.add_kv_proj   5 attn2.to_out.0
+ *   6 ffn.net.0.proj   7 ffn.net.2
+ * Entry i: a_cat[i] [rank[i], K] bf16 (the stacked lora_A of every adapter on that GEMM) and b_cat[i] [N, rank[i]] bf16 (the
+ * stacked lora_B, each adapter's columns pre-scaled by its scaling); the fused targets (0, 3, 4) stack their parts along N
+ * (q | k | v, k | v), a part without an adapter holding zeros.  rank[i] % 8 == 0 (pad with zero rows / columns); 0 = no LoRA on
+ * that GEMM.  The GEMM then computes base + bf16(bf16(x a_cat^T) b_cat^T), the term added in the epilogue before GELU, gate,
+ * residual and the row statistics; an e4m3 weight keeps its FP8 rule for the base, the term reads the bf16 activations.
+ * Pointers are the caller's (16-byte aligned device memory, kept alive while set).  n == 0 clears every entry.  Anything
+ * invalid is refused before the handle changes.  ce_dit_workspace_bytes grows while a table is set (see there).  Refused at
+ * forward time with sequence parallelism and by ce_dit_forward_fp32. */
+#define CE_LORA_TARGETS 8
+int ce_dit_set_lora(ce_dit* h, const void* const* a_cat, const void* const* b_cat, const int32_t* rank, int n);
+
 /* Scratch bytes one forward needs for `batch` samples of latent geometry (frames, height, width) and text_len tokens.
  * A handle holding FP8 weights needs M * max(D, ffn_dim) bytes + M floats more (M = batch * tokens): the quantized rows.
  * With FP8 attention on: M * 2D bytes + M * 2H floats (q | k and their scales) + batch * D * Lpad bytes + batch * D floats
- * (V^T and its scales; Lpad = tokens rounded up to 32). */
+ * (V^T and its scales; Lpad = tokens rounded up to 32).
+ * While a LoRA table is set (ce_dit_set_lora): Mx * R_max + Mx * max(3D, ffn_dim) bf16 more, the down-projection and the
+ * low-rank term of one GEMM at a time (Mx = max(M, batch * text_len, batch * 257), R_max the largest rank of the table). */
 int64_t ce_dit_workspace_bytes(const ce_dit* h, int batch, int frames, int height, int width, int text_len);
 
 /* ChronoEditTransformer3DModel.forward (:397-476).
@@ -445,6 +462,11 @@ typedef struct ce_linear_fp8_args {
   const float* w_scale;
 } ce_linear_fp8_args;
 int ce_linear_fp8_ex(const ce_linear_fp8_args* args, void* stream);
+
+/* The two GEMMs above with run-time LoRA's epilogue addend: term [M, ldt] bf16 (ldt % 8 == 0, ldt >= N, 16-byte aligned) is
+ * added as y = bf16(bf16(acc + bias) + term) before GELU, gate, residual and the row statistics.  out_f32 is refused. */
+int ce_linear_lora_bf16(const ce_linear_args* args, const void* term, int ldt, void* stream);
+int ce_linear_lora_fp8(const ce_linear_fp8_args* args, const void* term, int ldt, void* stream);
 
 /* Per-row e4m3 quantization of x [rows, K] bf16 (K % 16 == 0, ldx % 8 == 0, ldq % 16 == 0): scale[m] = max_k |x| / 448
  * (1 for a zero row), q[m, k] = e4m3 bits of cvt.rn.satfinite(x / scale[m]), the division in IEEE fp32. */
