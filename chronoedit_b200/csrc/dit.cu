@@ -134,6 +134,7 @@ SpLayout sp_layout(int64_t B, int64_t L, int64_t D, int64_t No, int world) {
 // every call whose full sample fits.
 constexpr int64_t kSlotFlagsBytes = 1024;
 int64_t slot_bytes(int64_t region_bytes) { return std::max<int64_t>(0, (region_bytes - kSlotFlagsBytes) / 2) & ~int64_t(1023); }
+int64_t slot_region_bytes(int64_t sample_bytes) { return kSlotFlagsBytes + 2 * ((sample_bytes + 1023) & ~int64_t(1023)); }
 
 // Keys of the FP8 attention's V^T rows: L rounded up to the 32-key groups of its layout.
 int vt_keys(int L) { return (L + 31) / 32 * 32; }
@@ -457,25 +458,17 @@ static int time_path(ce_dit* h, cudaStream_t s, const Weights& W, const float* t
   return CE_OK;
 }
 
-// Batch split: the refusals of a split call, all before its first launch.  `sample_elems`: elements of one output sample.
-static int bp_check(const ce_dit* h, const char* who, int batch, int64_t sample_elems, bool block_capture, cudaStream_t s) {
-  const SeqPar& bp = h->bp;
-  if (batch % bp.world != 0)
-    return fail(CE_ERR_INVALID, std::string(who) + ": batch split: a batch of " + std::to_string(batch) + " does not divide over " +
-                                    std::to_string(bp.world) + " ranks.  Only a call that carries the whole CFG pair is split: the unchanged "
-                                    "diffusers pipeline's batch-1 calls are not split (it calls with the prompt and the negative prompt "
-                                    "one at a time).  Run the pair as one batch-2 call, or switch the split off (ce_dit_bp_configure with "
-                                    "world 1)");
-  const int64_t need = (int64_t)batch * sample_elems * (int64_t)sizeof(bf16), slot = slot_bytes(bp.region_bytes);
+// The refusals of a slot group's call (the batch split's `bp`, the call pair's `cp`), before its first launch: a sample of `need` bytes
+// larger than a slot of the group's region (sized by `region_fn`), and a capturing stream.
+static int slot_check(const SeqPar& g, const std::string& who, const char* region_fn, int64_t need, cudaStream_t s) {
+  const int64_t slot = slot_bytes(g.region_bytes);
   if (need > slot)
-    return fail(CE_ERR_WORKSPACE, std::string(who) + ": batch split: the call's sample needs a slot of " + std::to_string(need) +
-                                      " bytes, the peer region holds slots of " + std::to_string(slot) + " (ce_dit_bp_region_bytes)");
-  CE_REQUIRE(!block_capture, std::string(who) + ": batch split: no block capture / block0_out (each rank runs only its own samples)");
+    return fail(CE_ERR_WORKSPACE, who + ": the call's sample needs a slot of " + std::to_string(need) +
+                                      " bytes, the peer region holds slots of " + std::to_string(slot) + " (" + region_fn + ")");
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   CE_CHECK_CUDA(cudaStreamIsCapturing(s, &cs));
   CE_REQUIRE(cs == cudaStreamCaptureStatusNone,
-             std::string(who) + ": batch split: the stream is capturing (the exchange's barrier epoch advances every call, so it cannot be "
-                                "replayed from a graph)");
+             who + ": the stream is capturing (the exchange's barrier epoch advances every call, so it cannot be replayed from a graph)");
   return CE_OK;
 }
 
@@ -505,12 +498,32 @@ static int slot_exchange(ce_dit* h, SeqPar& g, const void* own, void* dst, int64
   return CE_OK;
 }
 
-// Batch split: the exchange that ends every split call.  This rank's samples, already at their offset in the caller's buffer, go into
-// every peer's slot; the other ranks' samples come from the own slot into the caller's buffer.
-static int bp_exchange(ce_dit* h, void* sample, int batch, int64_t sample_elems, cudaStream_t s) {
+// Address of sample `first` of a [batch, ...] tensor with `per_sample` bytes per sample (NULL stays NULL, so the forward's own null
+// check still sees it).
+template <class T>
+static T* sample_at(T* p, int first, int64_t per_sample) {
+  return p ? reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(p) + first * per_sample) : nullptr;
+}
+
+// Batch split: rank r of W computes samples [r B / W, (r + 1) B / W) of the call with `local(first, count)`, the entry's forward on its
+// slice of the inputs and of `sample` (the token split, when configured too, runs on them unchanged).  Then the exchange: the rank's
+// samples, already in place in `sample`, go into every peer's slot, and the other ranks' samples come from its own slot.
+template <class Local>
+static int split_batch(ce_dit* h, const char* who, int batch, int frames, int height, int width, int text_len, void* sample,
+                       void* stream_v, Local&& local) {
   SeqPar& bp = h->bp;
-  const int64_t part = (int64_t)(batch / bp.world) * sample_elems * (int64_t)sizeof(bf16);
-  return slot_exchange(h, bp, reinterpret_cast<uint8_t*>(sample) + bp.rank * part, sample, part, part, s);
+  CE_TRY(validate_geometry(h, batch, frames, height, width, text_len));
+  if (batch % bp.world != 0)
+    return fail(CE_ERR_INVALID, std::string(who) + ": batch split: a batch of " + std::to_string(batch) + " does not divide over " +
+                                    std::to_string(bp.world) + " ranks.  Only a call that carries the whole CFG pair is split: the unchanged "
+                                    "diffusers pipeline's batch-1 calls are not split (it calls with the prompt and the negative prompt "
+                                    "one at a time).  Run the pair as one batch-2 call, or switch the split off (ce_dit_bp_configure with "
+                                    "world 1)");
+  const int64_t need = (int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16), part = need / bp.world;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
+  CE_TRY(slot_check(bp, std::string(who) + ": batch split", "ce_dit_bp_region_bytes", need, s));
+  CE_TRY(local(bp.rank * (batch / bp.world), batch / bp.world));
+  return slot_exchange(h, bp, static_cast<uint8_t*>(sample) + bp.rank * part, sample, part, part, s);
 }
 
 // ---- internals shared with dit_fp32.cu
@@ -609,8 +622,7 @@ int ce_dit_sp_host_barrier(ce_dit* h, int timeout_ms) { return sp_set_host_barri
 
 int64_t ce_dit_bp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width, int world) {
   if (!h || world < 2 || world > 8 || batch < 1 || batch > 8 || batch % world != 0 || frames < 1 || height < 1 || width < 1) return -1;
-  const int64_t sample = (int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16);
-  return kSlotFlagsBytes + 2 * ((sample + 1023) & ~int64_t(1023));
+  return slot_region_bytes((int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16));
 }
 
 int ce_dit_bp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes) {
@@ -624,8 +636,7 @@ int ce_dit_bp_host_barrier(ce_dit* h, int timeout_ms) { return sp_set_host_barri
 
 int64_t ce_dit_cp_region_bytes(const ce_dit* h, int batch, int frames, int height, int width) {
   if (!h || batch < 1 || batch > 8 || frames < 1 || height < 1 || width < 1) return -1;
-  const int64_t sample = (int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16);
-  return kSlotFlagsBytes + 2 * ((sample + 1023) & ~int64_t(1023));
+  return slot_region_bytes((int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16));
 }
 
 int ce_dit_cp_configure(ce_dit* h, int rank, int world, void* const* region_ptrs, int64_t region_bytes) {
@@ -646,16 +657,8 @@ int ce_dit_cp_exchange(ce_dit* h, const void* own_sample, void* other_sample, in
   CE_REQUIRE(((reinterpret_cast<uintptr_t>(own_sample) | reinterpret_cast<uintptr_t>(other_sample)) & 1) == 0,
              "ce_dit_cp_exchange: the samples must be bf16-aligned");
   const int64_t need = (int64_t)batch * h->cfg.out_channels * frames * height * width * (int64_t)sizeof(bf16);
-  const int64_t slot = slot_bytes(h->cp.region_bytes);
-  if (need > slot)
-    return fail(CE_ERR_WORKSPACE, "ce_dit_cp_exchange: the call's sample needs a slot of " + std::to_string(need) +
-                                      " bytes, the peer region holds slots of " + std::to_string(slot) + " (ce_dit_cp_region_bytes)");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  CE_CHECK_CUDA(cudaStreamIsCapturing(s, &cs));
-  CE_REQUIRE(cs == cudaStreamCaptureStatusNone,
-             "ce_dit_cp_exchange: the stream is capturing (the exchange's barrier epoch advances every pair, so it cannot be replayed from "
-             "a graph)");
+  CE_TRY(slot_check(h->cp, "ce_dit_cp_exchange", "ce_dit_cp_region_bytes", need, s));
   return slot_exchange(h, h->cp, own_sample, other_sample, need, 0, s);
 }
 
@@ -714,18 +717,41 @@ int ce_dit_forward(ce_dit* h, const void* hidden_states, const float* timestep, 
                            width, text_len, workspace, workspace_bytes, block0_out, nullptr, 0, 0, stream_v);
 }
 
+static bool aligned256(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) == 0; }
+
+// The set-up of a forward and of a TeaCache-skipped forward, before their first launch: the checks both make (`inputs_given`: the
+// caller's inputs and sample are non-null), the weights, and the workspace carved as the forward carves it (the tokens this rank owns
+// under the token split; the layout ce_dit_workspace_bytes sizes), with the handle's FP8 and LoRA slices pointed into it.
+static int forward_setup(ce_dit* h, const char* who, bool inputs_given, int batch, int frames, int height, int width, int text_len,
+                         void* workspace, int64_t workspace_bytes, Weights& W, Workspace& ws) {
+  CE_REQUIRE(h && inputs_given && workspace, std::string(who) + ": null argument");
+  CE_TRY(check_device());
+  CE_TRY(validate_geometry(h, batch, frames, height, width, text_len));
+  CE_TRY(resolve_weights(h, W));
+  const ce_dit_config& c = h->cfg;
+  const int L = frames * (height / c.patch_h) * (width / c.patch_w) / h->sp.world;
+  ws = carve(c, workspace, batch, L, text_len, 257, W.fp8, h->attn_fp8, h->lora_rmax);
+  if (ws.bytes > workspace_bytes)
+    return fail(CE_ERR_WORKSPACE, std::string(who) + ": workspace too small: need " + std::to_string(ws.bytes) + " bytes, got " +
+                                      std::to_string(workspace_bytes));
+  CE_REQUIRE(aligned256(workspace), std::string(who) + ": workspace must be 256-byte aligned");
+  h->fp8_q = ws.fp8_q;
+  h->fp8_scale = ws.fp8_scale;
+  h->lora_mid = ws.lora_mid;
+  h->lora_term = ws.lora_term;
+  return CE_OK;
+}
+
 // The forward of the samples this rank computes (all of them without the batch split).
 static int forward_samples(ce_dit* h, const void* hidden_states, const float* timestep, const void* encoder_hidden_states,
                            const void* encoder_hidden_states_image, void* sample, int batch, int frames, int height, int width,
                            int text_len, void* workspace, int64_t workspace_bytes, void* block0_out, void* ctx_cache,
                            int64_t ctx_cache_bytes, int ctx_reuse, void* stream_v) {
-  CE_REQUIRE(h && hidden_states && timestep && encoder_hidden_states && sample && workspace, "ce_dit_forward: null argument");
   CE_REQUIRE(ctx_reuse == 0 || ctx_cache != nullptr, "ce_dit_forward_ex: ctx_reuse needs a context cache");
-  int rc = check_device();
-  if (rc) return rc;
-  if ((rc = validate_geometry(h, batch, frames, height, width, text_len))) return rc;
   Weights W;
-  if ((rc = resolve_weights(h, W))) return rc;
+  Workspace ws;
+  CE_TRY(forward_setup(h, "ce_dit_forward", hidden_states && timestep && encoder_hidden_states && sample, batch, frames, height, width,
+                       text_len, workspace, workspace_bytes, W, ws));
   const ce_dit_config& c = h->cfg;
   CE_REQUIRE((c.image_dim > 0) == (encoder_hidden_states_image != nullptr),
              "ce_dit_forward: encoder_hidden_states_image must be given iff the model has an image embedder");
@@ -748,21 +774,14 @@ static int forward_samples(ce_dit* h, const void* hidden_states, const float* ti
   if (spx && lay.bytes > sp.region_bytes) return fail(CE_ERR_WORKSPACE, "sequence parallel: peer region too small (ce_dit_sp_region_bytes)");
   CE_REQUIRE(!(spx && W.fp8), "sequence parallelism is not built for FP8 weights: run the FP8 mode on one GPU");
   CE_REQUIRE(!(spx && !h->lora.empty()), "sequence parallelism is not built for run-time LoRA: clear it first (ce_dit_set_lora with n = 0)");
-  Workspace ws = carve(c, workspace, B, L, Lt, Li, W.fp8, h->attn_fp8, h->lora_rmax);
-  if (ws.bytes > workspace_bytes)
-    return fail(CE_ERR_WORKSPACE, "workspace too small: need " + std::to_string(ws.bytes) + " bytes, got " + std::to_string(workspace_bytes));
-  CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
   bf16* const rec = reinterpret_cast<bf16*>(h->resid_rec);
   if (rec) {
     CE_REQUIRE(!spx, "TeaCache residual record: sequence parallelism is not built for it");
     CE_REQUIRE(h->resid_rec_bytes >= (int64_t)M * D * (int64_t)sizeof(bf16),
                "TeaCache residual record: buffer too small for this forward (needs batch * tokens * inner dim bf16)");
   }
-  if ((rc = ensure_rope(h, frames, hp, wp, s))) return rc;   // always the full table [Lfull, 64]
-  h->fp8_q = ws.fp8_q;
-  h->fp8_scale = ws.fp8_scale;
-  h->lora_mid = ws.lora_mid;
-  h->lora_term = ws.lora_term;
+  int rc = ensure_rope(h, frames, hp, wp, s);   // always the full table [Lfull, 64]
+  if (rc) return rc;
   // run-time LoRA entry of layer i's GEMM `target`, or null
   auto lora_of = [&](int i, int target) { return h->lora.empty() ? nullptr : &h->lora[(size_t)i * CE_LORA_TARGETS + target]; };
   // step-invariant context (text / image embedders and every block's cross-attention K/V, :52-60, :147-165): kept in the
@@ -770,7 +789,7 @@ static int forward_samples(ce_dit* h, const void* hidden_states, const float* ti
   const int64_t kv_t_elems = (int64_t)B * Lt * 2 * D, kv_i_elems = c.image_dim > 0 ? (int64_t)B * Li * 2 * D : 0;
   const int64_t ctx_layer_bytes = ((kv_t_elems + kv_i_elems) * (int64_t)sizeof(bf16) + 255) & ~int64_t(255);
   if (ctx_cache) {
-    CE_REQUIRE((reinterpret_cast<uintptr_t>(ctx_cache) & 255) == 0, "ce_dit_forward_ex: context cache must be 256-byte aligned");
+    CE_REQUIRE(aligned256(ctx_cache), "ce_dit_forward_ex: context cache must be 256-byte aligned");
     CE_REQUIRE(ctx_cache_bytes >= ctx_layer_bytes * c.num_layers, "ce_dit_forward_ex: context cache too small (ce_dit_context_cache_bytes)");
   }
   auto kv_text_of = [&](int layer) { return ctx_cache ? reinterpret_cast<bf16*>(reinterpret_cast<uint8_t*>(ctx_cache) + layer * ctx_layer_bytes) : ws.kv_text; };
@@ -968,11 +987,6 @@ static int forward_samples(ce_dit* h, const void* hidden_states, const float* ti
   return CE_OK;
 }
 
-// Byte address of sample `first` of a [batch, ...] tensor with `per_sample` bytes per sample (NULL stays NULL).
-static const void* sample_at(const void* p, int first, int64_t per_sample) {
-  return p ? static_cast<const uint8_t*>(p) + first * per_sample : nullptr;
-}
-
 int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timestep, const void* encoder_hidden_states,
                       const void* encoder_hidden_states_image, void* sample, int batch, int frames, int height, int width,
                       int text_len, void* workspace, int64_t workspace_bytes, void* block0_out, void* ctx_cache,
@@ -980,26 +994,20 @@ int ce_dit_forward_ex(ce_dit* h, const void* hidden_states, const float* timeste
   if (!h || h->bp.world <= 1)
     return forward_samples(h, hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image, sample, batch, frames, height,
                            width, text_len, workspace, workspace_bytes, block0_out, ctx_cache, ctx_cache_bytes, ctx_reuse, stream_v);
-  // batch split: this rank's samples through the forward above (the token split, when configured too, runs on them unchanged), then
-  // the exchange
-  CE_REQUIRE(hidden_states && timestep && encoder_hidden_states && sample && workspace, "ce_dit_forward: null argument");
-  CE_TRY(validate_geometry(h, batch, frames, height, width, text_len));
+  CE_REQUIRE(block0_out == nullptr && h->capture.empty(),
+             "ce_dit_forward_ex: batch split: no block capture / block0_out (each rank runs only its own samples)");
   const ce_dit_config& c = h->cfg;
-  const int64_t pixels = (int64_t)frames * height * width, out_elems = c.out_channels * pixels;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
-  CE_TRY(bp_check(h, "ce_dit_forward_ex", batch, out_elems, block0_out != nullptr || !h->capture.empty(), s));
-  const int Bl = batch / h->bp.world, s0 = h->bp.rank * Bl;
-  CE_TRY(forward_samples(h, sample_at(hidden_states, s0, c.in_channels * pixels * 2), timestep + s0,
-                         sample_at(encoder_hidden_states, s0, (int64_t)text_len * c.text_dim * 2),
-                         sample_at(encoder_hidden_states_image, s0, (int64_t)257 * c.image_dim * 2),
-                         const_cast<void*>(sample_at(sample, s0, out_elems * 2)), Bl, frames, height, width, text_len, workspace,
-                         workspace_bytes, nullptr, ctx_cache, ctx_cache_bytes, ctx_reuse, stream_v));
-  return bp_exchange(h, sample, batch, out_elems, s);
+  const int64_t pixels = (int64_t)frames * height * width;
+  return split_batch(h, "ce_dit_forward_ex", batch, frames, height, width, text_len, sample, stream_v, [&](int s0, int Bl) {
+    return forward_samples(h, sample_at(hidden_states, s0, c.in_channels * pixels * 2), sample_at(timestep, s0, sizeof(float)),
+                           sample_at(encoder_hidden_states, s0, (int64_t)text_len * c.text_dim * 2),
+                           sample_at(encoder_hidden_states_image, s0, (int64_t)257 * c.image_dim * 2),
+                           sample_at(sample, s0, c.out_channels * pixels * 2), Bl, frames, height, width, text_len, workspace,
+                           workspace_bytes, nullptr, ctx_cache, ctx_cache_bytes, ctx_reuse, stream_v);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------- TeaCache
-static bool aligned256(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) == 0; }
-
 // The probe's scratch: sinusoid [B, freq_dim] f32, h1 and temb [B, D] f32, temb [B, D] bf16.
 static int64_t probe_bytes(const ce_dit_config& c, int B, float** sin_emb, float** h1, float** temb_f32, bf16** temb_bf16, void* base) {
   Bump b(base);
@@ -1055,26 +1063,18 @@ int ce_dit_set_residual_record(ce_dit* h, void* buf, int64_t bytes) {
 static int forward_cached_samples(ce_dit* h, const void* hidden_states, const float* timestep, const void* residual,
                                   int64_t residual_bytes, void* sample, int batch, int frames, int height, int width, int text_len,
                                   void* workspace, int64_t workspace_bytes, void* stream_v) {
-  CE_REQUIRE(h && hidden_states && timestep && residual && sample && workspace, "ce_dit_forward_cached: null argument");
+  Weights W;
+  Workspace ws;
+  CE_TRY(forward_setup(h, "ce_dit_forward_cached", hidden_states && timestep && residual && sample, batch, frames, height, width, text_len,
+                       workspace, workspace_bytes, W, ws));
   CE_REQUIRE(h->sp.world <= 1, "ce_dit_forward_cached: TeaCache is not built for sequence parallelism");
-  CE_REQUIRE(aligned256(residual) && aligned256(workspace), "ce_dit_forward_cached: residual and workspace must be 256-byte aligned");
-  int rc = validate_geometry(h, batch, frames, height, width, text_len);
-  if (rc) return rc;
+  CE_REQUIRE(aligned256(residual), "ce_dit_forward_cached: residual must be 256-byte aligned");
   const ce_dit_config& c = h->cfg;
   const int B = batch, hp = height / c.patch_h, wp = width / c.patch_w;
   const int L = frames * hp * wp, M = B * L, D = D_of(c), Kp = c.in_channels * 4, No = c.out_channels * 4;
   CE_REQUIRE(residual_bytes >= (int64_t)M * D * (int64_t)sizeof(bf16),
              "ce_dit_forward_cached: residual too small for this geometry (batch * tokens * inner dim bf16)");
-  Weights W;
-  if ((rc = resolve_weights(h, W))) return rc;
-  Workspace ws = carve(c, workspace, B, L, text_len, 257, W.fp8, h->attn_fp8);
-  if (ws.bytes > workspace_bytes)
-    return fail(CE_ERR_WORKSPACE, "ce_dit_forward_cached: workspace too small: need " + std::to_string(ws.bytes) + " bytes, got " +
-                                      std::to_string(workspace_bytes));
-  if ((rc = check_device())) return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
-  h->fp8_q = ws.fp8_q;
-  h->fp8_scale = ws.fp8_scale;
   const bool st = D % 256 == 0;
   const RowPartials px = st ? RowPartials{ws.stats_x, D / 256, D / 256, 256} : RowPartials{};
   h->launches = 0;
@@ -1088,13 +1088,13 @@ static int forward_cached_samples(ce_dit* h, const void* hidden_states, const fl
     g.stats_out = ws.stats_x;
     g.stats_mode = 1;
   }
-  if ((rc = linear(h, s, W.patch, ws.patches, M, D, Kp, ws.x, g))) return rc;
-  if ((rc = time_path(h, s, W, timestep, B, ws.sin_emb, ws.h1, ws.temb_f32, ws.temb_bf16, nullptr))) return rc;
+  CE_TRY(linear(h, s, W.patch, ws.patches, M, D, Kp, ws.x, g));
+  CE_TRY(time_path(h, s, W, timestep, B, ws.sin_emb, ws.h1, ws.temb_f32, ws.temb_bf16, nullptr));
   LAUNCH(CAT_OTHER, 0.0, launch_add_table(W.head_table, 1, ws.temb_bf16, D, ws.modf, B, D, 2, s, /*chunk 1 = scale*/ 0x2u));
   LAUNCH(CAT_ROWS, 4.0 * M * D, launch_layernorm(ws.x, D, ws.xn, D, M, D, c.eps, ws.modf + D, ws.modf, 2 * D, L, nullptr, nullptr, 1, px, s));
   GemmArgs gh;
   gh.epi = EPI_BIAS;
-  if ((rc = linear(h, s, W.proj_out, ws.xn, M, No, D, ws.yout, gh))) return rc;
+  CE_TRY(linear(h, s, W.proj_out, ws.xn, M, No, D, ws.yout, gh));
   LAUNCH(CAT_OTHER, 0.0, launch_unpatchify(ws.yout, No, reinterpret_cast<bf16*>(sample), B, c.out_channels, frames, height, width, s));
   return CE_OK;
 }
@@ -1106,17 +1106,13 @@ int ce_dit_forward_cached(ce_dit* h, const void* hidden_states, const float* tim
     return forward_cached_samples(h, hidden_states, timestep, residual, residual_bytes, sample, batch, frames, height, width, text_len,
                                   workspace, workspace_bytes, stream_v);
   // batch split: the residual is this rank's, [batch / world * tokens, D]; a skipped call ends in the same exchange as a computed one
-  CE_REQUIRE(hidden_states && timestep && residual && sample && workspace, "ce_dit_forward_cached: null argument");
-  CE_TRY(validate_geometry(h, batch, frames, height, width, text_len));
   const ce_dit_config& c = h->cfg;
-  const int64_t pixels = (int64_t)frames * height * width, out_elems = c.out_channels * pixels;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
-  CE_TRY(bp_check(h, "ce_dit_forward_cached", batch, out_elems, false, s));
-  const int Bl = batch / h->bp.world, s0 = h->bp.rank * Bl;
-  CE_TRY(forward_cached_samples(h, sample_at(hidden_states, s0, c.in_channels * pixels * 2), timestep + s0, residual, residual_bytes,
-                                const_cast<void*>(sample_at(sample, s0, out_elems * 2)), Bl, frames, height, width, text_len, workspace,
-                                workspace_bytes, stream_v));
-  return bp_exchange(h, sample, batch, out_elems, s);
+  const int64_t pixels = (int64_t)frames * height * width;
+  return split_batch(h, "ce_dit_forward_cached", batch, frames, height, width, text_len, sample, stream_v, [&](int s0, int Bl) {
+    return forward_cached_samples(h, sample_at(hidden_states, s0, c.in_channels * pixels * 2), sample_at(timestep, s0, sizeof(float)),
+                                  residual, residual_bytes, sample_at(sample, s0, c.out_channels * pixels * 2), Bl, frames, height, width,
+                                  text_len, workspace, workspace_bytes, stream_v);
+  });
 }
 
 int64_t ce_dit_host_staging_bytes(const ce_dit* h, int batch, int frames, int height, int width, int text_len) {

@@ -160,6 +160,26 @@ def _release_peer_regions(obj, entry: str, attr: str = "_sp_state") -> None:
     setattr(obj, attr, None)
 
 
+def _enable_split(obj, who: str, group, disable, region_bytes, configure) -> int:
+    """What every enable_* does: refuse without a process group, `disable(obj)` and stop at world 1; otherwise size the region
+    with `region_bytes(world)`, open the peer regions, hand them to `configure` (a configure_* function) and wait for every rank.
+    Returns the region size in bytes."""
+    from ._lib import CEError
+
+    if not dist.is_initialized():
+        raise CEError(f"{who} needs an initialised torch.distributed process group (one process per GPU)")
+    disable(obj)
+    world = dist.get_world_size(group)
+    if world == 1:
+        return 0
+    n = region_bytes(world)
+    with torch.cuda.device(obj.device):
+        ptrs, state = _open_peer_regions(n, group)
+        configure(obj, dist.get_rank(group), ptrs, n, state)
+    dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
+    return int(n)
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # Sequence parallelism for single-edit latency (SURVEY.md section 8(f) row 2)
 # ----------------------------------------------------------------------------------------------------------------------
@@ -173,20 +193,8 @@ def enable_sequence_parallel(model, batch: int, frames: int, height: int, width:
     rank -- computes 1/world of the tokens per rank, exchanges q/k/v and the attention output by peer stores over NVLink inside the
     kernels (no collective call on the data path), and returns the same full sample on every rank, bit-identical to the single-GPU
     forward.  Geometry-specific: call again for another latent shape.  Returns the region size in bytes."""
-    from ._lib import CEError
-
-    if not dist.is_initialized():
-        raise CEError("enable_sequence_parallel needs an initialised torch.distributed process group (one process per GPU)")
-    disable_sequence_parallel(model)
-    world = dist.get_world_size(group)
-    if world == 1:
-        return 0
-    n = sp_region_bytes(model, batch, frames, height, width, world)
-    with torch.cuda.device(model.device):
-        ptrs, state = _open_peer_regions(n, group)
-        configure_sequence_parallel(model, dist.get_rank(group), ptrs, n, state)
-    dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
-    return int(n)
+    return _enable_split(model, "enable_sequence_parallel", group, disable_sequence_parallel,
+                         lambda world: sp_region_bytes(model, batch, frames, height, width, world), configure_sequence_parallel)
 
 
 def sp_region_bytes(model, batch: int, frames: int, height: int, width: int, world: int) -> int:
@@ -242,21 +250,11 @@ def enable_cfg_parallel(model, batch: int, frames: int, height: int, width: int,
     """
     from ._lib import CEError
 
-    if not dist.is_initialized():
-        raise CEError("enable_cfg_parallel needs an initialised torch.distributed process group (one process per GPU)")
     if getattr(model, "_cp_state", None):   # before any region is allocated; ce_dit_bp_configure refuses it too
         raise CEError("enable_cfg_parallel: the call-pair split (enable_cfg_parallel_calls) is on: the two CFG splits are exclusive, "
                       "disable it first")
-    disable_cfg_parallel(model)
-    world = dist.get_world_size(group)
-    if world == 1:
-        return 0
-    n = cfg_region_bytes(model, batch, frames, height, width, world)
-    with torch.cuda.device(model.device):
-        ptrs, state = _open_peer_regions(n, group)
-        configure_cfg_parallel(model, dist.get_rank(group), ptrs, n, state)
-    dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
-    return int(n)
+    return _enable_split(model, "enable_cfg_parallel", group, disable_cfg_parallel,
+                         lambda world: cfg_region_bytes(model, batch, frames, height, width, world), configure_cfg_parallel)
 
 
 def cfg_region_bytes(model, batch: int, frames: int, height: int, width: int, world: int) -> int:
@@ -320,23 +318,17 @@ def enable_cfg_parallel_calls(model, batch: int, frames: int, height: int, width
     """
     from ._lib import CEError
 
-    if not dist.is_initialized():
-        raise CEError("enable_cfg_parallel_calls needs an initialised torch.distributed process group (one process per GPU)")
     if getattr(model, "_bp_state", None):   # before any region is allocated; ce_dit_cp_configure refuses it too
         raise CEError("enable_cfg_parallel_calls: the batch split (enable_cfg_parallel) is on: the two CFG splits are exclusive, "
                       "disable it first")
-    disable_cfg_parallel_calls(model)
-    world = dist.get_world_size(group)
-    if world == 1:
-        return 0
-    if world != 2:
-        raise CEError(f"enable_cfg_parallel_calls: a CFG pair has two calls: the group must have 2 ranks, not {world}")
-    n = cfg_calls_region_bytes(model, batch, frames, height, width)
-    with torch.cuda.device(model.device):
-        ptrs, state = _open_peer_regions(n, group)
-        configure_cfg_parallel_calls(model, dist.get_rank(group), ptrs, n, state)
-    dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
-    return int(n)
+
+    def region_bytes(world):
+        if world != 2:
+            raise CEError(f"enable_cfg_parallel_calls: a CFG pair has two calls: the group must have 2 ranks, not {world}")
+        return cfg_calls_region_bytes(model, batch, frames, height, width)
+
+    return _enable_split(model, "enable_cfg_parallel_calls", group, disable_cfg_parallel_calls, region_bytes,
+                         configure_cfg_parallel_calls)
 
 
 def cfg_calls_region_bytes(model, batch: int, frames: int, height: int, width: int) -> int:
@@ -394,20 +386,8 @@ def enable_vae_sequence_parallel(vae, height: int, width: int, group=None) -> in
     `height` x `width` is the edit's pixel geometry: one configuration serves the encode of any 1 + 4k frames at that size and the
     decode of any latent frame count at height / 8 x width / 8.  Allocates this rank's peer region (ce_ipc_alloc), exchanges the CUDA
     IPC handles through torch.distributed and configures the handle (ce_vae_sp_configure).  Returns the region size in bytes."""
-    from ._lib import CEError
-
-    if not dist.is_initialized():
-        raise CEError("enable_vae_sequence_parallel needs an initialised torch.distributed process group (one process per GPU)")
-    disable_vae_sequence_parallel(vae)
-    world = dist.get_world_size(group)
-    if world == 1:
-        return 0
-    n = vae_sp_region_bytes(vae, height, width, world)
-    with torch.cuda.device(vae.device):
-        ptrs, state = _open_peer_regions(n, group)
-        configure_vae_sequence_parallel(vae, dist.get_rank(group), ptrs, n, state)
-    dist.barrier(group=group)   # every region exists, is zeroed and is mapped everywhere before the first flag is written
-    return int(n)
+    return _enable_split(vae, "enable_vae_sequence_parallel", group, disable_vae_sequence_parallel,
+                         lambda world: vae_sp_region_bytes(vae, height, width, world), configure_vae_sequence_parallel)
 
 
 def vae_sp_region_bytes(vae, height: int, width: int, world: int) -> int:
