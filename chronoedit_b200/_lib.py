@@ -139,6 +139,9 @@ SIGNATURES = {
     "ce_encoder_last_launch_count": (c_int64, [c_void_p]),
     "ce_umt5_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "ce_clip_vision_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p]),
+    "ce_encoder_set_weight_fp32": (c_int, [c_void_p, c_char_p, c_void_p, c_int64]),
+    "ce_clip_vision_fp32_workspace_bytes": (c_int64, [c_void_p, c_int]),
+    "ce_clip_vision_encode_fp32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "ce_vae_create": (c_int, [c_void_p, POINTER(c_void_p)]),
     "ce_vae_destroy": (None, [c_void_p]),
     "ce_vae_set_weight": (c_int, [c_void_p, c_char_p, c_void_p, c_int64]),

@@ -4,11 +4,8 @@
 // SURVEY.md section 7 hard part 3).  Same operator order as ChronoEditTransformer3DModel.forward
 // (/root/reference/chronoedit_diffusers/transformer_chronoedit.py:397-476) evaluated in fp32 like the reference's own fp32 run.
 //
-// Every matrix product still runs on the wgmma GEMM of gemm.cu: an fp32 operand x is split into two bf16 terms
-// hi = bf16(x), lo = bf16(x - hi) (|x - hi - lo| <= 2^-17 |x|), and A.W^T is evaluated as ONE bf16 GEMM over a K axis three times
-// as long -- A' = [A_hi | A_lo | A_hi], W' = [W_hi | W_hi | W_lo], i.e. A_hi.W_hi + A_lo.W_hi + A_hi.W_lo, fp32 accumulation in
-// registers, fp32 store (the dropped A_lo.W_lo term is 2^-18 relative).  Attention is S = Q.K^T (same split GEMM, fp32 S in HBM),
-// an fp32 row softmax, and O = P.V with P and V^T split the same way.  Everything elementwise is a plain fp32 SIMT kernel.
+// Every matrix product still runs on the wgmma GEMM of gemm.cu, with every fp32 operand split into two bf16 terms, and attention
+// is a split-GEMM S, an fp32 row softmax and a split-GEMM P.V (fp32_chain.cuh).  Everything elementwise is a plain fp32 SIMT kernel.
 // This path trades speed for precision (3x the MMA work, S materialised) and exists for parity checks only.
 #include <math.h>
 
@@ -17,96 +14,12 @@
 
 #include "../../include/chronoedit_b200.h"
 #include "elementwise.cuh"
-#include "gemm.cuh"
+#include "fp32_chain.cuh"
 
 using namespace ce;
 
 namespace {
 
-// out[r, :] (bf16, 3*Kp wide) from x[r, 0:K] fp32 (leading dim ldx); A layout [hi | lo | hi], W layout [hi | hi | lo]; columns
-// K..Kp-1 of each third are zero
-__global__ void split3_kernel(const float* __restrict__ x, int ldx, int rows, int K, int Kp, bf16* __restrict__ out, int w_layout) {
-  const size_t total = (size_t)rows * Kp;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i % Kp);
-    const size_t r = i / Kp;
-    float v = c < K ? x[r * ldx + c] : 0.f;
-    const bf16 hi = __float2bfloat16_rn(v);
-    const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-    bf16* o = out + r * 3 * (size_t)Kp;
-    o[c] = hi;
-    o[Kp + c] = w_layout ? hi : lo;
-    o[2 * Kp + c] = w_layout ? lo : hi;
-  }
-}
-// W layout of the TRANSPOSE: out[n, :] over k from x[k, n]  (V^T for the P.V product); x [K, ldx], n < N
-__global__ void split3_transposed_kernel(const float* __restrict__ x, int ldx, int K, int Kp, int N, bf16* __restrict__ out) {
-  const size_t total = (size_t)N * Kp;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int k = (int)(i % Kp);
-    const int n = (int)(i / Kp);
-    float v = k < K ? x[(size_t)k * ldx + n] : 0.f;
-    const bf16 hi = __float2bfloat16_rn(v);
-    const bf16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-    bf16* o = out + (size_t)n * 3 * Kp;
-    o[k] = hi;
-    o[Kp + k] = hi;
-    o[2 * Kp + k] = lo;
-  }
-}
-
-__device__ __forceinline__ float act_f(float y, int act) {
-  if (act == 1) return 0.5f * y * (1.0f + tanhf(0.7978845608028654f * (y + 0.044715f * y * y * y)));  // GELU(tanh)
-  if (act == 2) return 0.5f * y * (1.0f + erff(y * 0.7071067811865476f));                              // GELU(erf)
-  if (act == 3) return y / (1.0f + expf(-y));                                                          // SiLU
-  return y;
-}
-// y[r, c] = act(y[r, c] + bias[c])
-__global__ void bias_act_kernel(float* __restrict__ y, int ldy, int rows, int N, const float* __restrict__ bias, int act) {
-  const size_t total = (size_t)rows * N;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i % N);
-    const size_t r = i / N;
-    float v = y[r * ldy + c] + (bias ? bias[c] : 0.f);
-    y[r * ldy + c] = act_f(v, act);
-  }
-}
-// x[r, c] += y[r, c] * (gate ? gate[b(r), c] : 1)
-__global__ void resid_kernel(float* __restrict__ x, const float* __restrict__ y, int rows, int D, const float* __restrict__ gate,
-                             int gate_stride, int rows_per_batch) {
-  const size_t total = (size_t)rows * D;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i % D);
-    const size_t r = i / D;
-    const float g = gate ? gate[(r / rows_per_batch) * gate_stride + c] : 1.0f;
-    x[i] = x[i] + y[i] * g;
-  }
-}
-// one warp per row: y = LN(x) * (1 + scale) + shift   or   LN(x) * w + b   (two-pass variance, fp32)
-__global__ void layernorm_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int rows, int D, float eps,
-                                     const float* __restrict__ scale, const float* __restrict__ shift, int mod_stride, int rows_per_batch,
-                                     const float* __restrict__ w, const float* __restrict__ b) {
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  const float* xr = x + (size_t)row * D;
-  float s = 0.f;
-  for (int i = lane; i < D; i += 32) s += xr[i];
-  const float mean = warp_sum(s) / D;
-  float ss = 0.f;
-  for (int i = lane; i < D; i += 32) {
-    const float d = xr[i] - mean;
-    ss += d * d;
-  }
-  const float rstd = rsqrtf(warp_sum(ss) / D + eps);
-  const int bi = row / rows_per_batch;
-  for (int i = lane; i < D; i += 32) {
-    float v = (xr[i] - mean) * rstd;
-    if (scale) v = v * (1.0f + scale[(size_t)bi * mod_stride + i]) + shift[(size_t)bi * mod_stride + i];
-    else if (w) v = v * w[i] + b[i];
-    y[(size_t)row * D + i] = v;
-  }
-}
 // in place, one warp per row: x = x * rsqrt(mean(x^2) + eps) * w, then optional interleaved RoPE (cos/sin [L, hd/2])
 __global__ void rmsnorm_rope_f32_kernel(float* __restrict__ x, int ldx, int rows, int D, float eps, const float* __restrict__ w,
                                         const float* __restrict__ rc, const float* __restrict__ rs, int L, int hd) {
@@ -208,10 +121,6 @@ Ws32 carve32(const ce_dit_config& c, void* base, int B, int L, int Lt, int Li) {
   return w;
 }
 
-// One Linear of the fp32 model: weight [N, K], bias [N].
-struct Lin32 {
-  const float *w = nullptr, *b = nullptr;
-};
 struct Layer32 {
   const float* table;   // scale_shift_table [6, D]
   Lin32 q, k, v, out1, q2, k2, v2, add_k, add_v, out2, ffn1, ffn2;
@@ -276,57 +185,9 @@ int resolve_weights32(const WeightMap& map, const ce_dit_config& c, Weights32& w
 }
 
 // The launches of the fp32 forward.  They are not counted: ce_dit_last_launch_count reports the last bf16 forward.
-struct Ctx32 {
-  Ws32 ws;
-  Launcher run;
-  // out[M, ldo] (fp32) = act(A[M, K] (lda) . W[N, K]^T + bias)
-  int linear(const float* A, int lda, int M, int K, const Lin32& w, int N, float* out, int ldo, int act) {
-    const int Kp = up8(K);
-    CE_TRY(run.kernel(split3_kernel, grid_for((size_t)M * Kp), TPB, A, lda, M, K, Kp, ws.Ap, 0));
-    CE_TRY(run.kernel(split3_kernel, grid_for((size_t)N * Kp), TPB, w.w, K, N, K, Kp, ws.Wp, 1));
-    GemmArgs g;
-    g.M = M; g.N = N; g.K = 3 * Kp;
-    g.out = nullptr; g.ldo = 0; g.out_f32 = out; g.ld_f32 = ldo;
-    g.bias = nullptr; g.epi = EPI_BIAS;
-    CE_TRY(run([&] { return launch_gemm_bf16(ws.Ap, 3 * Kp, ws.Wp, 3 * Kp, g, run.s); }));
-    if (w.b || act) CE_TRY(run.kernel(bias_act_kernel, grid_for((size_t)M * N), TPB, out, ldo, M, N, w.b, act));
-    return CE_OK;
-  }
-  int layernorm(const float* x, float* y, int rows, int D, float eps, const float* scale, const float* shift, int mod_stride, int rpb,
-                const float* w, const float* b) {
-    return run.kernel(layernorm_f32_kernel, (rows + 7) / 8, 256, x, y, rows, D, eps, scale, shift, mod_stride, rpb > 0 ? rpb : rows, w, b);
-  }
+struct Ctx32 : Fp32Chain {
   int rms(float* x, int ldx, int rows, int D, float eps, const float* w, const float* rc_, const float* rs_, int L, int hd) {
     return run.kernel(rmsnorm_rope_f32_kernel, (rows + 7) / 8, 256, x, ldx, rows, D, eps, w, rc_, rs_, L, hd);
-  }
-  // out[b, i, h*hd:(h+1)*hd] = softmax(q k^T * scale) v   for every (b, h); q [B*Lq, D], k / v [B*Lk, D]
-  int attention(const float* q, const float* k, const float* v, float* out, int B, int H, int Lq, int Lk, int D, int hd, float scale) {
-    const int Lk8 = up8(Lk);
-    for (int b = 0; b < B; ++b)
-      for (int hh = 0; hh < H; ++hh) {
-        const float* qh = q + (size_t)b * Lq * D + hh * hd;
-        const float* kh = k + (size_t)b * Lk * D + hh * hd;
-        const float* vh = v + (size_t)b * Lk * D + hh * hd;
-        // S[Lq, Lk8]: rows Lk..Lk8-1 of the "weight" operand are zero-padded by giving split3 rows = Lk8 over a zeroed tail
-        CE_CHECK_CUDA(cudaMemsetAsync(ws.Wp, 0, (size_t)Lk8 * 3 * up8(hd) * sizeof(bf16), run.s));
-        {
-          const int Kp = up8(hd);
-          CE_TRY(run.kernel(split3_kernel, grid_for((size_t)Lq * Kp), TPB, qh, D, Lq, hd, Kp, ws.Ap, 0));
-          CE_TRY(run.kernel(split3_kernel, grid_for((size_t)Lk * Kp), TPB, kh, D, Lk, hd, Kp, ws.Wp, 1));
-          GemmArgs g;
-          g.M = Lq; g.N = Lk8; g.K = 3 * Kp; g.out_f32 = ws.S; g.ld_f32 = Lk8;
-          CE_TRY(run([&] { return launch_gemm_bf16(ws.Ap, 3 * Kp, ws.Wp, 3 * Kp, g, run.s); }));
-        }
-        CE_TRY(run([&] { return launch_softmax_rows_f32(ws.S, Lk8, ws.P, Lk8, Lq, Lk, scale, run.s); }));
-        {  // O = P . V : P [Lq, Lk8] (padded columns are 0), V^T as the "weight" operand [hd, Lk8] (keys >= Lk zero-filled)
-          CE_TRY(run.kernel(split3_kernel, grid_for((size_t)Lq * Lk8), TPB, ws.P, Lk8, Lq, Lk8, Lk8, ws.Ap, 0));
-          CE_TRY(run.kernel(split3_transposed_kernel, grid_for((size_t)hd * Lk8), TPB, vh, D, Lk, Lk8, hd, ws.Wp));
-          GemmArgs g;
-          g.M = Lq; g.N = hd; g.K = 3 * Lk8; g.out_f32 = out + (size_t)b * Lq * D + hh * hd; g.ld_f32 = D;
-          CE_TRY(run([&] { return launch_gemm_bf16(ws.Ap, 3 * Lk8, ws.Wp, 3 * Lk8, g, run.s); }));
-        }
-      }
-    return CE_OK;
   }
 };
 
@@ -367,8 +228,8 @@ int ce_dit_forward_fp32(ce_dit* h, const float* hidden_states, const float* time
   const int B = batch, hp = height / c.patch_h, wp = width / c.patch_w, L = frames * hp * wp, M = B * L;
   const int H = c.num_attention_heads, hd = c.attention_head_dim, D = H * hd, F = c.ffn_dim, Lt = text_len, Li = 257;
   const int Kp = c.in_channels * 4, No = c.out_channels * 4;
-  Ctx32 X{carve32(c, workspace, B, L, Lt, Li), Launcher{s, nullptr}};
-  Ws32& ws = X.ws;
+  const Ws32 ws = carve32(c, workspace, B, L, Lt, Li);
+  Ctx32 X{{Launcher{s, nullptr}, ws.Ap, ws.Wp, ws.S, ws.P}};
   if (ws.bytes > workspace_bytes) return fail(CE_ERR_WORKSPACE, "fp32 validation workspace too small: need " + std::to_string(ws.bytes));
   CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256-byte aligned");
   const float *rope_c, *rope_s;
@@ -383,7 +244,7 @@ int ce_dit_forward_fp32(ce_dit* h, const float* hidden_states, const float* time
   CE_TRY(X.linear(ws.sin_emb, c.freq_dim, B, c.freq_dim, W.time1, D, ws.h1, D, 3));
   CE_TRY(X.linear(ws.h1, D, B, D, W.time2, D, ws.temb, D, 0));
   CE_CHECK_CUDA(cudaMemcpyAsync(ws.h1, ws.temb, (size_t)B * D * 4, cudaMemcpyDeviceToDevice, s));
-  CE_TRY(X.run.kernel(bias_act_kernel, grid_for((size_t)B * D), TPB, ws.h1, D, B, D, nullptr, 3));   // act_fn(temb)
+  CE_TRY(X.bias_act(ws.h1, D, B, D, nullptr, 3));   // act_fn(temb)
   CE_TRY(X.linear(ws.h1, D, B, D, W.time_proj, 6 * D, ws.tproj, 6 * D, 0));
   CE_TRY(X.linear(encoder_hidden_states, c.text_dim, B * Lt, c.text_dim, W.text1, D, ws.text1, D, 1));
   CE_TRY(X.linear(ws.text1, D, B * Lt, D, W.text2, D, ws.ctx_text, D, 0));
@@ -408,7 +269,7 @@ int ce_dit_forward_fp32(ce_dit* h, const float* hidden_states, const float* time
     CE_TRY(X.rms(ws.k, D, M, D, c.eps, l.norm_k, rope_c, rope_s, L, hd));
     CE_TRY(X.attention(ws.q, ws.k, ws.v, ws.attn, B, H, L, L, D, hd, scale));
     CE_TRY(X.linear(ws.attn, D, M, D, l.out1, D, ws.xn, D, 0));
-    CE_TRY(X.run.kernel(resid_kernel, grid_for((size_t)M * D), TPB, ws.x, ws.xn, M, D, mod + 2 * D, 6 * D, L));
+    CE_TRY(X.resid(ws.x, ws.xn, M, D, mod + 2 * D, 6 * D, L));
     // 2. cross-attention (:284-286)
     CE_TRY(X.layernorm(ws.x, ws.xn, M, D, c.eps, nullptr, nullptr, 0, 0, l.norm2_w, l.norm2_b));
     CE_TRY(X.linear(ws.xn, D, M, D, l.q2, D, ws.q, D, 0));
@@ -425,12 +286,12 @@ int ce_dit_forward_fp32(ce_dit* h, const float* hidden_states, const float* time
       CE_TRY(X.run.kernel(add_inplace_kernel, grid_for((size_t)M * D), TPB, ws.attn, ws.attn2, (size_t)M * D));
     }
     CE_TRY(X.linear(ws.attn, D, M, D, l.out2, D, ws.xn, D, 0));
-    CE_TRY(X.run.kernel(resid_kernel, grid_for((size_t)M * D), TPB, ws.x, ws.xn, M, D, nullptr, 0, 1));
+    CE_TRY(X.resid(ws.x, ws.xn, M, D, nullptr, 0, 1));
     // 3. feed-forward (:289-293)
     CE_TRY(X.layernorm(ws.x, ws.xn, M, D, c.eps, mod + 4 * D, mod + 3 * D, 6 * D, L, nullptr, nullptr));
     CE_TRY(X.linear(ws.xn, D, M, D, l.ffn1, F, ws.h, F, 1));
     CE_TRY(X.linear(ws.h, F, M, F, l.ffn2, D, ws.xn, D, 0));
-    CE_TRY(X.run.kernel(resid_kernel, grid_for((size_t)M * D), TPB, ws.x, ws.xn, M, D, mod + 5 * D, 6 * D, L));
+    CE_TRY(X.resid(ws.x, ws.xn, M, D, mod + 5 * D, 6 * D, L));
     if (i == 0 && block_out) CE_CHECK_CUDA(cudaMemcpyAsync(block_out, ws.x, (size_t)M * D * 4, cudaMemcpyDeviceToDevice, s));
   }
   // head (:451-467)

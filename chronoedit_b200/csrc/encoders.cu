@@ -8,13 +8,19 @@
 // kernels of elementwise.cu.  Head dims are 64 (UMT5) and 80 (CLIP ViT-H), sequence lengths 512 and 257: attention is
 // gemm_attention (gemm.cu) per sample, whose one row-softmax launch over all heads applies the reference's bf16 rounding of the
 // scores and the T5 position bias / key mask or the CLIP scale.  All rounding points of the reference's bf16 eager path are kept.
+//
+// ce_clip_vision_encode_fp32 is the same CLIP chain in fp32 -- fp32 pixels, weights, residual stream and output -- as the
+// reference CLI loads the image encoder (scripts/run_inference_diffusers.py:333-337, torch_dtype=torch.float32).  Its products,
+// attention and LayerNorms are the fp32 chain of fp32_chain.cuh (split-bf16 GEMMs, fp32 softmax), shared with the DiT's fp32 mode.
 #include <math.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
 #include "../../include/chronoedit_b200.h"
 #include "elementwise.cuh"
+#include "fp32_chain.cuh"
 #include "gemm.cuh"
 
 using namespace ce;
@@ -22,6 +28,7 @@ using namespace ce;
 struct ce_encoder {
   ce_encoder_config cfg;
   WeightMap w;
+  WeightMap w32;   // fp32 CLIP parameters (ce_encoder_set_weight_fp32), under their transformers names
   int64_t launches = 0;
 };
 
@@ -183,6 +190,107 @@ GemmAttention attention_of(const EncWs& ws, const ce_encoder_config& c, int b, i
   return a;
 }
 
+// ---- fp32 CLIP ----------------------------------------------------------------------------------------------------------------
+// im2row for the patch convolution in fp32: patches[(b, gy, gx), (c, dy, dx)] = px[b, c, gy*ps + dy, gx*ps + dx], K = 3 * ps * ps
+__global__ void clip_patchify_f32_kernel(const float* __restrict__ px, float* __restrict__ A, int B, int S, int ps) {
+  const int g = S / ps, K = 3 * ps * ps;
+  const size_t total = (size_t)B * g * g * K;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int k = (int)(i % K);
+    size_t r = i / K;
+    const int gx = (int)(r % g); r /= g;
+    const int gy = (int)(r % g);
+    const int b = (int)(r / g);
+    const int c = k / (ps * ps), dy = (k / ps) % ps, dx = k % ps;
+    A[i] = px[(((size_t)b * 3 + c) * S + gy * ps + dy) * S + gx * ps + dx];
+  }
+}
+// x[b, 0, :] = cls + pos[0];  x[b, 1 + p, :] = patch[b, p, :] + pos[1 + p]   (fp32; x is [B, L, D], patch [B, L-1, D])
+__global__ void clip_embed_f32_kernel(const float* __restrict__ patch, const float* __restrict__ cls, const float* __restrict__ pos,
+                                      float* __restrict__ x, int B, int L, int D) {
+  const size_t total = (size_t)B * L * D;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int d = (int)(i % D);
+    const size_t r = i / D;
+    const int t = (int)(r % L);
+    const int b = (int)(r / L);
+    const float e = t == 0 ? cls[d] : patch[((size_t)b * (L - 1) + (t - 1)) * D + d];
+    x[i] = e + pos[(size_t)t * D + d];
+  }
+}
+// x = x * sigmoid(1.702 x)   (CLIP "quick_gelu", fp32 as torch evaluates it)
+__global__ void quick_gelu_f32_kernel(float* __restrict__ x, size_t n) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = x[i];
+    x[i] = v * (1.0f / (1.0f + expf(-1.702f * v)));
+  }
+}
+
+// Rows are B * L, packed (the fp32 GEMM stores any row count, so no per-sample padding).
+struct ClipWs32 {
+  float *x, *xn, *q, *k, *v, *attn, *y, *h, *part, *patches, *S, *P;
+  bf16 *Ap, *Wp;
+  int64_t bytes;
+};
+ClipWs32 carve_clip32(const ce_encoder_config& c, void* base, int B) {
+  const int g = c.image_size / c.patch_size, L = 1 + g * g, L8 = up8(L), D = c.d_model, F = c.d_ff, hd = c.d_kv;
+  const int K = 3 * c.patch_size * c.patch_size;
+  const int64_t M = (int64_t)B * L, P = (int64_t)B * g * g;
+  Bump b(base);
+  ClipWs32 w;
+  w.x = b.take<float>(M * D); w.xn = b.take<float>(M * D);
+  w.q = b.take<float>(M * D); w.k = b.take<float>(M * D); w.v = b.take<float>(M * D);
+  w.attn = b.take<float>(M * D); w.y = b.take<float>(M * D); w.h = b.take<float>(M * F); w.part = b.take<float>(std::max((int64_t)L * L8, M * std::max(D, F)));
+  w.patches = b.take<float>(P * K);
+  w.S = b.take<float>((int64_t)L * L8); w.P = b.take<float>((int64_t)L * L8);
+  // the split operands of the largest product on each side: the Linears (patch, q / k / v / out, fc1, fc2), S and P.V
+  const int64_t a_elems = std::max({split_elems(P, K, 6), split_elems(M, D, 6), split_elems(M, F, 6), split_elems(L, hd, 6), split_elems(L, L8, 6)});
+  const int64_t w_elems = std::max({split_elems(D, K, 6), split_elems(D, D, 6), split_elems(F, D, 6), split_elems(D, F, 6), split_elems(L8, hd, 6),
+                                    split_elems(hd, L8, 6)});
+  w.Ap = b.take<bf16>(a_elems); w.Wp = b.take<bf16>(w_elems);
+  w.bytes = b.bytes();
+  return w;
+}
+
+struct ClipLayer32 {
+  const float *ln1_w, *ln1_b, *ln2_w, *ln2_b;
+  Lin32 q, k, v, out, fc1, fc2;
+};
+// Every fp32 parameter ce_clip_vision_encode_fp32 reads, under its transformers name, unfused.
+struct ClipWeights32 {
+  Lin32 patch;   // patch_embedding.weight [D, 3, ps, ps] read as [D, 3 * ps * ps]; no bias
+  const float *cls = nullptr, *pos = nullptr, *pre_ln_w = nullptr, *pre_ln_b = nullptr;
+  std::vector<ClipLayer32> layers;
+};
+int resolve_clip32(const ce_encoder* h, ClipWeights32& w) {
+  const ce_encoder_config& c = h->cfg;
+  const int64_t D = c.d_model, F = c.d_ff, g = c.image_size / c.patch_size;
+  WeightLookup r{h->w32};
+  auto lin = [&](const std::string& m, int64_t N, int64_t K) { return Lin32{r.f32(m + ".weight", N * K), r.f32(m + ".bias", N)}; };
+  const std::string vm = "vision_model.";
+  w.patch.w = r.f32(vm + "embeddings.patch_embedding.weight", D * 3 * c.patch_size * c.patch_size);
+  w.cls = r.f32(vm + "embeddings.class_embedding", D);
+  w.pos = r.f32(vm + "embeddings.position_embedding.weight", (1 + g * g) * D);
+  w.pre_ln_w = r.f32(vm + "pre_layrnorm.weight", D);
+  w.pre_ln_b = r.f32(vm + "pre_layrnorm.bias", D);
+  for (int l = 0; l < c.num_layers; ++l) {
+    const std::string p = vm + "encoder.layers." + std::to_string(l) + ".";
+    ClipLayer32 L;
+    L.ln1_w = r.f32(p + "layer_norm1.weight", D);
+    L.ln1_b = r.f32(p + "layer_norm1.bias", D);
+    L.q = lin(p + "self_attn.q_proj", D, D);
+    L.k = lin(p + "self_attn.k_proj", D, D);
+    L.v = lin(p + "self_attn.v_proj", D, D);
+    L.out = lin(p + "self_attn.out_proj", D, D);
+    L.ln2_w = r.f32(p + "layer_norm2.weight", D);
+    L.ln2_b = r.f32(p + "layer_norm2.bias", D);
+    L.fc1 = lin(p + "mlp.fc1", F, D);
+    L.fc2 = lin(p + "mlp.fc2", D, F);
+    w.layers.push_back(L);
+  }
+  return r.rc;
+}
+
 }  // namespace
 
 extern "C" {
@@ -209,6 +317,16 @@ int64_t ce_encoder_workspace_bytes(const ce_encoder* h, int batch, int seq_len) 
   return carve(h->cfg, nullptr, batch, seq_len).bytes;
 }
 int64_t ce_encoder_last_launch_count(const ce_encoder* h) { return h ? h->launches : 0; }
+
+int ce_encoder_set_weight_fp32(ce_encoder* h, const char* name, const float* ptr, int64_t numel) {
+  CE_REQUIRE(h, "ce_encoder_set_weight_fp32: null handle");
+  return register_weight(h->w32, "ce_encoder_set_weight_fp32", name, ptr, 1, numel);
+}
+
+int64_t ce_clip_vision_fp32_workspace_bytes(const ce_encoder* h, int batch) {
+  if (!h || h->cfg.kind != 1 || batch < 1) return -1;
+  return carve_clip32(h->cfg, nullptr, batch).bytes;
+}
 
 // UMT5EncoderModel.forward(input_ids [B, L] int64, attention_mask -> valid_len[b] leading valid tokens) -> last_hidden_state [B, L, D]
 int ce_umt5_encode(ce_encoder* h, const int64_t* input_ids, const int32_t* valid_len_host, void* last_hidden_state, int batch, int seq_len,
@@ -311,6 +429,54 @@ int ce_clip_vision_encode(ce_encoder* h, const void* pixel_values, void* out, in
   }
   for (int b = 0; b < B; ++b)
     CE_CHECK_CUDA(cudaMemcpyAsync(reinterpret_cast<bf16*>(out) + (size_t)b * L * D, ws.x + (size_t)b * L8 * D, (size_t)L * D * 2, cudaMemcpyDeviceToDevice, s));
+  return CE_OK;
+}
+
+// The same call in fp32, on the parameters registered with ce_encoder_set_weight_fp32: transformers' CLIPVisionModel loaded in fp32.
+int ce_clip_vision_encode_fp32(ce_encoder* h, const float* pixel_values, float* out, int batch, int layers_to_run, void* workspace,
+                               int64_t workspace_bytes, void* stream_v) {
+  CE_REQUIRE(h && pixel_values && out && workspace, "ce_clip_vision_encode_fp32: null argument");
+  const ce_encoder_config& c = h->cfg;
+  CE_REQUIRE(c.kind == 1, "ce_clip_vision_encode_fp32: handle is not a CLIP vision encoder");
+  CE_REQUIRE(batch >= 1, "ce_clip_vision_encode_fp32: batch >= 1");
+  CE_REQUIRE(layers_to_run >= 0 && layers_to_run <= c.num_layers, "ce_clip_vision_encode_fp32: layers_to_run");
+  CE_REQUIRE(!h->w32.empty(), "ce_clip_vision_encode_fp32: the handle has no fp32 weights (register them with ce_encoder_set_weight_fp32)");
+  ClipWeights32 W;
+  CE_TRY(resolve_clip32(h, W));
+  const ClipWs32 ws = carve_clip32(c, workspace, batch);
+  if (ws.bytes > workspace_bytes)
+    return fail(CE_ERR_WORKSPACE, "ce_clip_vision_encode_fp32: workspace too small, need " + std::to_string(ws.bytes));
+  CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "ce_clip_vision_encode_fp32: workspace must be 256-byte aligned");
+  CE_TRY(check_device());
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_v);
+  const int B = batch, g = c.image_size / c.patch_size, L = 1 + g * g, M = B * L, D = c.d_model, H = c.num_heads, hd = c.d_kv, F = c.d_ff;
+  const int K = 3 * c.patch_size * c.patch_size;
+  Fp32Chain X{Launcher{s, &h->launches}, ws.Ap, ws.Wp, ws.S, ws.P, 6, ws.part};
+  h->launches = 0;
+  // embeddings: patch conv as im2row + GEMM (no bias), class token, position embedding, pre_layrnorm
+  CE_TRY(X.run.kernel(clip_patchify_f32_kernel, grid_for((size_t)B * g * g * K), TPB, pixel_values, ws.patches, B, c.image_size, c.patch_size));
+  CE_TRY(X.linear(ws.patches, K, B * g * g, K, W.patch, D, ws.y, D, 0));
+  CE_TRY(X.run.kernel(clip_embed_f32_kernel, grid_for((size_t)M * D), TPB, ws.y, W.cls, W.pos, ws.xn, B, L, D));
+  CE_TRY(X.layernorm(ws.xn, ws.x, M, D, c.eps, nullptr, nullptr, 0, 0, W.pre_ln_w, W.pre_ln_b));
+  const float scale = 1.0f / sqrtf((float)hd);
+  for (int l = 0; l < layers_to_run; ++l) {
+    const ClipLayer32& lw = W.layers[l];
+    // x = x + out_proj(attn(LayerNorm1(x)))
+    CE_TRY(X.layernorm(ws.x, ws.xn, M, D, c.eps, nullptr, nullptr, 0, 0, lw.ln1_w, lw.ln1_b));
+    CE_TRY(X.linear(ws.xn, D, M, D, lw.q, D, ws.q, D, 0));
+    CE_TRY(X.linear(ws.xn, D, M, D, lw.k, D, ws.k, D, 0));
+    CE_TRY(X.linear(ws.xn, D, M, D, lw.v, D, ws.v, D, 0));
+    CE_TRY(X.attention(ws.q, ws.k, ws.v, ws.attn, B, H, L, L, D, hd, scale));
+    CE_TRY(X.linear(ws.attn, D, M, D, lw.out, D, ws.y, D, 0));
+    CE_TRY(X.resid(ws.x, ws.y, M, D, nullptr, 0, 1));
+    // x = x + fc2(act(fc1(LayerNorm2(x))))
+    CE_TRY(X.layernorm(ws.x, ws.xn, M, D, c.eps, nullptr, nullptr, 0, 0, lw.ln2_w, lw.ln2_b));
+    CE_TRY(X.linear(ws.xn, D, M, D, lw.fc1, F, ws.h, F, c.hidden_act == 1 ? 2 : 0));   // 1 gelu (erf); 0 quick_gelu, a pass of its own
+    if (c.hidden_act == 0) CE_TRY(X.run.kernel(quick_gelu_f32_kernel, grid_for((size_t)M * F), TPB, ws.h, (size_t)M * F));
+    CE_TRY(X.linear(ws.h, F, M, F, lw.fc2, D, ws.y, D, 0));
+    CE_TRY(X.resid(ws.x, ws.y, M, D, nullptr, 0, 1));
+  }
+  CE_CHECK_CUDA(cudaMemcpyAsync(out, ws.x, (size_t)M * D * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return CE_OK;
 }
 

@@ -6,10 +6,16 @@
 Same constructor configuration fields, same parameter names as the transformers modules (their `state_dict()` loads unchanged),
 same call surface as far as the pipeline touches it.  All arithmetic runs in libchronoedit_b200.so (`ce_umt5_encode`,
 `ce_clip_vision_encode`: wgmma GEMMs + row kernels, csrc/encoders.cu); PyTorch owns memory and streams.  No CPU path.
+
+`from_pretrained` reads a local transformers-format directory (config.json + model.safetensors or its sharded index).  CLIP also runs
+in fp32 (`torch_dtype=torch.float32`, `ce_clip_vision_encode_fp32`), as the reference CLI loads it
+(run_inference_diffusers.py:333-337); the text encoder is bf16 only, as the pipeline loads it.
 """
 from __future__ import annotations
 
+import json
 import math
+import os
 from types import SimpleNamespace
 from typing import Dict, Optional
 
@@ -17,6 +23,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from ._checkpoint import load_safetensors
 from ._lib import CEError, EncoderConfigC, check, current_stream, ptr
 
 
@@ -37,9 +44,17 @@ def _reg(mod: nn.Module, dotted: str, shape, dtype=torch.bfloat16, device=None) 
     mod.register_parameter(parts[-1], nn.Parameter(torch.empty(shape, dtype=dtype, device=device), requires_grad=False))
 
 
+def _read_config(pretrained_model_name_or_path: str, subfolder: Optional[str], fields) -> tuple:
+    root = os.path.join(pretrained_model_name_or_path, subfolder) if subfolder else pretrained_model_name_or_path
+    with open(os.path.join(root, "config.json")) as f:
+        cfg = json.load(f)
+    return root, {k: cfg[k] for k in fields if k in cfg}
+
+
 class _Base(nn.Module):
     def __init__(self):
         super().__init__()
+        self._fp32 = False
         self._handle = None
         self._packed = False
         self._keep: Dict[str, torch.Tensor] = {}
@@ -47,7 +62,7 @@ class _Base(nn.Module):
 
     @property
     def dtype(self) -> torch.dtype:
-        return torch.bfloat16
+        return torch.float32 if self._fp32 else torch.bfloat16
 
     @property
     def device(self) -> torch.device:
@@ -73,10 +88,14 @@ class _Base(nn.Module):
     def _set(self, name: str, t: torch.Tensor) -> None:
         t = t.contiguous()
         self._keep[name] = t
-        check(_lib.lib().ce_encoder_set_weight(self._handle, name.encode(), ptr(t), t.numel()))
+        set_weight = _lib.lib().ce_encoder_set_weight_fp32 if self._fp32 else _lib.lib().ce_encoder_set_weight
+        check(set_weight(self._handle, name.encode(), ptr(t), t.numel()))
 
     def _workspace(self, B: int, L: int) -> torch.Tensor:
-        n = _lib.lib().ce_encoder_workspace_bytes(self._handle, B, L)
+        if self._fp32:
+            n = _lib.lib().ce_clip_vision_fp32_workspace_bytes(self._handle, B)
+        else:
+            n = _lib.lib().ce_encoder_workspace_bytes(self._handle, B, L)
         if n < 0:
             check(-1)
         if self._ws is None or self._ws.numel() < n or self._ws.device != self.device:
@@ -121,6 +140,20 @@ class UMT5EncoderModel(_Base):
         sd = {k: v for k, v in state_dict.items() if k != "encoder.embed_tokens.weight"}   # tied to shared.weight in transformers
         self._packed = False
         return super().load_state_dict(sd, strict=strict, assign=assign)
+
+    @classmethod
+    def from_pretrained(cls, pretrained_model_name_or_path: str, subfolder: Optional[str] = None, torch_dtype: Optional[torch.dtype] = None,
+                        device=None, **unused) -> "UMT5EncoderModel":
+        """`UMT5EncoderModel.from_pretrained(model_id, subfolder="text_encoder")` for a LOCAL transformers-format directory (config.json +
+        model.safetensors or model.safetensors.index.json).  bf16 only: the pipeline runs the text encoder in its own bf16."""
+        if torch_dtype not in (None, torch.bfloat16):
+            raise CEError(f"UMT5EncoderModel: torch_dtype {torch_dtype} is not built; the text encoder runs in bf16 only")
+        fields = ("vocab_size", "d_model", "d_kv", "d_ff", "num_layers", "num_heads", "relative_attention_num_buckets",
+                  "relative_attention_max_distance", "layer_norm_epsilon", "feed_forward_proj")
+        root, cfg = _read_config(pretrained_model_name_or_path, subfolder, fields)
+        model = cls(**cfg, device=device or "cpu")
+        load_safetensors(model, root, "model", skip=lambda k: k == "encoder.embed_tokens.weight")   # tied to shared.weight
+        return model
 
     # T5 bucket function (transformers UMT5Attention._relative_position_bucket, bidirectional), host code
     def _bucket(self, rel: torch.Tensor) -> torch.Tensor:
@@ -220,39 +253,56 @@ class CLIPVisionModel(_Base):
 
     def __init__(self, hidden_size: int = 1280, intermediate_size: int = 5120, num_hidden_layers: int = 32, num_attention_heads: int = 16,
                  image_size: int = 224, patch_size: int = 14, hidden_act: str = "gelu", layer_norm_eps: float = 1e-5, num_channels: int = 3, *,
-                 device=None, **unused):
+                 torch_dtype: Optional[torch.dtype] = None, device=None, **unused):
         super().__init__()
         if hidden_act not in ("gelu", "quick_gelu") or num_channels != 3 or hidden_size % num_attention_heads:
             raise CEError("CLIPVisionModel: hidden_act must be gelu or quick_gelu, 3 input channels")
+        if torch_dtype not in (None, torch.bfloat16, torch.float32):
+            raise CEError(f"CLIPVisionModel: torch_dtype {torch_dtype} is not built; use torch.bfloat16 or torch.float32")
+        self._fp32 = torch_dtype == torch.float32
+        dt = self.dtype
         self.config = _Cfg(hidden_size=hidden_size, intermediate_size=intermediate_size, num_hidden_layers=num_hidden_layers,
                            num_attention_heads=num_attention_heads, image_size=image_size, patch_size=patch_size, hidden_act=hidden_act,
                            layer_norm_eps=layer_norm_eps, num_channels=num_channels)
         D, F = hidden_size, intermediate_size
         n_pos = 1 + (image_size // patch_size) ** 2
         vm = "vision_model."
-        _reg(self, vm + "embeddings.class_embedding", (D,), device=device)
-        _reg(self, vm + "embeddings.patch_embedding.weight", (D, 3, patch_size, patch_size), device=device)
-        _reg(self, vm + "embeddings.position_embedding.weight", (n_pos, D), device=device)
+        _reg(self, vm + "embeddings.class_embedding", (D,), dtype=dt, device=device)
+        _reg(self, vm + "embeddings.patch_embedding.weight", (D, 3, patch_size, patch_size), dtype=dt, device=device)
+        _reg(self, vm + "embeddings.position_embedding.weight", (n_pos, D), dtype=dt, device=device)
         for n in ("pre_layrnorm", "post_layernorm"):
-            _reg(self, vm + n + ".weight", (D,), device=device)
-            _reg(self, vm + n + ".bias", (D,), device=device)
+            _reg(self, vm + n + ".weight", (D,), dtype=dt, device=device)
+            _reg(self, vm + n + ".bias", (D,), dtype=dt, device=device)
         for l in range(num_hidden_layers):
             p = vm + f"encoder.layers.{l}."
             for n in ("q_proj", "k_proj", "v_proj", "out_proj"):
-                _reg(self, p + f"self_attn.{n}.weight", (D, D), device=device)
-                _reg(self, p + f"self_attn.{n}.bias", (D,), device=device)
+                _reg(self, p + f"self_attn.{n}.weight", (D, D), dtype=dt, device=device)
+                _reg(self, p + f"self_attn.{n}.bias", (D,), dtype=dt, device=device)
             for n in ("layer_norm1", "layer_norm2"):
-                _reg(self, p + n + ".weight", (D,), device=device)
-                _reg(self, p + n + ".bias", (D,), device=device)
-            _reg(self, p + "mlp.fc1.weight", (F, D), device=device)
-            _reg(self, p + "mlp.fc1.bias", (F,), device=device)
-            _reg(self, p + "mlp.fc2.weight", (D, F), device=device)
-            _reg(self, p + "mlp.fc2.bias", (D,), device=device)
+                _reg(self, p + n + ".weight", (D,), dtype=dt, device=device)
+                _reg(self, p + n + ".bias", (D,), dtype=dt, device=device)
+            _reg(self, p + "mlp.fc1.weight", (F, D), dtype=dt, device=device)
+            _reg(self, p + "mlp.fc1.bias", (F,), dtype=dt, device=device)
+            _reg(self, p + "mlp.fc2.weight", (D, F), dtype=dt, device=device)
+            _reg(self, p + "mlp.fc2.bias", (D,), dtype=dt, device=device)
 
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):
         sd = {k: v for k, v in state_dict.items() if not k.endswith("position_ids")}   # non-parameter buffer of older transformers
         self._packed = False
         return super().load_state_dict(sd, strict=strict, assign=assign)
+
+    @classmethod
+    def from_pretrained(cls, pretrained_model_name_or_path: str, subfolder: Optional[str] = None, torch_dtype: Optional[torch.dtype] = None,
+                        device=None, **unused) -> "CLIPVisionModel":
+        """`CLIPVisionModel.from_pretrained(model_id, subfolder="image_encoder", torch_dtype=torch.float32)` (run_inference_diffusers.py:333-337)
+        for a LOCAL transformers-format directory (config.json + model.safetensors or model.safetensors.index.json).  torch_dtype as the
+        constructor takes it: None or torch.bfloat16 gives the bf16 encoder, torch.float32 the fp32 one."""
+        fields = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "image_size", "patch_size", "hidden_act",
+                  "layer_norm_eps", "num_channels")
+        root, cfg = _read_config(pretrained_model_name_or_path, subfolder, fields)
+        model = cls(**cfg, torch_dtype=torch_dtype, device=device or "cpu")
+        load_safetensors(model, root, "model", skip=lambda k: k.endswith("position_ids"))   # buffer of older transformers
+        return model
 
     @torch.no_grad()
     def _pack(self) -> None:
@@ -263,6 +313,14 @@ class CLIPVisionModel(_Base):
                                     c.num_attention_heads, c.layer_norm_eps, c.image_size, c.patch_size, 1 if c.hidden_act == "gelu" else 0))
         self._keep = {}
         params = dict(self.named_parameters())
+        if self._fp32:   # the parameters as they are, under their own names (post_layernorm is not read)
+            for n, p in params.items():
+                if p.dtype != torch.float32:
+                    p.data = p.data.float()
+                if "post_layernorm" not in n:
+                    self._set(n, p.data)
+            self._packed = True
+            return
         for n, p in params.items():
             if p.dtype != torch.bfloat16:
                 p.data = p.data.to(torch.bfloat16)
@@ -295,12 +353,13 @@ class CLIPVisionModel(_Base):
         B = pixel_values.shape[0]
         if tuple(pixel_values.shape[1:]) != (3, c.image_size, c.image_size):
             raise CEError(f"CLIPVisionModel expects pixel_values [B, 3, {c.image_size}, {c.image_size}]")
-        px = pixel_values.to(device=self.device, dtype=torch.bfloat16).contiguous()
+        px = pixel_values.to(device=self.device, dtype=self.dtype).contiguous()
         L = 1 + (c.image_size // c.patch_size) ** 2
-        out = torch.empty(B, L, c.hidden_size, dtype=torch.bfloat16, device=self.device)
+        out = torch.empty(B, L, c.hidden_size, dtype=self.dtype, device=self.device)
         ws = self._workspace(B, L)
+        encode = _lib.lib().ce_clip_vision_encode_fp32 if self._fp32 else _lib.lib().ce_clip_vision_encode
         with torch.cuda.device(self.device):
-            check(_lib.lib().ce_clip_vision_encode(self._handle, ptr(px), ptr(out), B, int(layers_to_run), ptr(ws), ws.numel(), current_stream()))
+            check(encode(self._handle, ptr(px), ptr(out), B, int(layers_to_run), ptr(ws), ws.numel(), current_stream()))
         return out
 
     @torch.no_grad()

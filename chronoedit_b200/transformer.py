@@ -20,6 +20,7 @@ import torch.nn as nn
 
 from . import _lib
 from . import teacache as _tc
+from ._checkpoint import load_safetensors
 from ._lib import CEError, DiTConfigC, check, current_stream, ptr
 
 # reference `_keep_in_fp32_modules` (transformer_chronoedit.py:338)
@@ -1249,30 +1250,10 @@ class ChronoEditTransformer3DModel(nn.Module):
                         **unused) -> "ChronoEditTransformer3DModel":
         """Load a diffusers-format checkpoint directory (config.json + diffusion_pytorch_model*.safetensors), the layout
         `run_inference_diffusers.py:349-353` reads.  Local paths only (no hub download)."""
-        from safetensors import safe_open
-
         root = os.path.join(pretrained_model_name_or_path, subfolder) if subfolder else pretrained_model_name_or_path
         with open(os.path.join(root, cls.config_name)) as f:
             cfg = json.load(f)
         model = cls.from_config(cfg, torch_dtype=torch_dtype, device=device or "cpu")
-        index = os.path.join(root, "diffusion_pytorch_model.safetensors.index.json")
-        if os.path.exists(index):
-            with open(index) as f:
-                files = sorted(set(json.load(f)["weight_map"].values()))
-        else:
-            files = ["diffusion_pytorch_model.safetensors"]
-        params = dict(model.named_parameters())
-        seen = set()
-        for fn in files:
-            with safe_open(os.path.join(root, fn), framework="pt", device="cpu") as sf:
-                for k in sf.keys():
-                    if "norm_added_q" in k:  # `_keys_to_ignore_on_load_unexpected` (transformer_chronoedit.py:339)
-                        continue
-                    if k not in params:
-                        raise CEError(f"unexpected key in checkpoint: {k}")
-                    params[k].data.copy_(sf.get_tensor(k).reshape(params[k].shape))
-                    seen.add(k)
-        missing = sorted(set(params) - seen)
-        if missing:
-            raise CEError(f"checkpoint is missing {len(missing)} parameters, first: {missing[0]}")
+        # `_keys_to_ignore_on_load_unexpected` (transformer_chronoedit.py:339)
+        load_safetensors(model, root, "diffusion_pytorch_model", skip=lambda k: "norm_added_q" in k)
         return model

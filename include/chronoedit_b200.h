@@ -351,6 +351,18 @@ int ce_umt5_encode(ce_encoder* h, const int64_t* input_ids, const int32_t* valid
  * (hidden_states[-2] = num_layers - 1 layers; 0 = the embeddings after pre_layrnorm). */
 int ce_clip_vision_encode(ce_encoder* h, const void* pixel_values, void* out, int batch, int layers_to_run, void* workspace,
                           int64_t workspace_bytes, void* stream);
+/* The CLIP call in fp32, as the reference CLI loads the image encoder (CLIPVisionModel.from_pretrained(..., torch_dtype=torch.float32)):
+ * pixel_values [B, 3, S, S] fp32 -> out [B, 1 + (S/ps)^2, d_model] fp32, after `layers_to_run` encoder layers.  Parameters are
+ * registered with ce_encoder_set_weight_fp32, fp32, under their transformers names UNFUSED ("...self_attn.q_proj.weight", the LayerNorms
+ * without a suffix, "vision_model.embeddings.patch_embedding.weight" as it is, [D, 3, ps, ps]); post_layernorm is not read.  Products
+ * run on the wgmma GEMM with every fp32 operand split into three bf16 terms (csrc/fp32_chain.cuh), within rtol 1e-3 / atol 1e-4 of
+ * transformers' fp32 CLIPVisionModel at ViT-H/14 (tests/test_gpu_clip_fp32.py).
+ * Refused before any launch: a UMT5 handle, a handle without fp32 weights, a missing or mis-sized weight, and a workspace smaller than
+ * ce_clip_vision_fp32_workspace_bytes(h, batch) or not 256-byte aligned. */
+int ce_encoder_set_weight_fp32(ce_encoder* h, const char* name, const float* ptr, int64_t numel);
+int64_t ce_clip_vision_fp32_workspace_bytes(const ce_encoder* h, int batch);   /* -1 for a UMT5 handle or batch < 1 */
+int ce_clip_vision_encode_fp32(ce_encoder* h, const float* pixel_values, float* out, int batch, int layers_to_run, void* workspace,
+                               int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Individual hot-path operators (used by the handles above; exported for operator-level parity tests / profiling)
