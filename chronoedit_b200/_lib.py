@@ -149,6 +149,10 @@ SIGNATURES = {
     "ce_vae_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "ce_vae_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "ce_vae_last_launch_count": (c_int64, [c_void_p]),
+    "ce_vae_set_weight_fp32": (c_int, [c_void_p, c_char_p, c_void_p, c_int64]),
+    "ce_vae_workspace_bytes_fp32": (c_int64, [c_void_p, c_int, c_int, c_int, c_int]),
+    "ce_vae_encode_fp32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
+    "ce_vae_decode_fp32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "ce_vae_sp_region_bytes": (c_int64, [c_void_p, c_int, c_int, c_int]),
     "ce_vae_sp_configure": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64]),
     "ce_vae_sp_host_barrier": (c_int, [c_void_p, c_int]),
@@ -187,6 +191,7 @@ SIGNATURES = {
     "ce_im2row_bf16": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int,
                                c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "ce_conv3d_cl_ex_bf16": (c_int, [POINTER(Conv3dArgsC), c_void_p]),
+    "ce_conv3d_cl_ex_fp32": (c_int, [POINTER(Conv3dArgsC), c_void_p, c_void_p]),
     "ce_gemm_attention_bf16": (c_int, [POINTER(GemmAttentionArgsC), c_void_p]),
 }
 

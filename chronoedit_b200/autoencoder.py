@@ -165,6 +165,26 @@ def pack_parameter(name: str, w: torch.Tensor) -> torch.Tensor:
     return out.reshape(cout, -1).contiguous()
 
 
+def pack_parameter_fp32(name: str, w: torch.Tensor) -> torch.Tensor:
+    """Reference layout -> the layout ce_vae_set_weight_fp32 documents: convolution weights (every one, the small ones included) as
+    [Cout, taps, Cin_pad / 64, 3, 64] bf16 with W_hi | W_hi | W_lo per 64-channel block, the split the fp32 convolution multiplies
+    with its input's hi / lo pair; everything else fp32 as it is."""
+    w = w.detach().to(torch.float32)
+    base = name[: -len(".weight")] if name.endswith(".weight") else None
+    if base is None or base.endswith("to_qkv") or base.endswith(".proj"):
+        return w.reshape(w.shape[0], -1).contiguous() if base else w.reshape(-1).contiguous()
+    if w.dim() == 4:
+        w = w[:, :, None]
+    cout, cin, kt, kh, kw = w.shape
+    cp = _round_up(cin, 64)
+    full = torch.zeros(cout, kt * kh * kw, cp, dtype=torch.float32, device=w.device)
+    full[:, :, :cin] = w.permute(0, 2, 3, 4, 1).reshape(cout, kt * kh * kw, cin)
+    full = full.reshape(cout, kt * kh * kw, cp // 64, 64)
+    hi = full.to(torch.bfloat16)
+    lo = (full - hi.float()).to(torch.bfloat16)
+    return torch.stack((hi, hi, lo), dim=3).reshape(cout, -1).contiguous()
+
+
 class AutoencoderKLWan(nn.Module):
     """See module docstring.  Defaults = Wan2.1 VAE (wan2pt1.py:597-605)."""
 
@@ -173,19 +193,21 @@ class AutoencoderKLWan(nn.Module):
                  dropout: float = 0.0, latents_mean: Optional[List[float]] = None, latents_std: Optional[List[float]] = None,
                  *, torch_dtype: torch.dtype = torch.bfloat16, device=None, clamp_output: bool = True):
         super().__init__()
-        if torch_dtype != torch.bfloat16:
-            raise CEError("chronoedit_b200 VAE computes in bf16 (run_inference_diffusers.py:341-345 loads it in bf16)")
+        if torch_dtype not in (torch.bfloat16, torch.float32):
+            raise CEError("chronoedit_b200 VAE computes in bf16 (run_inference_diffusers.py:341-345 loads it in bf16) or in fp32 "
+                          f"(the reference pipeline's example loads it in fp32), not {torch_dtype}")
         if len(dim_mult) != 4 or len(temperal_downsample) != 3 or len(attn_scales) != 0:
             raise CEError("only the Wan2.1 layout (4 stages, no extra attention scales) is built")
         self.config = _Config(base_dim=base_dim, z_dim=z_dim, dim_mult=list(dim_mult), num_res_blocks=num_res_blocks,
                               attn_scales=list(attn_scales), temperal_downsample=list(temperal_downsample), dropout=dropout,
                               latents_mean=list(latents_mean or LATENTS_MEAN), latents_std=list(latents_std or LATENTS_STD))
         self.temperal_downsample = list(temperal_downsample)
+        self._dtype = torch_dtype   # what encode / decode compute in, whatever .to() later does to the parameters
         self.z_dim = z_dim
         self.clamp_output = clamp_output
         self._shapes = _param_shapes(base_dim, z_dim, tuple(dim_mult), num_res_blocks, tuple(temperal_downsample))
         for name, shape in self._shapes.items():
-            self._register(name, nn.Parameter(torch.empty(shape, dtype=torch.bfloat16, device=device), requires_grad=False))
+            self._register(name, nn.Parameter(torch.empty(shape, dtype=torch_dtype, device=device), requires_grad=False))
         self._handle = None
         self._packed: Dict[str, torch.Tensor] = {}
         self._is_packed = False
@@ -203,7 +225,8 @@ class AutoencoderKLWan(nn.Module):
 
     @property
     def dtype(self) -> torch.dtype:
-        return torch.bfloat16
+        """torch.bfloat16, or torch.float32 for a VAE built or loaded with torch_dtype=torch.float32 (fp32 encode / decode)."""
+        return self._dtype
 
     @property
     def device(self) -> torch.device:
@@ -238,10 +261,11 @@ class AutoencoderKLWan(nn.Module):
             raise CEError("AutoencoderKLWan must live on a CUDA (sm_90) device; there is no CPU path")
         self._ensure_handle()
         packed = {}
+        fp32 = self.dtype == torch.float32
         for name, p in self.named_parameters():
-            t = pack_parameter(name, p.data)
+            t = (pack_parameter_fp32 if fp32 else pack_parameter)(name, p.data)
             packed[name] = t
-            check(L.ce_vae_set_weight(self._handle, name.encode(), ptr(t), t.numel()))
+            check((L.ce_vae_set_weight_fp32 if fp32 else L.ce_vae_set_weight)(self._handle, name.encode(), ptr(t), t.numel()))
         self._packed = packed
         self._is_packed = True
 
@@ -252,16 +276,25 @@ class AutoencoderKLWan(nn.Module):
         return self._ws
 
     # ------------------------------------------------------------------------------------------ encode / decode
+    # An fp32 VAE computes in fp32 and returns fp32.  It widens a bf16 x or z to fp32 (exact), so the unchanged pipeline's
+    # prepare_latents, which casts the conditioning video to the transformer's bf16 before vae.encode, runs; diffusers' fp32 Conv3d
+    # would reject that input instead.
+    def _check_fp32_single_gpu(self) -> None:
+        if self.dtype == torch.float32 and self._sp_state:
+            raise CEError("the fp32 VAE does not run split over GPUs (parallel.enable_vae_sequence_parallel is built for bf16 only)")
+
     @torch.no_grad()
     def encode(self, x: torch.Tensor, return_dict: bool = True):
-        """x [B,3,T,H,W] in [-1,1], T = 1+4k, H and W multiples of 8 -> posterior (mean|logvar [B,2z,1+k,H/8,W/8])."""
+        """x [B,3,T,H,W] in [-1,1], T = 1+4k, H and W multiples of 8 -> posterior (mean|logvar [B,2z,1+k,H/8,W/8]), in the VAE's
+        dtype."""
         if x.dim() != 5 or x.shape[1] != 3:
             raise CEError("encode expects [B, 3, T, H, W]")
         B, _, T, H, W = x.shape
         if T < 1 or (T - 1) % 4 != 0 or H % 8 != 0 or W % 8 != 0:
             raise CEError("encode expects T = 1 + 4k frames and H, W multiples of 8")
-        x = x.to(device=self.device, dtype=torch.bfloat16).contiguous()
-        out = torch.empty(B, 2 * self.z_dim, 1 + (T - 1) // 4, H // 8, W // 8, dtype=torch.bfloat16, device=self.device)
+        self._check_fp32_single_gpu()
+        x = x.to(device=self.device, dtype=self.dtype).contiguous()
+        out = torch.empty(B, 2 * self.z_dim, 1 + (T - 1) // 4, H // 8, W // 8, dtype=self.dtype, device=self.device)
         self._native_encode(x, out)
         post = DiagonalGaussianDistribution(out)
         if not return_dict:
@@ -270,12 +303,13 @@ class AutoencoderKLWan(nn.Module):
 
     @torch.no_grad()
     def decode(self, z: torch.Tensor, return_dict: bool = True):
-        """z [B,z_dim,Tl,h,w] -> video [B,3,1+4(Tl-1),8h,8w] (clamped to [-1,1] like diffusers)."""
+        """z [B,z_dim,Tl,h,w] -> video [B,3,1+4(Tl-1),8h,8w] (clamped to [-1,1] like diffusers), in the VAE's dtype."""
         if z.dim() != 5 or z.shape[1] != self.z_dim:
             raise CEError(f"decode expects [B, {self.z_dim}, T, h, w]")
         B, _, Tl, h, w = z.shape
-        z = z.to(device=self.device, dtype=torch.bfloat16).contiguous()
-        out = torch.empty(B, 3, 1 + 4 * (Tl - 1), 8 * h, 8 * w, dtype=torch.bfloat16, device=self.device)
+        self._check_fp32_single_gpu()
+        z = z.to(device=self.device, dtype=self.dtype).contiguous()
+        out = torch.empty(B, 3, 1 + 4 * (Tl - 1), 8 * h, 8 * w, dtype=self.dtype, device=self.device)
         self._native_decode(z, out)
         if not return_dict:
             return (out,)
@@ -287,28 +321,32 @@ class AutoencoderKLWan(nn.Module):
         if not self._is_packed:
             self.pack_weights()
         L = _lib.lib()
+        fp32 = self.dtype == torch.float32
         B, _, T, H, W = x.shape
-        n = L.ce_vae_workspace_bytes(self._handle, 0, T, H, W)
+        n = (L.ce_vae_workspace_bytes_fp32 if fp32 else L.ce_vae_workspace_bytes)(self._handle, 0, T, H, W)
         if n < 0:
             check(-1)
         ws = self._workspace(n)
+        encode = L.ce_vae_encode_fp32 if fp32 else L.ce_vae_encode
         with torch.cuda.device(self.device):
             for b in range(B):
-                check(L.ce_vae_encode(self._handle, ptr(x[b]), ptr(out[b]), T, H, W, ptr(ws), ws.numel(), current_stream()))
+                check(encode(self._handle, ptr(x[b]), ptr(out[b]), T, H, W, ptr(ws), ws.numel(), current_stream()))
 
     def _native_decode(self, z: torch.Tensor, out: torch.Tensor) -> None:
         if not self._is_packed:
             self.pack_weights()
         L = _lib.lib()
+        fp32 = self.dtype == torch.float32
         B, _, Tl, h, w = z.shape
-        n = L.ce_vae_workspace_bytes(self._handle, 1, Tl, h, w)
+        n = (L.ce_vae_workspace_bytes_fp32 if fp32 else L.ce_vae_workspace_bytes)(self._handle, 1, Tl, h, w)
         if n < 0:
             check(-1)
         ws = self._workspace(n)
+        decode = L.ce_vae_decode_fp32 if fp32 else L.ce_vae_decode
         with torch.cuda.device(self.device):
             for b in range(B):
-                check(L.ce_vae_decode(self._handle, ptr(z[b]), ptr(out[b]), Tl, h, w, int(self.clamp_output), ptr(ws), ws.numel(),
-                                      current_stream()))
+                check(decode(self._handle, ptr(z[b]), ptr(out[b]), Tl, h, w, int(self.clamp_output), ptr(ws), ws.numel(),
+                             current_stream()))
 
     def launches(self) -> int:
         return int(_lib.lib().ce_vae_last_launch_count(self._handle)) if self._handle else 0
@@ -425,7 +463,8 @@ class AutoencoderKLWan(nn.Module):
                         device=None, **unused) -> "AutoencoderKLWan":
         """`AutoencoderKLWan.from_pretrained(model_id, subfolder="vae", torch_dtype=torch.bfloat16)` (run_inference_diffusers.py:341-345)
         for a LOCAL diffusers checkpoint directory: config.json + diffusion_pytorch_model[.safetensors | sharded index].  Also accepts a
-        directory / file holding the original `Wan2.1_VAE.pth`-style names (the twin's)."""
+        directory / file holding the original `Wan2.1_VAE.pth`-style names (the twin's).  torch_dtype=torch.float32 keeps the
+        checkpoint's fp32 values and builds the fp32 VAE."""
         import json
         import os
 
@@ -449,5 +488,5 @@ class AutoencoderKLWan(nn.Module):
             with safe_open(os.path.join(root, fn), framework="pt", device="cpu") as sf:
                 for k in sf.keys():
                     sd[k] = sf.get_tensor(k)
-        model.load_state_dict({k: v.to(torch.bfloat16) for k, v in sd.items()}, strict=True)
+        model.load_state_dict({k: v.to(model.dtype) for k, v in sd.items()}, strict=True)
         return model

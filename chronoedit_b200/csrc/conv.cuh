@@ -34,4 +34,18 @@ struct ConvArgs {
 
 int launch_conv3d_cl(const ConvArgs& a, cudaStream_t stream);
 
+// The same convolution in fp32 (the fp32 VAE).  The activation arrives as its split pair: x [Tin, Hin, Win, 2, Cin] bf16 holds
+// hi = bf16(v) then lo = bf16(v - hi) of every pixel's channels, and the weight is packed [Cout, taps, Cin_pad / 64, 3, 64] bf16 as
+// W_hi | W_hi | W_lo per 64-channel block, so that the K loop sums A_hi.W_hi + A_lo.W_hi + A_hi.W_lo (fp32_chain.cuh's rule) in
+// fp32.  ConvArgs supplies the geometry, x and w; its bias, y and resid are not read.  The epilogue adds bias (fp32) and resid (fp32,
+// y's layout) and stores y (fp32: channels-last, split_time interleave, or planar with the optional clamp) and / or the split pair
+// of y, [frame, oh, ow, 2, C], for a convolution that reads it next.
+struct ConvF32 {
+  const float* bias = nullptr;
+  const float* resid = nullptr;
+  float* y = nullptr;
+  bf16* y_pair = nullptr;
+};
+int launch_conv3d_cl_f32(const ConvArgs& a, const ConvF32& f, cudaStream_t stream);
+
 }  // namespace ce

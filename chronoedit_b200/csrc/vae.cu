@@ -23,6 +23,7 @@
 
 #include "../../include/chronoedit_b200.h"
 #include "conv.cuh"
+#include "fp32_chain.cuh"
 #include "gemm.cuh"
 #include "seqpar.cuh"
 #include "vae_kernels.cuh"
@@ -32,6 +33,7 @@ using namespace ce;
 struct ce_vae {
   ce_vae_config cfg;
   WeightMap w;
+  WeightMap w32;   // the fp32 VAE's (ce_vae_set_weight_fp32)
   int64_t launches = 0;
   SeqPar sp;   // the split over ranks (ce_vae_sp_configure): world == 1 means off
 };
@@ -655,6 +657,346 @@ int vae_sp_layout(ce_vae* h, int H, int W, int world, VaeSpLayout& L) {
   return CE_OK;
 }
 
+// ---------------------------------------------------------------------------------------------- fp32
+// The same chain in fp32 (AutoencoderKLWan loaded in fp32): fp32 activations, fp32 parameters, the operator order and chunking of
+// run_encode / run_decode on one GPU.  Every convolution is launch_conv3d_cl_f32 reading the split pair of its input (conv.cuh); the
+// row kernels and the convolutions' epilogues write that pair where a convolution reads it next, and the causal history is kept as
+// the pair.  The mid attention is Fp32Chain's (6-term split products, fp32 row softmax).
+
+struct Act32 {   // fp32 [T, H, W, C] and / or its pair [T, H, W, 2, C]
+  float* f = nullptr;
+  bf16* pair = nullptr;
+  int T = 0, H = 0, W = 0, C = 0;
+  size_t pixels() const { return (size_t)T * H * W; }
+};
+
+struct Stream32 {   // input pair of one streaming convolution: `hist` history frames, then the chunk
+  bf16* p = nullptr;
+  int hist = 0, tcap = 0, H = 0, W = 0, C = 0;
+  bool primed = false;
+  size_t frame() const { return (size_t)H * W * 2 * C; }
+};
+
+// Scratch is two arenas used in turn, one per block: a block's temporaries and output go into the arena its input is not in, which
+// it resets first (what that arena held was the input of the block before, consumed by now).  A whole chunk's activations at 720p
+// would not fit beside the fp32 stream buffers.
+struct Run32 {
+  ce_vae* h;
+  cudaStream_t s;
+  bool dry;
+  Bump persist;
+  Bump arena[2];
+  int cur = 0;
+  int64_t arena_max[2] = {0, 0};
+  std::map<std::string, Stream32> streams;
+  WeightLookup weights{h->w32};
+  Launcher run{s, &h->launches};
+  int rc = 0;
+
+  Run32(ce_vae* h_, cudaStream_t s_, uint8_t* persist_base, uint8_t* arena0, uint8_t* arena1)
+      : h(h_), s(s_), dry(persist_base == nullptr), persist(persist_base), arena{Bump(arena0), Bump(arena1)} {}
+
+  template <class T>
+  T* take(size_t n) {
+    T* p = arena[cur].take<T>((int64_t)n);
+    arena_max[cur] = std::max(arena_max[cur], arena[cur].off);
+    return p;
+  }
+  void next_block() {
+    cur ^= 1;
+    arena[cur].off = 0;
+  }
+  void new_chunk() {
+    arena[0].off = arena[1].off = 0;
+    cur = 0;
+  }
+  int64_t arena_bytes(int i) const { return (arena_max[i] + 255) & ~int64_t(255); }
+  Act32 act(int T, int H, int W, int C, bool f, bool pair) {
+    Act32 a;
+    a.T = T; a.H = H; a.W = W; a.C = C;
+    if (f) a.f = take<float>(a.pixels() * C);
+    if (pair) a.pair = take<bf16>(a.pixels() * 2 * C);
+    return a;
+  }
+  int64_t workspace_bytes() const { return persist.bytes() + arena_bytes(0) + arena_bytes(1) + 256; }
+  template <class Launch>
+  void launch(Launch&& l) {
+    if (!dry && !rc) rc = run(l);
+  }
+  void copy(void* dst, const void* src, size_t bytes) {
+    if (!dry && !rc && cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess) rc = fail(CE_ERR_CUDA, "vae fp32: copy");
+  }
+
+  Stream32& stream(const std::string& name, int hist, int tcap, int H, int W, int C) {
+    auto it = streams.find(name);
+    if (it != streams.end()) return it->second;
+    Stream32 b;
+    b.hist = hist; b.tcap = tcap; b.H = H; b.W = W; b.C = C;
+    b.p = persist.take<bf16>((int64_t)(hist + tcap) * b.frame());
+    if (!dry && hist > 0 && cudaMemsetAsync(b.p, 0, hist * b.frame() * 2, s) != cudaSuccess && !rc) rc = fail(CE_ERR_CUDA, "vae fp32: memset");
+    return streams.emplace(name, b).first->second;
+  }
+  bf16* chunk_of(Stream32& b, int T) {
+    if (T > b.tcap && !rc) rc = fail(CE_ERR_INVALID, "vae fp32: chunk larger than the planned stream buffer");
+    return at(b.p, b.hist * b.frame());
+  }
+  void push_history(Stream32& b, int T) {   // history <- last `hist` frames of [history ; chunk]
+    for (int i = 0; i < b.hist; ++i) copy(at(b.p, i * b.frame()), at(b.p, (T + i) * b.frame()), b.frame() * 2);
+  }
+
+  void rms(const Act32& x, const std::string& gamma, float* y, bf16* y_pair, bool silu) {
+    const float* g = weights.any<float>(gamma, x.C);
+    launch([&] { return launch_rms_silu_cl_f32(x.f, g, y, y_pair, x.pixels(), x.C, silu ? 1 : 0, s); });
+  }
+  // convolution of the pair `in` ([Tin] frames, history included) into out's fp32 and / or pair
+  void conv(const std::string& name, const bf16* in, int Tin, int Hin, int Win, int Cin, const Act32& out, int kt, int kh, int kw, int st,
+            int sh, int sw, int ph, int pw, const float* resid = nullptr, int split_time = 0, int t_base = 0) {
+    ConvArgs a;
+    a.Cout = split_time ? out.C * 2 : out.C; a.Cin_pad = round_up(Cin, 64);
+    a.w = weights.any<bf16>(name + ".weight", (int64_t)a.Cout * kt * kh * kw * a.Cin_pad * 3);
+    ConvF32 f;
+    f.bias = weights.any<float>(name + ".bias", a.Cout);
+    f.resid = resid; f.y = out.f; f.y_pair = out.pair;
+    a.x = in; a.Tin = Tin; a.Hin = Hin; a.Win = Win; a.Cin = Cin;
+    a.kt = kt; a.kh = kh; a.kw = kw; a.st = st; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw;
+    a.t_base = t_base;
+    a.Tout = split_time ? out.T / 2 : out.T; a.Hout = out.H; a.Wout = out.W;
+    a.split_time = split_time;
+    launch([&] { return launch_conv3d_cl_f32(a, f, s); });
+  }
+  void causal_conv(const std::string& name, Stream32& b, int T, const Act32& out, int kh, const float* resid = nullptr, int split_time = 0) {
+    conv(name, b.p, b.hist + T, b.H, b.W, b.C, out, 3, kh, kh, 1, 1, 1, kh / 2, kh / 2, resid, split_time);
+    push_history(b, T);
+    b.primed = true;
+  }
+
+  // ResidualBlock.forward (wan2pt1.py:201-220); the output carries its pair for the shortcut or the convolution after it
+  Act32 res_block(const std::string& n, const Act32& x, int Cout, int tcap) {
+    next_block();
+    Stream32& sa = stream(n + ".residual.2", 2, tcap, x.H, x.W, x.C);
+    rms(x, n + ".residual.0.gamma", nullptr, chunk_of(sa, x.T), true);
+    Act32 t1 = act(x.T, x.H, x.W, Cout, true, false);
+    causal_conv(n + ".residual.2", sa, x.T, t1, 3);
+    Stream32& sb = stream(n + ".residual.6", 2, tcap, x.H, x.W, Cout);
+    rms(t1, n + ".residual.3.gamma", nullptr, chunk_of(sb, x.T), true);
+    const float* hres = x.f;
+    if (x.C != Cout) {
+      if (!dry && !x.pair && !rc) rc = fail(CE_ERR_INVALID, "vae fp32: a shortcut input without its pair");
+      Act32 sc = act(x.T, x.H, x.W, Cout, true, false);
+      conv(n + ".shortcut", x.pair, x.T, x.H, x.W, x.C, sc, 1, 1, 1, 1, 1, 1, 0, 0);
+      hres = sc.f;
+    }
+    Act32 out = act(x.T, x.H, x.W, Cout, true, true);
+    causal_conv(n + ".residual.6", sb, x.T, out, 3, hres);
+    return out;
+  }
+
+  // AttentionBlock.forward (wan2pt1.py:240-259): per frame, one head of width C over H*W tokens
+  Act32 attn_block(const std::string& n, const Act32& x) {
+    next_block();
+    const int C = x.C, L = x.H * x.W, L8 = up8(L), Cp = up8(C);
+    Act32 xn = act(x.T, x.H, x.W, C, true, false);
+    rms(x, n + ".norm.gamma", xn.f, nullptr, false);
+    Lin32 qkv_w, proj_w;
+    qkv_w.w = weights.any<float>(n + ".to_qkv.weight", (int64_t)3 * C * C);
+    qkv_w.b = weights.any<float>(n + ".to_qkv.bias", 3 * C);
+    proj_w.w = weights.any<float>(n + ".proj.weight", (int64_t)C * C);
+    proj_w.b = weights.any<float>(n + ".proj.bias", C);
+    Act32 out = act(x.T, x.H, x.W, C, true, false);
+    float* qkv = take<float>((size_t)L * 3 * C);
+    float* o = take<float>((size_t)L * 3 * C);   // attention output in columns [0, C) (Fp32Chain::attention's row stride is qkv's)
+    Fp32Chain X{run, nullptr, nullptr, nullptr, nullptr, 6, nullptr};
+    X.Ap = take<bf16>((size_t)split_elems(L, std::max(Cp, L8), 6));
+    X.Wp = take<bf16>((size_t)std::max({split_elems(3 * C, C, 6), split_elems(L8, C, 6), split_elems(C, L8, 6)}));
+    X.S = take<float>((size_t)L * L8);
+    X.P = take<float>((size_t)L * L8);
+    X.part = take<float>((size_t)L * std::max(3 * C, L8));
+    const float scale = 1.0f / sqrtf((float)C);
+    for (int f = 0; f < x.T && !dry && !rc; ++f) {
+      const size_t off = (size_t)f * L * C;
+      if ((rc = X.linear(xn.f + off, C, L, C, qkv_w, 3 * C, qkv, 3 * C, 0))) break;
+      if ((rc = X.attention(qkv, qkv + C, qkv + 2 * C, o, 1, 1, L, L, 3 * C, C, scale))) break;
+      if ((rc = X.linear(o, 3 * C, L, C, proj_w, C, out.f + off, C, 0))) break;
+      rc = X.resid(out.f + off, x.f + off, L, C, nullptr, 0, L);
+    }
+    return out;
+  }
+
+  // Resample upsample2d / upsample3d (wan2pt1.py:112-143)
+  Act32 upsample(const std::string& n, Act32 x, bool temporal, int tcap_in) {
+    next_block();
+    const int C = x.C;
+    if (temporal) {
+      Stream32& st = stream(n + ".time_conv", 2, tcap_in, x.H, x.W, C);
+      if (!st.primed) {
+        st.primed = true;   // first chunk: "Rep" -- no temporal doubling, history stays zero
+      } else {
+        copy(chunk_of(st, x.T), x.pair, x.pixels() * 2 * C * 2);
+        Act32 y = act(2 * x.T, x.H, x.W, C, true, false);
+        causal_conv(n + ".time_conv", st, x.T, y, 1, nullptr, /*split_time=*/1);
+        x = y;
+      }
+    }
+    bf16* up = take<bf16>(x.pixels() * 4 * 2 * C);
+    launch([&] { return launch_upsample2x_cl_f32(x.f, up, x.T, x.H, x.W, C, s); });
+    Act32 out = act(x.T, 2 * x.H, 2 * x.W, C / 2, true, true);
+    conv(n + ".resample.1", up, x.T, 2 * x.H, 2 * x.W, C, out, 1, 3, 3, 1, 1, 1, 1, 1);
+    return out;
+  }
+
+  // Resample downsample2d / downsample3d (wan2pt1.py:145-159): ZeroPad2d(0,1,0,1) is the TMA's zero fill past the edge
+  Act32 downsample(const std::string& n, const Act32& x, bool temporal, int tcap_out_spatial) {
+    next_block();
+    const int C = x.C, Ho = (x.H + 1 - 3) / 2 + 1, Wo = (x.W + 1 - 3) / 2 + 1;
+    if (!temporal) {
+      Act32 out = act(x.T, Ho, Wo, C, true, true);
+      conv(n + ".resample.1", x.pair, x.T, x.H, x.W, C, out, 1, 3, 3, 1, 2, 2, 0, 0);
+      return out;
+    }
+    Stream32& st = stream(n + ".time_conv", 1, tcap_out_spatial, Ho, Wo, C);
+    Act32 sp;
+    sp.T = x.T; sp.H = Ho; sp.W = Wo; sp.C = C;
+    sp.pair = chunk_of(st, x.T);
+    if (!st.primed) {   // first chunk passes through and becomes the history (:147-150)
+      st.primed = true;
+      sp.f = take<float>(sp.pixels() * C);
+      conv(n + ".resample.1", x.pair, x.T, x.H, x.W, C, sp, 1, 3, 3, 1, 2, 2, 0, 0);
+      push_history(st, x.T);
+      return sp;   // its pair is the chunk, which nothing rewrites before the next chunk
+    }
+    conv(n + ".resample.1", x.pair, x.T, x.H, x.W, C, sp, 1, 3, 3, 1, 2, 2, 0, 0);
+    Act32 out = act((1 + x.T - 3) / 2 + 1, Ho, Wo, C, true, true);
+    conv(n + ".time_conv", st.p, 1 + x.T, Ho, Wo, C, out, 3, 1, 1, 2, 1, 1, 0, 0);
+    push_history(st, x.T);
+    return out;
+  }
+};
+
+// z planar [zc, Tl, h, w] fp32 -> video planar [3, 1+4(Tl-1), 8h, 8w] fp32 (run_decode in fp32)
+int run_decode_fp32(Run32& R, const float* z, float* video, int Tl, int h, int w, int clamp) {
+  const ce_vae_config& c = R.h->cfg;
+  const int top = top_dim(c), zc = c.z_dim, T_px = 1 + 4 * (Tl - 1);
+  bf16* zpair = R.persist.take<bf16>((int64_t)Tl * h * w * 2 * zc);
+  R.launch([&] { return launch_planar_to_pair(z, zc, (size_t)Tl * h * w, zpair, zc, R.s); });
+  std::vector<LayerSpec> layers = decoder_layers(c);
+  int t_out = 0;
+  for (int i = 0; i < Tl && !R.rc; ++i) {
+    R.new_chunk();
+    int cap = 1;
+    Stream32& s1 = R.stream("decoder.conv1", 2, 1, h, w, zc);
+    Act32 x0;
+    x0.T = 1; x0.H = h; x0.W = w; x0.C = zc;
+    x0.pair = R.chunk_of(s1, 1);
+    R.conv("conv2", zpair, Tl, h, w, zc, x0, 1, 1, 1, 1, 1, 1, 0, 0, nullptr, 0, /*t_base=*/i);
+    Act32 x = R.act(1, h, w, top, true, true);
+    R.causal_conv("decoder.conv1", s1, 1, x, 3);
+    x = R.res_block("decoder.middle.0", x, top, cap);
+    x = R.attn_block("decoder.middle.1", x);
+    x = R.res_block("decoder.middle.2", x, top, cap);
+    int idx = 0;
+    for (const LayerSpec& l : layers) {
+      const std::string n = "decoder.upsamples." + std::to_string(idx++);
+      if (l.res) {
+        x = R.res_block(n, x, l.cout, cap);
+      } else {
+        x = R.upsample(n, x, l.mode == 1, cap);
+        if (l.mode == 1) cap *= 2;
+      }
+    }
+    Stream32& sh = R.stream("decoder.head.2", 2, cap, x.H, x.W, x.C);
+    R.rms(x, "decoder.head.0.gamma", nullptr, R.chunk_of(sh, x.T), true);
+    ConvArgs a;
+    a.x = sh.p; a.Tin = sh.hist + x.T; a.Hin = x.H; a.Win = x.W; a.Cin = x.C;
+    a.Cout = 3; a.Cin_pad = round_up(x.C, 64);
+    a.w = R.weights.any<bf16>("decoder.head.2.weight", (int64_t)3 * 27 * a.Cin_pad * 3);
+    ConvF32 f;
+    f.bias = R.weights.any<float>("decoder.head.2.bias", 3);
+    f.y = video;
+    a.kt = 3; a.kh = 3; a.kw = 3; a.ph = 1; a.pw = 1;
+    a.Tout = x.T; a.Hout = x.H; a.Wout = x.W;
+    a.planar_out = 1; a.clamp = clamp; a.planar_T = T_px; a.planar_t0 = t_out;
+    R.launch([&] { return launch_conv3d_cl_f32(a, f, R.s); });
+    R.push_history(sh, x.T);
+    t_out += x.T;
+  }
+  if (!R.rc && t_out != T_px) return fail(CE_ERR_INVALID, "vae decode fp32: produced frame count mismatch");
+  return R.rc;
+}
+
+// video planar [3, T, H, W] fp32 -> moments planar [2 zc, Tl, H/8, W/8] fp32 (run_encode in fp32)
+int run_encode_fp32(Run32& R, const float* video, float* moments, int T, int H, int Wd) {
+  const ce_vae_config& c = R.h->cfg;
+  const int top = top_dim(c), zc = c.z_dim;
+  const int Tl = 1 + (T - 1) / 4, h = H / 8, w = Wd / 8;
+  std::vector<LayerSpec> layers = encoder_layers(c);
+  // the video's pair with the 3 channels padded to 8 (16-byte pixel rows); encoder.conv1 reads its own past frames as the history
+  bf16* vpair = R.persist.take<bf16>((int64_t)T * H * Wd * 2 * 8);
+  R.launch([&] { return launch_planar_to_pair(video, 3, (size_t)T * H * Wd, vpair, 8, R.s); });
+  bf16* enc_out = R.persist.take<bf16>((int64_t)Tl * h * w * 2 * 2 * zc);   // head outputs of every chunk, as the pair
+  int t_lat = 0;
+  for (int f0 = 0; f0 < T && !R.rc;) {
+    const int Tc = f0 == 0 ? 1 : 4;
+    R.new_chunk();
+    int cap = 4;
+    Act32 x = R.act(Tc, H, Wd, c.dim, true, true);
+    R.conv("encoder.conv1", vpair, T, H, Wd, 8, x, 3, 3, 3, 1, 1, 1, 1, 1, nullptr, 0, /*t_base=*/f0 - 2);
+    for (size_t li = 0; li < layers.size(); ++li) {
+      const LayerSpec& l = layers[li];
+      const std::string n = "encoder.downsamples." + std::to_string(li);
+      if (l.res) {
+        x = R.res_block(n, x, l.cout, cap);
+      } else {
+        x = R.downsample(n, x, l.mode == 1, cap);
+        if (l.mode == 1) cap = cap > 1 ? cap / 2 : 1;
+      }
+    }
+    x = R.res_block("encoder.middle.0", x, top, cap);
+    x = R.attn_block("encoder.middle.1", x);
+    x = R.res_block("encoder.middle.2", x, top, cap);
+    Stream32& sh = R.stream("encoder.head.2", 2, cap, x.H, x.W, x.C);
+    R.rms(x, "encoder.head.0.gamma", nullptr, R.chunk_of(sh, x.T), true);
+    if (x.H != h || x.W != w) return fail(CE_ERR_INVALID, "vae encode fp32: spatial size mismatch (H, W must be multiples of 8)");
+    Act32 o;
+    o.T = x.T; o.H = h; o.W = w; o.C = 2 * zc;
+    o.pair = at(enc_out, (size_t)t_lat * h * w * 2 * 2 * zc);
+    R.causal_conv("encoder.head.2", sh, x.T, o, 3);
+    t_lat += x.T;
+    f0 += Tc;
+  }
+  if (!R.rc && t_lat != Tl) return fail(CE_ERR_INVALID, "vae encode fp32: produced frame count mismatch");
+  // conv1 (1x1x1, 2z -> 2z), then planar moments = mean | logvar
+  R.new_chunk();
+  Act32 q = R.act(Tl, h, w, 2 * zc, true, false);
+  R.conv("conv1", enc_out, Tl, h, w, 2 * zc, q, 1, 1, 1, 1, 1, 1, 0, 0);
+  R.launch([&] { return launch_cl_to_planar_f32(q.f, 2 * zc, moments, q.pixels(), 2 * zc, R.s); });
+  return R.rc;
+}
+
+int run_fp32(ce_vae* h, bool decode, const float* in, float* out, int frames, int height, int width, int clamp, void* workspace,
+             int64_t workspace_bytes, int64_t* need_out, void* stream) {
+  CE_TRY(check_geometry(h, frames, height, width, decode));
+  if (h->sp.world > 1)
+    return fail(CE_ERR_INVALID, "vae fp32: the VAE split over GPUs (ce_vae_sp_configure) is built for bf16 only; configure world = 1");
+  CE_REQUIRE(!h->w32.empty(), "vae fp32: the handle has no fp32 weights (register them with ce_vae_set_weight_fp32)");
+  Run32 plan(h, nullptr, nullptr, nullptr, nullptr);
+  int rc = decode ? run_decode_fp32(plan, nullptr, nullptr, frames, height, width, 0) : run_encode_fp32(plan, nullptr, nullptr, frames, height, width);
+  if (rc || (rc = plan.weights.rc)) return rc;
+  const int64_t need = plan.workspace_bytes();
+  if (need_out) {
+    *need_out = need;
+    return CE_OK;
+  }
+  CE_TRY(check_device());
+  CE_REQUIRE(in && out && workspace, "vae fp32: null argument");
+  CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "vae fp32: workspace must be 256-byte aligned");
+  if (need > workspace_bytes)
+    return fail(CE_ERR_WORKSPACE, "vae fp32: workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(workspace_bytes));
+  uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
+  Run32 R(h, reinterpret_cast<cudaStream_t>(stream), base, base + plan.persist.bytes(), base + plan.persist.bytes() + plan.arena_bytes(0));
+  h->launches = 0;
+  return decode ? run_decode_fp32(R, in, out, frames, height, width, clamp) : run_encode_fp32(R, in, out, frames, height, width);
+}
+
 }  // namespace
 
 extern "C" {
@@ -734,6 +1076,26 @@ int ce_vae_decode(ce_vae* h, const void* z, void* video, int latent_frames, int 
   return run(h, true, z, video, latent_frames, latent_height, latent_width, clamp, workspace, workspace_bytes, stream);
 }
 
+int ce_vae_set_weight_fp32(ce_vae* h, const char* name, const void* ptr, int64_t numel) {
+  CE_REQUIRE(h, "ce_vae_set_weight_fp32: null handle");
+  return register_weight(h->w32, "ce_vae_set_weight_fp32", name, ptr, -1, numel);
+}
+
+int64_t ce_vae_workspace_bytes_fp32(ce_vae* h, int decode, int frames, int height, int width) {
+  int64_t need = -1;
+  return run_fp32(h, decode != 0, nullptr, nullptr, frames, height, width, 0, nullptr, 0, &need, nullptr) ? -1 : need;
+}
+
+int ce_vae_encode_fp32(ce_vae* h, const float* video, float* moments, int frames, int height, int width, void* workspace,
+                       int64_t workspace_bytes, void* stream) {
+  return run_fp32(h, false, video, moments, frames, height, width, 0, workspace, workspace_bytes, nullptr, stream);
+}
+
+int ce_vae_decode_fp32(ce_vae* h, const float* z, float* video, int latent_frames, int latent_height, int latent_width, int clamp,
+                       void* workspace, int64_t workspace_bytes, void* stream) {
+  return run_fp32(h, true, z, video, latent_frames, latent_height, latent_width, clamp, workspace, workspace_bytes, nullptr, stream);
+}
+
 int64_t ce_vae_last_launch_count(const ce_vae* h) { return h ? h->launches : 0; }
 
 int64_t ce_vae_sp_region_bytes(ce_vae* h, int height, int width, int world) {
@@ -783,6 +1145,25 @@ int ce_conv3d_cl_ex_bf16(const ce_conv3d_args* args, void* stream) {
   a.resid = reinterpret_cast<const bf16*>(args->resid); a.split_time = args->split_time;
   a.planar_out = args->planar_out; a.clamp = args->clamp; a.planar_T = args->planar_T; a.planar_t0 = args->planar_t0;
   return launch_conv3d_cl(a, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int ce_conv3d_cl_ex_fp32(const ce_conv3d_args* args, void* y_pair, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(args != nullptr, "ce_conv3d_cl_ex_fp32: null args");
+  ConvArgs a;
+  a.x = reinterpret_cast<const bf16*>(args->x); a.Tin = args->Tin; a.Hin = args->Hin; a.Win = args->Win; a.Cin = args->Cin;
+  a.w = reinterpret_cast<const bf16*>(args->w);
+  a.Cout = args->Cout; a.Cin_pad = args->Cin_pad;
+  a.kt = args->kt; a.kh = args->kh; a.kw = args->kw; a.st = args->st; a.sh = args->sh; a.sw = args->sw; a.ph = args->ph; a.pw = args->pw;
+  a.t_base = args->t_base;
+  a.Tout = args->Tout; a.Hout = args->Hout; a.Wout = args->Wout;
+  a.split_time = args->split_time;
+  a.planar_out = args->planar_out; a.clamp = args->clamp; a.planar_T = args->planar_T; a.planar_t0 = args->planar_t0;
+  ConvF32 f;
+  f.bias = reinterpret_cast<const float*>(args->bias); f.resid = reinterpret_cast<const float*>(args->resid);
+  f.y = reinterpret_cast<float*>(args->y); f.y_pair = reinterpret_cast<bf16*>(y_pair);
+  return launch_conv3d_cl_f32(a, f, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int ce_rms_silu_cl_bf16(const void* x, const void* gamma, void* y, int64_t pixels, int C, int apply_silu, void* stream) {

@@ -1,5 +1,6 @@
 // HBM-bound kernels of the Wan VAE path (channels-last bf16): RMS_norm(+SiLU), nearest 2x upsample, im2row for the
-// few small-Cin convolutions, layout conversion.
+// few small-Cin convolutions, layout conversion; and the fp32 VAE's RMS_norm(+SiLU), upsample and layout conversions, which write
+// the split pair its convolutions read.
 #include "vae_kernels.cuh"
 
 namespace ce {
@@ -127,7 +128,89 @@ __global__ void cl_to_planar_kernel(const bf16* __restrict__ cl, int C, bf16* __
   }
 }
 
+// ---- fp32 (the fp32 VAE)
+__device__ __forceinline__ void store_pair(bf16* p, int C, float v) {   // p = &pair[pixel][0][c]
+  const bf16 hi = __float2bfloat16_rn(v);
+  p[0] = hi;
+  p[C] = __float2bfloat16_rn(v - __bfloat162float(hi));
+}
+
+// RMS_norm.forward (wan2pt1.py:74-75) in fp32: F.normalize (x / max(||x||, 1e-12)) * sqrt(C) * gamma, then SiLU.  One warp per pixel.
+__global__ void __launch_bounds__(256)
+rms_silu_cl_f32_kernel(const float* __restrict__ x, const float* __restrict__ gamma, float* __restrict__ y, bf16* __restrict__ y_pair,
+                       size_t pixels, int C, int apply_silu) {
+  const int lane = threadIdx.x & 31;
+  const float sqrt_c = sqrtf((float)C);
+  for (size_t p = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; p < pixels; p += ((size_t)gridDim.x * blockDim.x) >> 5) {
+    const float* xr = x + p * C;
+    float ss = 0.f;
+    for (int c = lane; c < C; c += 32) ss += xr[c] * xr[c];
+    const float n = fmaxf(sqrtf(warp_sum(ss)), 1e-12f);
+    for (int c = lane; c < C; c += 32) {
+      float v = xr[c] / n * sqrt_c * gamma[c];
+      if (apply_silu) v = v / (1.0f + expf(-v));
+      if (y_pair) store_pair(y_pair + p * 2 * C + c, C, v);
+      else y[p * C + c] = v;
+    }
+  }
+}
+
+// out[t, 2h+a, 2w+b, :] = in[t, h, w, :] (nearest-exact), stored as the pair
+__global__ void upsample2x_cl_f32_kernel(const float* __restrict__ in, bf16* __restrict__ out, int T, int H, int W, int C) {
+  const size_t total = (size_t)T * (2 * H) * (2 * W) * C;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    size_t r = i / C;
+    const int ow = (int)(r % (2 * W)); r /= (2 * W);
+    const int oh = (int)(r % (2 * H));
+    const int t = (int)(r / (2 * H));
+    store_pair(out + (i / C) * 2 * C + c, C, in[(((size_t)t * H + (oh >> 1)) * W + (ow >> 1)) * C + c]);
+  }
+}
+
+__global__ void planar_to_pair_kernel(const float* __restrict__ planar, int C, size_t pixels, bf16* __restrict__ pair, int Cp) {
+  const size_t total = pixels * Cp;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % Cp);
+    const size_t p = i / Cp;
+    store_pair(pair + p * 2 * Cp + c, Cp, c < C ? planar[(size_t)c * pixels + p] : 0.f);
+  }
+}
+
+__global__ void cl_to_planar_f32_kernel(const float* __restrict__ cl, int C, float* __restrict__ planar, size_t pixels, int Cout) {
+  const size_t total = pixels * Cout;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x)
+    planar[i] = cl[(i % pixels) * C + i / pixels];
+}
+
 }  // namespace
+
+int launch_rms_silu_cl_f32(const float* x, const float* gamma, float* y, bf16* y_pair, size_t pixels, int C, int apply_silu,
+                           cudaStream_t stream) {
+  CE_REQUIRE(x && gamma && (y == nullptr) != (y_pair == nullptr) && C > 0, "rms_silu fp32: null pointer, or not exactly one output");
+  rms_silu_cl_f32_kernel<<<grid_for(pixels * 32), TPB, 0, stream>>>(x, gamma, y, y_pair, pixels, C, apply_silu);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
+
+int launch_upsample2x_cl_f32(const float* in, bf16* out_pair, int T, int H, int W, int C, cudaStream_t stream) {
+  upsample2x_cl_f32_kernel<<<grid_for((size_t)T * 4 * H * W * C), TPB, 0, stream>>>(in, out_pair, T, H, W, C);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
+
+int launch_planar_to_pair(const float* planar, int C, size_t pixels, bf16* pair, int Cp, cudaStream_t stream) {
+  CE_REQUIRE(Cp >= C, "planar_to_pair: Cp >= C");
+  planar_to_pair_kernel<<<grid_for(pixels * Cp), TPB, 0, stream>>>(planar, C, pixels, pair, Cp);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
+
+int launch_cl_to_planar_f32(const float* cl, int C, float* planar, size_t pixels, int Cout, cudaStream_t stream) {
+  cl_to_planar_f32_kernel<<<grid_for(pixels * Cout), TPB, 0, stream>>>(cl, C, planar, pixels, Cout);
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
 
 int launch_rms_silu_cl(const bf16* x, const bf16* gamma, bf16* y, size_t pixels, int C, int apply_silu, cudaStream_t stream) {
   CE_REQUIRE(C % 8 == 0 && C <= 512, "rms_silu: C % 8, C <= 512");

@@ -385,9 +385,18 @@ def enable_vae_sequence_parallel(vae, height: int, width: int, group=None) -> in
 
     `height` x `width` is the edit's pixel geometry: one configuration serves the encode of any 1 + 4k frames at that size and the
     decode of any latent frame count at height / 8 x width / 8.  Allocates this rank's peer region (ce_ipc_alloc), exchanges the CUDA
-    IPC handles through torch.distributed and configures the handle (ce_vae_sp_configure).  Returns the region size in bytes."""
+    IPC handles through torch.distributed and configures the handle (ce_vae_sp_configure).  Returns the region size in bytes.
+    The split is built for the bf16 VAE only: an fp32 VAE is refused before anything is allocated."""
+    _refuse_fp32_vae(vae)
     return _enable_split(vae, "enable_vae_sequence_parallel", group, disable_vae_sequence_parallel,
                          lambda world: vae_sp_region_bytes(vae, height, width, world), configure_vae_sequence_parallel)
+
+
+def _refuse_fp32_vae(vae) -> None:
+    from ._lib import CEError
+
+    if vae.dtype == torch.float32:
+        raise CEError("the VAE split over GPUs is built for the bf16 VAE only; this VAE was loaded in fp32")
 
 
 def vae_sp_region_bytes(vae, height: int, width: int, world: int) -> int:
@@ -406,6 +415,7 @@ def configure_vae_sequence_parallel(vae, rank: int, region_ptrs: Sequence[int], 
     (ce_vae_sp_configure).  `state` is kept as `vae._sp_state` and holds what disable_vae_sequence_parallel releases: the own region
     under "own" (ce_ipc_free, after a barrier on the process group under "group") and the opened peer mappings under "opened"
     (ce_ipc_close)."""
+    _refuse_fp32_vae(vae)
     _configure_peer_regions(vae, "ce_vae_sp_configure", rank, region_ptrs, region_bytes, state)
 
 

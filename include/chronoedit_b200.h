@@ -294,6 +294,24 @@ int ce_vae_decode(ce_vae* h, const void* z, void* video, int latent_frames, int 
                   void* workspace, int64_t workspace_bytes, void* stream);
 int64_t ce_vae_last_launch_count(const ce_vae* h);
 
+/* The VAE in fp32, as the reference pipeline loads it (AutoencoderKLWan.from_pretrained(..., torch_dtype=torch.float32)): the calls
+ * above with fp32 in and fp32 out, on parameters registered with ce_vae_set_weight_fp32 (a map of their own) under the same names:
+ *   convolution weights [Cout, Cin, kt, kh, kw] fp32 -> [Cout, taps, Cin_pad / 64, 3, 64] bf16 with taps ordered (dt, dh, dw), Cin_pad
+ *     = Cin rounded up to 64 (zero filled) and, per 64-channel block, hi = bf16(w), hi again, lo = bf16(w - hi) -- every convolution,
+ *     the small ones included;
+ *   "*.gamma" [C], biases [Cout], attention "to_qkv.weight" [3C, C] and "proj.weight" [C, C]: fp32 as they are.
+ * Convolutions run on the wgmma implicit GEMM with both operands split into two bf16 terms (A_hi.W_hi + A_lo.W_hi + A_hi.W_lo, fp32
+ * accumulation), the mid attention on 6-term split GEMMs with an fp32 softmax, everything else in fp32 (csrc/vae.cu).
+ * Refused before any launch: a handle split over GPUs (ce_vae_sp_configure with world > 1), a handle without fp32 weights, a missing or
+ * mis-sized weight, and a workspace smaller than ce_vae_workspace_bytes_fp32 or not 256-byte aligned.  ce_vae_workspace_bytes_fp32
+ * returns -1 on any of the refusals it can see (geometry, split, weights). */
+int ce_vae_set_weight_fp32(ce_vae* h, const char* name, const void* ptr, int64_t numel);
+int64_t ce_vae_workspace_bytes_fp32(ce_vae* h, int decode, int frames, int height, int width);
+int ce_vae_encode_fp32(ce_vae* h, const float* video, float* moments, int frames, int height, int width, void* workspace,
+                       int64_t workspace_bytes, void* stream);
+int ce_vae_decode_fp32(ce_vae* h, const float* z, float* video, int latent_frames, int latent_height, int latent_width, int clamp,
+                       void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * The VAE split over the `world` ranks of a node (one process per GPU), for the latency of one edit: rank r encodes and
  * decodes latent rows [r h / world, (r + 1) h / world) (and the matching rows at every resolution), exchanges only the rows
@@ -552,6 +570,10 @@ typedef struct ce_conv3d_args {
   int32_t planar_T, planar_t0;
 } ce_conv3d_args;
 int ce_conv3d_cl_ex_bf16(const ce_conv3d_args* args, void* stream);
+/* The fp32 VAE's convolution with the same arguments, read as: x the split pair [Tin, Hin, Win, 2, Cin] bf16 (hi = bf16(v) then
+ * lo = bf16(v - hi) for each pixel's channels), w packed as for ce_vae_set_weight_fp32, bias [Cout] fp32, resid fp32 in y's layout,
+ * y fp32 (or NULL when only y_pair is wanted; not with planar_out), y_pair optional: the split pair of y [frames, Hout, Wout, 2, C]. */
+int ce_conv3d_cl_ex_fp32(const ce_conv3d_args* args, void* y_pair, void* stream);
 
 /* Multi-head self-attention composed of GEMMs over one sequence of L tokens, as the VAE mid-block (H = 1, dk = D) and both
  * encoders run it; I = H * dk, L8 = L rounded up to 8.
