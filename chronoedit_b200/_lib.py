@@ -82,6 +82,15 @@ class GemmAttentionArgsC(ctypes.Structure):   # ce_gemm_attention_args
     ]
 
 
+class TileBlendArgsC(ctypes.Structure):   # ce_vae_tile_blend_args
+    _fields_ = [
+        ("fp32", c_int32), ("tile", c_void_p), ("C", c_int32), ("T", c_int32), ("th", c_int32), ("tw", c_int32), ("above", c_void_p),
+        ("above_h", c_int32), ("left", c_void_p), ("left_w", c_int32), ("out", c_void_p), ("out_h", c_int32), ("out_w", c_int32),
+        ("oy", c_int32), ("ox", c_int32), ("crop_h", c_int32), ("crop_w", c_int32), ("clamp", c_int32), ("strip", c_void_p),
+        ("strip_h", c_int32), ("tail", c_void_p), ("tail_w", c_int32),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/chronoedit_b200.h declares
 SIGNATURES = {
     "ce_abi_version": (c_int, []),
@@ -153,6 +162,17 @@ SIGNATURES = {
     "ce_vae_workspace_bytes_fp32": (c_int64, [c_void_p, c_int, c_int, c_int, c_int]),
     "ce_vae_encode_fp32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "ce_vae_decode_fp32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
+    "ce_vae_workspace_bytes_tiled": (c_int64, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "ce_vae_encode_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64,
+                                    c_void_p]),
+    "ce_vae_decode_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                    c_int64, c_void_p]),
+    "ce_vae_workspace_bytes_tiled_fp32": (c_int64, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "ce_vae_encode_tiled_fp32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                         c_int64, c_void_p]),
+    "ce_vae_decode_tiled_fp32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                         c_void_p, c_int64, c_void_p]),
+    "ce_vae_tile_blend": (c_int, [POINTER(TileBlendArgsC), c_void_p]),
     "ce_vae_sp_region_bytes": (c_int64, [c_void_p, c_int, c_int, c_int]),
     "ce_vae_sp_configure": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64]),
     "ce_vae_sp_host_barrier": (c_int, [c_void_p, c_int]),

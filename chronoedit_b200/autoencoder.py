@@ -1,6 +1,7 @@
 """H100-native drop-in for diffusers `AutoencoderKLWan` as `ChronoEditPipeline` uses it.
 
-What the unchanged pipeline touches (pipeline_chronoedit.py:119-129, 185-186, 427-445, 672, 765-781):
+What the unchanged pipeline touches (pipeline_chronoedit.py:119-129, 185-186, 427-445, 672, 765-781), plus the memory switches
+scripts call on it (enable_tiling / disable_tiling / enable_slicing / disable_slicing):
     vae.encode(x).latent_dist.mode() / .sample(generator)      x  [B,3,T,H,W] in [-1,1]
     vae.decode(z, return_dict=False)[0]                         z  [B,16,Tl,h,w]
     vae.config.z_dim / .latents_mean / .latents_std, vae.temperal_downsample, vae.dtype
@@ -27,6 +28,10 @@ LATENTS_MEAN = [-0.7571, -0.7089, -0.9113, 0.1075, -0.1745, 0.9653, -0.1517, 1.5
                 0.4134, -0.0715, 0.5517, -0.3632, -0.1922, -0.9497, 0.2503, -0.2921]
 LATENTS_STD = [2.8184, 1.4541, 2.3275, 2.6558, 1.2196, 1.7708, 2.6052, 2.0743,
                3.2687, 2.1526, 2.8652, 1.5579, 1.6382, 1.1253, 2.8251, 1.9160]
+
+# diffusers' tiled_decode returns the blended tiles without the [-1, 1] clamp its untiled decode applies ([diffusers-mem],
+# DESIGN.md "Tiled VAE"); flip this to clamp the tiled output as well
+TILED_DECODE_CLAMPS = False
 
 # convolutions that run as im2row + GEMM (Cin < 64); every other convolution is the implicit-GEMM kernel
 SMALL_CONVS = ("encoder.conv1", "decoder.conv1", "conv1", "conv2")
@@ -213,6 +218,13 @@ class AutoencoderKLWan(nn.Module):
         self._is_packed = False
         self._ws: Optional[torch.Tensor] = None
         self._sp_state: Optional[Dict] = None   # the split over ranks (parallel.enable_vae_sequence_parallel)
+        # diffusers' memory switches (enable_tiling / enable_slicing), with its defaults; sizes in pixels
+        self.use_slicing = False
+        self.use_tiling = False
+        self.tile_sample_min_height = 256
+        self.tile_sample_min_width = 256
+        self.tile_sample_stride_height = 192
+        self.tile_sample_stride_width = 192
 
     def _register(self, dotted: str, p: nn.Parameter) -> None:
         mod = self
@@ -275,6 +287,38 @@ class AutoencoderKLWan(nn.Module):
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         return self._ws
 
+    # ------------------------------------------------------------------------------------------ memory switches
+    def enable_tiling(self, tile_sample_min_height: Optional[int] = None, tile_sample_min_width: Optional[int] = None,
+                      tile_sample_stride_height: Optional[int] = None, tile_sample_stride_width: Optional[int] = None) -> None:
+        """Encode and decode frames larger than one tile tile by tile (diffusers' `enable_tiling`): the VAE's memory is then bounded by
+        the tile size, whatever the frame size.  Sizes not given keep their current values.  Sizes and strides must be multiples of 8
+        pixels with stride <= size (the C library refuses anything else at the first tiled call)."""
+        self.use_tiling = True
+        self.tile_sample_min_height = tile_sample_min_height or self.tile_sample_min_height
+        self.tile_sample_min_width = tile_sample_min_width or self.tile_sample_min_width
+        self.tile_sample_stride_height = tile_sample_stride_height or self.tile_sample_stride_height
+        self.tile_sample_stride_width = tile_sample_stride_width or self.tile_sample_stride_width
+
+    def disable_tiling(self) -> None:
+        self.use_tiling = False
+
+    def enable_slicing(self) -> None:
+        """diffusers' `enable_slicing`: encode and decode a batch one sample at a time.  The samples of a batch already run one after
+        another here, so this only records the switch."""
+        self.use_slicing = True
+
+    def disable_slicing(self) -> None:
+        self.use_slicing = False
+
+    def _tiles(self) -> Tuple[int, int, int, int]:
+        return (self.tile_sample_min_height, self.tile_sample_min_width, self.tile_sample_stride_height, self.tile_sample_stride_width)
+
+    def _tiled_encode(self, H: int, W: int) -> bool:   # diffusers' AutoencoderKLWan._encode
+        return self.use_tiling and (W > self.tile_sample_min_width or H > self.tile_sample_min_height)
+
+    def _tiled_decode(self, h: int, w: int) -> bool:   # diffusers' AutoencoderKLWan._decode, in latents
+        return self.use_tiling and (w > self.tile_sample_min_width // 8 or h > self.tile_sample_min_height // 8)
+
     # ------------------------------------------------------------------------------------------ encode / decode
     # An fp32 VAE computes in fp32 and returns fp32.  It widens a bf16 x or z to fp32 (exact), so the unchanged pipeline's
     # prepare_latents, which casts the conditioning video to the transformer's bf16 before vae.encode, runs; diffusers' fp32 Conv3d
@@ -286,16 +330,22 @@ class AutoencoderKLWan(nn.Module):
     @torch.no_grad()
     def encode(self, x: torch.Tensor, return_dict: bool = True):
         """x [B,3,T,H,W] in [-1,1], T = 1+4k, H and W multiples of 8 -> posterior (mean|logvar [B,2z,1+k,H/8,W/8]), in the VAE's
-        dtype."""
+        dtype.  With tiling on and a frame larger than one tile, tiled as diffusers' tiled_encode."""
         if x.dim() != 5 or x.shape[1] != 3:
             raise CEError("encode expects [B, 3, T, H, W]")
         B, _, T, H, W = x.shape
         if T < 1 or (T - 1) % 4 != 0 or H % 8 != 0 or W % 8 != 0:
             raise CEError("encode expects T = 1 + 4k frames and H, W multiples of 8")
         self._check_fp32_single_gpu()
+        tiled = self._tiled_encode(H, W)
+        if tiled:
+            self._check_tiling_single_gpu()
         x = x.to(device=self.device, dtype=self.dtype).contiguous()
         out = torch.empty(B, 2 * self.z_dim, 1 + (T - 1) // 4, H // 8, W // 8, dtype=self.dtype, device=self.device)
-        self._native_encode(x, out)
+        if tiled:
+            self._native_tiled(x, out, decode=False)
+        else:
+            self._native_encode(x, out)
         post = DiagonalGaussianDistribution(out)
         if not return_dict:
             return (post,)
@@ -303,14 +353,21 @@ class AutoencoderKLWan(nn.Module):
 
     @torch.no_grad()
     def decode(self, z: torch.Tensor, return_dict: bool = True):
-        """z [B,z_dim,Tl,h,w] -> video [B,3,1+4(Tl-1),8h,8w] (clamped to [-1,1] like diffusers), in the VAE's dtype."""
+        """z [B,z_dim,Tl,h,w] -> video [B,3,1+4(Tl-1),8h,8w] (clamped to [-1,1] like diffusers), in the VAE's dtype.  With tiling
+        on and a latent frame larger than one tile, tiled as diffusers' tiled_decode (not clamped)."""
         if z.dim() != 5 or z.shape[1] != self.z_dim:
             raise CEError(f"decode expects [B, {self.z_dim}, T, h, w]")
         B, _, Tl, h, w = z.shape
         self._check_fp32_single_gpu()
+        tiled = self._tiled_decode(h, w)
+        if tiled:
+            self._check_tiling_single_gpu()
         z = z.to(device=self.device, dtype=self.dtype).contiguous()
         out = torch.empty(B, 3, 1 + 4 * (Tl - 1), 8 * h, 8 * w, dtype=self.dtype, device=self.device)
-        self._native_decode(z, out)
+        if tiled:
+            self._native_tiled(z, out, decode=True)
+        else:
+            self._native_decode(z, out)
         if not return_dict:
             return (out,)
         return DecoderOutput(sample=out)
@@ -347,6 +404,32 @@ class AutoencoderKLWan(nn.Module):
             for b in range(B):
                 check(decode(self._handle, ptr(z[b]), ptr(out[b]), Tl, h, w, int(self.clamp_output), ptr(ws), ws.numel(),
                              current_stream()))
+
+    def _check_tiling_single_gpu(self) -> None:
+        if self._sp_state:
+            raise CEError("tiling is not built for the VAE split over GPUs (parallel.enable_vae_sequence_parallel); disable one of them")
+
+    def _native_tiled(self, x: torch.Tensor, out: torch.Tensor, decode: bool) -> None:
+        """Tiled encode (x = video) or decode (x = z), one sample at a time.  The tiled decode does not clamp (TILED_DECODE_CLAMPS)."""
+        if not self._is_packed:
+            self.pack_weights()
+        L = _lib.lib()
+        fp32 = self.dtype == torch.float32
+        B, _, T, H, W = x.shape
+        tiles = self._tiles()
+        n = (L.ce_vae_workspace_bytes_tiled_fp32 if fp32 else L.ce_vae_workspace_bytes_tiled)(self._handle, int(decode), T, H, W, *tiles)
+        if n < 0:
+            check(-1)
+        ws = self._workspace(n)
+        with torch.cuda.device(self.device):
+            for b in range(B):
+                if decode:
+                    fn = L.ce_vae_decode_tiled_fp32 if fp32 else L.ce_vae_decode_tiled
+                    check(fn(self._handle, ptr(x[b]), ptr(out[b]), T, H, W, *tiles, int(TILED_DECODE_CLAMPS and self.clamp_output),
+                             ptr(ws), ws.numel(), current_stream()))
+                else:
+                    fn = L.ce_vae_encode_tiled_fp32 if fp32 else L.ce_vae_encode_tiled
+                    check(fn(self._handle, ptr(x[b]), ptr(out[b]), T, H, W, *tiles, ptr(ws), ws.numel(), current_stream()))
 
     def launches(self) -> int:
         return int(_lib.lib().ce_vae_last_launch_count(self._handle)) if self._handle else 0

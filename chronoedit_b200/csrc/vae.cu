@@ -14,6 +14,9 @@
 // moves them into the halo rows (zero past the global top and bottom: the convolution's own zero padding).  The mid attention
 // gathers its normalised frame into every rank's region and computes the rank's query rows only; the outputs are gathered the same
 // way.  Every output element sums the same terms in the same order as on one GPU, so each rank returns the single-GPU bits.
+//
+// Tiled (ce_vae_encode_tiled / ce_vae_decode_tiled, diffusers' enable_tiling): run_tiled walks a grid of overlapping tiles, runs the
+// untiled chain on each and blends it with its neighbours (tile_blend_kernel, vae_kernels.cu); see the section above run_tiled.
 #include <math.h>
 
 #include <algorithm>
@@ -997,6 +1000,176 @@ int run_fp32(ce_vae* h, bool decode, const float* in, float* out, int frames, in
   return decode ? run_decode_fp32(R, in, out, frames, height, width, clamp) : run_encode_fp32(R, in, out, frames, height, width);
 }
 
+// ---------------------------------------------------------------------------------------------- tiled encode / decode
+// diffusers AutoencoderKLWan.tiled_encode / tiled_decode: the frame is cut into overlapping tiles, each tile is a fresh untiled
+// encode or decode (its own causal cache), and each result is blended with its blended upper and left neighbours (blend_v, then
+// blend_h) and cropped to the stride.  Tiles are walked row-major in C; a tile is blended right after it is computed, which gives
+// the same values as diffusers' blend-after-everything because a tile only reads neighbours that come before it.  What a later tile
+// reads of a blended tile is kept, nothing else: the last blend_v rows of every tile of the previous and the current grid row (the
+// strips) and the last blend_h columns of the previous and the current tile (the tails).
+
+struct TileSpec {   // pixels, multiples of 8
+  int min_h, min_w, stride_h, stride_w;
+};
+
+// One untiled encode or decode of a tile in `ws`, or with ws == null only its workspace need.  The caller resets the launch count.
+int run_tile(ce_vae* h, bool decode, bool fp32, const void* in, void* out, int frames, int H, int W, uint8_t* ws, int64_t* need,
+             cudaStream_t s) {
+  if (fp32) {
+    Run32 plan(h, nullptr, nullptr, nullptr, nullptr);
+    int rc = decode ? run_decode_fp32(plan, nullptr, nullptr, frames, H, W, 0) : run_encode_fp32(plan, nullptr, nullptr, frames, H, W);
+    if (rc || (rc = plan.weights.rc)) return rc;
+    if (need) *need = plan.workspace_bytes();
+    if (!ws) return CE_OK;
+    Run32 R(h, s, ws, ws + plan.persist.bytes(), ws + plan.persist.bytes() + plan.arena_bytes(0));
+    return decode ? run_decode_fp32(R, static_cast<const float*>(in), static_cast<float*>(out), frames, H, W, 0)
+                  : run_encode_fp32(R, static_cast<const float*>(in), static_cast<float*>(out), frames, H, W);
+  }
+  Run plan(h, nullptr, nullptr, nullptr);
+  int rc = decode ? run_decode(plan, nullptr, nullptr, frames, H, W, 0) : run_encode(plan, nullptr, nullptr, frames, H, W);
+  if (rc || (rc = plan.weights.rc)) return rc;
+  if (need) *need = plan.workspace_bytes();
+  if (!ws) return CE_OK;
+  Run R(h, s, ws, ws + plan.persist.bytes());
+  return decode ? run_decode(R, static_cast<const bf16*>(in), static_cast<bf16*>(out), frames, H, W, 0)
+                : run_encode(R, static_cast<const bf16*>(in), static_cast<bf16*>(out), frames, H, W);
+}
+
+// The grid in latent units: tile (i, j) covers latent rows [i sh, i sh + min(mh, h - i sh)) and the matching columns.  A decode tile's
+// input is those latents and its output 8x them in pixels; an encode tile's input is the pixels and its output the latents.
+struct TileGrid {
+  bool decode, fp32;
+  int es;                        // element bytes
+  int Cin, Tin, Cout, Tout;      // input [Cin, Tin, ...], output [Cout, Tout, ...]
+  int h, w;                      // latent geometry
+  int mh, mw, sh, sw;            // tile size and stride, latents
+  int rows, cols;
+  int in_f, out_f;               // input / output units per latent: (1, 8) decode, (8, 1) encode
+  int bv, bw;                    // blend extents, output units
+  int lat_h(int i) const { return std::min(mh, h - i * sh); }
+  int lat_w(int j) const { return std::min(mw, w - j * sw); }
+};
+
+struct TileLayout {
+  int64_t run_bytes = 0;
+  uint8_t *run = nullptr, *stage = nullptr, *tile = nullptr, *strip[2] = {nullptr, nullptr}, *tail[2] = {nullptr, nullptr};
+  int64_t strip_slot = 0;        // bytes of one tile's strip
+  int64_t bytes = 0;
+};
+
+int tile_grid(const ce_vae* h, bool decode, bool fp32, int frames, int height, int width, const TileSpec& ts, TileGrid& g) {
+  CE_TRY(check_geometry(h, frames, height, width, decode));
+  if (h->sp.world > 1)
+    return fail(CE_ERR_INVALID, "vae tiled: tiling is not built for the VAE split over GPUs (ce_vae_sp_configure); configure world = 1");
+  CE_REQUIRE(ts.min_h >= 8 && ts.min_w >= 8 && ts.stride_h >= 8 && ts.stride_w >= 8 && ts.min_h % 8 == 0 && ts.min_w % 8 == 0 &&
+                 ts.stride_h % 8 == 0 && ts.stride_w % 8 == 0,
+             "vae tiled: tile sizes and strides must be positive multiples of 8 pixels");
+  CE_REQUIRE(ts.stride_h <= ts.min_h && ts.stride_w <= ts.min_w, "vae tiled: a stride larger than the tile leaves pixels no tile covers");
+  CE_REQUIRE(!fp32 || !h->w32.empty(), "vae tiled fp32: the handle has no fp32 weights (register them with ce_vae_set_weight_fp32)");
+  g.decode = decode;
+  g.fp32 = fp32;
+  g.es = fp32 ? 4 : 2;
+  const int zc = h->cfg.z_dim;
+  g.h = decode ? height : height / 8;
+  g.w = decode ? width : width / 8;
+  g.mh = ts.min_h / 8; g.mw = ts.min_w / 8; g.sh = ts.stride_h / 8; g.sw = ts.stride_w / 8;
+  g.rows = (g.h + g.sh - 1) / g.sh;
+  g.cols = (g.w + g.sw - 1) / g.sw;
+  g.in_f = decode ? 1 : 8;
+  g.out_f = decode ? 8 : 1;
+  g.Cin = decode ? zc : 3;
+  g.Tin = frames;
+  g.Cout = decode ? 3 : 2 * zc;
+  g.Tout = decode ? 1 + 4 * (frames - 1) : 1 + (frames - 1) / 4;
+  g.bv = (g.mh - g.sh) * g.out_f;
+  g.bw = (g.mw - g.sw) * g.out_f;
+  return CE_OK;
+}
+
+// Workspace: one tile's untiled run (the largest of the at most four tile shapes) | the staged input tile | the tile's output |
+// two rows of strips | two tails.  Only the strips grow with the frame, by one tile's strip per tile column.
+int tile_layout(ce_vae* h, const TileGrid& g, uint8_t* base, TileLayout& L) {
+  L = TileLayout();
+  for (int i : {0, g.rows - 1})
+    for (int j : {0, g.cols - 1}) {
+      int64_t need = 0;
+      const int th = g.lat_h(i) * g.in_f, tw = g.lat_w(j) * g.in_f;
+      CE_TRY(run_tile(h, g.decode, g.fp32, nullptr, nullptr, g.Tin, th, tw, nullptr, &need, nullptr));
+      L.run_bytes = std::max(L.run_bytes, need);
+    }
+  const int64_t mh = std::min(g.mh, g.h), mw = std::min(g.mw, g.w);
+  Bump b(base);
+  L.run = b.take<uint8_t>(L.run_bytes);
+  L.stage = b.take<uint8_t>((int64_t)g.Cin * g.Tin * mh * g.in_f * mw * g.in_f * g.es);
+  L.tile = b.take<uint8_t>((int64_t)g.Cout * g.Tout * mh * g.out_f * mw * g.out_f * g.es);
+  L.strip_slot = ((int64_t)g.Cout * g.Tout * std::min<int64_t>(g.bv, mh * g.out_f) * mw * g.out_f * g.es + 255) & ~int64_t(255);
+  for (int k = 0; k < 2; ++k) L.strip[k] = b.take<uint8_t>(g.rows > 1 && g.bv > 0 ? g.cols * L.strip_slot : 0);
+  for (int k = 0; k < 2; ++k)
+    L.tail[k] = b.take<uint8_t>(g.cols > 1 ? (int64_t)g.Cout * g.Tout * mh * g.out_f * std::min<int64_t>(g.bw, mw * g.out_f) * g.es : 0);
+  L.bytes = b.bytes() + 256;
+  return CE_OK;
+}
+
+int run_tiled(ce_vae* h, bool decode, bool fp32, const void* in, void* out, int frames, int height, int width, const TileSpec& ts,
+              int clamp, void* workspace, int64_t workspace_bytes, int64_t* need_out, void* stream) {
+  TileGrid g;
+  CE_TRY(tile_grid(h, decode, fp32, frames, height, width, ts, g));
+  TileLayout L;
+  CE_TRY(tile_layout(h, g, nullptr, L));
+  if (need_out) {
+    *need_out = L.bytes;
+    return CE_OK;
+  }
+  CE_TRY(check_device());
+  CE_REQUIRE(in && out && workspace, "vae tiled: null argument");
+  CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "vae tiled: workspace must be 256-byte aligned");
+  if (L.bytes > workspace_bytes)
+    return fail(CE_ERR_WORKSPACE, "vae tiled: workspace too small: need " + std::to_string(L.bytes) + " bytes, got " + std::to_string(workspace_bytes));
+  CE_TRY(tile_layout(h, g, reinterpret_cast<uint8_t*>(workspace), L));
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  Launcher launch{s, &h->launches};
+  h->launches = 0;
+  const int IH = g.h * g.in_f, IW = g.w * g.in_f;
+  for (int i = 0; i < g.rows; ++i)
+    for (int j = 0; j < g.cols; ++j) {
+      const int lh = g.lat_h(i), lw = g.lat_w(j);
+      const int ih = lh * g.in_f, iw = lw * g.in_f;
+      // the tile's input, contiguous: [Cin, Tin, ih, iw] out of [Cin, Tin, IH, IW]
+      cudaMemcpy3DParms p = {};
+      p.srcPtr = make_cudaPitchedPtr(const_cast<void*>(in), (size_t)IW * g.es, (size_t)IW, (size_t)IH);
+      p.srcPos = make_cudaPos((size_t)j * g.sw * g.in_f * g.es, (size_t)i * g.sh * g.in_f, 0);
+      p.dstPtr = make_cudaPitchedPtr(L.stage, (size_t)iw * g.es, (size_t)iw, (size_t)ih);
+      p.extent = make_cudaExtent((size_t)iw * g.es, (size_t)ih, (size_t)g.Cin * g.Tin);
+      p.kind = cudaMemcpyDeviceToDevice;
+      CE_CHECK_CUDA(cudaMemcpy3DAsync(&p, s));
+      CE_TRY(run_tile(h, decode, fp32, L.stage, L.tile, g.Tin, ih, iw, L.run, nullptr, s));
+      TileBlend b;
+      b.fp32 = fp32;
+      b.tile = L.tile; b.C = g.Cout; b.T = g.Tout; b.th = lh * g.out_f; b.tw = lw * g.out_f;
+      if (i > 0 && g.bv > 0) {
+        b.above = L.strip[(i - 1) & 1] + j * L.strip_slot;
+        b.above_h = std::min(g.bv, g.lat_h(i - 1) * g.out_f);
+      }
+      if (j > 0 && g.bw > 0) {
+        b.left = L.tail[(j - 1) & 1];
+        b.left_w = std::min(g.bw, g.lat_w(j - 1) * g.out_f);
+      }
+      b.out = out; b.out_h = g.h * g.out_f; b.out_w = g.w * g.out_f;
+      b.oy = i * g.sh * g.out_f; b.ox = j * g.sw * g.out_f; b.crop_h = g.sh * g.out_f; b.crop_w = g.sw * g.out_f;
+      b.clamp = clamp;
+      if (i + 1 < g.rows && g.bv > 0) {
+        b.strip = L.strip[i & 1] + j * L.strip_slot;
+        b.strip_h = std::min(g.bv, b.th);
+      }
+      if (j + 1 < g.cols && g.bw > 0) {
+        b.tail = L.tail[j & 1];
+        b.tail_w = std::min(g.bw, b.tw);
+      }
+      CE_TRY(launch([&] { return launch_tile_blend(b, s); }));
+    }
+  return CE_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1097,6 +1270,68 @@ int ce_vae_decode_fp32(ce_vae* h, const float* z, float* video, int latent_frame
 }
 
 int64_t ce_vae_last_launch_count(const ce_vae* h) { return h ? h->launches : 0; }
+
+static int64_t tiled_bytes(ce_vae* h, bool fp32, int decode, int frames, int height, int width, int mh, int mw, int sh, int sw) {
+  int64_t need = -1;
+  return run_tiled(h, decode != 0, fp32, nullptr, nullptr, frames, height, width, TileSpec{mh, mw, sh, sw}, 0, nullptr, 0, &need, nullptr)
+             ? -1
+             : need;
+}
+
+int64_t ce_vae_workspace_bytes_tiled(ce_vae* h, int decode, int frames, int height, int width, int tile_min_height, int tile_min_width,
+                                     int tile_stride_height, int tile_stride_width) {
+  return tiled_bytes(h, false, decode, frames, height, width, tile_min_height, tile_min_width, tile_stride_height, tile_stride_width);
+}
+
+int64_t ce_vae_workspace_bytes_tiled_fp32(ce_vae* h, int decode, int frames, int height, int width, int tile_min_height, int tile_min_width,
+                                          int tile_stride_height, int tile_stride_width) {
+  return tiled_bytes(h, true, decode, frames, height, width, tile_min_height, tile_min_width, tile_stride_height, tile_stride_width);
+}
+
+int ce_vae_encode_tiled(ce_vae* h, const void* video, void* moments, int frames, int height, int width, int tile_min_height, int tile_min_width,
+                        int tile_stride_height, int tile_stride_width, void* workspace, int64_t workspace_bytes, void* stream) {
+  return run_tiled(h, false, false, video, moments, frames, height, width,
+                   TileSpec{tile_min_height, tile_min_width, tile_stride_height, tile_stride_width}, 0, workspace, workspace_bytes, nullptr, stream);
+}
+
+int ce_vae_decode_tiled(ce_vae* h, const void* z, void* video, int latent_frames, int latent_height, int latent_width, int tile_min_height,
+                        int tile_min_width, int tile_stride_height, int tile_stride_width, int clamp, void* workspace, int64_t workspace_bytes,
+                        void* stream) {
+  return run_tiled(h, true, false, z, video, latent_frames, latent_height, latent_width,
+                   TileSpec{tile_min_height, tile_min_width, tile_stride_height, tile_stride_width}, clamp, workspace, workspace_bytes, nullptr,
+                   stream);
+}
+
+int ce_vae_encode_tiled_fp32(ce_vae* h, const float* video, float* moments, int frames, int height, int width, int tile_min_height,
+                             int tile_min_width, int tile_stride_height, int tile_stride_width, void* workspace, int64_t workspace_bytes,
+                             void* stream) {
+  return run_tiled(h, false, true, video, moments, frames, height, width,
+                   TileSpec{tile_min_height, tile_min_width, tile_stride_height, tile_stride_width}, 0, workspace, workspace_bytes, nullptr, stream);
+}
+
+int ce_vae_decode_tiled_fp32(ce_vae* h, const float* z, float* video, int latent_frames, int latent_height, int latent_width, int tile_min_height,
+                             int tile_min_width, int tile_stride_height, int tile_stride_width, int clamp, void* workspace,
+                             int64_t workspace_bytes, void* stream) {
+  return run_tiled(h, true, true, z, video, latent_frames, latent_height, latent_width,
+                   TileSpec{tile_min_height, tile_min_width, tile_stride_height, tile_stride_width}, clamp, workspace, workspace_bytes, nullptr,
+                   stream);
+}
+
+int ce_vae_tile_blend(const ce_vae_tile_blend_args* args, void* stream) {
+  int rc = check_device();
+  if (rc) return rc;
+  CE_REQUIRE(args != nullptr, "ce_vae_tile_blend: null args");
+  TileBlend b;
+  b.fp32 = args->fp32;
+  b.tile = args->tile; b.C = args->C; b.T = args->T; b.th = args->th; b.tw = args->tw;
+  b.above = args->above; b.above_h = args->above_h;
+  b.left = args->left; b.left_w = args->left_w;
+  b.out = args->out; b.out_h = args->out_h; b.out_w = args->out_w; b.oy = args->oy; b.ox = args->ox;
+  b.crop_h = args->crop_h; b.crop_w = args->crop_w; b.clamp = args->clamp;
+  b.strip = args->strip; b.strip_h = args->strip_h;
+  b.tail = args->tail; b.tail_w = args->tail_w;
+  return launch_tile_blend(b, reinterpret_cast<cudaStream_t>(stream));
+}
 
 int64_t ce_vae_sp_region_bytes(ce_vae* h, int height, int width, int world) {
   CE_REQUIRE(h, "ce_vae_sp_region_bytes: null handle");

@@ -1,7 +1,9 @@
 // HBM-bound kernels of the Wan VAE path (channels-last bf16): RMS_norm(+SiLU), nearest 2x upsample, im2row for the
-// few small-Cin convolutions, layout conversion; and the fp32 VAE's RMS_norm(+SiLU), upsample and layout conversions, which write
-// the split pair its convolutions read.
+// few small-Cin convolutions, layout conversion; the fp32 VAE's RMS_norm(+SiLU), upsample and layout conversions, which write
+// the split pair its convolutions read; and the tiled VAE's blend of one tile with its neighbours (bf16 and fp32).
 #include "vae_kernels.cuh"
+
+#include <algorithm>
 
 namespace ce {
 
@@ -183,7 +185,127 @@ __global__ void cl_to_planar_f32_kernel(const float* __restrict__ cl, int C, flo
     planar[i] = cl[(i % pixels) * C + i / pixels];
 }
 
+// ---- tiled encode / decode: the blend of one tile with its blended neighbours, and its crop
+template <class E, int V>
+struct alignas(sizeof(E) * V) Vec {
+  E v[V];
+};
+__device__ __forceinline__ float to_f(bf16 x) { return __bfloat162float(x); }
+__device__ __forceinline__ float to_f(float x) { return x; }
+template <class E>
+__device__ __forceinline__ E from_f(float x);
+template <>
+__device__ __forceinline__ bf16 from_f<bf16>(float x) { return __float2bfloat16_rn(x); }
+template <>
+__device__ __forceinline__ float from_f<float>(float x) { return x; }
+
+// diffusers' blend step  b[k] = a[-e + k] * (1 - k / e) + b[k] * (k / e)  as torch evaluates it on a tensor of type E: the weights are
+// Python floats (double) converted to fp32, each product is rounded to E, then the sum is (no fused multiply-add anywhere).
+template <class E>
+__device__ __forceinline__ float blend_step(float a, float b, int k, int e) {
+  const double r = (double)k / (double)e;
+  const float wa = (float)(1.0 - r), wb = (float)r;
+  const float pa = to_f(from_f<E>(__fmul_rn(a, wa))), pb = to_f(from_f<E>(__fmul_rn(b, wb)));
+  return to_f(from_f<E>(__fadd_rn(pa, pb)));
+}
+
+// One thread per V consecutive columns of a tile row: the tile's value, blended vertically with the stored rows of the tile above and
+// then horizontally with the stored columns of the tile to its left, stored to the output crop, the strip and the tail (TileBlend).
+template <class E, int V>
+__global__ void __launch_bounds__(256) tile_blend_kernel(TileBlend b) {
+  using Vt = Vec<E, V>;
+  const int nv = b.tw / V;
+  const int ev = b.above ? min(b.above_h, b.th) : 0, eh = b.left ? min(b.left_w, b.tw) : 0;
+  const size_t total = (size_t)b.C * b.T * b.th * nv;
+  const E* tile = static_cast<const E*>(b.tile);
+  const E* above = static_cast<const E*>(b.above);
+  const E* left = static_cast<const E*>(b.left);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int x0 = (int)(i % nv) * V;
+    const size_t r = i / nv;
+    const int y = (int)(r % b.th);
+    const size_t plane = r / b.th;
+    Vt t = *reinterpret_cast<const Vt*>(tile + r * b.tw + x0);
+    float v[V];
+#pragma unroll
+    for (int k = 0; k < V; ++k) v[k] = to_f(t.v[k]);
+    if (y < ev) {
+      const Vt a = *reinterpret_cast<const Vt*>(above + (plane * b.above_h + b.above_h - ev + y) * b.tw + x0);
+#pragma unroll
+      for (int k = 0; k < V; ++k) v[k] = blend_step<E>(to_f(a.v[k]), v[k], y, ev);
+    }
+    if (x0 < eh) {   // V divides eh: the whole vector is inside the extent
+      const Vt a = *reinterpret_cast<const Vt*>(left + r * b.left_w + b.left_w - eh + x0);
+#pragma unroll
+      for (int k = 0; k < V; ++k) v[k] = blend_step<E>(to_f(a.v[k]), v[k], x0 + k, eh);
+    }
+#pragma unroll
+    for (int k = 0; k < V; ++k) t.v[k] = from_f<E>(v[k]);
+    if (b.strip && y >= b.th - b.strip_h)
+      *reinterpret_cast<Vt*>(static_cast<E*>(b.strip) + (plane * b.strip_h + y - (b.th - b.strip_h)) * b.tw + x0) = t;
+    if (b.tail && x0 >= b.tw - b.tail_w)
+      *reinterpret_cast<Vt*>(static_cast<E*>(b.tail) + r * b.tail_w + x0 - (b.tw - b.tail_w)) = t;
+    const int oy = b.oy + y, ox = b.ox + x0;
+    if (y < b.crop_h && x0 < b.crop_w && oy < b.out_h && ox < b.out_w) {
+      if (b.clamp) {
+#pragma unroll
+        for (int k = 0; k < V; ++k) t.v[k] = from_f<E>(fminf(fmaxf(v[k], -1.0f), 1.0f));
+      }
+      *reinterpret_cast<Vt*>(static_cast<E*>(b.out) + (plane * b.out_h + oy) * b.out_w + ox) = t;
+    }
+  }
+}
+
+int gcd_int(int a, int b) {
+  while (b) {
+    const int t = a % b;
+    a = b;
+    b = t;
+  }
+  return a;
+}
+
 }  // namespace
+
+int tile_blend_vector(const TileBlend& b) {
+  int g = b.tw;
+  const int eh = b.left ? std::min(b.left_w, b.tw) : 0;
+  for (int v : {b.left ? b.left_w : 0, eh, b.out_w, b.ox, b.crop_w < b.tw ? b.crop_w : 0, b.tail ? b.tail_w : 0}) g = gcd_int(g, v);
+  for (const void* p : {b.tile, b.above, b.left, (const void*)b.out, (const void*)b.strip, (const void*)b.tail}) {
+    const int misaligned = (int)(reinterpret_cast<uintptr_t>(p) & 15) / (b.fp32 ? 4 : 2);   // elements past a 16-byte boundary
+    if (misaligned) g = gcd_int(g, misaligned);
+  }
+  const int vmax = b.fp32 ? 4 : 8;
+  int v = 1;
+  while (v < vmax && g % (2 * v) == 0) v *= 2;
+  return v;
+}
+
+int launch_tile_blend(const TileBlend& b, cudaStream_t stream) {
+  CE_REQUIRE(b.tile && b.out && b.C > 0 && b.T > 0 && b.th > 0 && b.tw > 0 && b.out_h > 0 && b.out_w > 0 && b.oy >= 0 && b.ox >= 0,
+             "tile blend: null tile / output or empty extents");
+  CE_REQUIRE(!b.above || b.above_h > 0, "tile blend: above rows");
+  CE_REQUIRE(!b.left || b.left_w > 0, "tile blend: left columns");
+  CE_REQUIRE(!b.strip || (b.strip_h > 0 && b.strip_h <= b.th), "tile blend: strip rows must be 1 .. th");
+  CE_REQUIRE(!b.tail || (b.tail_w > 0 && b.tail_w <= b.tw), "tile blend: tail columns must be 1 .. tw");
+  const int v = tile_blend_vector(b);
+  const size_t n = (size_t)b.C * b.T * b.th * (b.tw / v);
+  const int grid = grid_for(n);
+#define CE_TILE_BLEND(E, V) tile_blend_kernel<E, V><<<grid, TPB, 0, stream>>>(b)
+  if (b.fp32) {
+    if (v == 4) CE_TILE_BLEND(float, 4);
+    else if (v == 2) CE_TILE_BLEND(float, 2);
+    else CE_TILE_BLEND(float, 1);
+  } else {
+    if (v == 8) CE_TILE_BLEND(bf16, 8);
+    else if (v == 4) CE_TILE_BLEND(bf16, 4);
+    else if (v == 2) CE_TILE_BLEND(bf16, 2);
+    else CE_TILE_BLEND(bf16, 1);
+  }
+#undef CE_TILE_BLEND
+  CE_CHECK_CUDA(cudaGetLastError());
+  return CE_OK;
+}
 
 int launch_rms_silu_cl_f32(const float* x, const float* gamma, float* y, bf16* y_pair, size_t pixels, int C, int apply_silu,
                            cudaStream_t stream) {

@@ -22,4 +22,29 @@ int launch_planar_to_pair(const float* planar, int C, size_t pixels, bf16* pair,
 // planar[c, p] = cl[p, c] for c < Cout, fp32
 int launch_cl_to_planar_f32(const float* cl, int C, float* planar, size_t pixels, int Cout, cudaStream_t stream);
 
+// One tile of a tiled encode or decode (diffusers' blend_v then blend_h, in place, then the crop).  Every tensor is planar
+// [C, T, rows, cols] in the tile's dtype (bf16 or fp32, `fp32`).  The tile [C, T, th, tw] is blended with the last `above_h` rows
+// of the blended tile above (`above` [C, T, above_h, tw], extent min(above_h, th)) and then with the last `left_w` columns of the
+// blended tile to its left (`left` [C, T, th, left_w], extent min(left_w, tw)); a null neighbour is no blend.  The blended values go
+// to: out [C, T, out_h, out_w] at (oy, ox) for tile rows < crop_h and columns < crop_w, clipped to out (clamped to [-1, 1] if
+// clamp); strip [C, T, strip_h, tw] = the last strip_h rows; tail [C, T, th, tail_w] = the last tail_w columns (null: not kept).
+struct TileBlend {
+  const void* tile = nullptr;
+  int C = 0, T = 0, th = 0, tw = 0;
+  const void* above = nullptr;
+  int above_h = 0;
+  const void* left = nullptr;
+  int left_w = 0;
+  void* out = nullptr;
+  int out_h = 0, out_w = 0, oy = 0, ox = 0, crop_h = 0, crop_w = 0, clamp = 0;
+  void* strip = nullptr;
+  int strip_h = 0;
+  void* tail = nullptr;
+  int tail_w = 0;
+  int fp32 = 0;
+};
+int launch_tile_blend(const TileBlend& b, cudaStream_t stream);
+// elements per 16-byte access the launch uses for these extents (8 / 4 / 2 / 1 bf16, 4 / 2 / 1 fp32)
+int tile_blend_vector(const TileBlend& b);
+
 }  // namespace ce

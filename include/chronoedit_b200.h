@@ -312,6 +312,55 @@ int ce_vae_encode_fp32(ce_vae* h, const float* video, float* moments, int frames
 int ce_vae_decode_fp32(ce_vae* h, const float* z, float* video, int latent_frames, int latent_height, int latent_width, int clamp,
                        void* workspace, int64_t workspace_bytes, void* stream);
 
+/* Tiled encode / decode (diffusers AutoencoderKLWan.tiled_encode / tiled_decode, what enable_tiling() switches on): the same inputs
+ * and outputs as the calls above, computed tile by tile.  Tile sizes and strides are in pixels, multiples of 8, stride <= size.
+ * Tiles start every stride (latent stride = stride / 8) and cover `size` (smaller at the right and bottom edges); each is a fresh
+ * untiled encode or decode (its own causal cache, never clamped).  In grid order each result is blended in place with the blended
+ * tile above (diffusers' blend_v over min(size - stride, both heights) rows) and then with the blended tile to its left (blend_h),
+ * and its first stride x stride is written to the output (blend extents and crops in latent units when encoding, in pixels when
+ * decoding).  clamp != 0 clamps the decoded pixels to [-1, 1] as they are written.
+ * The workspace (ce_vae_workspace_bytes_tiled[_fp32], -1 on refusal) is one tile's untiled workspace plus the staged input and output
+ * tile plus the last size - stride rows of every tile of two grid rows and the last size - stride columns of two tiles: it does not
+ * grow with the height, and grows with the width by those rows only.  Refused before any launch: a handle split over GPUs
+ * (ce_vae_sp_configure with world > 1), sizes or strides that are not positive multiples of 8, a stride larger than the size, and
+ * everything the untiled call refuses. */
+int64_t ce_vae_workspace_bytes_tiled(ce_vae* h, int decode, int frames, int height, int width, int tile_min_height, int tile_min_width,
+                                     int tile_stride_height, int tile_stride_width);
+int ce_vae_encode_tiled(ce_vae* h, const void* video, void* moments, int frames, int height, int width, int tile_min_height, int tile_min_width,
+                        int tile_stride_height, int tile_stride_width, void* workspace, int64_t workspace_bytes, void* stream);
+int ce_vae_decode_tiled(ce_vae* h, const void* z, void* video, int latent_frames, int latent_height, int latent_width, int tile_min_height,
+                        int tile_min_width, int tile_stride_height, int tile_stride_width, int clamp, void* workspace, int64_t workspace_bytes,
+                        void* stream);
+int64_t ce_vae_workspace_bytes_tiled_fp32(ce_vae* h, int decode, int frames, int height, int width, int tile_min_height, int tile_min_width,
+                                          int tile_stride_height, int tile_stride_width);
+int ce_vae_encode_tiled_fp32(ce_vae* h, const float* video, float* moments, int frames, int height, int width, int tile_min_height,
+                             int tile_min_width, int tile_stride_height, int tile_stride_width, void* workspace, int64_t workspace_bytes,
+                             void* stream);
+int ce_vae_decode_tiled_fp32(ce_vae* h, const float* z, float* video, int latent_frames, int latent_height, int latent_width, int tile_min_height,
+                             int tile_min_width, int tile_stride_height, int tile_stride_width, int clamp, void* workspace,
+                             int64_t workspace_bytes, void* stream);
+/* Test aid: the blend launch of one tile.  Planar [C, T, rows, cols] tensors of one dtype (fp32 != 0: fp32, else bf16).  The tile
+ * [C, T, th, tw] is blended with the last above_h rows of the blended tile above (above [C, T, above_h, tw]; extent min(above_h, th)),
+ * then with the last left_w columns of the blended tile to its left (left [C, T, th, left_w]; extent min(left_w, tw)); null = none.
+ * Its rows < crop_h and columns < crop_w go to out [C, T, out_h, out_w] at (oy, ox), clipped to out; the last strip_h rows to strip
+ * [C, T, strip_h, tw] and the last tail_w columns to tail [C, T, th, tail_w] (null: not written). */
+typedef struct ce_vae_tile_blend_args {
+  int32_t fp32;
+  const void* tile;
+  int32_t C, T, th, tw;
+  const void* above;
+  int32_t above_h;
+  const void* left;
+  int32_t left_w;
+  void* out;
+  int32_t out_h, out_w, oy, ox, crop_h, crop_w, clamp;
+  void* strip;
+  int32_t strip_h;
+  void* tail;
+  int32_t tail_w;
+} ce_vae_tile_blend_args;
+int ce_vae_tile_blend(const ce_vae_tile_blend_args* args, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * The VAE split over the `world` ranks of a node (one process per GPU), for the latency of one edit: rank r encodes and
  * decodes latent rows [r h / world, (r + 1) h / world) (and the matching rows at every resolution), exchanges only the rows
