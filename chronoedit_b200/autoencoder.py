@@ -372,64 +372,46 @@ class AutoencoderKLWan(nn.Module):
             return (out,)
         return DecoderOutput(sample=out)
 
-    # the two places the VAE reaches the C ABI; samples of a batch are independent streams (each has its own causal cache in
-    # the reference too), run back to back on the current stream
+    # the seams encode / decode reach the C ABI through (tests stand in for them), all one call of _native
     def _native_encode(self, x: torch.Tensor, out: torch.Tensor) -> None:
-        if not self._is_packed:
-            self.pack_weights()
-        L = _lib.lib()
-        fp32 = self.dtype == torch.float32
-        B, _, T, H, W = x.shape
-        n = (L.ce_vae_workspace_bytes_fp32 if fp32 else L.ce_vae_workspace_bytes)(self._handle, 0, T, H, W)
-        if n < 0:
-            check(-1)
-        ws = self._workspace(n)
-        encode = L.ce_vae_encode_fp32 if fp32 else L.ce_vae_encode
-        with torch.cuda.device(self.device):
-            for b in range(B):
-                check(encode(self._handle, ptr(x[b]), ptr(out[b]), T, H, W, ptr(ws), ws.numel(), current_stream()))
+        self._native(x, out, decode=False, tiled=False)
 
     def _native_decode(self, z: torch.Tensor, out: torch.Tensor) -> None:
+        self._native(z, out, decode=True, tiled=False)
+
+    def _native_tiled(self, x: torch.Tensor, out: torch.Tensor, decode: bool) -> None:
+        self._native(x, out, decode=decode, tiled=True)
+
+    # (fp32, tiled) -> the workspace query and the encode / decode entry points
+    _SYMBOLS = {
+        (False, False): ("ce_vae_workspace_bytes", "ce_vae_encode", "ce_vae_decode"),
+        (True, False): ("ce_vae_workspace_bytes_fp32", "ce_vae_encode_fp32", "ce_vae_decode_fp32"),
+        (False, True): ("ce_vae_workspace_bytes_tiled", "ce_vae_encode_tiled", "ce_vae_decode_tiled"),
+        (True, True): ("ce_vae_workspace_bytes_tiled_fp32", "ce_vae_encode_tiled_fp32", "ce_vae_decode_tiled_fp32"),
+    }
+
+    def _native(self, x: torch.Tensor, out: torch.Tensor, decode: bool, tiled: bool) -> None:
+        """Encode (x = video) or decode (x = z), tiled or not.  Samples of a batch are independent streams (each has its own causal
+        cache in the reference too), run back to back on the current stream.  The tiled decode does not clamp (TILED_DECODE_CLAMPS)."""
         if not self._is_packed:
             self.pack_weights()
         L = _lib.lib()
-        fp32 = self.dtype == torch.float32
-        B, _, Tl, h, w = z.shape
-        n = (L.ce_vae_workspace_bytes_fp32 if fp32 else L.ce_vae_workspace_bytes)(self._handle, 1, Tl, h, w)
+        query, enc, dec = (getattr(L, name) for name in self._SYMBOLS[(self.dtype == torch.float32, tiled)])
+        B, _, T, H, W = x.shape
+        tiles = self._tiles() if tiled else ()
+        n = query(self._handle, int(decode), T, H, W, *tiles)
         if n < 0:
             check(-1)
         ws = self._workspace(n)
-        decode = L.ce_vae_decode_fp32 if fp32 else L.ce_vae_decode
+        clamp = (int(self.clamp_output and (TILED_DECODE_CLAMPS or not tiled)),) if decode else ()
+        fn = dec if decode else enc
         with torch.cuda.device(self.device):
             for b in range(B):
-                check(decode(self._handle, ptr(z[b]), ptr(out[b]), Tl, h, w, int(self.clamp_output), ptr(ws), ws.numel(),
-                             current_stream()))
+                check(fn(self._handle, ptr(x[b]), ptr(out[b]), T, H, W, *tiles, *clamp, ptr(ws), ws.numel(), current_stream()))
 
     def _check_tiling_single_gpu(self) -> None:
         if self._sp_state:
             raise CEError("tiling is not built for the VAE split over GPUs (parallel.enable_vae_sequence_parallel); disable one of them")
-
-    def _native_tiled(self, x: torch.Tensor, out: torch.Tensor, decode: bool) -> None:
-        """Tiled encode (x = video) or decode (x = z), one sample at a time.  The tiled decode does not clamp (TILED_DECODE_CLAMPS)."""
-        if not self._is_packed:
-            self.pack_weights()
-        L = _lib.lib()
-        fp32 = self.dtype == torch.float32
-        B, _, T, H, W = x.shape
-        tiles = self._tiles()
-        n = (L.ce_vae_workspace_bytes_tiled_fp32 if fp32 else L.ce_vae_workspace_bytes_tiled)(self._handle, int(decode), T, H, W, *tiles)
-        if n < 0:
-            check(-1)
-        ws = self._workspace(n)
-        with torch.cuda.device(self.device):
-            for b in range(B):
-                if decode:
-                    fn = L.ce_vae_decode_tiled_fp32 if fp32 else L.ce_vae_decode_tiled
-                    check(fn(self._handle, ptr(x[b]), ptr(out[b]), T, H, W, *tiles, int(TILED_DECODE_CLAMPS and self.clamp_output),
-                             ptr(ws), ws.numel(), current_stream()))
-                else:
-                    fn = L.ce_vae_encode_tiled_fp32 if fp32 else L.ce_vae_encode_tiled
-                    check(fn(self._handle, ptr(x[b]), ptr(out[b]), T, H, W, *tiles, ptr(ws), ws.numel(), current_stream()))
 
     def launches(self) -> int:
         return int(_lib.lib().ce_vae_last_launch_count(self._handle)) if self._handle else 0

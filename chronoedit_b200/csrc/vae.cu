@@ -8,6 +8,9 @@
 // (3->dim, z->top, 2z->2z) go through im2row + the wgmma GEMM; RMS_norm+SiLU / upsample are the row kernels of
 // vae_kernels.cu; the single-head mid attention is gemm_attention (gemm.cu) with H = 1.
 //
+// fp32 (ce_vae_*_fp32, AutoencoderKLWan loaded in fp32) runs the same walk: only Run's primitives know the precision (see Run).
+// Every entry point plans and runs through vae_call, which refuses in one order for all of them.
+//
 // Split over the ranks of a node (ce_vae_sp_configure): rank r owns latent rows [r h / W, (r + 1) h / W) and the matching rows at
 // every resolution of the encoder and decoder.  Every buffer that feeds a convolution with three kernel rows holds the band plus one
 // halo row above and below; the neighbours store their edge rows into this rank's peer region, a barrier orders it, and a local copy
@@ -43,19 +46,23 @@ struct ce_vae {
 
 namespace {
 
+// An activation [T, H, W, C]: p is what a convolution reads (bf16, or the fp32 activation's split pair [T, H, W, 2, C]), f the fp32
+// values where they exist.
 struct Act {
   bf16* p = nullptr;
+  float* f = nullptr;
   int T = 0, H = 0, W = 0, C = 0;
   size_t frame() const { return (size_t)H * W * C; }
-  size_t numel() const { return (size_t)T * frame(); }
   size_t pixels() const { return (size_t)T * H * W; }
 };
 
 struct StreamBuf {  // input buffer of one streaming (causal) convolution: `hist` history frames, then the chunk
   bf16* p = nullptr;
   int hist = 0, tcap = 0, H = 0, W = 0, C = 0;
+  int pair = 1;         // 2 in fp32: the frames hold the split pair [H, W, 2, C]
   bool halo = false;    // split: every frame is a band with one halo row above and below (H counts them)
   bool primed = false;  // false until the first chunk went through (used for the "Rep" / pass-through first chunks)
+  size_t frame() const { return (size_t)H * W * pair * C; }
 };
 
 // Byte offsets inside a rank's peer region for one pixel geometry H x W, the same for every frame count.
@@ -72,23 +79,35 @@ struct VaeSpLayout {
   int64_t bytes = 0;
 };
 
+struct Planar {   // a convolution's planar [C, T, H, W] store: output frame t goes to frame t0 + t of T
+  int T, t0, clamp;
+};
+
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 template <class T>
 T* at(T* p, size_t off) {   // planning passes carry null pointers
   return p ? p + off : nullptr;
 }
 
-// One encode or decode call.  `dry` = planning pass: the same walk without launches, in which the two bump allocators measure the
-// workspace and every weight is looked up with its packed element count before anything is launched.
+// One encode or decode call in bf16 or fp32.  A planning pass (dry) is the same walk without launches, in which the bump allocators
+// measure the workspace and every weight is looked up with its packed element count before anything is launched.  Only the primitives
+// below (rms, conv, the upsample, the mid attention, the stems and the encode's tail) know the precision: bf16 activations, or fp32
+// activations whose convolutions read their split pair (launch_conv3d_cl_f32, conv.cuh), with the causal history kept as the pair and
+// the mid attention Fp32Chain's (6-term split products, fp32 row softmax).
 struct Run {
   ce_vae* h;
+  bool fp32;
   cudaStream_t s;
-  bool dry;
-  Bump persist;   // from the front of the workspace: stream buffers, collected outputs
-  Bump scratch;   // after the persistent region; reset per chunk
-  int64_t scratch_max = 0;
+  bool dry = true;
+  Bump persist{nullptr};   // from the front of the workspace: stream buffers, converted inputs, collected outputs
+  // Scratch after the persistent region, reset per chunk.  fp32 uses two arenas in turn, one per block: a block's temporaries and
+  // output go into the arena its input is not in, which it resets first (what that arena held was the input of the block before,
+  // consumed by now); a whole chunk's fp32 activations at 720p would not fit beside the fp32 stream buffers.  bf16 uses one.
+  Bump arena[2] = {Bump(nullptr), Bump(nullptr)};
+  int cur = 0;
+  int64_t arena_max[2] = {0, 0};
   std::map<std::string, StreamBuf> streams;
-  WeightLookup weights{h->w};
+  WeightLookup weights{fp32 ? h->w32 : h->w};
   Launcher run{s, &h->launches};
   int rc = 0;
   // the split: this rank's band is latent rows [band0, band1) of `rows`; world == 1: the whole frame
@@ -97,29 +116,52 @@ struct Run {
   const VaeSpLayout* lay = nullptr;   // null when planning
   int64_t halo_row_max = 0;           // the largest halo row of a chunk (T W C bf16), in bytes
 
-  Run(ce_vae* h_, cudaStream_t s_, uint8_t* persist_base, uint8_t* scratch_base, int rank_ = 0, int world_ = 1)
-      : h(h_), s(s_), dry(persist_base == nullptr), persist(persist_base), scratch(scratch_base), rank(rank_), world(world_) {}
+  Run(ce_vae* h_, bool fp32_, int rank_, int world_, cudaStream_t s_ = nullptr) : h(h_), fp32(fp32_), s(s_), rank(rank_), world(world_) {}
+  // a launching pass: the buffers go into `ws` as the planning pass `plan` measured them
+  void bind(uint8_t* ws, const Run& plan) {
+    dry = false;
+    persist = Bump(ws);
+    arena[0] = Bump(ws + plan.persist.bytes());
+    arena[1] = Bump(ws + plan.persist.bytes() + plan.arena_bytes(0));
+  }
 
   bool split() const { return world > 1; }
+  int pair() const { return fp32 ? 2 : 1; }
   void set_band(int latent_rows) {
     rows = latent_rows;
     band0 = (int)((int64_t)rank * latent_rows / world);
     band1 = (int)((int64_t)(rank + 1) * latent_rows / world);
   }
 
-  void* take_scratch_bytes(size_t bytes) {
-    void* p = scratch.take<uint8_t>((int64_t)bytes);
-    if (scratch.off > scratch_max) scratch_max = scratch.off;
+  template <class T>
+  T* take(size_t n) {
+    T* p = arena[cur].take<T>((int64_t)n);
+    arena_max[cur] = std::max(arena_max[cur], arena[cur].off);
     return p;
   }
-  Act scratch_act(int T, int H, int W, int C) {
+  void next_block() {
+    if (!fp32) return;
+    cur ^= 1;
+    arena[cur].off = 0;
+  }
+  void new_chunk() {
+    arena[0].off = arena[1].off = 0;
+    cur = 0;
+  }
+  int64_t arena_bytes(int i) const { return (arena_max[i] + 255) & ~int64_t(255); }
+  int64_t workspace_bytes() const { return persist.bytes() + arena_bytes(0) + arena_bytes(1) + 256; }
+  // a scratch activation: bf16, or fp32 values and (with `with_pair`) the pair a convolution reads
+  Act act(int T, int H, int W, int C, bool with_pair = true) {
     Act a;
     a.T = T; a.H = H; a.W = W; a.C = C;
-    a.p = reinterpret_cast<bf16*>(take_scratch_bytes(a.numel() * 2));
+    if (!fp32) {
+      a.p = take<bf16>(a.pixels() * C);
+    } else {
+      a.f = take<float>(a.pixels() * C);
+      if (with_pair) a.p = take<bf16>(a.pixels() * 2 * C);
+    }
     return a;
   }
-  void reset_scratch() { scratch.off = 0; }
-  int64_t workspace_bytes() const { return persist.bytes() + ((scratch_max + 255) & ~int64_t(255)) + 256; }
 
   template <class Launch>
   void launch(Launch&& l) {
@@ -128,6 +170,9 @@ struct Run {
   void cuda(cudaError_t e) {
     if (e != cudaSuccess && !rc) rc = fail(CE_ERR_CUDA, cudaGetErrorString(e));
   }
+  void copy(void* dst, const void* src, size_t bytes) {
+    if (!dry && !rc) cuda(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s));
+  }
 
   // ---- streaming conv input buffers
   StreamBuf& stream(const std::string& name, int hist, int tcap, int H, int W_, int C, bool halo = false) {
@@ -135,34 +180,25 @@ struct Run {
     if (it != streams.end()) return it->second;
     StreamBuf b;
     b.halo = halo && split();
-    b.hist = hist; b.tcap = tcap; b.H = b.halo ? H + 2 : H; b.W = W_; b.C = C;
-    const size_t elems = (size_t)(hist + tcap) * b.H * W_ * C;
+    b.hist = hist; b.tcap = tcap; b.H = b.halo ? H + 2 : H; b.W = W_; b.C = C; b.pair = pair();
+    const size_t elems = (size_t)(hist + tcap) * b.frame();
     b.p = persist.take<bf16>((int64_t)elems);
     // zero history = causal zero padding; split: also the halo rows past the global edge, which nothing writes
-    const size_t zero = split() ? elems : (size_t)hist * b.H * W_ * C;
+    const size_t zero = split() ? elems : (size_t)hist * b.frame();
     if (!dry && zero > 0) cuda(cudaMemsetAsync(b.p, 0, zero * 2, s));
     return streams.emplace(name, b).first->second;
   }
   Act chunk_of(StreamBuf& b, int T) {
     Act a;
     a.T = T; a.H = b.H; a.W = b.W; a.C = b.C;
-    a.p = b.p ? b.p + (size_t)b.hist * a.frame() : nullptr;
+    a.p = at(b.p, (size_t)b.hist * b.frame());
     if (T > b.tcap && !rc) rc = fail(CE_ERR_INVALID, "vae: chunk larger than the planned stream buffer");
     return a;
   }
   // history <- last `hist` frames of [history ; chunk of T frames]
   void push_history(StreamBuf& b, int T) {
-    if (dry || b.hist == 0) return;
-    const size_t fb = (size_t)b.H * b.W * b.C * 2;
-    for (int i = 0; i < b.hist; ++i) {  // ascending order: sources are always at or after the destination
-      const int src = T + i;            // frame index inside [hist ; chunk]
-      cuda(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(b.p) + (size_t)i * fb, reinterpret_cast<uint8_t*>(b.p) + (size_t)src * fb, fb,
-                           cudaMemcpyDeviceToDevice, s));
-    }
-  }
-  void copy(const Act& src, bf16* dst) {
-    if (dry) return;
-    cuda(cudaMemcpyAsync(dst, src.p, src.numel() * 2, cudaMemcpyDeviceToDevice, s));
+    for (int i = 0; i < b.hist; ++i)   // ascending order: sources are always at or after the destination
+      copy(at(b.p, i * b.frame()), at(b.p, (T + i) * b.frame()), b.frame() * 2);
   }
 
   // ---- the exchange between ranks
@@ -212,37 +248,58 @@ struct Run {
     if (rank < world - 1) copy_2d(b + (band + 1) * row, fr, slot(rank, 1), row, row, T);
   }
 
-  // ---- primitive ops
-  void rms(const Act& x, const std::string& gamma_name, bf16* y, bool silu) {
+  // ---- primitive ops: the only code that knows the precision
+  // RMS_norm (+ SiLU) of x into y: bf16, or fp32 into y's fp32 values and / or its pair
+  void rms(const Act& x, const std::string& gamma_name, const Act& y, bool silu) {
+    if (fp32) {
+      const float* g = weights.any<float>(gamma_name, x.C);
+      launch([&] { return launch_rms_silu_cl_f32(x.f, g, y.f, y.p, x.pixels(), x.C, silu ? 1 : 0, s); });
+      return;
+    }
     const bf16* g = weights.any<bf16>(gamma_name, x.C);
-    launch([&] { return launch_rms_silu_cl(x.p, g, y, x.pixels(), x.C, silu ? 1 : 0, s); });
+    launch([&] { return launch_rms_silu_cl(x.p, g, y.p, x.pixels(), x.C, silu ? 1 : 0, s); });
   }
-  // rms into the chunk of a stream buffer; with halo rows one launch per frame (a frame's band rows are not next to the next frame's)
-  void rms_into(const Act& x, const std::string& gamma_name, const StreamBuf& b, bf16* y, bool silu) {
+  // rms into the chunk y of a stream buffer; with halo rows one launch per frame (a frame's band rows are not next to the next frame's)
+  void rms_into(const Act& x, const std::string& gamma_name, const StreamBuf& b, const Act& y, bool silu) {
     if (!b.halo) return rms(x, gamma_name, y, silu);
     for (int f = 0; f < x.T; ++f) {
-      Act xf = x;
+      Act xf = x, yf = y;
       xf.T = 1; xf.p = at(x.p, f * x.frame());
-      rms(xf, gamma_name, at(y, f * (x.frame() + 2 * (size_t)x.W * x.C) + (size_t)x.W * x.C), silu);
+      yf.p = at(y.p, f * (x.frame() + 2 * (size_t)x.W * x.C) + (size_t)x.W * x.C);
+      rms(xf, gamma_name, yf, silu);
     }
   }
-  // implicit-GEMM conv reading `in` = [Tin frames] (history included) -> out
-  void conv(const std::string& name, const bf16* in, int Tin, int Hin, int Win, int Cin, Act& out, int kt, int kh, int kw, int st, int sh,
-            int sw, int ph, int pw, const bf16* resid = nullptr, int split_time = 0, int t_base = 0) {
+  // implicit-GEMM conv reading `in` = [Tin frames] (history included) -> out (bf16, or fp32 values and / or pair), plus resid's values;
+  // with `planar` the output is stored planar into out.p (bf16) or out.f (fp32)
+  void conv(const std::string& name, const bf16* in, int Tin, int Hin, int Win, int Cin, const Act& out, int kt, int kh, int kw, int st,
+            int sh, int sw, int ph, int pw, const Act& resid = Act(), int split_time = 0, int t_base = 0, const Planar* planar = nullptr) {
     ConvArgs a;
     a.Cout = split_time ? out.C * 2 : out.C; a.Cin_pad = round_up(Cin, 64);
-    a.w = weights.any<bf16>(name + ".weight", (int64_t)a.Cout * kt * kh * kw * a.Cin_pad);
-    a.bias = weights.any<bf16>(name + ".bias", a.Cout);
+    // fp32: the weight's bf16 hi | hi | lo split (pack_parameter_fp32)
+    a.w = weights.any<bf16>(name + ".weight", (int64_t)a.Cout * kt * kh * kw * a.Cin_pad * (fp32 ? 3 : 1));
     a.x = in; a.Tin = Tin; a.Hin = Hin; a.Win = Win; a.Cin = Cin;
     a.kt = kt; a.kh = kh; a.kw = kw; a.st = st; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw;
     a.t_base = t_base;
-    a.y = out.p; a.Tout = split_time ? out.T / 2 : out.T; a.Hout = out.H; a.Wout = out.W;
-    a.resid = resid; a.split_time = split_time;
-    launch([&] { return launch_conv3d_cl(a, s); });
+    a.Tout = split_time ? out.T / 2 : out.T; a.Hout = out.H; a.Wout = out.W;
+    a.split_time = split_time;
+    if (planar) {
+      a.planar_out = 1; a.clamp = planar->clamp; a.planar_T = planar->T; a.planar_t0 = planar->t0;
+    }
+    if (!fp32) {
+      a.bias = weights.any<bf16>(name + ".bias", a.Cout);
+      a.y = out.p; a.resid = resid.p;
+      launch([&] { return launch_conv3d_cl(a, s); });
+      return;
+    }
+    ConvF32 f;
+    f.bias = weights.any<float>(name + ".bias", a.Cout);
+    f.resid = resid.f; f.y = out.f; f.y_pair = out.p;
+    launch([&] { return launch_conv3d_cl_f32(a, f, s); });
   }
   // streaming causal conv (kt = 3): x is already in the stream buffer's chunk region; halo rows replace the rows' zero padding
-  void causal_conv(const std::string& name, StreamBuf& b, int T, Act& out, int kh, const bf16* resid = nullptr, int split_time = 0) {
-    conv(name, b.p, b.hist + T, b.H, b.W, b.C, out, 3, kh, kh, 1, 1, 1, b.halo ? 0 : kh / 2, kh / 2, resid, split_time);
+  void causal_conv(const std::string& name, StreamBuf& b, int T, const Act& out, int kh, const Act& resid = Act(), int split_time = 0,
+                   const Planar* planar = nullptr) {
+    conv(name, b.p, b.hist + T, b.H, b.W, b.C, out, 3, kh, kh, 1, 1, 1, b.halo ? 0 : kh / 2, kh / 2, resid, split_time, 0, planar);
     push_history(b, T);
     b.primed = true;
   }
@@ -250,38 +307,133 @@ struct Run {
             const bf16* resid = nullptr, int ldr = 0) {
     if (!dry && !rc) rc = run_gemm(run, A, lda, Wt, ldw, M, N, K, out, ldo, bias, epi, resid, ldr);
   }
+  // bf16 small-Cin conv: im2row + GEMM.  x addressed by strides (planar or channels-last); output row oh reads rows oh + dh - ph of x
+  void small_conv(const std::string& name, const bf16* x, size_t sc, size_t st_, size_t sh, size_t sw, int Tin, int Hin, int Win, int Cin,
+                  int t_base, int kt, int kh, bf16* out, int ldo, int Tout, int Hout, int ph, int Cout) {
+    const int K = kt * kh * kh * Cin, Kpad = round_up(K, 8);
+    bf16* A = take<bf16>((size_t)Tout * Hout * Win * Kpad);
+    const bf16* w = weights.any<bf16>(name + ".weight", (int64_t)Cout * Kpad);
+    const bf16* b = weights.any<bf16>(name + ".bias", Cout);
+    launch([&] {
+      return launch_im2row(x, sc, st_, sh, sw, Tin, Hin, Win, Cin, A, Kpad, Tout, Hout, Win, kt, kh, kh, ph, kh / 2, t_base, s);
+    });
+    gemm(A, Kpad, w, Kpad, Tout * Hout * Win, Cout, Kpad, out, ldo, b);
+  }
+  // the caller's planar input [C, pixels] as the stems read it: bf16 in place, fp32 as its pair [pixels, 2, Cp] in the persistent region
+  const bf16* stem_input(const void* x, int C, int Cp, size_t pixels) {
+    if (!fp32) return static_cast<const bf16*>(x);
+    bf16* pair = persist.take<bf16>((int64_t)pixels * 2 * Cp);
+    launch([&] { return launch_planar_to_pair(static_cast<const float*>(x), C, pixels, pair, Cp, s); });
+    return pair;
+  }
+  // the caller's planar output: bf16 as a convolution's out.p, fp32 as its out.f
+  Act caller_out(void* y, int T, int H, int W, int C) {
+    Act a;
+    a.T = T; a.H = H; a.W = W; a.C = C;
+    if (fp32) a.f = static_cast<float*>(y);
+    else a.p = static_cast<bf16*>(y);
+    return a;
+  }
+  // nearest 2x upsample of x into scratch, as the convolution after it reads it (bf16, or the fp32 pair)
+  bf16* upsample2x(const Act& x) {
+    bf16* up = take<bf16>(x.pixels() * 4 * pair() * x.C);
+    if (fp32) launch([&] { return launch_upsample2x_cl_f32(x.f, up, x.T, x.H, x.W, x.C, s); });
+    else launch([&] { return launch_upsample2x_cl(x.p, up, x.T, x.H, x.W, x.C, s); });
+    return up;
+  }
+
+  // encoder.conv1 (3x3x3 causal, Cin = 3) of chunk frames f0 .. into x, straight from the whole video (its own past frames are the
+  // history).  bf16: im2row + GEMM over the planar video; split: the band's pixel rows and the rows around it, read from the row above
+  // the band on (zero padding only at the global top and bottom).  fp32: the implicit conv on the video's pair, 3 channels padded to 8.
+  void encoder_stem(const bf16* video, const Act& x, int T, int H, int Wd, int f0) {
+    if (fp32) return conv("encoder.conv1", video, T, H, Wd, 8, x, 3, 3, 3, 1, 1, 1, 1, 1, Act(), 0, /*t_base=*/f0 - 2);
+    const int skip = band0 > 0 ? 8 * band0 - 1 : 0;
+    small_conv("encoder.conv1", at(video, (size_t)skip * Wd), (size_t)T * H * Wd, (size_t)H * Wd, (size_t)Wd, 1, T, H - skip, Wd, 3,
+               /*t_base=*/f0 - 2, 3, 3, x.p, x.C, x.T, x.H, band0 > 0 ? 0 : 1, x.C);
+  }
+  // conv2 (1x1x1 on latent frame i of z [zc, Tl, h, w]) into decoder.conv1's stream buffer, then decoder.conv1 (3x3x3 causal) into a
+  // new scratch activation of `top` channels.  bf16: both as im2row + GEMM; split: conv2 writes the band's rows and the halo rows
+  // that exist, read from the whole z.  fp32: both implicit convs on the pair.
+  Act decoder_stem(const bf16* z, int i, int Tl, int lh, int lw, int top) {
+    const int zc = h->cfg.z_dim, a = band0, nb = band1 - band0;
+    StreamBuf& s1 = stream("decoder.conv1", 2, 1, nb, lw, zc, true);
+    Act x0 = chunk_of(s1, 1);
+    if (fp32) {
+      conv("conv2", z, Tl, lh, lw, zc, x0, 1, 1, 1, 1, 1, 1, 0, 0, Act(), 0, /*t_base=*/i);
+      Act x = act(1, nb, lw, top);
+      causal_conv("decoder.conv1", s1, 1, x, 3);
+      return x;
+    }
+    const size_t zplane = (size_t)Tl * lh * lw;
+    if (!s1.halo) {
+      small_conv("conv2", z, zplane, (size_t)lh * lw, (size_t)lw, 1, Tl, lh, lw, zc, /*t_base=*/i, 1, 1, x0.p, zc, 1, lh, 0, zc);
+    } else {
+      const int lo = std::max(a - 1, 0), hi = std::min(a + nb + 1, lh);
+      small_conv("conv2", at(z, (size_t)lo * lw), zplane, (size_t)lh * lw, (size_t)lw, 1, Tl, hi - lo, lw, zc, /*t_base=*/i, 1, 1,
+                 at(x0.p, (size_t)(lo - a + 1) * lw * zc), zc, 1, hi - lo, 0, zc);
+    }
+    Act x = act(1, nb, lw, top);
+    small_conv("decoder.conv1", s1.p, 1, (size_t)s1.H * lw * zc, (size_t)lw * zc, (size_t)zc, s1.hist + 1, s1.H, lw, zc, 0, 3, 3, x.p, top, 1,
+               nb, s1.halo ? 0 : 1, top);
+    push_history(s1, 1);
+    return x;
+  }
+  // conv1 (1x1x1, 2z -> 2z) of the collected head outputs [P, 2z] (bf16, or the fp32 pair), then planar moments = mean | logvar.  bf16
+  // runs it as a GEMM; split: each rank's band is gathered into every rank's moments.
+  void encode_tail(const bf16* enc_out, void* moments, int Tl, int nb, int w) {
+    const int zc = h->cfg.z_dim;
+    const size_t P = (size_t)Tl * nb * w;
+    if (fp32) {
+      Act q = act(Tl, nb, w, 2 * zc, false);
+      conv("conv1", enc_out, Tl, nb, w, 2 * zc, q, 1, 1, 1, 1, 1, 1, 0, 0);
+      launch([&] { return launch_cl_to_planar_f32(q.f, 2 * zc, static_cast<float*>(moments), P, 2 * zc, s); });
+      return;
+    }
+    bf16* q = take<bf16>(P * 2 * zc);
+    const bf16* w1 = weights.any<bf16>("conv1.weight", (int64_t)4 * zc * zc);
+    gemm(enc_out, 2 * zc, w1, 2 * zc, (int)P, 2 * zc, 2 * zc, q, 2 * zc, weights.any<bf16>("conv1.bias", 2 * zc));
+    if (!split()) {
+      launch([&] { return launch_cl_to_planar(q, 2 * zc, static_cast<bf16*>(moments), P, 2 * zc, s); });
+      return;
+    }
+    bf16* band = take<bf16>(P * 2 * zc);   // the band's moments, planar
+    launch([&] { return launch_cl_to_planar(q, 2 * zc, band, P, 2 * zc, s); });
+    for (int t = 0; t < Tl; ++t) gather_moments(band, static_cast<bf16*>(moments), t, Tl, 2 * zc, w);
+  }
 
   // ---- blocks
   // ResidualBlock.forward (wan2pt1.py:201-220).  halo_out (split only): the output feeds a stride-2 downsample, so it is written
   // with halo rows (one launch per frame) and its edge rows are exchanged.
   Act res_block(const std::string& n, const Act& x, int Cout, int tcap, bool halo_out = false) {
+    next_block();
     StreamBuf& sa = stream(n + ".residual.2", 2, tcap, x.H, x.W, x.C, true);
     Act a_in = chunk_of(sa, x.T);
-    rms_into(x, n + ".residual.0.gamma", sa, a_in.p, true);
+    rms_into(x, n + ".residual.0.gamma", sa, a_in, true);
     if (sa.halo) halo_exchange(a_in.p, x.T, x.H, x.W, x.C);
-    Act t1 = scratch_act(x.T, x.H, x.W, Cout);
+    Act t1 = act(x.T, x.H, x.W, Cout, false);
     causal_conv(n + ".residual.2", sa, x.T, t1, 3);
     StreamBuf& sb = stream(n + ".residual.6", 2, tcap, x.H, x.W, Cout, true);
     Act b_in = chunk_of(sb, x.T);
-    rms_into(t1, n + ".residual.3.gamma", sb, b_in.p, true);
+    rms_into(t1, n + ".residual.3.gamma", sb, b_in, true);
     if (sb.halo) halo_exchange(b_in.p, x.T, x.H, x.W, Cout);
-    const bf16* hres = x.p;
+    Act hres = x;
     if (x.C != Cout) {
-      Act sc = scratch_act(x.T, x.H, x.W, Cout);
-      conv(n + ".shortcut", x.p, x.T, x.H, x.W, x.C, sc, 1, 1, 1, 1, 1, 1, 0, 0);
-      hres = sc.p;
+      if (!dry && !x.p && !rc) rc = fail(CE_ERR_INVALID, "vae fp32: a shortcut input without its pair");
+      hres = act(x.T, x.H, x.W, Cout, false);
+      conv(n + ".shortcut", x.p, x.T, x.H, x.W, x.C, hres, 1, 1, 1, 1, 1, 1, 0, 0);
     }
     if (!(halo_out && split())) {
-      Act out = scratch_act(x.T, x.H, x.W, Cout);
+      Act out = act(x.T, x.H, x.W, Cout);
       causal_conv(n + ".residual.6", sb, x.T, out, 3, hres);
       return out;
     }
-    Act out = scratch_act(x.T, x.H + 2, x.W, Cout);
+    Act out = act(x.T, x.H + 2, x.W, Cout);
     const size_t row = (size_t)x.W * Cout;
     for (int f = 0; f < x.T; ++f) {
-      Act of = out;
+      Act of = out, rf = hres;
       of.T = 1; of.H = x.H; of.p = at(out.p, f * out.frame() + row);
-      conv(n + ".residual.6", sb.p, sb.hist + x.T, sb.H, sb.W, sb.C, of, 3, 3, 3, 1, 1, 1, 0, 1, at(hres, f * x.H * row), 0, f);
+      rf.p = at(hres.p, f * x.H * row);
+      conv(n + ".residual.6", sb.p, sb.hist + x.T, sb.H, sb.W, sb.C, of, 3, 3, 3, 1, 1, 1, 0, 1, rf, 0, f);
     }
     push_history(sb, x.T);
     sb.primed = true;
@@ -290,15 +442,21 @@ struct Run {
     return out;
   }
 
-  // AttentionBlock.forward (wan2pt1.py:240-259): per frame, single head of width C over H*W tokens.  Split: every rank stores its band
-  // of the normalised frame into every rank's region, computes q|k and V^T of the whole frame and S, softmax, P.V, the projection
-  // and the residual for its own rows.
+  // AttentionBlock.forward (wan2pt1.py:240-259): per frame, single head of width C over H*W tokens.  Split (bf16): every rank stores
+  // its band of the normalised frame into every rank's region, computes q|k and V^T of the whole frame and S, softmax, P.V, the
+  // projection and the residual for its own rows.
   Act attn_block(const std::string& n, const Act& x) {
+    next_block();
+    Act xn = act(x.T, x.H, x.W, x.C, false);
+    rms(x, n + ".norm.gamma", xn, false);
+    Act out = act(x.T, x.H, x.W, x.C, false);
+    if (fp32) attention_fp32(n, x, xn, out);
+    else attention(n, x, xn, out);
+    return out;
+  }
+  void attention(const std::string& n, const Act& x, const Act& xn, const Act& out) {
     const int C = x.C, P = rows * x.W, Ppad = round_up(P, 8);
     const int q0 = band0 * x.W, nq = x.H * x.W;
-    Act xn = scratch_act(x.T, x.H, x.W, C);
-    rms(x, n + ".norm.gamma", xn.p, false);
-    Act out = scratch_act(x.T, x.H, x.W, C);
     GemmAttention a;
     a.wqk = weights.any<bf16>(n + ".to_qkv.weight", (int64_t)3 * C * C);
     a.bqk = weights.any<bf16>(n + ".to_qkv.bias", 3 * C);
@@ -309,11 +467,11 @@ struct Run {
     a.L = P; a.D = C; a.H = 1; a.dk = C; a.kpv = P; a.q0 = q0; a.nq = nq;
     a.sc.rule = SOFTMAX_SCALED;
     a.sc.scale = 1.0f / sqrtf((float)C);
-    a.qk = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)P * 2 * C * 2));
-    a.vT = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)C * Ppad * 2));
-    a.S = reinterpret_cast<float*>(take_scratch_bytes((size_t)nq * Ppad * 4));
-    a.P = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)nq * Ppad * 2));
-    a.out = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)nq * C * 2));
+    a.qk = take<bf16>((size_t)P * 2 * C);
+    a.vT = take<bf16>((size_t)C * Ppad);
+    a.S = take<float>((size_t)nq * Ppad);
+    a.P = take<bf16>((size_t)nq * Ppad);
+    a.out = take<bf16>((size_t)nq * C);
     a.ldo = C;
     for (int f = 0; f < x.T && !dry && !rc; ++f) {
       a.x = xn.p + (size_t)f * nq * C;
@@ -330,32 +488,54 @@ struct Run {
       if (!rc) rc = gemm_attention(run, a);
       gemm(a.out, C, wproj, C, nq, C, C, out.p + (size_t)f * nq * C, C, bproj, EPI_BIAS_RESID, x.p + (size_t)f * nq * C, C);   // proj + identity
     }
-    return out;
+  }
+  void attention_fp32(const std::string& n, const Act& x, const Act& xn, const Act& out) {
+    const int C = x.C, L = x.H * x.W, L8 = up8(L), Cp = up8(C);
+    Lin32 qkv_w, proj_w;
+    qkv_w.w = weights.any<float>(n + ".to_qkv.weight", (int64_t)3 * C * C);
+    qkv_w.b = weights.any<float>(n + ".to_qkv.bias", 3 * C);
+    proj_w.w = weights.any<float>(n + ".proj.weight", (int64_t)C * C);
+    proj_w.b = weights.any<float>(n + ".proj.bias", C);
+    float* qkv = take<float>((size_t)L * 3 * C);
+    float* o = take<float>((size_t)L * 3 * C);   // attention output in columns [0, C) (Fp32Chain::attention's row stride is qkv's)
+    Fp32Chain X{run, nullptr, nullptr, nullptr, nullptr, 6, nullptr};
+    X.Ap = take<bf16>((size_t)split_elems(L, std::max(Cp, L8), 6));
+    X.Wp = take<bf16>((size_t)std::max({split_elems(3 * C, C, 6), split_elems(L8, C, 6), split_elems(C, L8, 6)}));
+    X.S = take<float>((size_t)L * L8);
+    X.P = take<float>((size_t)L * L8);
+    X.part = take<float>((size_t)L * std::max(3 * C, L8));
+    const float scale = 1.0f / sqrtf((float)C);
+    for (int f = 0; f < x.T && !dry && !rc; ++f) {
+      const size_t off = (size_t)f * L * C;
+      if ((rc = X.linear(xn.f + off, C, L, C, qkv_w, 3 * C, qkv, 3 * C, 0))) break;
+      if ((rc = X.attention(qkv, qkv + C, qkv + 2 * C, o, 1, 1, L, L, 3 * C, C, scale))) break;
+      if ((rc = X.linear(o, 3 * C, L, C, proj_w, C, out.f + off, C, 0))) break;
+      rc = X.resid(out.f + off, x.f + off, L, C, nullptr, 0, L);
+    }
   }
 
   // Resample upsample2d / upsample3d (wan2pt1.py:112-143)
   Act upsample(const std::string& n, Act x, bool temporal, int tcap_in) {
+    next_block();
     const int C = x.C;
     if (temporal) {
       StreamBuf& st = stream(n + ".time_conv", 2, tcap_in, x.H, x.W, C);
       if (!st.primed) {
         st.primed = true;  // first chunk: "Rep" -- no temporal doubling, history stays zero (:116-120, 128-129)
       } else {
-        Act in = chunk_of(st, x.T);
-        copy(x, in.p);
-        Act y = scratch_act(2 * x.T, x.H, x.W, C);
-        causal_conv(n + ".time_conv", st, x.T, y, 1, nullptr, /*split_time=*/1);
+        copy(chunk_of(st, x.T).p, x.p, x.pixels() * pair() * C * 2);
+        Act y = act(2 * x.T, x.H, x.W, C, false);
+        causal_conv(n + ".time_conv", st, x.T, y, 1, Act(), /*split_time=*/1);
         x = y;
       }
     }
     if (!split()) {
-      Act up = scratch_act(x.T, 2 * x.H, 2 * x.W, C);
-      launch([&] { return launch_upsample2x_cl(x.p, up.p, x.T, x.H, x.W, C, s); });
-      Act out = scratch_act(x.T, 2 * x.H, 2 * x.W, C / 2);
-      conv(n + ".resample.1", up.p, up.T, up.H, up.W, C, out, 1, 3, 3, 1, 1, 1, 1, 1);
+      const bf16* up = upsample2x(x);
+      Act out = act(x.T, 2 * x.H, 2 * x.W, C / 2);
+      conv(n + ".resample.1", up, x.T, 2 * x.H, 2 * x.W, C, out, 1, 3, 3, 1, 1, 1, 1, 1);
       return out;
     }
-    Act up = scratch_act(x.T, 2 * x.H + 2, 2 * x.W, C);   // halo'd: one launch per frame into the band rows
+    Act up = act(x.T, 2 * x.H + 2, 2 * x.W, C);   // halo'd: one launch per frame into the band rows
     for (int f = 0; f < x.T; ++f) {
       const bf16* xf = at(x.p, f * x.frame());
       bf16* uf = at(up.p, f * up.frame() + (size_t)2 * x.W * C);
@@ -363,49 +543,43 @@ struct Run {
     }
     zero_edges(up.p, x.T, 2 * x.H, 2 * x.W, C);
     halo_exchange(up.p, x.T, 2 * x.H, 2 * x.W, C);
-    Act out = scratch_act(x.T, 2 * x.H, 2 * x.W, C / 2);
+    Act out = act(x.T, 2 * x.H, 2 * x.W, C / 2);
     conv(n + ".resample.1", up.p, up.T, up.H, up.W, C, out, 1, 3, 3, 1, 1, 1, 0, 1);
     return out;
   }
 
-  // Resample downsample2d / downsample3d (wan2pt1.py:145-159).  Split: x is halo'd; ph = -1 skips its row above, and the row below
-  // the band (zero at the global bottom) is what ZeroPad2d(0,1,0,1) and the stride-2 window read there.
+  // Resample downsample2d / downsample3d (wan2pt1.py:145-159): ZeroPad2d(0,1,0,1) is the zero fill past the edge.  Split: x is
+  // halo'd; ph = -1 skips its row above, and the row below the band (zero at the global bottom) is what ZeroPad2d(0,1,0,1) and the
+  // stride-2 window read there.
   Act downsample(const std::string& n, const Act& x, bool temporal, int tcap_out_spatial) {
+    next_block();
     const int C = x.C, band = split() ? x.H - 2 : x.H, ph = split() ? -1 : 0;
     const int Ho = (band + 1 - 3) / 2 + 1, Wo = (x.W + 1 - 3) / 2 + 1;
     if (!temporal) {
-      Act out = scratch_act(x.T, Ho, Wo, C);
-      conv(n + ".resample.1", x.p, x.T, x.H, x.W, C, out, 1, 3, 3, 1, 2, 2, ph, 0);  // ZeroPad2d(0,1,0,1) = OOB zero fill
+      Act out = act(x.T, Ho, Wo, C);
+      conv(n + ".resample.1", x.p, x.T, x.H, x.W, C, out, 1, 3, 3, 1, 2, 2, ph, 0);
       return out;
     }
     StreamBuf& st = stream(n + ".time_conv", 1, tcap_out_spatial, Ho, Wo, C);
     Act sp = chunk_of(st, x.T);
+    const bool first = !st.primed;
+    if (first && fp32) sp.f = take<float>(sp.pixels() * C);
     conv(n + ".resample.1", x.p, x.T, x.H, x.W, C, sp, 1, 3, 3, 1, 2, 2, ph, 0);
-    if (!st.primed) {  // first chunk passes through and becomes the history (:147-150)
+    if (first) {  // first chunk passes through and becomes the history (:147-150)
       st.primed = true;
-      Act out = scratch_act(x.T, Ho, Wo, C);
-      copy(sp, out.p);
+      Act out = sp;   // fp32: the chunk itself, whose pair nothing rewrites before the next chunk; bf16: a copy in scratch
+      if (!fp32) {
+        out = act(x.T, Ho, Wo, C);
+        copy(out.p, sp.p, sp.pixels() * C * 2);
+      }
       push_history(st, x.T);
       return out;
     }
     const int To = (1 + x.T - 3) / 2 + 1;
-    Act out = scratch_act(To, Ho, Wo, C);
+    Act out = act(To, Ho, Wo, C);
     conv(n + ".time_conv", st.p, 1 + x.T, Ho, Wo, C, out, 3, 1, 1, 2, 1, 1, 0, 0);
     push_history(st, x.T);
     return out;
-  }
-
-  // small-Cin conv: im2row + GEMM.  x addressed by strides (planar or channels-last); output row oh reads rows oh + dh - ph of x
-  void small_conv(const std::string& name, const bf16* x, size_t sc, size_t st_, size_t sh, size_t sw, int Tin, int Hin, int Win, int Cin,
-                  int t_base, int kt, int kh, bf16* out, int ldo, int Tout, int Hout, int ph, int Cout) {
-    const int K = kt * kh * kh * Cin, Kpad = round_up(K, 8);
-    bf16* A = reinterpret_cast<bf16*>(take_scratch_bytes((size_t)Tout * Hout * Win * Kpad * 2));
-    const bf16* w = weights.any<bf16>(name + ".weight", (int64_t)Cout * Kpad);
-    const bf16* b = weights.any<bf16>(name + ".bias", Cout);
-    launch([&] {
-      return launch_im2row(x, sc, st_, sh, sw, Tin, Hin, Win, Cin, A, Kpad, Tout, Hout, Win, kt, kh, kh, ph, kh / 2, t_base, s);
-    });
-    gemm(A, Kpad, w, Kpad, Tout * Hout * Win, Cout, Kpad, out, ldo, b);
   }
 
   // ---- gathering the outputs (split)
@@ -484,34 +658,18 @@ std::vector<LayerSpec> decoder_layers(const ce_vae_config& c) {
 
 // ---------------------------------------------------------------------------------------------- decode
 // WanVAE_.decode (wan2pt1.py:543-560) + Decoder3d.forward (:412-456); z planar [zc, Tl, h, w] -> video planar [3, 1+4(Tl-1), 8h, 8w]
-int run_decode(Run& R, const bf16* z, bf16* video, int Tl, int h, int w, int clamp) {
+int run_decode(Run& R, const void* z, void* video, int Tl, int h, int w, int clamp) {
   const ce_vae_config& c = R.h->cfg;
   const int top = top_dim(c), zc = c.z_dim;
   const int T_px = 1 + 4 * (Tl - 1);
-  const size_t zplane = (size_t)Tl * h * w;
+  const bf16* zin = R.stem_input(z, zc, zc, (size_t)Tl * h * w);
   R.set_band(h);
-  const int a = R.band0, nb = R.band1 - R.band0;   // the band's latent rows
   std::vector<LayerSpec> layers = decoder_layers(c);
   int t_out = 0;
   for (int i = 0; i < Tl && !R.rc; ++i) {
-    R.reset_scratch();
+    R.new_chunk();
     int cap = 1;  // frames a non-first chunk carries at the current depth (x2 after every upsample3d): stream capacity
-    // conv2 (1x1x1 on the planar z) -> straight into the stream buffer of decoder.conv1; split: the band's rows and the halo rows
-    // that exist, read from the whole z
-    StreamBuf& s1 = R.stream("decoder.conv1", 2, 1, nb, w, zc, true);
-    Act x0 = R.chunk_of(s1, 1);
-    if (!s1.halo) {
-      R.small_conv("conv2", z, zplane, (size_t)h * w, (size_t)w, 1, Tl, h, w, zc, /*t_base=*/i, 1, 1, x0.p, zc, 1, h, 0, zc);
-    } else {
-      const int lo = std::max(a - 1, 0), hi = std::min(a + nb + 1, h);
-      R.small_conv("conv2", at(z, (size_t)lo * w), zplane, (size_t)h * w, (size_t)w, 1, Tl, hi - lo, w, zc, /*t_base=*/i, 1, 1,
-                   at(x0.p, (size_t)(lo - a + 1) * w * zc), zc, 1, hi - lo, 0, zc);
-    }
-    // decoder.conv1: 3x3x3 causal with Cin = z_dim: im2row over [history ; chunk] (channels-last) + GEMM
-    Act x = R.scratch_act(1, nb, w, top);
-    R.small_conv("decoder.conv1", s1.p, 1, (size_t)s1.H * w * zc, (size_t)w * zc, (size_t)zc, s1.hist + 1, s1.H, w, zc, 0, 3, 3, x.p, top, 1, nb,
-                 s1.halo ? 0 : 1, top);
-    R.push_history(s1, 1);
+    Act x = R.decoder_stem(zin, i, Tl, h, w, top);
     x = R.res_block("decoder.middle.0", x, top, cap);
     x = R.attn_block("decoder.middle.1", x);
     x = R.res_block("decoder.middle.2", x, top, cap);
@@ -529,25 +687,16 @@ int run_decode(Run& R, const bf16* z, bf16* video, int Tl, int h, int w, int cla
     // then gathered)
     StreamBuf& sh = R.stream("decoder.head.2", 2, cap, x.H, x.W, x.C, true);
     Act hin = R.chunk_of(sh, x.T);
-    R.rms_into(x, "decoder.head.0.gamma", sh, hin.p, true);
+    R.rms_into(x, "decoder.head.0.gamma", sh, hin, true);
     if (sh.halo) R.halo_exchange(hin.p, x.T, x.H, x.W, x.C);
-    {
-      ConvArgs a;
-      a.x = sh.p; a.Tin = sh.hist + x.T; a.Hin = sh.H; a.Win = x.W; a.Cin = x.C;
-      a.Cout = 3; a.Cin_pad = round_up(x.C, 64);
-      a.w = R.weights.any<bf16>("decoder.head.2.weight", (int64_t)3 * 27 * a.Cin_pad);
-      a.bias = R.weights.any<bf16>("decoder.head.2.bias", 3);
-      a.kt = 3; a.kh = 3; a.kw = 3; a.ph = sh.halo ? 0 : 1; a.pw = 1;
-      a.y = video; a.Tout = x.T; a.Hout = x.H; a.Wout = x.W;
-      a.planar_out = 1; a.clamp = clamp; a.planar_T = T_px; a.planar_t0 = t_out;
-      if (R.split()) {
-        a.y = reinterpret_cast<bf16*>(R.take_scratch_bytes((size_t)3 * x.T * x.H * x.W * 2));
-        a.planar_T = x.T; a.planar_t0 = 0;
-      }
-      R.launch([&] { return launch_conv3d_cl(a, R.s); });
-      R.push_history(sh, x.T);
-      if (R.split()) R.gather_video(a.y, video, T_px, t_out, x.T, 8 * h, x.W);
+    Act o = R.caller_out(video, x.T, x.H, x.W, 3);
+    Planar pl{T_px, t_out, clamp};
+    if (R.split()) {
+      o.p = R.take<bf16>((size_t)3 * x.T * x.H * x.W);
+      pl = Planar{x.T, 0, clamp};
     }
+    R.causal_conv("decoder.head.2", sh, x.T, o, 3, Act(), 0, &pl);
+    if (R.split()) R.gather_video(o.p, static_cast<bf16*>(video), T_px, t_out, x.T, 8 * h, x.W);
     t_out += x.T;
   }
   if (!R.rc && t_out != T_px) return fail(CE_ERR_INVALID, "vae decode: produced frame count mismatch");
@@ -555,27 +704,24 @@ int run_decode(Run& R, const bf16* z, bf16* video, int Tl, int h, int w, int cla
 }
 
 // ---------------------------------------------------------------------------------------------- encode
-// WanVAE_.encode (wan2pt1.py:502-533) + Encoder3d.forward (:315-357); video planar [3, T, H, W] -> mean planar [zc, Tl, H/8, W/8]
-int run_encode(Run& R, const bf16* video, bf16* mu, int T, int H, int Wd) {
+// WanVAE_.encode (wan2pt1.py:502-533) + Encoder3d.forward (:315-357); video planar [3, T, H, W] -> moments planar [2 zc, Tl, H/8, W/8]
+int run_encode(Run& R, const void* video, void* moments, int T, int H, int Wd) {
   const ce_vae_config& c = R.h->cfg;
   const int top = top_dim(c), zc = c.z_dim;
   const int Tl = 1 + (T - 1) / 4, h = H / 8, w = Wd / 8;
+  const bf16* vin = R.stem_input(video, 3, 8, (size_t)T * H * Wd);
   R.set_band(h);
   const int nb = R.band1 - R.band0;   // the band's latent rows
   std::vector<LayerSpec> layers = encoder_layers(c);
-  bf16* enc_out = R.persist.take<bf16>((int64_t)Tl * nb * w * 2 * zc);  // head outputs of every chunk, channels-last
+  const size_t out_frame = (size_t)nb * w * 2 * zc * R.pair();
+  bf16* enc_out = R.persist.take<bf16>((int64_t)(Tl * out_frame));  // head outputs of every chunk, channels-last (fp32: the pair)
   int t_lat = 0;
   for (int f0 = 0; f0 < T && !R.rc;) {
     const int Tc = f0 == 0 ? 1 : 4;
-    R.reset_scratch();
+    R.new_chunk();
     int cap = 4;
-    Act x = R.scratch_act(Tc, 8 * nb, Wd, c.dim);
-    // encoder.conv1: 3x3x3 causal with Cin = 3 straight from the planar video (its own past frames are the history).  Split: the
-    // band's pixel rows and the rows around it, read from the whole video from the row above the band on (zero padding only at the
-    // global top and bottom)
-    const int skip = R.band0 > 0 ? 8 * R.band0 - 1 : 0;
-    R.small_conv("encoder.conv1", at(video, (size_t)skip * Wd), (size_t)T * H * Wd, (size_t)H * Wd, (size_t)Wd, 1, T, H - skip, Wd, 3,
-                 /*t_base=*/f0 - 2, 3, 3, x.p, c.dim, Tc, 8 * nb, R.band0 > 0 ? 0 : 1, c.dim);
+    Act x = R.act(Tc, 8 * nb, Wd, c.dim);
+    R.encoder_stem(vin, x, T, H, Wd, f0);
     for (size_t li = 0; li < layers.size(); ++li) {
       const LayerSpec& l = layers[li];
       const std::string n = "encoder.downsamples." + std::to_string(li);
@@ -591,31 +737,25 @@ int run_encode(Run& R, const bf16* video, bf16* mu, int T, int H, int Wd) {
     x = R.res_block("encoder.middle.2", x, top, cap);
     StreamBuf& sh = R.stream("encoder.head.2", 2, cap, x.H, x.W, x.C, true);
     Act hin = R.chunk_of(sh, x.T);
-    R.rms_into(x, "encoder.head.0.gamma", sh, hin.p, true);
+    R.rms_into(x, "encoder.head.0.gamma", sh, hin, true);
     if (sh.halo) R.halo_exchange(hin.p, x.T, x.H, x.W, x.C);
+    if (x.H != nb || x.W != w) return fail(CE_ERR_INVALID, "vae encode: spatial size mismatch (H, W must be multiples of 8)");
     Act o;
     o.T = x.T; o.H = x.H; o.W = x.W; o.C = 2 * zc;
-    o.p = R.dry ? nullptr : enc_out + (size_t)t_lat * nb * w * 2 * zc;
-    if (x.H != nb || x.W != w) return fail(CE_ERR_INVALID, "vae encode: spatial size mismatch (H, W must be multiples of 8)");
+    o.p = at(enc_out, t_lat * out_frame);
     R.causal_conv("encoder.head.2", sh, x.T, o, 3);
     t_lat += x.T;
     f0 += Tc;
   }
   if (!R.rc && t_lat != Tl) return fail(CE_ERR_INVALID, "vae encode: produced frame count mismatch");
-  // conv1 (1x1x1, 2z -> 2z) then keep the first z channels (posterior mean)
-  R.reset_scratch();
-  const size_t P = (size_t)Tl * nb * w;
-  bf16* q = reinterpret_cast<bf16*>(R.take_scratch_bytes(P * 2 * zc * 2));
-  const bf16* w1 = R.weights.any<bf16>("conv1.weight", (int64_t)4 * zc * zc);
-  R.gemm(enc_out, 2 * zc, w1, 2 * zc, (int)P, 2 * zc, 2 * zc, q, 2 * zc, R.weights.any<bf16>("conv1.bias", 2 * zc));
-  if (!R.split()) {
-    R.launch([&] { return launch_cl_to_planar(q, 2 * zc, mu, P, 2 * zc, R.s); });  // moments = mean | logvar
-    return R.rc;
-  }
-  bf16* band = reinterpret_cast<bf16*>(R.take_scratch_bytes(P * 2 * zc * 2));   // the band's moments, planar
-  R.launch([&] { return launch_cl_to_planar(q, 2 * zc, band, P, 2 * zc, R.s); });
-  for (int t = 0; t < Tl; ++t) R.gather_moments(band, mu, t, Tl, 2 * zc, w);
+  R.new_chunk();
+  R.encode_tail(enc_out, moments, Tl, nb, w);
   return R.rc;
+}
+
+// One encode or decode: `R` plans (dry) or launches.  A planning pass leaves the first missing or mis-sized weight in R.weights.rc.
+int walk(Run& R, bool decode, const void* in, void* out, int frames, int height, int width, int clamp) {
+  return decode ? run_decode(R, in, out, frames, height, width, clamp) : run_encode(R, in, out, frames, height, width);
 }
 
 int check_geometry(const ce_vae* h, int T, int H, int W, bool decode) {
@@ -642,9 +782,9 @@ int count_temporal(const ce_vae_config& c) { return (c.temporal_downsample[0] !=
 int vae_sp_layout(ce_vae* h, int H, int W, int world, VaeSpLayout& L) {
   const ce_vae_config& c = h->cfg;
   const int lh = H / 8, lw = W / 8;
-  Run enc(h, nullptr, nullptr, nullptr, 0, world), dec(h, nullptr, nullptr, nullptr, 0, world);
-  CE_TRY(run_encode(enc, nullptr, nullptr, 5, H, W));
-  CE_TRY(run_decode(dec, nullptr, nullptr, 2, lh, lw, 0));
+  Run enc(h, false, 0, world), dec(h, false, 0, world);
+  CE_TRY(walk(enc, false, nullptr, nullptr, 5, H, W, 0));
+  CE_TRY(walk(dec, true, nullptr, nullptr, 2, lh, lw, 0));
   auto al = [](int64_t v) { return (v + 1023) & ~int64_t(1023); };
   L = VaeSpLayout();
   L.flags = 0;
@@ -660,344 +800,58 @@ int vae_sp_layout(ce_vae* h, int H, int W, int world, VaeSpLayout& L) {
   return CE_OK;
 }
 
-// ---------------------------------------------------------------------------------------------- fp32
-// The same chain in fp32 (AutoencoderKLWan loaded in fp32): fp32 activations, fp32 parameters, the operator order and chunking of
-// run_encode / run_decode on one GPU.  Every convolution is launch_conv3d_cl_f32 reading the split pair of its input (conv.cuh); the
-// row kernels and the convolutions' epilogues write that pair where a convolution reads it next, and the causal history is kept as
-// the pair.  The mid attention is Fp32Chain's (6-term split products, fp32 row softmax).
-
-struct Act32 {   // fp32 [T, H, W, C] and / or its pair [T, H, W, 2, C]
-  float* f = nullptr;
-  bf16* pair = nullptr;
-  int T = 0, H = 0, W = 0, C = 0;
-  size_t pixels() const { return (size_t)T * H * W; }
-};
-
-struct Stream32 {   // input pair of one streaming convolution: `hist` history frames, then the chunk
-  bf16* p = nullptr;
-  int hist = 0, tcap = 0, H = 0, W = 0, C = 0;
-  bool primed = false;
-  size_t frame() const { return (size_t)H * W * 2 * C; }
-};
-
-// Scratch is two arenas used in turn, one per block: a block's temporaries and output go into the arena its input is not in, which
-// it resets first (what that arena held was the input of the block before, consumed by now).  A whole chunk's activations at 720p
-// would not fit beside the fp32 stream buffers.
-struct Run32 {
-  ce_vae* h;
-  cudaStream_t s;
-  bool dry;
-  Bump persist;
-  Bump arena[2];
-  int cur = 0;
-  int64_t arena_max[2] = {0, 0};
-  std::map<std::string, Stream32> streams;
-  WeightLookup weights{h->w32};
-  Launcher run{s, &h->launches};
-  int rc = 0;
-
-  Run32(ce_vae* h_, cudaStream_t s_, uint8_t* persist_base, uint8_t* arena0, uint8_t* arena1)
-      : h(h_), s(s_), dry(persist_base == nullptr), persist(persist_base), arena{Bump(arena0), Bump(arena1)} {}
-
-  template <class T>
-  T* take(size_t n) {
-    T* p = arena[cur].take<T>((int64_t)n);
-    arena_max[cur] = std::max(arena_max[cur], arena[cur].off);
-    return p;
-  }
-  void next_block() {
-    cur ^= 1;
-    arena[cur].off = 0;
-  }
-  void new_chunk() {
-    arena[0].off = arena[1].off = 0;
-    cur = 0;
-  }
-  int64_t arena_bytes(int i) const { return (arena_max[i] + 255) & ~int64_t(255); }
-  Act32 act(int T, int H, int W, int C, bool f, bool pair) {
-    Act32 a;
-    a.T = T; a.H = H; a.W = W; a.C = C;
-    if (f) a.f = take<float>(a.pixels() * C);
-    if (pair) a.pair = take<bf16>(a.pixels() * 2 * C);
-    return a;
-  }
-  int64_t workspace_bytes() const { return persist.bytes() + arena_bytes(0) + arena_bytes(1) + 256; }
-  template <class Launch>
-  void launch(Launch&& l) {
-    if (!dry && !rc) rc = run(l);
-  }
-  void copy(void* dst, const void* src, size_t bytes) {
-    if (!dry && !rc && cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess) rc = fail(CE_ERR_CUDA, "vae fp32: copy");
-  }
-
-  Stream32& stream(const std::string& name, int hist, int tcap, int H, int W, int C) {
-    auto it = streams.find(name);
-    if (it != streams.end()) return it->second;
-    Stream32 b;
-    b.hist = hist; b.tcap = tcap; b.H = H; b.W = W; b.C = C;
-    b.p = persist.take<bf16>((int64_t)(hist + tcap) * b.frame());
-    if (!dry && hist > 0 && cudaMemsetAsync(b.p, 0, hist * b.frame() * 2, s) != cudaSuccess && !rc) rc = fail(CE_ERR_CUDA, "vae fp32: memset");
-    return streams.emplace(name, b).first->second;
-  }
-  bf16* chunk_of(Stream32& b, int T) {
-    if (T > b.tcap && !rc) rc = fail(CE_ERR_INVALID, "vae fp32: chunk larger than the planned stream buffer");
-    return at(b.p, b.hist * b.frame());
-  }
-  void push_history(Stream32& b, int T) {   // history <- last `hist` frames of [history ; chunk]
-    for (int i = 0; i < b.hist; ++i) copy(at(b.p, i * b.frame()), at(b.p, (T + i) * b.frame()), b.frame() * 2);
-  }
-
-  void rms(const Act32& x, const std::string& gamma, float* y, bf16* y_pair, bool silu) {
-    const float* g = weights.any<float>(gamma, x.C);
-    launch([&] { return launch_rms_silu_cl_f32(x.f, g, y, y_pair, x.pixels(), x.C, silu ? 1 : 0, s); });
-  }
-  // convolution of the pair `in` ([Tin] frames, history included) into out's fp32 and / or pair
-  void conv(const std::string& name, const bf16* in, int Tin, int Hin, int Win, int Cin, const Act32& out, int kt, int kh, int kw, int st,
-            int sh, int sw, int ph, int pw, const float* resid = nullptr, int split_time = 0, int t_base = 0) {
-    ConvArgs a;
-    a.Cout = split_time ? out.C * 2 : out.C; a.Cin_pad = round_up(Cin, 64);
-    a.w = weights.any<bf16>(name + ".weight", (int64_t)a.Cout * kt * kh * kw * a.Cin_pad * 3);
-    ConvF32 f;
-    f.bias = weights.any<float>(name + ".bias", a.Cout);
-    f.resid = resid; f.y = out.f; f.y_pair = out.pair;
-    a.x = in; a.Tin = Tin; a.Hin = Hin; a.Win = Win; a.Cin = Cin;
-    a.kt = kt; a.kh = kh; a.kw = kw; a.st = st; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw;
-    a.t_base = t_base;
-    a.Tout = split_time ? out.T / 2 : out.T; a.Hout = out.H; a.Wout = out.W;
-    a.split_time = split_time;
-    launch([&] { return launch_conv3d_cl_f32(a, f, s); });
-  }
-  void causal_conv(const std::string& name, Stream32& b, int T, const Act32& out, int kh, const float* resid = nullptr, int split_time = 0) {
-    conv(name, b.p, b.hist + T, b.H, b.W, b.C, out, 3, kh, kh, 1, 1, 1, kh / 2, kh / 2, resid, split_time);
-    push_history(b, T);
-    b.primed = true;
-  }
-
-  // ResidualBlock.forward (wan2pt1.py:201-220); the output carries its pair for the shortcut or the convolution after it
-  Act32 res_block(const std::string& n, const Act32& x, int Cout, int tcap) {
-    next_block();
-    Stream32& sa = stream(n + ".residual.2", 2, tcap, x.H, x.W, x.C);
-    rms(x, n + ".residual.0.gamma", nullptr, chunk_of(sa, x.T), true);
-    Act32 t1 = act(x.T, x.H, x.W, Cout, true, false);
-    causal_conv(n + ".residual.2", sa, x.T, t1, 3);
-    Stream32& sb = stream(n + ".residual.6", 2, tcap, x.H, x.W, Cout);
-    rms(t1, n + ".residual.3.gamma", nullptr, chunk_of(sb, x.T), true);
-    const float* hres = x.f;
-    if (x.C != Cout) {
-      if (!dry && !x.pair && !rc) rc = fail(CE_ERR_INVALID, "vae fp32: a shortcut input without its pair");
-      Act32 sc = act(x.T, x.H, x.W, Cout, true, false);
-      conv(n + ".shortcut", x.pair, x.T, x.H, x.W, x.C, sc, 1, 1, 1, 1, 1, 1, 0, 0);
-      hres = sc.f;
-    }
-    Act32 out = act(x.T, x.H, x.W, Cout, true, true);
-    causal_conv(n + ".residual.6", sb, x.T, out, 3, hres);
-    return out;
-  }
-
-  // AttentionBlock.forward (wan2pt1.py:240-259): per frame, one head of width C over H*W tokens
-  Act32 attn_block(const std::string& n, const Act32& x) {
-    next_block();
-    const int C = x.C, L = x.H * x.W, L8 = up8(L), Cp = up8(C);
-    Act32 xn = act(x.T, x.H, x.W, C, true, false);
-    rms(x, n + ".norm.gamma", xn.f, nullptr, false);
-    Lin32 qkv_w, proj_w;
-    qkv_w.w = weights.any<float>(n + ".to_qkv.weight", (int64_t)3 * C * C);
-    qkv_w.b = weights.any<float>(n + ".to_qkv.bias", 3 * C);
-    proj_w.w = weights.any<float>(n + ".proj.weight", (int64_t)C * C);
-    proj_w.b = weights.any<float>(n + ".proj.bias", C);
-    Act32 out = act(x.T, x.H, x.W, C, true, false);
-    float* qkv = take<float>((size_t)L * 3 * C);
-    float* o = take<float>((size_t)L * 3 * C);   // attention output in columns [0, C) (Fp32Chain::attention's row stride is qkv's)
-    Fp32Chain X{run, nullptr, nullptr, nullptr, nullptr, 6, nullptr};
-    X.Ap = take<bf16>((size_t)split_elems(L, std::max(Cp, L8), 6));
-    X.Wp = take<bf16>((size_t)std::max({split_elems(3 * C, C, 6), split_elems(L8, C, 6), split_elems(C, L8, 6)}));
-    X.S = take<float>((size_t)L * L8);
-    X.P = take<float>((size_t)L * L8);
-    X.part = take<float>((size_t)L * std::max(3 * C, L8));
-    const float scale = 1.0f / sqrtf((float)C);
-    for (int f = 0; f < x.T && !dry && !rc; ++f) {
-      const size_t off = (size_t)f * L * C;
-      if ((rc = X.linear(xn.f + off, C, L, C, qkv_w, 3 * C, qkv, 3 * C, 0))) break;
-      if ((rc = X.attention(qkv, qkv + C, qkv + 2 * C, o, 1, 1, L, L, 3 * C, C, scale))) break;
-      if ((rc = X.linear(o, 3 * C, L, C, proj_w, C, out.f + off, C, 0))) break;
-      rc = X.resid(out.f + off, x.f + off, L, C, nullptr, 0, L);
-    }
-    return out;
-  }
-
-  // Resample upsample2d / upsample3d (wan2pt1.py:112-143)
-  Act32 upsample(const std::string& n, Act32 x, bool temporal, int tcap_in) {
-    next_block();
-    const int C = x.C;
-    if (temporal) {
-      Stream32& st = stream(n + ".time_conv", 2, tcap_in, x.H, x.W, C);
-      if (!st.primed) {
-        st.primed = true;   // first chunk: "Rep" -- no temporal doubling, history stays zero
-      } else {
-        copy(chunk_of(st, x.T), x.pair, x.pixels() * 2 * C * 2);
-        Act32 y = act(2 * x.T, x.H, x.W, C, true, false);
-        causal_conv(n + ".time_conv", st, x.T, y, 1, nullptr, /*split_time=*/1);
-        x = y;
-      }
-    }
-    bf16* up = take<bf16>(x.pixels() * 4 * 2 * C);
-    launch([&] { return launch_upsample2x_cl_f32(x.f, up, x.T, x.H, x.W, C, s); });
-    Act32 out = act(x.T, 2 * x.H, 2 * x.W, C / 2, true, true);
-    conv(n + ".resample.1", up, x.T, 2 * x.H, 2 * x.W, C, out, 1, 3, 3, 1, 1, 1, 1, 1);
-    return out;
-  }
-
-  // Resample downsample2d / downsample3d (wan2pt1.py:145-159): ZeroPad2d(0,1,0,1) is the TMA's zero fill past the edge
-  Act32 downsample(const std::string& n, const Act32& x, bool temporal, int tcap_out_spatial) {
-    next_block();
-    const int C = x.C, Ho = (x.H + 1 - 3) / 2 + 1, Wo = (x.W + 1 - 3) / 2 + 1;
-    if (!temporal) {
-      Act32 out = act(x.T, Ho, Wo, C, true, true);
-      conv(n + ".resample.1", x.pair, x.T, x.H, x.W, C, out, 1, 3, 3, 1, 2, 2, 0, 0);
-      return out;
-    }
-    Stream32& st = stream(n + ".time_conv", 1, tcap_out_spatial, Ho, Wo, C);
-    Act32 sp;
-    sp.T = x.T; sp.H = Ho; sp.W = Wo; sp.C = C;
-    sp.pair = chunk_of(st, x.T);
-    if (!st.primed) {   // first chunk passes through and becomes the history (:147-150)
-      st.primed = true;
-      sp.f = take<float>(sp.pixels() * C);
-      conv(n + ".resample.1", x.pair, x.T, x.H, x.W, C, sp, 1, 3, 3, 1, 2, 2, 0, 0);
-      push_history(st, x.T);
-      return sp;   // its pair is the chunk, which nothing rewrites before the next chunk
-    }
-    conv(n + ".resample.1", x.pair, x.T, x.H, x.W, C, sp, 1, 3, 3, 1, 2, 2, 0, 0);
-    Act32 out = act((1 + x.T - 3) / 2 + 1, Ho, Wo, C, true, true);
-    conv(n + ".time_conv", st.p, 1 + x.T, Ho, Wo, C, out, 3, 1, 1, 2, 1, 1, 0, 0);
-    push_history(st, x.T);
-    return out;
-  }
-};
-
-// z planar [zc, Tl, h, w] fp32 -> video planar [3, 1+4(Tl-1), 8h, 8w] fp32 (run_decode in fp32)
-int run_decode_fp32(Run32& R, const float* z, float* video, int Tl, int h, int w, int clamp) {
-  const ce_vae_config& c = R.h->cfg;
-  const int top = top_dim(c), zc = c.z_dim, T_px = 1 + 4 * (Tl - 1);
-  bf16* zpair = R.persist.take<bf16>((int64_t)Tl * h * w * 2 * zc);
-  R.launch([&] { return launch_planar_to_pair(z, zc, (size_t)Tl * h * w, zpair, zc, R.s); });
-  std::vector<LayerSpec> layers = decoder_layers(c);
-  int t_out = 0;
-  for (int i = 0; i < Tl && !R.rc; ++i) {
-    R.new_chunk();
-    int cap = 1;
-    Stream32& s1 = R.stream("decoder.conv1", 2, 1, h, w, zc);
-    Act32 x0;
-    x0.T = 1; x0.H = h; x0.W = w; x0.C = zc;
-    x0.pair = R.chunk_of(s1, 1);
-    R.conv("conv2", zpair, Tl, h, w, zc, x0, 1, 1, 1, 1, 1, 1, 0, 0, nullptr, 0, /*t_base=*/i);
-    Act32 x = R.act(1, h, w, top, true, true);
-    R.causal_conv("decoder.conv1", s1, 1, x, 3);
-    x = R.res_block("decoder.middle.0", x, top, cap);
-    x = R.attn_block("decoder.middle.1", x);
-    x = R.res_block("decoder.middle.2", x, top, cap);
-    int idx = 0;
-    for (const LayerSpec& l : layers) {
-      const std::string n = "decoder.upsamples." + std::to_string(idx++);
-      if (l.res) {
-        x = R.res_block(n, x, l.cout, cap);
-      } else {
-        x = R.upsample(n, x, l.mode == 1, cap);
-        if (l.mode == 1) cap *= 2;
-      }
-    }
-    Stream32& sh = R.stream("decoder.head.2", 2, cap, x.H, x.W, x.C);
-    R.rms(x, "decoder.head.0.gamma", nullptr, R.chunk_of(sh, x.T), true);
-    ConvArgs a;
-    a.x = sh.p; a.Tin = sh.hist + x.T; a.Hin = x.H; a.Win = x.W; a.Cin = x.C;
-    a.Cout = 3; a.Cin_pad = round_up(x.C, 64);
-    a.w = R.weights.any<bf16>("decoder.head.2.weight", (int64_t)3 * 27 * a.Cin_pad * 3);
-    ConvF32 f;
-    f.bias = R.weights.any<float>("decoder.head.2.bias", 3);
-    f.y = video;
-    a.kt = 3; a.kh = 3; a.kw = 3; a.ph = 1; a.pw = 1;
-    a.Tout = x.T; a.Hout = x.H; a.Wout = x.W;
-    a.planar_out = 1; a.clamp = clamp; a.planar_T = T_px; a.planar_t0 = t_out;
-    R.launch([&] { return launch_conv3d_cl_f32(a, f, R.s); });
-    R.push_history(sh, x.T);
-    t_out += x.T;
-  }
-  if (!R.rc && t_out != T_px) return fail(CE_ERR_INVALID, "vae decode fp32: produced frame count mismatch");
-  return R.rc;
-}
-
-// video planar [3, T, H, W] fp32 -> moments planar [2 zc, Tl, H/8, W/8] fp32 (run_encode in fp32)
-int run_encode_fp32(Run32& R, const float* video, float* moments, int T, int H, int Wd) {
-  const ce_vae_config& c = R.h->cfg;
-  const int top = top_dim(c), zc = c.z_dim;
-  const int Tl = 1 + (T - 1) / 4, h = H / 8, w = Wd / 8;
-  std::vector<LayerSpec> layers = encoder_layers(c);
-  // the video's pair with the 3 channels padded to 8 (16-byte pixel rows); encoder.conv1 reads its own past frames as the history
-  bf16* vpair = R.persist.take<bf16>((int64_t)T * H * Wd * 2 * 8);
-  R.launch([&] { return launch_planar_to_pair(video, 3, (size_t)T * H * Wd, vpair, 8, R.s); });
-  bf16* enc_out = R.persist.take<bf16>((int64_t)Tl * h * w * 2 * 2 * zc);   // head outputs of every chunk, as the pair
-  int t_lat = 0;
-  for (int f0 = 0; f0 < T && !R.rc;) {
-    const int Tc = f0 == 0 ? 1 : 4;
-    R.new_chunk();
-    int cap = 4;
-    Act32 x = R.act(Tc, H, Wd, c.dim, true, true);
-    R.conv("encoder.conv1", vpair, T, H, Wd, 8, x, 3, 3, 3, 1, 1, 1, 1, 1, nullptr, 0, /*t_base=*/f0 - 2);
-    for (size_t li = 0; li < layers.size(); ++li) {
-      const LayerSpec& l = layers[li];
-      const std::string n = "encoder.downsamples." + std::to_string(li);
-      if (l.res) {
-        x = R.res_block(n, x, l.cout, cap);
-      } else {
-        x = R.downsample(n, x, l.mode == 1, cap);
-        if (l.mode == 1) cap = cap > 1 ? cap / 2 : 1;
-      }
-    }
-    x = R.res_block("encoder.middle.0", x, top, cap);
-    x = R.attn_block("encoder.middle.1", x);
-    x = R.res_block("encoder.middle.2", x, top, cap);
-    Stream32& sh = R.stream("encoder.head.2", 2, cap, x.H, x.W, x.C);
-    R.rms(x, "encoder.head.0.gamma", nullptr, R.chunk_of(sh, x.T), true);
-    if (x.H != h || x.W != w) return fail(CE_ERR_INVALID, "vae encode fp32: spatial size mismatch (H, W must be multiples of 8)");
-    Act32 o;
-    o.T = x.T; o.H = h; o.W = w; o.C = 2 * zc;
-    o.pair = at(enc_out, (size_t)t_lat * h * w * 2 * 2 * zc);
-    R.causal_conv("encoder.head.2", sh, x.T, o, 3);
-    t_lat += x.T;
-    f0 += Tc;
-  }
-  if (!R.rc && t_lat != Tl) return fail(CE_ERR_INVALID, "vae encode fp32: produced frame count mismatch");
-  // conv1 (1x1x1, 2z -> 2z), then planar moments = mean | logvar
-  R.new_chunk();
-  Act32 q = R.act(Tl, h, w, 2 * zc, true, false);
-  R.conv("conv1", enc_out, Tl, h, w, 2 * zc, q, 1, 1, 1, 1, 1, 1, 0, 0);
-  R.launch([&] { return launch_cl_to_planar_f32(q.f, 2 * zc, moments, q.pixels(), 2 * zc, R.s); });
-  return R.rc;
-}
-
-int run_fp32(ce_vae* h, bool decode, const float* in, float* out, int frames, int height, int width, int clamp, void* workspace,
-             int64_t workspace_bytes, int64_t* need_out, void* stream) {
+// One untiled encode or decode, bf16 or fp32, split over the configured ranks.  Every entry refuses in this order: the handle and
+// the geometry; the precision's and the split's refusals; the planning pass, which checks every weight; with need != null, the
+// answer to the workspace query; the device; the arguments; the split's capture and region checks, all before its first barrier;
+// the workspace size.  The launch count restarts at zero.
+int vae_call(ce_vae* h, bool decode, bool fp32, const void* in, void* out, int frames, int height, int width, int clamp, void* workspace,
+             int64_t workspace_bytes, int64_t* need, void* stream) {
   CE_TRY(check_geometry(h, frames, height, width, decode));
-  if (h->sp.world > 1)
+  if (fp32 && h->sp.world > 1)
     return fail(CE_ERR_INVALID, "vae fp32: the VAE split over GPUs (ce_vae_sp_configure) is built for bf16 only; configure world = 1");
-  CE_REQUIRE(!h->w32.empty(), "vae fp32: the handle has no fp32 weights (register them with ce_vae_set_weight_fp32)");
-  Run32 plan(h, nullptr, nullptr, nullptr, nullptr);
-  int rc = decode ? run_decode_fp32(plan, nullptr, nullptr, frames, height, width, 0) : run_encode_fp32(plan, nullptr, nullptr, frames, height, width);
-  if (rc || (rc = plan.weights.rc)) return rc;
-  const int64_t need = plan.workspace_bytes();
-  if (need_out) {
-    *need_out = need;
+  CE_REQUIRE(!fp32 || !h->w32.empty(), "vae fp32: the handle has no fp32 weights (register them with ce_vae_set_weight_fp32)");
+  Run plan(h, fp32, h->sp.rank, h->sp.world);
+  CE_TRY(walk(plan, decode, nullptr, nullptr, frames, height, width, 0));
+  CE_TRY(plan.weights.rc);
+  if (need) {
+    *need = plan.workspace_bytes();
     return CE_OK;
   }
+  const std::string who = fp32 ? "vae fp32: " : "vae: ";
   CE_TRY(check_device());
-  CE_REQUIRE(in && out && workspace, "vae fp32: null argument");
-  CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "vae fp32: workspace must be 256-byte aligned");
-  if (need > workspace_bytes)
-    return fail(CE_ERR_WORKSPACE, "vae fp32: workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(workspace_bytes));
-  uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
-  Run32 R(h, reinterpret_cast<cudaStream_t>(stream), base, base + plan.persist.bytes(), base + plan.persist.bytes() + plan.arena_bytes(0));
+  CE_REQUIRE(in && out && workspace, who + "null argument");
+  CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, who + "workspace must be 256-byte aligned");
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  VaeSpLayout lay;
+  if (plan.split()) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CE_CHECK_CUDA(cudaStreamIsCapturing(s, &cs));
+    CE_REQUIRE(cs == cudaStreamCaptureStatusNone, "vae sequence parallel: the stream is capturing (the split VAE cannot be captured)");
+    const int H = decode ? 8 * height : height, W = decode ? 8 * width : width;
+    CE_TRY(vae_sp_layout(h, H, W, h->sp.world, lay));
+    if (lay.bytes > h->sp.region_bytes)
+      return fail(CE_ERR_WORKSPACE, "vae sequence parallel: a " + std::to_string(H) + " x " + std::to_string(W) + " call needs a peer region of " +
+                                        std::to_string(lay.bytes) + " bytes, the handle was configured with " +
+                                        std::to_string(h->sp.region_bytes) + " (ce_vae_sp_region_bytes)");
+  }
+  const int64_t bytes = plan.workspace_bytes();
+  if (bytes > workspace_bytes)
+    return fail(CE_ERR_WORKSPACE, who + "workspace too small: need " + std::to_string(bytes) + " bytes, got " + std::to_string(workspace_bytes));
+  Run R(h, fp32, h->sp.rank, h->sp.world, s);
+  R.bind(reinterpret_cast<uint8_t*>(workspace), plan);
+  R.lay = &lay;
   h->launches = 0;
-  return decode ? run_decode_fp32(R, in, out, frames, height, width, clamp) : run_encode_fp32(R, in, out, frames, height, width);
+  int rc = walk(R, decode, in, out, frames, height, width, clamp);
+  if (!rc && R.split()) {   // nobody stores into a peer's region (next call) before the peer has read it
+    R.barrier();
+    rc = R.rc;
+  }
+  return rc;
+}
+
+int64_t workspace_query(ce_vae* h, bool decode, bool fp32, int frames, int height, int width) {
+  int64_t need = -1;
+  return vae_call(h, decode, fp32, nullptr, nullptr, frames, height, width, 0, nullptr, 0, &need, nullptr) ? -1 : need;
 }
 
 // ---------------------------------------------------------------------------------------------- tiled encode / decode
@@ -1011,29 +865,6 @@ int run_fp32(ce_vae* h, bool decode, const float* in, float* out, int frames, in
 struct TileSpec {   // pixels, multiples of 8
   int min_h, min_w, stride_h, stride_w;
 };
-
-// One untiled encode or decode of a tile in `ws`, or with ws == null only its workspace need.  The caller resets the launch count.
-int run_tile(ce_vae* h, bool decode, bool fp32, const void* in, void* out, int frames, int H, int W, uint8_t* ws, int64_t* need,
-             cudaStream_t s) {
-  if (fp32) {
-    Run32 plan(h, nullptr, nullptr, nullptr, nullptr);
-    int rc = decode ? run_decode_fp32(plan, nullptr, nullptr, frames, H, W, 0) : run_encode_fp32(plan, nullptr, nullptr, frames, H, W);
-    if (rc || (rc = plan.weights.rc)) return rc;
-    if (need) *need = plan.workspace_bytes();
-    if (!ws) return CE_OK;
-    Run32 R(h, s, ws, ws + plan.persist.bytes(), ws + plan.persist.bytes() + plan.arena_bytes(0));
-    return decode ? run_decode_fp32(R, static_cast<const float*>(in), static_cast<float*>(out), frames, H, W, 0)
-                  : run_encode_fp32(R, static_cast<const float*>(in), static_cast<float*>(out), frames, H, W);
-  }
-  Run plan(h, nullptr, nullptr, nullptr);
-  int rc = decode ? run_decode(plan, nullptr, nullptr, frames, H, W, 0) : run_encode(plan, nullptr, nullptr, frames, H, W);
-  if (rc || (rc = plan.weights.rc)) return rc;
-  if (need) *need = plan.workspace_bytes();
-  if (!ws) return CE_OK;
-  Run R(h, s, ws, ws + plan.persist.bytes());
-  return decode ? run_decode(R, static_cast<const bf16*>(in), static_cast<bf16*>(out), frames, H, W, 0)
-                : run_encode(R, static_cast<const bf16*>(in), static_cast<bf16*>(out), frames, H, W);
-}
 
 // The grid in latent units: tile (i, j) covers latent rows [i sh, i sh + min(mh, h - i sh)) and the matching columns.  A decode tile's
 // input is those latents and its output 8x them in pixels; an encode tile's input is the pixels and its output the latents.
@@ -1094,7 +925,7 @@ int tile_layout(ce_vae* h, const TileGrid& g, uint8_t* base, TileLayout& L) {
     for (int j : {0, g.cols - 1}) {
       int64_t need = 0;
       const int th = g.lat_h(i) * g.in_f, tw = g.lat_w(j) * g.in_f;
-      CE_TRY(run_tile(h, g.decode, g.fp32, nullptr, nullptr, g.Tin, th, tw, nullptr, &need, nullptr));
+      CE_TRY(vae_call(h, g.decode, g.fp32, nullptr, nullptr, g.Tin, th, tw, 0, nullptr, 0, &need, nullptr));
       L.run_bytes = std::max(L.run_bytes, need);
     }
   const int64_t mh = std::min(g.mh, g.h), mw = std::min(g.mw, g.w);
@@ -1142,7 +973,9 @@ int run_tiled(ce_vae* h, bool decode, bool fp32, const void* in, void* out, int 
       p.extent = make_cudaExtent((size_t)iw * g.es, (size_t)ih, (size_t)g.Cin * g.Tin);
       p.kind = cudaMemcpyDeviceToDevice;
       CE_CHECK_CUDA(cudaMemcpy3DAsync(&p, s));
-      CE_TRY(run_tile(h, decode, fp32, L.stage, L.tile, g.Tin, ih, iw, L.run, nullptr, s));
+      const int64_t launched = h->launches;   // vae_call counts the tile's launches from zero
+      CE_TRY(vae_call(h, decode, fp32, L.stage, L.tile, g.Tin, ih, iw, 0, L.run, L.run_bytes, nullptr, stream));
+      h->launches += launched;
       TileBlend b;
       b.fp32 = fp32;
       b.tile = L.tile; b.C = g.Cout; b.T = g.Tout; b.th = lh * g.out_f; b.tw = lw * g.out_f;
@@ -1170,6 +1003,19 @@ int run_tiled(ce_vae* h, bool decode, bool fp32, const void* in, void* out, int 
   return CE_OK;
 }
 
+// The fields of a convolution's arguments that do not depend on its precision (bias, output and residual do).
+ConvArgs conv_args(const ce_conv3d_args& c) {
+  ConvArgs a;
+  a.x = reinterpret_cast<const bf16*>(c.x); a.Tin = c.Tin; a.Hin = c.Hin; a.Win = c.Win; a.Cin = c.Cin;
+  a.w = reinterpret_cast<const bf16*>(c.w); a.Cout = c.Cout; a.Cin_pad = c.Cin_pad;
+  a.kt = c.kt; a.kh = c.kh; a.kw = c.kw; a.st = c.st; a.sh = c.sh; a.sw = c.sw; a.ph = c.ph; a.pw = c.pw;
+  a.t_base = c.t_base;
+  a.Tout = c.Tout; a.Hout = c.Hout; a.Wout = c.Wout;
+  a.split_time = c.split_time;
+  a.planar_out = c.planar_out; a.clamp = c.clamp; a.planar_T = c.planar_T; a.planar_t0 = c.planar_t0;
+  return a;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1193,60 +1039,17 @@ int ce_vae_set_weight(ce_vae* h, const char* name, const void* ptr, int64_t nume
 }
 
 int64_t ce_vae_workspace_bytes(ce_vae* h, int decode, int frames, int height, int width) {
-  if (check_geometry(h, frames, height, width, decode != 0)) return -1;
-  Run plan(h, nullptr, nullptr, nullptr, h->sp.rank, h->sp.world);
-  int rc = decode ? run_decode(plan, nullptr, nullptr, frames, height, width, 0) : run_encode(plan, nullptr, nullptr, frames, height, width);
-  return rc || plan.weights.rc ? -1 : plan.workspace_bytes();
-}
-
-static int run(ce_vae* h, bool decode, const void* in, void* out, int frames, int height, int width, int clamp, void* workspace,
-               int64_t workspace_bytes, void* stream) {
-  int rc = check_device();
-  if (rc) return rc;
-  if ((rc = check_geometry(h, frames, height, width, decode))) return rc;
-  CE_REQUIRE(in && out && workspace, "vae: null argument");
-  CE_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "vae: workspace must be 256-byte aligned");
-  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  VaeSpLayout lay;
-  if (h->sp.world > 1) {   // every refusal of the split comes before its first barrier
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    CE_CHECK_CUDA(cudaStreamIsCapturing(s, &cs));
-    CE_REQUIRE(cs == cudaStreamCaptureStatusNone, "vae sequence parallel: the stream is capturing (the split VAE cannot be captured)");
-    const int H = decode ? 8 * height : height, W = decode ? 8 * width : width;
-    CE_TRY(vae_sp_layout(h, H, W, h->sp.world, lay));
-    if (lay.bytes > h->sp.region_bytes)
-      return fail(CE_ERR_WORKSPACE, "vae sequence parallel: a " + std::to_string(H) + " x " + std::to_string(W) + " call needs a peer region of " +
-                                        std::to_string(lay.bytes) + " bytes, the handle was configured with " +
-                                        std::to_string(h->sp.region_bytes) + " (ce_vae_sp_region_bytes)");
-  }
-  // plan first: sizes of the persistent region (stream buffers) and of the per-chunk scratch
-  Run plan(h, nullptr, nullptr, nullptr, h->sp.rank, h->sp.world);
-  rc = decode ? run_decode(plan, nullptr, nullptr, frames, height, width, 0) : run_encode(plan, nullptr, nullptr, frames, height, width);
-  if (rc || (rc = plan.weights.rc)) return rc;
-  const int64_t need = plan.workspace_bytes();
-  if (need > workspace_bytes)
-    return fail(CE_ERR_WORKSPACE, "vae: workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(workspace_bytes));
-  uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
-  Run R(h, s, base, base + plan.persist.bytes(), h->sp.rank, h->sp.world);
-  R.lay = &lay;
-  h->launches = 0;
-  rc = decode ? run_decode(R, reinterpret_cast<const bf16*>(in), reinterpret_cast<bf16*>(out), frames, height, width, clamp)
-              : run_encode(R, reinterpret_cast<const bf16*>(in), reinterpret_cast<bf16*>(out), frames, height, width);
-  if (!rc && R.split()) {   // nobody stores into a peer's region (next call) before the peer has read it
-    R.barrier();
-    rc = R.rc;
-  }
-  return rc;
+  return workspace_query(h, decode != 0, false, frames, height, width);
 }
 
 int ce_vae_encode(ce_vae* h, const void* video, void* mean, int frames, int height, int width, void* workspace, int64_t workspace_bytes,
                   void* stream) {
-  return run(h, false, video, mean, frames, height, width, 0, workspace, workspace_bytes, stream);
+  return vae_call(h, false, false, video, mean, frames, height, width, 0, workspace, workspace_bytes, nullptr, stream);
 }
 
 int ce_vae_decode(ce_vae* h, const void* z, void* video, int latent_frames, int latent_height, int latent_width, int clamp, void* workspace,
                   int64_t workspace_bytes, void* stream) {
-  return run(h, true, z, video, latent_frames, latent_height, latent_width, clamp, workspace, workspace_bytes, stream);
+  return vae_call(h, true, false, z, video, latent_frames, latent_height, latent_width, clamp, workspace, workspace_bytes, nullptr, stream);
 }
 
 int ce_vae_set_weight_fp32(ce_vae* h, const char* name, const void* ptr, int64_t numel) {
@@ -1255,18 +1058,17 @@ int ce_vae_set_weight_fp32(ce_vae* h, const char* name, const void* ptr, int64_t
 }
 
 int64_t ce_vae_workspace_bytes_fp32(ce_vae* h, int decode, int frames, int height, int width) {
-  int64_t need = -1;
-  return run_fp32(h, decode != 0, nullptr, nullptr, frames, height, width, 0, nullptr, 0, &need, nullptr) ? -1 : need;
+  return workspace_query(h, decode != 0, true, frames, height, width);
 }
 
 int ce_vae_encode_fp32(ce_vae* h, const float* video, float* moments, int frames, int height, int width, void* workspace,
                        int64_t workspace_bytes, void* stream) {
-  return run_fp32(h, false, video, moments, frames, height, width, 0, workspace, workspace_bytes, nullptr, stream);
+  return vae_call(h, false, true, video, moments, frames, height, width, 0, workspace, workspace_bytes, nullptr, stream);
 }
 
 int ce_vae_decode_fp32(ce_vae* h, const float* z, float* video, int latent_frames, int latent_height, int latent_width, int clamp,
                        void* workspace, int64_t workspace_bytes, void* stream) {
-  return run_fp32(h, true, z, video, latent_frames, latent_height, latent_width, clamp, workspace, workspace_bytes, nullptr, stream);
+  return vae_call(h, true, true, z, video, latent_frames, latent_height, latent_width, clamp, workspace, workspace_bytes, nullptr, stream);
 }
 
 int64_t ce_vae_last_launch_count(const ce_vae* h) { return h ? h->launches : 0; }
@@ -1370,15 +1172,10 @@ int ce_conv3d_cl_ex_bf16(const ce_conv3d_args* args, void* stream) {
   int rc = check_device();
   if (rc) return rc;
   CE_REQUIRE(args != nullptr, "ce_conv3d_cl_ex_bf16: null args");
-  ConvArgs a;
-  a.x = reinterpret_cast<const bf16*>(args->x); a.Tin = args->Tin; a.Hin = args->Hin; a.Win = args->Win; a.Cin = args->Cin;
-  a.w = reinterpret_cast<const bf16*>(args->w); a.bias = reinterpret_cast<const bf16*>(args->bias);
-  a.Cout = args->Cout; a.Cin_pad = args->Cin_pad;
-  a.kt = args->kt; a.kh = args->kh; a.kw = args->kw; a.st = args->st; a.sh = args->sh; a.sw = args->sw; a.ph = args->ph; a.pw = args->pw;
-  a.t_base = args->t_base;
-  a.y = reinterpret_cast<bf16*>(args->y); a.Tout = args->Tout; a.Hout = args->Hout; a.Wout = args->Wout;
-  a.resid = reinterpret_cast<const bf16*>(args->resid); a.split_time = args->split_time;
-  a.planar_out = args->planar_out; a.clamp = args->clamp; a.planar_T = args->planar_T; a.planar_t0 = args->planar_t0;
+  ConvArgs a = conv_args(*args);
+  a.bias = reinterpret_cast<const bf16*>(args->bias);
+  a.y = reinterpret_cast<bf16*>(args->y);
+  a.resid = reinterpret_cast<const bf16*>(args->resid);
   return launch_conv3d_cl(a, reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -1386,15 +1183,7 @@ int ce_conv3d_cl_ex_fp32(const ce_conv3d_args* args, void* y_pair, void* stream)
   int rc = check_device();
   if (rc) return rc;
   CE_REQUIRE(args != nullptr, "ce_conv3d_cl_ex_fp32: null args");
-  ConvArgs a;
-  a.x = reinterpret_cast<const bf16*>(args->x); a.Tin = args->Tin; a.Hin = args->Hin; a.Win = args->Win; a.Cin = args->Cin;
-  a.w = reinterpret_cast<const bf16*>(args->w);
-  a.Cout = args->Cout; a.Cin_pad = args->Cin_pad;
-  a.kt = args->kt; a.kh = args->kh; a.kw = args->kw; a.st = args->st; a.sh = args->sh; a.sw = args->sw; a.ph = args->ph; a.pw = args->pw;
-  a.t_base = args->t_base;
-  a.Tout = args->Tout; a.Hout = args->Hout; a.Wout = args->Wout;
-  a.split_time = args->split_time;
-  a.planar_out = args->planar_out; a.clamp = args->clamp; a.planar_T = args->planar_T; a.planar_t0 = args->planar_t0;
+  const ConvArgs a = conv_args(*args);
   ConvF32 f;
   f.bias = reinterpret_cast<const float*>(args->bias); f.resid = reinterpret_cast<const float*>(args->resid);
   f.y = reinterpret_cast<float*>(args->y); f.y_pair = reinterpret_cast<bf16*>(y_pair);

@@ -177,6 +177,29 @@ def test_vae_names_each_missing_or_short_weight(case):
                     assert got > 0, (name, decode, error())
 
 
+
+def test_vae_abi_checks_every_weight_before_a_launch():
+    """ce_vae_encode / ce_vae_decode name a missing or short weight before they ask for the device or look at the arguments (the
+    workspace here is not even 256-byte aligned)."""
+    weights = vae_weights(*VAE_CONFIGS["tiny"])
+    p = FAKE.ptr
+    for name in ("encoder.conv1.weight", "decoder.middle.1.to_qkv.weight", "decoder.head.2.bias", "conv1.weight",
+                 "encoder.downsamples.2.resample.1.weight", "decoder.upsamples.3.time_conv.weight"):
+        decode = not name.startswith("encoder") and name != "conv1.weight"
+        for w in ({**weights, name: weights[name] - 1}, {k: v for k, v in weights.items() if k != name}):
+            with Vae("tiny", w) as v:
+                rc = (v.lib.ce_vae_decode(v.h, p, p, 2, 4, 6, 0, p, 1 << 40, None) if decode else
+                      v.lib.ce_vae_encode(v.h, p, p, 5, 32, 48, p, 1 << 40, None))
+                assert rc == CE_ERR_MISSING_WEIGHT and names(name), (name, rc, error())
+
+
+@no_device
+def test_vae_abi_complete_set_reaches_the_device_check():
+    p = FAKE.ptr
+    with Vae("tiny", vae_weights(*VAE_CONFIGS["tiny"])) as v:
+        assert v.lib.ce_vae_decode(v.h, p, p, 2, 4, 6, 0, p, 1 << 40, None) == CE_ERR_NO_DEVICE
+        assert v.lib.ce_vae_encode(v.h, p, p, 5, 32, 48, p, 1 << 40, None) == CE_ERR_NO_DEVICE
+
 # ------------------------------------------------------------------------------------------------------------------ encoders
 UMT5 = dict(kind=0, vocab_size=4096, d_model=512, d_kv=64, d_ff=1024, num_layers=3, num_heads=8, eps=1e-6)
 CLIP = dict(kind=1, d_model=256, d_kv=64, d_ff=512, num_layers=3, num_heads=4, eps=1e-5, image_size=56, patch_size=14, hidden_act=0)
