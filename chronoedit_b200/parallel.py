@@ -140,14 +140,14 @@ def _configure_peer_regions(obj, entry: str, rank: int, region_ptrs: Sequence[in
     setattr(obj, attr, dict(state, rank=rank, world=world, bytes=region_bytes))
 
 
-def _release_peer_regions(obj, entry: str, attr: str = "_sp_state") -> None:
+def _release_peer_regions(obj, entry: str, attr: str = "_sp_state") -> bool:
     """Switches obj's handle back to one GPU (C configure `entry`, world 1), closes the opened peer mappings of the state obj.<attr>
-    and frees the own region once no rank of the state's group still maps it."""
+    and frees the own region once no rank of the state's group still maps it.  Returns False when obj had no such split on."""
     from . import _lib
 
     st = getattr(obj, attr, None)
     if not st:
-        return
+        return False
     L = _lib.lib()
     torch.cuda.synchronize(obj.device)
     getattr(L, entry)(obj._handle, 0, 1, None, 0)
@@ -158,6 +158,7 @@ def _release_peer_regions(obj, entry: str, attr: str = "_sp_state") -> None:
             dist.barrier(group=st.get("group"))
         L.ce_ipc_free(st["own"])
     setattr(obj, attr, None)
+    return True
 
 
 def _enable_split(obj, who: str, group, disable, region_bytes, configure) -> int:
@@ -202,8 +203,7 @@ def sp_region_bytes(model, batch: int, frames: int, height: int, width: int, wor
     from . import _lib
     from ._lib import CEError
 
-    if not model._packed:
-        model.pack_weights()
+    model._ensure_packed()
     n = _lib.lib().ce_dit_sp_region_bytes(model._handle, batch, frames, height, width, world)
     if n < 0:
         raise CEError(f"sequence parallel: tokens and heads must be divisible by the world size {world} (2 to 8)")
@@ -215,10 +215,9 @@ def configure_sequence_parallel(model, rank: int, region_ptrs: Sequence[int], re
     (ce_dit_sp_configure) and switch the model into sequence-parallel mode.  `state` is kept as `model._sp_state` (with "world" and
     "bytes" added) and holds whatever disable_sequence_parallel releases: the own region under "own" (freed with ce_ipc_free, after a
     barrier on the process group under "group") and the opened peer mappings under "opened" (closed with ce_ipc_close)."""
-    if not model._packed:
-        model.pack_weights()
+    model._ensure_packed()
     _configure_peer_regions(model, "ce_dit_sp_configure", rank, region_ptrs, region_bytes, state)
-    model._graphs = {}
+    model._invalidate("layout")
 
 
 def disable_sequence_parallel(model) -> None:
@@ -250,7 +249,7 @@ def enable_cfg_parallel(model, batch: int, frames: int, height: int, width: int,
     """
     from ._lib import CEError
 
-    if getattr(model, "_cp_state", None):   # before any region is allocated; ce_dit_bp_configure refuses it too
+    if dist.is_initialized() and model._cp_state:   # before any region is allocated; ce_dit_bp_configure refuses it too
         raise CEError("enable_cfg_parallel: the call-pair split (enable_cfg_parallel_calls) is on: the two CFG splits are exclusive, "
                       "disable it first")
     return _enable_split(model, "enable_cfg_parallel", group, disable_cfg_parallel,
@@ -274,14 +273,13 @@ def configure_cfg_parallel(model, rank: int, region_ptrs: Sequence[int], region_
     "bytes" added) and holds what disable_cfg_parallel releases, as for configure_sequence_parallel.  The token split's state
     (`model._sp_state`) is not touched."""
     _configure_peer_regions(model, "ce_dit_bp_configure", rank, region_ptrs, region_bytes, state, "_bp_state")
-    _drop_sample_caches(model)
+    model._invalidate("results")   # the context cache's K/V and the TeaCache states hold the old share of samples
 
 
 def disable_cfg_parallel(model) -> None:
     """Back to computing every sample of a call on this GPU; releases what enable_cfg_parallel allocated and opened."""
-    if getattr(model, "_bp_state", None):
-        _release_peer_regions(model, "ce_dit_bp_configure", "_bp_state")
-        _drop_sample_caches(model)
+    if _release_peer_regions(model, "ce_dit_bp_configure", "_bp_state"):
+        model._invalidate("results")
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -318,7 +316,7 @@ def enable_cfg_parallel_calls(model, batch: int, frames: int, height: int, width
     """
     from ._lib import CEError
 
-    if getattr(model, "_bp_state", None):   # before any region is allocated; ce_dit_cp_configure refuses it too
+    if dist.is_initialized() and model._bp_state:   # before any region is allocated; ce_dit_cp_configure refuses it too
         raise CEError("enable_cfg_parallel_calls: the batch split (enable_cfg_parallel) is on: the two CFG splits are exclusive, "
                       "disable it first")
 
@@ -349,29 +347,21 @@ def configure_cfg_parallel_calls(model, rank: int, region_ptrs: Sequence[int], r
     pair."""
     _configure_peer_regions(model, "ce_dit_cp_configure", rank, region_ptrs, region_bytes, state, "_cp_state")
     model._cp_pair = None
-    _drop_sample_caches(model)
+    model._invalidate("results")
 
 
 def disable_cfg_parallel_calls(model) -> None:
     """Back to computing every call on this GPU; releases what enable_cfg_parallel_calls allocated and opened.  A pair whose second
     call never came is dropped with a warning."""
-    if getattr(model, "_cp_state", None):
-        if getattr(model, "_cp_pair", None) is not None:
-            import warnings
+    if not _release_peer_regions(model, "ce_dit_cp_configure", "_cp_state"):
+        return
+    if model._cp_pair is not None:
+        import warnings
 
-            warnings.warn("disable_cfg_parallel_calls: the first call of a CFG pair is still open (its second call never came); "
-                          "dropping it")
-        model._cp_pair = None
-        _release_peer_regions(model, "ce_dit_cp_configure", "_cp_state")
-        _drop_sample_caches(model)
-
-
-def _drop_sample_caches(model) -> None:
-    """What a model keeps per sample of a call (the context cache's K/V, the TeaCache states) holds the samples of the old share, and
-    a captured graph has the old launches."""
-    model._graphs = {}
-    model.clear_context_cache()
-    model._drop_teacache_states()
+        warnings.warn("disable_cfg_parallel_calls: the first call of a CFG pair is still open (its second call never came); "
+                      "dropping it")
+    model._cp_pair = None
+    model._invalidate("results")
 
 
 # ----------------------------------------------------------------------------------------------------------------------

@@ -9,6 +9,7 @@ owns the memory and the stream.  There is no PyTorch fallback path.
 """
 from __future__ import annotations
 
+import contextlib
 import json
 import math
 import os
@@ -73,6 +74,24 @@ def fp8_attention_key_order() -> torch.Tensor:
     `stored[..., 32 g + p] = vt[..., 32 g + order[p]]`."""
     p = torch.arange(32)
     return 16 * (p // 16) + 8 * ((p % 4) // 2) + 2 * ((p % 16) // 4) + p % 2
+
+
+def _cond_entry(entries: list, slots: int, txt_in, img_in, new) -> Tuple[Dict[str, Any], bool]:
+    """(entry, hit) of the LRU cache, least recently used first, that the context cache and the TeaCache states share.  A hit needs
+    the SAME conditioning tensor objects the entry holds, at the same in-place versions: the unchanged pipeline passes the same
+    `prompt_embeds` / `negative_prompt_embeds` / `image_embeds` at every step (pipeline_chronoedit.py:715-735).  A miss appends
+    `new(evicted)` plus the key; `evicted` (the LRU entry when all `slots` are taken, else None) is dropped once `new` returned."""
+    ver = lambda t: None if t is None else t._version
+    for i, e in enumerate(entries):
+        if e["txt"] is txt_in and e["img"] is img_in and e["txt_v"] == ver(txt_in) and e["img_v"] == ver(img_in):
+            entries.append(entries.pop(i))   # by position, since list.remove would compare the entries' tensors with ==
+            return e, True
+    full = len(entries) >= slots
+    e = dict(new(entries[0] if full else None), txt=txt_in, img=img_in, txt_v=ver(txt_in), img_v=ver(img_in))
+    if full:
+        del entries[0]
+    entries.append(e)
+    return e, False
 
 
 @dataclass
@@ -257,6 +276,11 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._tc_next_slot = 0
         self._tc_probe: Dict[str, Any] = {}
         self._tc_records: list = []
+        # the splits over GPUs, set by chronoedit_b200.parallel: the token split, the batch split, the call pair and its open first call
+        self._sp_state: Optional[Dict[str, Any]] = None
+        self._bp_state: Optional[Dict[str, Any]] = None
+        self._cp_state: Optional[Dict[str, Any]] = None
+        self._cp_pair: Optional[Dict[str, Any]] = None
 
     # ------------------------------------------------------------------------------------------ plumbing
     @property
@@ -267,13 +291,27 @@ class ChronoEditTransformer3DModel(nn.Module):
     def device(self) -> torch.device:
         return self.patch_embedding.weight.device
 
+    def _invalidate(self, kind: str) -> None:
+        """Drop what a change of `kind` makes stale.
+        "results": the weights, the adapters or this rank's share of a call's samples changed, so what was computed from them
+            is stale: the context cache's K/V, the TeaCache states (their residuals) and the captured graphs.
+        "layout": the launch sequence or its scratch changed: the workspaces and the captured graphs (which hold their addresses).
+        "storage": the parameters are new tensors, maybe on another device, so the fused device buffers must be rebuilt (`_packed`)
+            and the TeaCache probe's buffers reallocated; drops both of the above."""
+        assert kind in ("results", "layout", "storage"), kind
+        if kind == "storage":
+            self._packed = False
+            self._tc_probe = {}
+        if kind != "layout":
+            self._ctx_cache = []
+            self._tc_states = []
+        if kind != "results":
+            self._workspaces = {}
+        self._graphs = {}
+
     def _apply(self, fn, *a, **k):
         # .to()/.cuda()/.cpu() re-allocate parameters: the fused device buffers must be rebuilt
-        self._packed = False
-        self._graphs = {}
-        self._ctx_cache = []
-        self._workspaces = {}
-        self._drop_teacache_states()
+        self._invalidate("storage")
         if self._lora_key is not None:   # the packed LoRA tables are rebuilt on the new device (or cleared from the handle)
             self._lora_key = ("moved",)
         self._lora_tables = {}
@@ -283,13 +321,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         if self._fp8:
             raise CEError("load_state_dict after enable_fp8(): the FP8 block weights are quantized from the bf16 ones; load the "
                           "checkpoint (and fuse any LoRA) first, then call enable_fp8()")
-        # new weights under the same prompt tensors: the cached cross-attention K/V and any captured graph are stale; with
-        # assign=True the parameters are new tensors, so the fused device buffers must be rebuilt as well
-        self._ctx_cache = []
-        self._graphs = {}
-        self._drop_teacache_states()   # the stored residuals came from the old weights
-        if assign:
-            self._packed = False
+        self._invalidate("storage" if assign else "results")
         return super().load_state_dict(state_dict, strict=strict, assign=assign)
 
     def __del__(self):
@@ -337,12 +369,8 @@ class ChronoEditTransformer3DModel(nn.Module):
                 holder.register_buffer("weight_fp8", q)
                 holder.register_buffer("weight_scale", s)
         self._fp8 = True
-        self._packed = False
         self._pack_keepalive = {}   # the fused bf16 QKV buffers
-        self._graphs = {}
-        self._ctx_cache = []
-        self._workspaces = {}
-        self._drop_teacache_states()
+        self._invalidate("storage")
 
     @property
     def fp8_attention_enabled(self) -> bool:
@@ -359,8 +387,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         if self._handle is not None:
             check(_lib.lib().ce_dit_set_attention_fp8(self._handle, int(enabled)))
         self._fp8_attention = enabled
-        self._graphs = {}
-        self._workspaces = {}
+        self._invalidate("layout")
 
     # ------------------------------------------------------------------------------------------ fp32 validation mode
     @torch.no_grad()
@@ -394,13 +421,10 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._refuse_cp("forward_fp32")
         if self._lora_active():
             raise CEError("forward_fp32 is not built for run-time LoRA (set_adapters): call disable_lora() first")
+        self._check_inputs(hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image)
         dev = self.device
         B, C, T, H, W = hidden_states.shape
-        x = hidden_states.to(device=dev, dtype=torch.float32).contiguous()
-        t = timestep.to(device=dev, dtype=torch.float32).reshape(-1)
-        t = (t.expand(B) if t.numel() == 1 and B > 1 else t).contiguous()
-        txt = encoder_hidden_states.to(device=dev, dtype=torch.float32).contiguous()
-        img = None if encoder_hidden_states_image is None else encoder_hidden_states_image.to(device=dev, dtype=torch.float32).contiguous()
+        x, t, txt, img = self._to_device(torch.float32, hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image)
         L = _lib.lib()
         Lt = txt.shape[1]
         n = L.ce_dit_fp32_workspace_bytes(self._handle, B, T, H, W, Lt)
@@ -483,21 +507,9 @@ class ChronoEditTransformer3DModel(nn.Module):
                 reg(n[: -len("_fp8")] if n.endswith(".weight_fp8") else n, b)
         check(L.ce_dit_weights_complete(self._handle))
         self._pack_keepalive = keep
+        if self._packed:   # a re-pack: what was computed from the replaced tensors is stale (an unpacked model has nothing cached)
+            self._invalidate("results")
         self._packed = True
-        self._ctx_cache = []   # cached K/V were projected with the previous weights
-        self._graphs = {}
-
-    def _workspace(self, B, T, H, W, Lt) -> torch.Tensor:
-        key = (B, T, H, W, Lt, str(self.device))
-        ws = self._workspaces.get(key)
-        if ws is None:
-            n = _lib.lib().ce_dit_workspace_bytes(self._handle, B, T, H, W, Lt)
-            if n < 0:
-                check(-1)
-            self._workspaces.clear()  # one live geometry at a time keeps the footprint bounded
-            ws = torch.empty(n, dtype=torch.uint8, device=self.device)
-            self._workspaces[key] = ws
-        return ws
 
     # ------------------------------------------------------------------------------------------ forward
     @torch.no_grad()
@@ -521,40 +533,21 @@ class ChronoEditTransformer3DModel(nn.Module):
 
             warnings.warn("Passing `scale` via `attention_kwargs` when not using the PEFT backend is ineffective "
                           "(LoRA must be fused with fuse_lora(lora_scale=...) before inference).")
-        if self._lora_active() and getattr(self, "_sp_state", None):
-            raise CEError("run-time LoRA (set_adapters) is not built for sequence parallelism: call disable_lora() or disable the "
-                          "sequence-parallel mode first")
+        self._refuse_token_split(lora=self._lora_active())
         dev = self.device
-        if hidden_states.dim() != 5:
-            raise CEError("hidden_states must be [B, C, T, H, W]")
+        self._check_inputs(hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image)
         B, C, T, H, W = hidden_states.shape
-        if C != self.config.in_channels:
-            raise CEError(f"hidden_states has {C} channels, model expects {self.config.in_channels}")
-        if (encoder_hidden_states_image is None) != (self.config.image_dim is None):
-            raise CEError("encoder_hidden_states_image must be passed iff the model was built with image_dim")
         if self._teacache is not None:
             if return_block0 or capture_layers:
                 raise CEError("return_block0 / capture_layers are not available while TeaCache is on (a skipped step runs no "
                               "blocks): call disable_teacache() first")
-            if getattr(self, "_sp_state", None):
-                raise CEError("TeaCache is not built for sequence parallelism: disable one of the two")
-        cp = getattr(self, "_cp_state", None)
+            self._refuse_token_split(teacache=True)
+        cp = self._cp_state
         role, pair = self._cp_role(hidden_states, timestep, encoder_hidden_states_image, return_block0, capture_layers) if cp else (0, None)
         computes = not cp or role == cp["rank"]
         self._lora_scale = lora_scale
         self._lora_sync(lora_scale)
-        x = hidden_states.to(device=dev, dtype=torch.bfloat16).contiguous()
-        t = timestep.to(device=dev, dtype=torch.float32).reshape(-1)
-        if t.numel() == 1 and B > 1:
-            t = t.expand(B)
-        t = t.contiguous()
-        txt = encoder_hidden_states.to(device=dev, dtype=torch.bfloat16).contiguous()
-        img = None
-        if encoder_hidden_states_image is not None:
-            img = encoder_hidden_states_image.to(device=dev, dtype=torch.bfloat16).contiguous()
-            if img.shape[1] != 257:
-                raise CEError("encoder_hidden_states_image must have 257 tokens (transformer_chronoedit.py:53)")
-        Lt = txt.shape[1]
+        x, t, txt, img = self._to_device(torch.bfloat16, hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image)
         out = torch.empty(B, self.config.out_channels, T, H, W, dtype=torch.bfloat16, device=dev)
         L_tok = T * (H // 2) * (W // 2)
         Dm = self.config.num_attention_heads * self.config.attention_head_dim
@@ -571,8 +564,8 @@ class ChronoEditTransformer3DModel(nn.Module):
             pass
         elif self._teacache is not None:
             self._teacache_forward(x, t, txt, img, out, encoder_hidden_states, encoder_hidden_states_image)
-        elif (self.use_cuda_graph and not caps and b0 is None and not getattr(self, "_sp_state", None)
-              and not getattr(self, "_bp_state", None) and not cp and not self._lora_active()):
+        elif (self.use_cuda_graph and not caps and b0 is None and not self._sp_state and not self._bp_state and not cp
+              and not self._lora_active()):
             out = self._graphed_forward(x, t, txt, img, encoder_hidden_states, encoder_hidden_states_image)
         else:
             self._native_forward(x, t, txt, img, out, b0, caps, encoder_hidden_states, encoder_hidden_states_image)
@@ -588,14 +581,63 @@ class ChronoEditTransformer3DModel(nn.Module):
         """(first, count) of the samples of a B-sample call this handle computes: its share under the batch split
         (parallel.enable_cfg_parallel), else all of them.  The workspace, the context cache and the TeaCache buffers are sized by
         `count`.  A batch the ranks do not divide is left whole here, for the forward to refuse."""
-        st = getattr(self, "_bp_state", None)
+        st = self._bp_state
         if not st or B % st["world"]:
             return 0, B
         n = B // st["world"]
         return st["rank"] * n, n
 
+    def _check_inputs(self, hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image, host: bool = False,
+                      out: Optional[torch.Tensor] = None) -> None:
+        """Refuse inputs whose extents disagree with the model, from tensor metadata alone.  The C library works out every extent
+        from the config and (B, T, H, W, Lt), so it cannot see a tensor that is too small.  With `host` (forward_host, whose C call
+        copies the inputs and the sample itself) the tensors must also be on the CPU: the timestep of any dtype, the others
+        contiguous bf16, and `out`, when given, of the sample's shape."""
+        c = self.config
+        if hidden_states.dim() != 5:
+            raise CEError("hidden_states must be [B, C, T, H, W]")
+        B, C, T, H, W = hidden_states.shape
+        if C != c.in_channels:
+            raise CEError(f"hidden_states has {C} channels, model expects {c.in_channels}")
+        img = encoder_hidden_states_image
+        if (img is None) != (c.image_dim is None):
+            raise CEError("encoder_hidden_states_image must be passed iff the model was built with image_dim")
+        if timestep.numel() not in (1, B):
+            raise CEError(f"timestep has {timestep.numel()} elements, expected 1 or B = {B}")
+        txt = encoder_hidden_states
+        for name, tns, dim in (("encoder_hidden_states", txt, c.text_dim), ("encoder_hidden_states_image", img, c.image_dim)):
+            if tns is not None and (tns.dim() != 3 or tns.shape[0] != B or tns.shape[2] != dim):
+                raise CEError(f"{name} must be [B, tokens, {dim}] with B = {B}, got {list(tns.shape)}")
+        if img is not None and img.shape[1] != 257:
+            raise CEError("encoder_hidden_states_image must have 257 tokens (transformer_chronoedit.py:53)")
+        if not host:
+            return
+        if timestep.device.type != "cpu":
+            raise CEError(f"forward_host expects a CPU timestep, got one on {timestep.device}")
+        for name, tns in (("hidden_states", hidden_states), ("encoder_hidden_states", txt), ("encoder_hidden_states_image", img),
+                          ("out", out)):
+            if tns is not None and (tns.device.type != "cpu" or tns.dtype != torch.bfloat16 or not tns.is_contiguous()):
+                raise CEError(f"forward_host expects contiguous CPU bf16 tensors: {name} is {tns.dtype} on {tns.device}"
+                              + ("" if tns.is_contiguous() else ", not contiguous"))
+        if out is not None and tuple(out.shape) != (B, c.out_channels, T, H, W):
+            raise CEError(f"out must be [B, out_channels, T, H, W] = {[B, c.out_channels, T, H, W]}, got {list(out.shape)}")
+
+    def _to_device(self, dtype, hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image):
+        """The checked inputs as the C forward reads them: contiguous on the module's device in `dtype`, the timestep fp32 [B]."""
+        cast = lambda a: None if a is None else a.to(device=self.device, dtype=dtype).contiguous()
+        t = timestep.to(device=self.device, dtype=torch.float32).reshape(-1).expand(hidden_states.shape[0]).contiguous()
+        return cast(hidden_states), t, cast(encoder_hidden_states), cast(encoder_hidden_states_image)
+
+    def _refuse_token_split(self, lora: bool = False, teacache: bool = False) -> None:
+        """Under the token split (parallel.enable_sequence_parallel): refuse run-time LoRA when `lora`, TeaCache when `teacache`."""
+        if self._sp_state and lora:
+            raise CEError("run-time LoRA (set_adapters) is not built for sequence parallelism: call disable_lora() or disable the "
+                          "sequence-parallel mode first")
+        if self._sp_state and teacache:
+            raise CEError("TeaCache is not built for sequence parallelism: disable one of the two")
+
     def _refuse_cp(self, who: str) -> None:
-        if getattr(self, "_cp_state", None):
+        if self._cp_state:
             raise CEError(f"{who} is not available with the call-pair split (parallel.enable_cfg_parallel_calls pairs the calls of "
                           "forward()): call parallel.disable_cfg_parallel_calls first")
 
@@ -611,7 +653,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         if self.device.type == "cuda" and torch.cuda.is_current_stream_capturing():
             raise CEError("call-pair split: the stream is capturing (the exchange's barrier epoch advances every pair, so it cannot "
                           "be replayed from a graph)")
-        pair = getattr(self, "_cp_pair", None)
+        pair = self._cp_pair
         if pair is None:
             return 0, None
         self._cp_pair = None
@@ -646,30 +688,55 @@ class ChronoEditTransformer3DModel(nn.Module):
         with torch.cuda.device(self.device):
             check(_lib.lib().ce_dit_cp_exchange(self._ensure_handle(), ptr(own), ptr(other), B, T, H, W, current_stream()))
 
+    def _ensure_packed(self) -> None:
+        if not self._packed:
+            self.pack_weights()
+
+    @contextlib.contextmanager
+    def _pre_launch(self, shape, Lt: int, cond=None):
+        """Around every native forward's C call: packs the weights if needed and yields this rank's workspace for a forward of
+        `shape` (B, C, T, H, W) with Lt text tokens and the context-cache slot (buffer, reuse flag) of `cond` = (txt_in, img_in, txt,
+        img), (None, 0) without.  A slot the call was to fill is dropped if the body raises: it is unfilled or only partly filled."""
+        self._ensure_packed()
+        B, _, T, H, W = shape
+        key = (self._local_samples(B)[1], T, H, W, Lt, str(self.device))
+        ws = self._workspaces.get(key)
+        if ws is None:
+            n = _lib.lib().ce_dit_workspace_bytes(self._handle, *key[:5])
+            if n < 0:
+                check(-1)
+            # one live geometry at a time keeps the footprint bounded; graphs captured on the old workspace go with it
+            self._invalidate("layout")
+            ws = self._workspaces[key] = torch.empty(n, dtype=torch.uint8, device=self.device)
+        ctx_buf, ctx_reuse = self._context_slot(*cond) if cond is not None and self.cache_context else (None, 0)
+        try:
+            yield ws, ctx_buf, ctx_reuse
+        except BaseException:
+            self._drop_unfilled(ctx_buf, ctx_reuse)
+            raise
+
+    def _forward_ex(self, x, t, txt, img, out, b0, ws, ctx_buf, ctx_reuse) -> None:
+        """ce_dit_forward_ex on the current stream, the one call of it the eager forward and the graph capture share."""
+        B, _, T, H, W = x.shape
+        with torch.cuda.device(self.device):
+            self._check_forward(_lib.lib().ce_dit_forward_ex(
+                self._handle, ptr(x), ptr(t), ptr(txt), ptr(img), ptr(out), B, T, H, W, txt.shape[1], ptr(ws), ws.numel(), ptr(b0),
+                ptr(ctx_buf), ctx_buf.numel() if ctx_buf is not None else 0, ctx_reuse, current_stream()), ctx_buf, ctx_reuse)
+
     def _native_forward(self, x, t, txt, img, out, b0, caps, txt_in, img_in) -> None:
         """The one place the DiT forward reaches the C ABI (ce_dit_forward_ex).  x [B,C,T,H,W] bf16, t [B] fp32, txt / img bf16,
         all contiguous on the module's device; `out` (and the optional block captures) are written in place."""
-        if not self._packed:
-            self.pack_weights()
-        B, _, T, H, W = x.shape
-        Lt = txt.shape[1]
         L = _lib.lib()
-        ws = self._workspace(self._local_samples(B)[1], T, H, W, Lt)
-        if caps:
-            lay = (_lib.c_int32 * len(caps))(*caps.keys())
-            dst = (_lib.c_void_p * len(caps))(*[v.data_ptr() for v in caps.values()])
-            check(L.ce_dit_set_capture(self._handle, lay, dst, len(caps)))
-        ctx_buf, ctx_reuse = (None, 0)
-        if self.cache_context:
-            ctx_buf, ctx_reuse = self._context_slot(txt_in, img_in, txt, img)
-        try:
-            with torch.cuda.device(self.device):
-                self._check_forward(L.ce_dit_forward_ex(self._handle, ptr(x), ptr(t), ptr(txt), ptr(img), ptr(out), B, T, H, W, Lt, ptr(ws),
-                                                        ws.numel(), ptr(b0), ptr(ctx_buf), ctx_buf.numel() if ctx_buf is not None else 0,
-                                                        ctx_reuse, current_stream()), ctx_buf, ctx_reuse)
-        finally:
+        with self._pre_launch(x.shape, txt.shape[1], (txt_in, img_in, txt, img)) as (ws, ctx_buf, ctx_reuse):
             if caps:
-                check(L.ce_dit_set_capture(self._handle, None, None, 0))
+                lay = (_lib.c_int32 * len(caps))(*caps.keys())
+                dst = (_lib.c_void_p * len(caps))(*[v.data_ptr() for v in caps.values()])
+                check(L.ce_dit_set_capture(self._handle, lay, dst, len(caps)))
+            try:
+                self._forward_ex(x, t, txt, img, out, b0, ws, ctx_buf, ctx_reuse)
+            finally:
+                if caps:
+                    check(L.ce_dit_set_capture(self._handle, None, None, 0))
 
     def _graphed_forward(self, x, t, txt, img, txt_in, img_in) -> torch.Tensor:
         """Replay (or, the second time a configuration is seen, capture) the forward as one CUDA graph.  A configuration = geometry +
@@ -677,80 +744,59 @@ class ChronoEditTransformer3DModel(nn.Module):
         runs eagerly: it packs weights, builds RoPE tables, opts kernels into their shared-memory sizes and fills the context cache
         -- none of which may happen during capture.  Inputs are copied into fixed staging tensors; the returned sample is a fresh
         tensor (a copy out of the graph's fixed output buffer)."""
-        if not self._packed:
-            self.pack_weights()
-        ctx_buf, ctx_reuse = (None, 0)
-        if self.cache_context:
-            ctx_buf, ctx_reuse = self._context_slot(txt_in, img_in, txt, img)
-        key = (tuple(x.shape), tuple(txt.shape), None if img is None else tuple(img.shape), None if ctx_buf is None else ctx_buf.data_ptr())
-        L = _lib.lib()
-        B, _, T, H, W = x.shape
-        Lt = txt.shape[1]
-
-        def launch(xs, ts, txts, imgs, outs, reuse):
-            ws = self._workspace(B, T, H, W, Lt)
-            with torch.cuda.device(self.device):
-                self._check_forward(L.ce_dit_forward_ex(self._handle, ptr(xs), ptr(ts), ptr(txts), ptr(imgs), ptr(outs), B, T, H, W, Lt,
-                                                        ptr(ws), ws.numel(), None, ptr(ctx_buf),
-                                                        ctx_buf.numel() if ctx_buf is not None else 0, reuse, current_stream()), ctx_buf, reuse)
-
-        g = self._graphs.get(key)
-        if g is None or (self.cache_context and not ctx_reuse):
-            # eager: first sight of this configuration, or the context has to be (re)computed into the slot
-            out = torch.empty(B, self.config.out_channels, T, H, W, dtype=torch.bfloat16, device=self.device)
-            launch(x, t, txt, img, out, ctx_reuse)
-            if g is None:
-                self._graphs[key] = {"graph": None}
-            return out
-        if g["graph"] is None:   # second sight: capture (with ctx_reuse = 1 when the context cache is on)
-            st = {"x": x.clone(), "t": t.clone(), "txt": txt.clone(), "img": None if img is None else img.clone(),
-                  "out": torch.empty(B, self.config.out_channels, T, H, W, dtype=torch.bfloat16, device=self.device)}
-            torch.cuda.synchronize(self.device)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                launch(st["x"], st["t"], st["txt"], st["img"], st["out"], 1 if self.cache_context else 0)
-            g.update(st)
-            g["graph"] = graph
-        g["x"].copy_(x)
-        g["t"].copy_(t)
-        if not self.cache_context:   # with the context cache the captured launches do not read the encoder states at all
-            g["txt"].copy_(txt)
-            if img is not None:
-                g["img"].copy_(img)
-        g["graph"].replay()
-        return g["out"].clone()
+        with self._pre_launch(x.shape, txt.shape[1], (txt_in, img_in, txt, img)) as (ws, ctx_buf, ctx_reuse):
+            key = (tuple(x.shape), tuple(txt.shape), None if img is None else tuple(img.shape),
+                   None if ctx_buf is None else ctx_buf.data_ptr())
+            B, _, T, H, W = x.shape
+            g = self._graphs.get(key)
+            if g is None or (self.cache_context and not ctx_reuse):
+                # eager: first sight of this configuration, or the context has to be (re)computed into the slot
+                out = torch.empty(B, self.config.out_channels, T, H, W, dtype=torch.bfloat16, device=self.device)
+                self._forward_ex(x, t, txt, img, out, None, ws, ctx_buf, ctx_reuse)
+                if g is None:
+                    self._graphs[key] = {"graph": None}
+                return out
+            if g["graph"] is None:   # second sight: capture (with ctx_reuse = 1 when the context cache is on)
+                st = {"x": x.clone(), "t": t.clone(), "txt": txt.clone(), "img": None if img is None else img.clone(),
+                      "out": torch.empty(B, self.config.out_channels, T, H, W, dtype=torch.bfloat16, device=self.device)}
+                torch.cuda.synchronize(self.device)
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    self._forward_ex(st["x"], st["t"], st["txt"], st["img"], st["out"], None, ws, ctx_buf, ctx_reuse)
+                g.update(st)
+                g["graph"] = graph
+            g["x"].copy_(x)
+            g["t"].copy_(t)
+            if not self.cache_context:   # with the context cache the captured launches do not read the encoder states at all
+                g["txt"].copy_(txt)
+                if img is not None:
+                    g["img"].copy_(img)
+            g["graph"].replay()
+            return g["out"].clone()
 
     def _context_slot(self, txt_in, img_in, txt, img):
-        """(cache buffer, reuse flag) for these encoder states.  A hit requires the SAME tensor objects the cache entry was
-        filled from (the entry holds references, so their storage cannot have been recycled) at the same in-place version
-        counter -- the unchanged pipeline passes the same `prompt_embeds` / `negative_prompt_embeds` / `image_embeds` objects at
-        every step (pipeline_chronoedit.py:715-735)."""
-        ver = lambda t: None if t is None else t._version
-        for i, e in enumerate(self._ctx_cache):
-            if e["txt"] is txt_in and e["img"] is img_in and e["txt_v"] == ver(txt_in) and e["img_v"] == ver(img_in):
-                # most recently used last; by position, since list.remove would compare the entries' tensors with ==
-                self._ctx_cache.append(self._ctx_cache.pop(i))
-                return e["buf"], 1
-        B, Lt = self._local_samples(txt.shape[0])[1], txt.shape[1]
-        n = _lib.lib().ce_dit_context_cache_bytes(self._handle, B, Lt)
-        if n < 0:
-            check(-1)
-        buf = None
-        if len(self._ctx_cache) >= self._ctx_slots:
-            old = self._ctx_cache.pop(0)
-            if old["buf"].numel() >= n and old["buf"].device == self.device:
-                buf = old["buf"]
-        if buf is None:
-            buf = torch.empty(n, dtype=torch.uint8, device=self.device)
-        self._ctx_cache.append(dict(txt=txt_in, img=img_in, txt_v=ver(txt_in), img_v=ver(img_in), buf=buf))
-        return buf, 0
+        """(cache buffer, reuse flag) for these encoder states: an entry of the conditioning-keyed LRU (`_cond_entry`).  A new entry
+        takes over the evicted one's buffer when it is large enough."""
+        def new(old):
+            n = _lib.lib().ce_dit_context_cache_bytes(self._handle, self._local_samples(txt.shape[0])[1], txt.shape[1])
+            if n < 0:
+                check(-1)
+            if old is not None and old["buf"].numel() >= n and old["buf"].device == self.device:
+                return dict(buf=old["buf"])
+            return dict(buf=torch.empty(n, dtype=torch.uint8, device=self.device))
+
+        e, hit = _cond_entry(self._ctx_cache, self._ctx_slots, txt_in, img_in, new)
+        return e["buf"], int(hit)
 
     def _check_forward(self, rc, ctx_buf, ctx_reuse) -> None:
-        """check(rc) of a forward call.  A forward that was to fill a context-cache slot and failed may have stopped before writing all
-        of it (the K/V of later layers are projected inside the layer loop), so the slot is dropped rather than reused."""
-        if rc != 0 and ctx_buf is not None and not ctx_reuse:
-            self._ctx_cache = [e for e in self._ctx_cache if e["buf"] is not ctx_buf]
+        """check(rc) of a forward call: a failed call drops the context-cache slot it was to fill (it may have stopped part way)."""
+        if rc != 0:
+            self._drop_unfilled(ctx_buf, ctx_reuse)
         check(rc)
+
+    def _drop_unfilled(self, ctx_buf, ctx_reuse) -> None:
+        if ctx_buf is not None and not ctx_reuse:
+            self._ctx_cache = [e for e in self._ctx_cache if e["buf"] is not ctx_buf]
 
     def clear_context_cache(self) -> None:
         self._ctx_cache = []
@@ -767,19 +813,18 @@ class ChronoEditTransformer3DModel(nn.Module):
         _tc.coefficients(tea_cache_model_id)   # raises on an unknown id, listing the supported ones
         if int(num_inference_steps) < 1:
             raise ValueError("num_inference_steps must be >= 1")
-        if getattr(self, "_sp_state", None):
-            raise CEError("TeaCache is not built for sequence parallelism: disable it first")
+        self._refuse_token_split(teacache=True)
         self._teacache = dict(thresh=float(tea_cache_l1_thresh), steps=int(num_inference_steps), model_id=tea_cache_model_id)
         self.reset_teacache()
 
     def disable_teacache(self) -> None:
         """Back to the plain forward.  The call records stay readable until the next enable_teacache / reset_teacache."""
         self._teacache = None
-        self._drop_teacache_states()
+        self._tc_states = []
 
     def reset_teacache(self) -> None:
         """Forget every conditioning's state and the call records: the next call of each conditioning is step 0."""
-        self._drop_teacache_states()
+        self._tc_states = []
         self._tc_records = []
         self._tc_next_slot = 0
 
@@ -792,26 +837,16 @@ class ChronoEditTransformer3DModel(nn.Module):
         """One record per forward since enable_teacache / reset_teacache: (slot, step, rel, acc, computed)."""
         return tuple(self._tc_records)
 
-    def _drop_teacache_states(self) -> None:
-        self._tc_states = []
-        self._tc_probe = {}
-
     def _teacache_state(self, txt_in, img_in) -> Dict[str, Any]:
-        """The state of this conditioning, keyed like `_context_slot`: the same tensor objects at the same version.  Up to
-        `_tc_slots` states, least recently used dropped first; a new state starts at step 0."""
-        ver = lambda t: None if t is None else t._version
-        for i, e in enumerate(self._tc_states):
-            if e["txt"] is txt_in and e["img"] is img_in and e["txt_v"] == ver(txt_in) and e["img_v"] == ver(img_in):
-                self._tc_states.append(self._tc_states.pop(i))
-                return e
-        if len(self._tc_states) >= self._tc_slots:
-            self._tc_states.pop(0)
-        c = self._teacache
-        e = dict(txt=txt_in, img=img_in, txt_v=ver(txt_in), img_v=ver(img_in), slot=self._tc_next_slot,
-                 policy=_tc.TeaCacheState(c["steps"], c["thresh"], c["model_id"]), prev=None, spare=None, resid=None, geom=None)
-        self._tc_next_slot += 1
-        self._tc_states.append(e)
-        return e
+        """The state of this conditioning: an entry of the conditioning-keyed LRU (`_cond_entry`) of up to `_tc_slots` states.  A
+        new state starts at step 0."""
+        def new(_):
+            c = self._teacache
+            self._tc_next_slot += 1
+            return dict(slot=self._tc_next_slot - 1, policy=_tc.TeaCacheState(c["steps"], c["thresh"], c["model_id"]), prev=None,
+                        spare=None, resid=None, geom=None)
+
+        return _cond_entry(self._tc_states, self._tc_slots, txt_in, img_in, new)[0]
 
     def _teacache_forward(self, x, t, txt, img, out, txt_in, img_in) -> None:
         """One TeaCache call: the probe (time path, and the two sums against the previous call's modulation when the rule
@@ -820,7 +855,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         split the rule sees only this rank's samples: the probe takes their timesteps, and the modulation and the residual are theirs."""
         B, _, T, H, W = x.shape
         D = self.config.num_attention_heads * self.config.attention_head_dim
-        bp = getattr(self, "_bp_state", None)
+        bp = self._bp_state
         if bp and B % bp["world"]:   # before the probe's launches; the forward itself would refuse it too
             raise CEError(f"batch split: a batch of {B} does not divide over {bp['world']} ranks.  Only a call that carries the whole CFG "
                           "pair is split: the unchanged diffusers pipeline's batch-1 calls are not split.  Run the pair as one batch-2 call")
@@ -850,8 +885,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         """ce_dit_teacache_probe: the timestep modulation of t into `cur` ([B * 6D] bf16); with `prev` also the two sums, read
         back through pinned memory (the only device-to-host read of a TeaCache call).  Returns (sum |cur - prev|, sum |prev|)
         or None."""
-        if not self._packed:
-            self.pack_weights()
+        self._ensure_packed()
         L = _lib.lib()
         B = t.numel()
         pr = self._tc_probe
@@ -888,8 +922,7 @@ class ChronoEditTransformer3DModel(nn.Module):
             return
         B, _, T, H, W = x.shape
         Lt = txt.shape[1]
-        ws = self._workspace(self._local_samples(B)[1], T, H, W, Lt)
-        with torch.cuda.device(self.device):
+        with self._pre_launch(x.shape, Lt) as (ws, _, _), torch.cuda.device(self.device):
             check(L.ce_dit_forward_cached(self._handle, ptr(x), ptr(t), ptr(resid), resid.numel() * 2, ptr(out), B, T, H, W, Lt,
                                           ptr(ws), ws.numel(), current_stream()))
 
@@ -901,36 +934,27 @@ class ChronoEditTransformer3DModel(nn.Module):
         C-ABI call (ce_dit_forward_host_ex).  Returns the host sample tensor (and, with `return_device_sample`, a view of the same
         sample still on the device -- valid until the next forward_host call -- for the scheduler step)."""
         self._refuse_cp("forward_host")
-        if self._lora_active() and getattr(self, "_sp_state", None):
-            raise CEError("run-time LoRA (set_adapters) is not built for sequence parallelism: call disable_lora() or disable the "
-                          "sequence-parallel mode first")
+        self._refuse_token_split(lora=self._lora_active())
+        self._check_inputs(hidden_states, timestep, encoder_hidden_states, encoder_hidden_states_image, host=True, out=out)
         self._lora_sync(self._lora_scale)   # no attention_kwargs here: the scale of the last forward() call
-        if not self._packed:
-            self.pack_weights()
         B, C, T, H, W = hidden_states.shape
         Lt = encoder_hidden_states.shape[1]
-        for tns in (hidden_states, encoder_hidden_states):
-            if tns.device.type != "cpu" or tns.dtype != torch.bfloat16 or not tns.is_contiguous():
-                raise CEError("forward_host expects contiguous CPU bf16 tensors")
-        t = timestep.to(torch.float32).contiguous()
+        t = timestep.to(torch.float32).reshape(-1).expand(B).contiguous()   # the C call copies B timesteps
         L = _lib.lib()
-        ws = self._workspace(self._local_samples(B)[1], T, H, W, Lt)
-        n = L.ce_dit_host_staging_bytes(self._handle, B, T, H, W, Lt)
-        st = self._workspaces.get("staging")
-        if st is None or st.numel() < n:
-            st = torch.empty(n, dtype=torch.uint8, device=self.device)
-            self._workspaces["staging"] = st
-        if out is None:
-            out = torch.empty(B, self.config.out_channels, T, H, W, dtype=torch.bfloat16).pin_memory()
-        ctx_buf, ctx_reuse = (None, 0)
-        if self.cache_context:
-            ctx_buf, ctx_reuse = self._context_slot(encoder_hidden_states, encoder_hidden_states_image, encoder_hidden_states,
-                                                    encoder_hidden_states_image)
-        with torch.cuda.device(self.device):
-            self._check_forward(L.ce_dit_forward_host_ex(self._handle, ptr(hidden_states), ptr(t), ptr(encoder_hidden_states),
-                                                         ptr(encoder_hidden_states_image), ptr(out), B, T, H, W, Lt, ptr(st), st.numel(),
-                                                         ptr(ws), ws.numel(), ptr(ctx_buf), ctx_buf.numel() if ctx_buf is not None else 0,
-                                                         ctx_reuse, current_stream()), ctx_buf, ctx_reuse)
+        cond = (encoder_hidden_states, encoder_hidden_states_image, encoder_hidden_states, encoder_hidden_states_image)
+        with self._pre_launch(hidden_states.shape, Lt, cond) as (ws, ctx_buf, ctx_reuse):
+            n = L.ce_dit_host_staging_bytes(self._handle, B, T, H, W, Lt)
+            st = self._workspaces.get("staging")
+            if st is None or st.numel() < n:
+                st = torch.empty(n, dtype=torch.uint8, device=self.device)
+                self._workspaces["staging"] = st
+            if out is None:
+                out = torch.empty(B, self.config.out_channels, T, H, W, dtype=torch.bfloat16).pin_memory()
+            with torch.cuda.device(self.device):
+                self._check_forward(L.ce_dit_forward_host_ex(
+                    self._handle, ptr(hidden_states), ptr(t), ptr(encoder_hidden_states), ptr(encoder_hidden_states_image), ptr(out),
+                    B, T, H, W, Lt, ptr(st), st.numel(), ptr(ws), ws.numel(), ptr(ctx_buf),
+                    ctx_buf.numel() if ctx_buf is not None else 0, ctx_reuse, current_stream()), ctx_buf, ctx_reuse)
         if not return_device_sample:
             return out
         off = L.ce_dit_host_staging_sample_offset(self._handle, B, T, H, W, Lt)
@@ -1029,7 +1053,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         self._lora_gen += 1
         if self._lora_set:
             self._lora_set = []
-            self._lora_changed()
+            self._invalidate("results")
 
     @torch.no_grad()
     def fuse_lora(self, *args, **kwargs) -> int:
@@ -1084,8 +1108,7 @@ class ChronoEditTransformer3DModel(nn.Module):
             self._lora_adapters.clear()   # merged: a second fuse_lora must not add them again
             self._lora_set = []           # and a (switched-off) run-time set of them is gone with them
             self._lora_gen += 1
-        self._ctx_cache = []              # cross-attention K/V cached from the old weights are stale
-        self._drop_teacache_states()      # and so are the TeaCache residuals
+        self._invalidate("results")
         return n
 
     # ------------------------------------------------------------------------------------------ run-time LoRA
@@ -1118,22 +1141,21 @@ class ChronoEditTransformer3DModel(nn.Module):
             raise CEError(f"set_adapters: an adapter is named twice in {names}")
         for n in names:
             self._lora_entries(n)
-        if names and getattr(self, "_sp_state", None):
-            raise CEError("run-time LoRA (set_adapters) is not built for sequence parallelism: disable the sequence-parallel mode first")
+        self._refuse_token_split(lora=bool(names))
         self._lora_set = list(zip(names, ws))
         self._lora_on = True
-        self._lora_changed()
+        self._invalidate("results")
         if self.device.type == "cuda":
             self._lora_sync(self._lora_scale)
 
     def disable_lora(self) -> None:
         """Switch the active set off (the forward is the plain one again); enable_lora() switches it back on."""
         self._lora_on = False
-        self._lora_changed()
+        self._invalidate("results")
 
     def enable_lora(self) -> None:
         self._lora_on = True
-        self._lora_changed()
+        self._invalidate("results")
 
     def delete_adapters(self, adapter_names) -> None:
         """Drop loaded adapters, and take them out of the active set."""
@@ -1147,7 +1169,7 @@ class ChronoEditTransformer3DModel(nn.Module):
         kept = [(n, w) for n, w in self._lora_set if n not in names]
         if kept != self._lora_set:
             self._lora_set = kept
-            self._lora_changed()
+            self._invalidate("results")
 
     def active_adapters(self) -> list:
         """The names of the set chosen with set_adapters, in activation order (also while disable_lora() has it off)."""
@@ -1155,12 +1177,6 @@ class ChronoEditTransformer3DModel(nn.Module):
 
     def _lora_active(self) -> bool:
         return self._lora_on and bool(self._lora_set)
-
-    def _lora_changed(self) -> None:
-        """A set, weight or on / off change: what was computed with the old set is stale."""
-        self._ctx_cache = []
-        self._graphs = {}
-        self._drop_teacache_states()
 
     def _lora_entries(self, name):
         """[(layer, target, part, A, B, alpha or None)] of a loaded adapter; refuses a module that is not a block linear layer."""
@@ -1210,7 +1226,7 @@ class ChronoEditTransformer3DModel(nn.Module):
     def _lora_sync(self, scale: float) -> None:
         """Bring the handle's LoRA tables to the active set at `scale` (attention_kwargs["scale"]).  Nothing happens while they are
         current, so the per-step path does no work for them; a new set packs the factors, a new scale only rescales B_cat
-        = bf16(B_raw * col_scale * scale) on the device.  Any change drops the workspaces and everything _lora_changed drops."""
+        = bf16(B_raw * col_scale * scale) on the device.  Any change drops the workspaces and what was computed with the old tables."""
         want = self._lora_active()
         key = (self._lora_gen, tuple(self._lora_set), str(self.device), float(scale)) if want else None
         if key == self._lora_key:
@@ -1233,8 +1249,8 @@ class ChronoEditTransformer3DModel(nn.Module):
             check(L.ce_dit_set_lora(h, None, None, None, 0))
             self._lora_tables = {}
         self._lora_key = key
-        self._workspaces = {}
-        self._lora_changed()
+        self._invalidate("results")   # what was computed with the old tables
+        self._invalidate("layout")    # their scratch is part of the workspace
 
     # ------------------------------------------------------------------------------------------ loading
     @classmethod

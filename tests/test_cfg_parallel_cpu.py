@@ -184,3 +184,30 @@ def test_teacache_under_the_batch_split_sizes_by_the_local_samples(host_only_con
         m(x[:1], torch.tensor([500]), txt[:1], img[:1])
     assert len(seen) == 4                                           # refused before the probe
     parallel.disable_cfg_parallel(m)
+
+
+# what each split's configure / disable drops: the model's "layout" (token split) and "results" (the CFG splits) kinds of change
+_RESULTS = ("_ctx_cache", "_tc_states", "_graphs")
+DROPS = {"token_split_configure": ("_workspaces", "_graphs"), "batch_split_configure": _RESULTS, "batch_split_disable": _RESULTS,
+         "call_pair_configure": _RESULTS, "call_pair_disable": _RESULTS}
+
+
+@pytest.mark.parametrize("event", sorted(DROPS))
+def test_split_changes_drop_their_caches(event, host_only_configure):
+    m, _ = _handle()
+    split, what = event.rsplit("_", 1)
+    configure = {"token_split": parallel.configure_sequence_parallel, "batch_split": parallel.configure_cfg_parallel,
+                 "call_pair": parallel.configure_cfg_parallel_calls}[split]
+    m._packed = True   # stands in for the weights the token split's configure would pack on a device
+    if what == "disable":
+        configure(m, 1, [4096, 8192], 1 << 20, {})
+    cached = {"_ctx_cache": [dict(buf=None)], "_tc_states": [dict()], "_graphs": {"k": 1}, "_workspaces": {"w": 2}}
+    for k, v in cached.items():
+        setattr(m, k, v)
+    if what == "disable":
+        {"batch_split": parallel.disable_cfg_parallel, "call_pair": parallel.disable_cfg_parallel_calls}[split](m)
+    else:
+        configure(m, 1, [4096, 8192], 1 << 20, {})
+    assert {k: getattr(m, k) == v for k, v in cached.items()} == {k: k not in DROPS[event] for k in cached}
+    for disable in (parallel.disable_sequence_parallel, parallel.disable_cfg_parallel, parallel.disable_cfg_parallel_calls):
+        disable(m)

@@ -129,6 +129,23 @@ def test_skipped_forward_against_the_oracle_head_and_batch_invariant():
 
 
 @gpu
+def test_pack_weights_drops_the_states():
+    """The lazy pack of the first call keeps the state it was made for; an explicit pack_weights() re-registers the weights, so the
+    residuals computed from the old ones are dropped, as load_state_dict and fuse_lora drop them."""
+    dev = torch.device("cuda", 0)
+    m, _, _, (x, t, text, img) = _tiny(dev, "bf16")
+    m.enable_teacache(1e9, num_inference_steps=4)
+    m(x, t, text, img)
+    m(x, t, text, img)
+    assert [r.step for r in m.teacache_records] == [0, 1] and m._tc_states
+    m.pack_weights()
+    assert m._tc_states == []
+    m(x, t, text, img)
+    torch.cuda.synchronize()
+    assert m.teacache_records[-1].step == 0 and m.teacache_records[-1].computed
+
+
+@gpu
 @pytest.mark.parametrize("name", ["edit_5f", "reason_cut"])
 def test_pipeline_with_teacache(name):
     from chronoedit_b200 import teacache as TCP

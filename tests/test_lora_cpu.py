@@ -182,3 +182,15 @@ def test_new_weights_drop_the_context_cache():
     m._ctx_cache = [dict(txt=None, img=None, txt_v=None, img_v=None, buf=None)]
     m.to(torch.bfloat16)
     assert m._ctx_cache == []
+
+
+def test_fuse_lora_drops_captured_graphs():
+    """A captured graph replays K/V projections of the weights fuse_lora changed, as the context cache would serve them."""
+    import chronoedit_b200 as ce
+
+    m = ce.ChronoEditTransformer3DModel(num_attention_heads=2, in_channels=36, ffn_dim=256, num_layers=1, image_dim=1280, added_kv_proj_dim=256,
+                                        text_dim=64, cache_context=True)
+    m._graphs, m._ctx_cache = {"k": object()}, [dict(buf=None)]
+    w = m.blocks[0].attn2.to_k.weight
+    m.fuse_lora({"blocks.0.attn2.to_k.lora_A.weight": torch.zeros(2, w.shape[1]), "blocks.0.attn2.to_k.lora_B.weight": torch.zeros(w.shape[0], 2)})
+    assert m._graphs == {} and m._ctx_cache == []

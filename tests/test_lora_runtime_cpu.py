@@ -189,7 +189,8 @@ def test_a_new_set_weight_or_scale_drops_cached_state():
     m.set_adapters("a")
     _run(m, inp)
     for change in (lambda: _run(m, inp, attention_kwargs={"scale": 0.5}), lambda: m.set_adapters("a", 0.3), m.disable_lora,
-                   m.enable_lora, lambda: m.set_adapters([])):
+                   m.enable_lora, lambda: (m.load_lora_adapter(_lora(m, 4, 5), adapter_name="a"), _run(m, inp)),
+                   lambda: m.set_adapters([])):
         m._ctx_cache, m._graphs, m._tc_states = [dict(buf=None)], {"k": 1}, [dict()]
         change()
         assert m._ctx_cache == [] and m._graphs == {} and m._tc_states == []

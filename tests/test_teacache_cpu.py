@@ -135,7 +135,7 @@ def test_geometry_change_forces_a_compute():
     assert r[2].rel is not None and r[2].acc == 0.0
 
 
-@pytest.mark.parametrize("how", ["to", "load_state_dict", "fuse_lora", "enable_fp8", "reset"])
+@pytest.mark.parametrize("how", ["to", "load_state_dict", "load_state_dict_assign", "fuse_lora", "enable_fp8", "reset"])
 def test_state_is_dropped(how):
     m = _mirror()
     m.enable_teacache(1e9, num_inference_steps=4)
@@ -146,6 +146,8 @@ def test_state_is_dropped(how):
         m.to("cpu")
     elif how == "load_state_dict":
         m.load_state_dict(dict(m.state_dict()))
+    elif how == "load_state_dict_assign":
+        m.load_state_dict({k: v.clone() for k, v in m.state_dict().items()}, assign=True)
     elif how == "fuse_lora":
         w = m.blocks[0].ffn.net[2].weight
         m.fuse_lora({"blocks.0.ffn.net.2.lora_A.weight": torch.zeros(2, w.shape[1], dtype=torch.bfloat16),
